@@ -28,6 +28,9 @@ METRIC = "DiffusionNetBlock forward Mverts/sec at V=200k,K=128,C=128; 1/2/4/8 GP
 WORKLOAD = "block_fwd V=200000 K=128 C=128, 1 mesh per GPU"      # identical in both arms (config.workload)
 
 
+DUMP_ROWS = 65536                                       # rows of the block output written by --dump-outputs
+
+
 def flops_per_vertex(K, C, r=NNZ_ROW):
     return 4 * K * C + 18 * C * C + 4 * r * C           # SURVEY.md 8d (reference op count)
 
@@ -37,7 +40,9 @@ def bytes_per_vertex(K, C, r=NNZ_ROW, s=4):
 
 
 def peaks():
-    p = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # fallback: NVIDIA's H100 SXM data-sheet peaks (dense, 700 W card), never reached in practice; MEASURED_PEAKS.json
+    # overrides them with measured rates
+    p = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data-sheet peak"}
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
             m = json.load(fh)
@@ -371,7 +376,7 @@ def run_aux(args, rank, world, local):
                     for (n1, p1), (n2, p2) in zip(net.named_parameters(), rnet.named_parameters()):
                         worst = max(worst, float((p1.grad - p2.grad).abs().max() / (p2.grad.abs().max() + 1e-30)))
                     gpu_base = {"value": V / (rms * 1e-3) / 1e6, "unit": "Mverts/s", "ms_per_step": rms,
-                                "kind": "reference", "how": "reference DiffusionNet, torch eager autograd on this B200, "
+                                "kind": "reference", "how": "reference DiffusionNet, torch eager autograd on this GPU, "
                                 "fp32 (TF32 off)", "speedup_ours": rms / ms, "max_rel_grad_diff_vs_ours": worst}
                 torch.backends.cuda.matmul.allow_tf32 = prev
             except Exception as exc:
@@ -474,18 +479,19 @@ def run_aux(args, rank, world, local):
                         rms, _ = timed(rf)
                         err = float((fwd() - rf()).abs().max() / rf().abs().max())
                     gpu_base = {"value": V / (rms * 1e-3) / 1e6, "unit": "Mverts/s", "ms_per_step": rms, "kind": "reference",
-                                "how": "reference DiffusionNet (4 x 256), torch eager on this B200, fp32 (TF32 off)",
+                                "how": "reference DiffusionNet (4 x 256), torch eager on this GPU, fp32 (TF32 off)",
                                 "speedup_ours": rms / ms, "max_rel_diff_vs_ours": err}
                 torch.backends.cuda.matmul.allow_tf32 = prev
             except Exception as exc:
                 gpu_base = {"unavailable": repr(exc)[:200]}
+        bf16_peak = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
         line.update({"metric": "DiffusionNet (4 blocks, C_width=256) forward Mverts/sec at V=200k,K=128, bf16 arithmetic",
                      "value": world * V / (ms * 1e-3) / 1e6, "ms_per_step": ms, "scaling": "weak", "dtype": "bf16 (fp32 accumulate, fp32 tensors in HBM)",
                      "config": {"workload": "config3 net_fwd V={} K=128 C=256 4 blocks, 1 mesh per GPU".format(V), "engine": eng,
                                 "block_ms": blk_ms, "block_stages_ms": stages},
-                     "roofline": {"bound": "tensor", "kernel": "rows_chain16_kernel (MiniMLP 768-256-256-256 + skip)",
-                                  "achieved": mlp_flops / (mlp_ms * 1e-3) / 1e12, "peak": pk["bf16_tflops_sustained"],
-                                  "unit": "TFLOP/s", "frac": mlp_flops / (mlp_ms * 1e-3) / 1e12 / pk["bf16_tflops_sustained"],
+                     "roofline": {"bound": "tensor", "kernel": "rows_chain_kernel (MiniMLP 768-256-256-256 + skip, one launch per 256-wide layer)",
+                                  "achieved": mlp_flops / (mlp_ms * 1e-3) / 1e12, "peak": bf16_peak,
+                                  "unit": "TFLOP/s", "frac": mlp_flops / (mlp_ms * 1e-3) / 1e12 / bf16_peak,
                                   "hbm_frac": 4.0 * V * C3 * 4 / (mlp_ms * 1e-3) / 1e9 / pk["hbm_gbs"],
                                   "block_tflops": blk_flops / (blk_ms * 1e-3) / 1e12,
                                   "block_hbm_frac_fp32_bytes": blk_bytes / (blk_ms * 1e-3) / 1e9 / pk["hbm_gbs"],
@@ -546,7 +552,13 @@ def main():
     ap.add_argument("--e2e-steps", type=int, default=8)
     ap.add_argument("--workload", default="block_fwd", choices=["block_fwd", "fwd_bwd", "train", "small_batch", "config3"],
                     help="block_fwd = the BASELINE metric (default); the others are BASELINE configs 2 / 5 / 4 / 3")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="block_fwd: after the timed steps, write the block output of the last timed step as float32 "
+                         "DIR/block_out_rows.npy (a fixed sample of {} of its rows: numpy default_rng(0).choice(V, {}, "
+                         "replace=False), sorted) so that two builds can be compared output for output".format(DUMP_ROWS, DUMP_ROWS))
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "block_fwd" or args.impl != "ours"):
+        ap.error("--dump-outputs is implemented for --impl ours --workload block_fwd")
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -607,6 +619,12 @@ def main():
     ev1.record()
     barrier()
     launches = lib.dn_kernel_launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        rows = np.sort(np.random.default_rng(0).choice(V, DUMP_ROWS, replace=False))
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "block_out_rows.npy"),
+                out[0][torch.from_numpy(rows).to(dev)].float().cpu().numpy())
     t_end = time.time()
     ms_total = torch.tensor([ev0.elapsed_time(ev1)], device=dev)
     if world > 1:
@@ -690,9 +708,6 @@ def main():
         lins = blk.mlp.linears()
         nprof = 10
         acc = [0.0] * len(dn.ops.PROFILE_STAGES)
-        import ctypes
-        lib.dn_debug_gf_gather_ms.restype = ctypes.c_float
-        gather_acc = 0.0
         with torch.no_grad():
             for it in range(nprof + 2):
                 prof = []
@@ -700,9 +715,7 @@ def main():
                                          [l.weight for l in lins], [l.bias for l in lins], True, profile=prof)
                 if it >= 2:
                     acc = [a + b for a, b in zip(acc, prof)]
-                    gather_acc += float(lib.dn_debug_gf_gather_ms())     # the x-only gather's share of stage [4] (0: old route)
         stages = {n + "_ms": a / nprof for n, a in zip(dn.ops.PROFILE_STAGES, acc)}
-        gather_x_ms = gather_acc / nprof
 
     # ---- the reference beside it (rank 0, N=1 only; bounded samples) ----
     cpu, gpu_base = None, None
@@ -726,7 +739,7 @@ def main():
             gms = a.elapsed_time(b) / 10
             torch.backends.cuda.matmul.allow_tf32 = prev
             gpu_base = {"value": V / (gms * 1e-3) / 1e6, "unit": "Mverts/s", "ms_per_step": gms, "kind": gkind,
-                        "how": "reference DiffusionNetBlock, torch eager on this B200, fp32 (TF32 off), inputs resident, "
+                        "how": "reference DiffusionNetBlock, torch eager on this GPU, fp32 (TF32 off), inputs resident, "
                                "10 steps after 3 warm-up",
                         "speedup_ours": gms / ms_step}
             del gstep
@@ -745,49 +758,23 @@ def main():
         tf32 = measure_tf32_peak(dev)
         C, K = C_WIDTH, K_EIG
         nnz = NNZ_ROW * V
-        # tensor-pipe work per fp32 product in TF32-pass equivalents: the default tc3x chain issues, per 32-wide K-stage,
-        # 4 kind::tf32 MMAs (hi*hi) + 4 kind::f16 bf16 MMAs (K = 16: both correction terms) = 8 MMA slots where plain
-        # 3xTF32 needs 12 -> 2 equivalents (DN_TC_HYBRID=0 restores 3); bf16 engine: half a TF32 pass
-        hybrid = os.environ.get("DN_TC_HYBRID", "1") != "0"
-        passes = {"tc3x": 2.0 if hybrid else 3.0, "tc1x": 1.0, "bf16": 0.5}.get(args.engine, 3.0)
+        # tensor-pipe work per fp32 product in TF32-pass equivalents: tc3x issues lo*hi + hi*lo + hi*hi (3 TF32 MMAs);
+        # bf16 engine: half a TF32 pass
+        passes = {"tc3x": 3.0, "tc1x": 1.0, "bf16": 0.5}.get(args.engine, 3.0)
         # algorithmic (minimum) HBM bytes and useful fp32 flops per launch of each kernel (DESIGN.md section 4)
         work = {
-            "to_basis": (4 * V * (K + C) + 4 * V, 2 * K * C * V, "to_basis_kernel (split-V tcgen05)"),
+            "to_basis": (4 * V * (K + C) + 4 * V, 2 * K * C * V, "to_basis_kernel (split-V wgmma)"),
             "spectral_scale": (0, 0, "(separate launch only on the SIMT engine; part of pack_weights_kernel here)"),
-            "pack_weights": (4 * 148 * K * C + 3 * 4 * (K * C + 2 * C * C + 5 * C * C), 0,
+            "pack_weights": (4 * 132 * K * C + 3 * 4 * (K * C + 2 * C * C + 5 * C * C), 0,
                              "pack_weights_kernel (split-V partial reduction + exp(-lambda t) scale + hi/lo weight pack)"),
-            # default route at C = 128 (DN_GF_TC=1): from_basis alone, then the gradient features as an x-only gather
-            # (writes [gX|gY]) + two tcgen05 GEMM launches with the inner product / tanh epilogue
-            "from_basis_pq": (4 * V * (K + C), 2 * K * C * V, "rows_chain3_kernel (from_basis)"),
-            "grad_features_gather": (4 * V * (C + 2 * C) + 12 * nnz + 4 * V + 4 * V * (2 * C + C), (4 * NNZ_ROW * C + 8 * C * C) * V,
-                                     "spmm_gxy_blk_kernel (x-only CSR gather) + 2 x rows_chain3_kernel ([gX|gY] W_rot, "
-                                     "tanh(gX*Bre+gY*Bim) epilogue)"),
-            "mlp": (4 * V * (3 * C + C), 10 * C * C * V, "rows_chain3_kernel (MiniMLP + skip, 3 fused layers)"),
+            "from_basis_pq": (4 * V * (K + C + 2 * C), (2 * K * C + 4 * C * C) * V, "rows_chain_kernel (from_basis, [P|Q])"),
+            "grad_features_gather": (4 * V * (3 * C + C) + 12 * nnz + 4 * V, 12 * NNZ_ROW * C * V,
+                                     "spmm_features_blk_kernel (CSR gather of x, P, Q + inner product + tanh)"),
+            "mlp": (4 * V * (3 * C + C), 10 * C * C * V, "rows_chain_kernel (MiniMLP + skip, 3 fused layers)"),
         }
-        try:   # per-launch DRAM traffic of each kernel from the committed ncu --set full capture of this command
-            with open(os.path.join(ROOT, "profiles", "r02_traffic.json")) as fh:
-                traffic = json.load(fh)
-        except Exception:
-            traffic = {}
-        tc_route = gather_x_ms > 0.0      # tensor-core gradient features (default at C = 128): stage [4] is three launches
-        if not tc_route:                  # commuted route (DN_GF_TC=0): [P|Q] fused behind from_basis, one gather kernel
-            work["from_basis_pq"] = (4 * V * (K + C + 2 * C), (2 * K * C + 4 * C * C) * V,
-                                     "rows_chain3_kernel (from_basis -> [P|Q], 2 fused layers)")
-            work["grad_features_gather"] = (4 * V * (3 * C + C) + 12 * nnz + 4 * V, 12 * NNZ_ROW * C * V,
-                                            "spmm_features_blk_kernel (CSR gather of x, P, Q + inner product + tanh)")
         kernels = []
         names = list(dn.ops.PROFILE_STAGES)
         times = {n: stages[n + "_ms"] for n in names}
-        if tc_route:
-            i = names.index("grad_features_gather")
-            names[i:i + 1] = ["grad_gather_x", "grad_dots_gemm"]
-            times["grad_gather_x"] = gather_x_ms
-            times["grad_dots_gemm"] = (stages["grad_features_gather_ms"] - gather_x_ms) / 2      # per launch (two launches)
-            work["grad_gather_x"] = (4 * V * (C + 2 * C) + 12 * nnz + 4 * V, 4 * NNZ_ROW * C * V,
-                                     "spmm_gxy_blk_kernel (x-only CSR gather, writes [gX|gY])")
-            # (the epilogue's second read of the 64 gX / gY columns it needs comes out of L2: not counted)
-            work["grad_dots_gemm"] = (4 * V * (2 * C + C // 2), 4 * C * C * V,
-                                      "rows_chain3_kernel ([gX|gY] W_rot for 64 channels, tanh(gX*Bre+gY*Bim) epilogue; one of 2 launches)")
         for name in names:
             ms = times[name]
             by, fl, kname = work[name]
@@ -799,22 +786,19 @@ def main():
             ent = {"stage": name, "kernel": kname, "ms": ms, "algorithmic_bytes": by, "useful_flops": fl,
                    "achieved_gbs": gbs, "hbm_frac": gbs / pk["hbm_gbs"],
                    "issued_tf32_tflops": passes * tfl, "tf32_frac": passes * tfl / tf32["tf32_tflops"],
-                   "bound": "tensor" if t_tc > t_hbm else "hbm", "floor_ms": max(t_tc, t_hbm) * 1e3,
-                   "traffic": traffic.get(name)}
+                   "bound": "tensor" if t_tc > t_hbm else "hbm", "floor_ms": max(t_tc, t_hbm) * 1e3}
             kernels.append(ent)
         dom = max(kernels, key=lambda e: e["ms"])
         if dom["bound"] == "tensor":
             roof = {"bound": "tensor", "achieved": dom["issued_tf32_tflops"], "peak": tf32["tf32_tflops"],
                     "unit": "TFLOP/s", "frac": dom["tf32_frac"],
-                    "note": "tensor-pipe work issued, in TF32-pass equivalents (tc3x: TF32 hi*hi + bf16 correction MMAs = 2 "
-                            "per fp32 product), over the cuBLAS TF32 GEMM rate measured in this run (burst); useful fp32 "
+                    "note": "tensor-pipe work issued, in TF32-pass equivalents (tc3x: 3 TF32 MMAs per fp32 product), over the cuBLAS TF32 GEMM rate measured in this run (burst); useful fp32 "
                             "flops are `achieved` / passes_equiv", "passes_equiv": passes}
         else:
             roof = {"bound": "hbm", "achieved": dom["achieved_gbs"], "peak": pk["hbm_gbs"], "unit": "GB/s",
                     "frac": dom["hbm_frac"],
                     "note": "algorithmic bytes per launch / CUDA-event time over the measured copy bandwidth"}
-        roof.update({"kernel": dom["kernel"], "ms": dom["ms"], "traffic": dom["traffic"],
-                     "traffic_source": "profiles/r02_traffic.json (one ncu --set full launch of this command)",
+        roof.update({"kernel": dom["kernel"], "ms": dom["ms"],
                      "peak_source": pk["source"], "tf32_peak": tf32, "bf16_peak_tflops": pk["bf16_tflops"],
                      "block_hbm_frac": bytes_per_vertex(K_EIG, C) * V / (ms_step * 1e-3) / 1e9 / pk["hbm_gbs"],
                      "block_tf32_frac": passes * (4 * K * C + 14 * C * C) * V / (ms_step * 1e-3) / 1e12 / tf32["tf32_tflops"]})
@@ -825,7 +809,7 @@ def main():
             "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": WORKLOAD, "engine": args.engine,
-                       "parallelism": "mesh-sharded x{}".format(world), "l2": "inputs (~330 MB/step) exceed the 126 MB L2",
+                       "parallelism": "mesh-sharded x{}".format(world), "l2": "inputs (~330 MB/step) exceed the 50 MB L2",
                        "gflop_per_step": flops_per_vertex(K_EIG, C_WIDTH) * V / 1e9,
                        "min_hbm_mb_per_step": bytes_per_vertex(K_EIG, C_WIDTH) * V / 1e6},
             "clocks": clocks, "gpu_launches": int(launches),

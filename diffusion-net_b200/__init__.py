@@ -1,4 +1,4 @@
-"""B200-native DiffusionNetBlock hot path behind the reference module API.
+"""H100-native (sm_90a) DiffusionNetBlock hot path behind the reference module API.
 
 Public surface mirrors ``diffusion_net`` (reference ``src/diffusion_net/__init__.py:1-3``):
 ``layers`` (DiffusionNet, DiffusionNetBlock, LearnedTimeDiffusion, SpatialGradientFeatures,

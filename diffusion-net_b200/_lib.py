@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI library (include/diffusion_net_b200.h).
 
 The shared object is built IN-TREE (``diffusion-net_b200/libdiffusion_net_b200.so``)
-with nvcc for sm_100a and loaded with ctypes -- plain pointers and sizes, no torch
+with nvcc for sm_90a (H100) and loaded with ctypes -- plain pointers and sizes, no torch
 types cross the boundary.  There is no CPU or library fallback: if the library is
 missing or a call fails, a RuntimeError is raised.
 """
@@ -14,10 +14,10 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libdiffusion_net_b200.so")
-SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_tc.cu", "dn_chain.cu", "dn_chain16.cu", "dn_capi.cu"]
+SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_tc.cu", "dn_capi.cu"]
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "diffusion_net_b200.h")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 ENGINE_SIMT, ENGINE_TC3X, ENGINE_TC1X, ENGINE_BF16 = 0, 1, 2, 3

@@ -27,9 +27,9 @@ constexpr int64_t kPartialFloats = 16ll << 20;  // 64 MiB split-V partial sums
 inline bool use_tc(int engine) { return engine == DN_ENGINE_TC3X || engine == DN_ENGINE_TC1X || engine == DN_ENGINE_BF16; }
 inline int tc_passes(int engine) { return engine == DN_ENGINE_TC1X ? 1 : (engine == DN_ENGINE_BF16 ? DN_PASSES_BF16 : 3); }
 
-// A tensor-core engine was requested but this contraction is outside the tcgen05 kernels' envelope and runs the exact
+// A tensor-core engine was requested but this contraction is outside the wgmma kernels' envelope and runs the exact
 // fp32 SIMT kernel instead (same result class or better, slower).  Said once per shape on stderr; DN_STRICT_TC=1 turns
-// it into DN_ERR_UNSUPPORTED so that a deployment never runs the slow path unnoticed.  A non-sm_100 device with a
+// it into DN_ERR_UNSUPPORTED so that a deployment never runs the slow path unnoticed.  A non-sm_90 device with a
 // tensor-core engine is always an error (DN_ERR_NOT_SM100): there is no multi-backend dispatch.
 int note_simt_fallback(const char* what, int K, int N) {
   static int strict = -1;
@@ -104,12 +104,12 @@ int run_chain(const DnRowsSrc& src, DnLayer* layers, int n_layers, int64_t V, in
 int to_basis_partials(const float* values, const float* basis, const float* massvec, int64_t V, int K, int C,
                       float* partial, int64_t partial_floats, int* P, int engine, cudaStream_t st) {
   if (use_tc(engine) && tc_supported_device() && tc_to_basis_supported(K, C) == DN_OK &&
-      (int64_t)148 * K * C <= partial_floats) {
+      (int64_t)dn_sm_count() * K * C <= partial_floats) {
     return tc_to_basis_partial(values, basis, massvec, V, K, C, partial, P, tc_passes(engine), st);
   }
   // wider than one accumulator set (C_width = 256): 128-column slices, each its own launch into the shared partials
   if (use_tc(engine) && tc_supported_device() && C > 128 && C % 128 == 0 && tc_to_basis_supported(K, 128) == DN_OK &&
-      (int64_t)148 * K * C <= partial_floats) {
+      (int64_t)dn_sm_count() * K * C <= partial_floats) {
     for (int c0 = 0; c0 < C; c0 += 128) {
       const int rc = tc_to_basis_partial(values + c0, basis, massvec, V, K, 128, partial + c0, P, tc_passes(engine), st, C, C);
       if (rc) return rc;
@@ -128,7 +128,7 @@ int to_basis_partials(const float* values, const float* basis, const float* mass
 int atb(const float* A, int64_t lda, int I, const float* B, int64_t ldb, int J, int64_t V, float* out, int64_t ld_out,
         int accumulate, float* part, int64_t part_floats, int engine, cudaStream_t st) {
   if (use_tc(engine) && tc_supported_device() && lda == I && ldb == J && tc_to_basis_supported(I, J) == DN_OK &&
-      (int64_t)148 * I * J <= part_floats) {
+      (int64_t)dn_sm_count() * I * J <= part_floats) {
     int P = 0;
     int rc = tc_to_basis_partial(B, A, nullptr, V, I, J, part, &P, tc_passes(engine), st);
     if (rc == DN_OK) return launch_reduce_partials_ld(part, P, I, J, out, ld_out, accumulate, st);
@@ -151,11 +151,6 @@ int one_layer(const DnRowsSrc& src, DnLayer& L, int64_t V, int engine, void* tc_
 }  // namespace
 
 long long g_dn_launches = 0;
-// bring-up: device time of the x-only gather inside stage [4] of the last dn_block_fwd_profile call (tools only)
-static cudaEvent_t g_gf_ev = nullptr;
-static float g_gf_gather_ms = 0.f;
-static bool g_gf_recorded = false;
-extern "C" float dn_debug_gf_gather_ms(void) { return g_gf_gather_ms; }
 
 extern "C" {
 
@@ -169,7 +164,7 @@ const char* dn_error_string(int code) {
     case DN_ERR_INVALID_ARGUMENT: return "diffusion_net_b200: invalid argument";
     case DN_ERR_UNSUPPORTED: return "diffusion_net_b200: unsupported shape/engine";
     case DN_ERR_WORKSPACE: return "diffusion_net_b200: workspace too small (see dn_workspace_bytes)";
-    case DN_ERR_NOT_SM100: return "diffusion_net_b200: tensor-core engine needs an sm_100 GPU";
+    case DN_ERR_NOT_SM100: return "diffusion_net_b200: tensor-core engine needs an sm_90 (H100) GPU";
     default: break;
   }
   if (code > 0) return cudaGetErrorString(static_cast<cudaError_t>(code));
@@ -361,7 +356,7 @@ int dn_learned_time_diffusion_bwd(const float* grad_out, const float* mass, cons
   int rc = to_basis_partials(grad_out, evecs, nullptr, V, K, C, partial, pf, &P, engine, st);
   if (rc) return rc;
   if (P > 4) {
-    // spectral_bwd walks the partials serially per channel: with the 148 split-V partials of the tensor-core kernel that
+    // spectral_bwd walks the partials serially per channel: with the ~132 split-V partials of the tensor-core kernel that
     // took 4.5 ms (V = 7k); sum them first (coalesced, parallel) and hand it one
     float* red = ws.take((int64_t)K * C);
     if (!red) return DN_ERR_WORKSPACE;
@@ -630,27 +625,9 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
   DnLayer L[3 + DN_MAX_LAYERS];
   L[0] = make_layer(S, C, 1, nullptr, 0, K, C, xd, C);
   int nfront = 1;
-  // Tensor-core gradient features (C_width = 128, learned rotations, fp32-grade / TF32 engines): gather only x_diffuse
-  // (gxy = [gradX x | gradY x], a third of the commuted route's gather traffic), then the complex-linear map as tcgen05
-  // GEMMs whose epilogue forms tanh(gX * Bre + gY * Bim) (layers.py:117-130) -- two launches of 64 channels each, so
-  // that the [Bre | Bim] accumulators (128 columns) ping-pong in TMEM.  DN_GF_TC=0 restores the commuted route
-  // ([P|Q] = x_diffuse [A_re; A_im]^T in front of a gather of x, P and Q).
-  static int gf_env = -1;
-  if (gf_env < 0) { const char* e = getenv("DN_GF_TC"); gf_env = (!e || atoi(e) != 0) ? 1 : 0; }
-  bool gf_tc = false;
-  DnRowsSrc src_gxy = one_src(pq, 2 * C, 2 * C);
-  if (p->with_gradient_features && rot && C == 128 && gf_env && use_tc(engine) && engine != DN_ENGINE_BF16 &&
-      tc_supported_device() && !(grad->patches && grad->patches->n_patches > 0)) {
-    for (int h = 0; h < 2; ++h) {
-      L[1 + h] = make_layer(p->A_re, C, 0, nullptr, 0, 2 * C, C, feat + h * 64, C);
-      L[1 + h].W2 = p->A_im; L[1 + h].rot_C = C; L[1 + h].rot_ch0 = h * 64;
-      L[1 + h].dots_src = pq + h * 64; L[1 + h].ld_dots = 2 * C; L[1 + h].dots_gy_col = C;
-    }
-    gf_tc = tc_rows_chain_supported(src_gxy, &L[1], 1, tc_passes(engine)) == DN_OK &&
-            tc_rows_chain_supported(src_gxy, &L[2], 1, tc_passes(engine)) == DN_OK;
-    if (gf_tc) nfront = 3;
-  }
-  if (p->with_gradient_features && !gf_tc) {
+  // gradient features, commuted route: [P|Q] = x_diffuse [A_re; A_im]^T as a dense layer in front of one CSR gather of
+  // x, P and Q that forms tanh(gX * Bre + gY * Bim) (layers.py:117-130)
+  if (p->with_gradient_features) {
     if (rot && npq > 256) {
       // [P|Q] wider than one tensor-core layer (C_width = 256): P and Q are separate layers writing the two halves
       L[1] = make_layer(p->A_re, C, 0, nullptr, 0, C, C, pq, npq);
@@ -690,17 +667,15 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
   const float* srcs[3] = {x_in, xd, feat};
   for (int q = 0; q < nsrc; ++q) { src_mlp.ptr[q] = srcs[q]; src_mlp.width[q] = C; src_mlp.ld[q] = C; }
   src_mlp.nsrc = nsrc;
-  // one launch packs (hi/lo split + UMMA layout) every weight the tensor-core kernels will stream
+  // one launch packs (hi/lo split + wgmma layout) every weight the tensor-core kernels will stream
   const bool tc = use_tc(engine) && tc_supported_device();
   const int passes = tc_passes(engine);
   const bool front_fused = tc && nfront == 2 && tc_rows_chain_supported(src_fb, &L[0], 2, passes) == DN_OK;
   bool tc_front = front_fused;
-  const DnRowsSrc& src_l12 = gf_tc ? src_gxy : src_pq;      // input of L[1], L[2]: raw gradients | x_diffuse
   if (tc && !front_fused) {
     tc_front = tc_rows_chain_supported(src_fb, &L[0], 1, passes) == DN_OK;
-    for (int l = 1; l < nfront; ++l) tc_front = tc_front && tc_rows_chain_supported(src_l12, &L[l], 1, passes) == DN_OK;
+    for (int l = 1; l < nfront; ++l) tc_front = tc_front && tc_rows_chain_supported(src_pq, &L[l], 1, passes) == DN_OK;
   }
-  if (gf_tc && !tc_front) return DN_ERR_UNSUPPORTED;         // (from_basis outside the envelope: cannot happen at C = 128)
   const bool tc_mlp = tc && tc_rows_chain_supported(src_mlp, &L[nfront], nm, passes) == DN_OK;
   if (head && !tc_mlp) return DN_ERR_UNSUPPORTED;
   // the spectral multiplier S = exp(-lambda t) * (reduced partial sums) is layer 0's weight: when the tensor-core path
@@ -737,7 +712,7 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
     if (front_fused) tc_choose_pack_fmt(src_fb, &L[0], 2, passes);
     else {
       tc_choose_pack_fmt(src_fb, &L[0], 1, passes);
-      for (int l = 1; l < nfront; ++l) tc_choose_pack_fmt(src_l12, &L[l], 1, passes);
+      for (int l = 1; l < nfront; ++l) tc_choose_pack_fmt(src_pq, &L[l], 1, passes);
     }
   }
   if (tc_mlp) tc_choose_pack_fmt(src_mlp, &L[nfront], nm, passes);
@@ -782,21 +757,12 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
     if ((rc = run_chain(src_fb, &L[0], 2, V, engine, nullptr, nullptr, tcws, tcws_bytes, st))) return rc;
   } else {
     if ((rc = run_chain(src_fb, &L[0], 1, V, engine, nullptr, nullptr, tcws, tcws_bytes, st))) return rc;
-    if (!gf_tc)
-      for (int l = 1; l < nfront; ++l)
-        if ((rc = run_chain(src_pq, &L[l], 1, V, engine, nullptr, nullptr, tcws, tcws_bytes, st))) return rc;
+    for (int l = 1; l < nfront; ++l)
+      if ((rc = run_chain(src_pq, &L[l], 1, V, engine, nullptr, nullptr, tcws, tcws_bytes, st))) return rc;
   }
   mark(4);
   // (a4+a5) sparse tangent gradient + complex inner product + tanh   [layers.py:216-226,128-130]
-  if (gf_tc) {
-    if ((rc = launch_spmm_gxy(grad, xd, V, C, pq, st))) return rc;
-    if (ev) {
-      if (!g_gf_ev) cudaEventCreate(&g_gf_ev);
-      if (g_gf_ev) { cudaEventRecord(g_gf_ev, st); g_gf_recorded = true; }
-    }
-    for (int l = 1; l < nfront; ++l)
-      if ((rc = tc_rows_chain(src_gxy, &L[l], 1, V, passes, tcws, tcws_bytes, st))) return rc;
-  } else if (p->with_gradient_features) {
+  if (p->with_gradient_features) {
     if ((rc = launch_spmm_features(grad, xd, pq, rot, V, C, feat, st))) return rc;
   }
   mark(5);
@@ -828,7 +794,7 @@ int dn_mesh_batch_plan(int n_meshes, const int32_t* n_rows_host, int sm_count, i
                        int32_t* tile_mesh_host, int32_t* tb_rows_host, int32_t* mesh_cta_begin_host) {
   if (n_meshes < 1 || !n_rows_host || !row_begin_host || !tile_mesh_host || !tb_rows_host || !mesh_cta_begin_host)
     return DN_ERR_INVALID_ARGUMENT;
-  if (sm_count < 1) sm_count = 148;
+  if (sm_count < 1) sm_count = 132;
   int64_t row = 0, chunks_total = 0;
   for (int b = 0; b < n_meshes; ++b) {
     if (n_rows_host[b] < 0) return DN_ERR_INVALID_ARGUMENT;
@@ -872,15 +838,12 @@ int dn_block_fwd_profile(const float* x_in, const float* mass, const float* eval
                          void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream, float* stage_ms_host) {
   if (!stage_ms_host) return DN_ERR_INVALID_ARGUMENT;
   cudaEvent_t ev[DN_PROFILE_STAGES + 1];
-  g_gf_recorded = false;
-  g_gf_gather_ms = 0.f;
   for (int i = 0; i <= DN_PROFILE_STAGES; ++i) DN_CUDA_TRY(cudaEventCreate(&ev[i]));
   int rc = block_fwd_impl(x_in, mass, evals, evecs, grad, p, V, K, C, out, workspace, ws_bytes, engine, stream, ev);
   if (rc == DN_OK) {
     rc = (int)cudaEventSynchronize(ev[DN_PROFILE_STAGES]);
     for (int i = 0; i < DN_PROFILE_STAGES && rc == DN_OK; ++i)
       rc = (int)cudaEventElapsedTime(&stage_ms_host[i], ev[i], ev[i + 1]);
-    if (rc == DN_OK && g_gf_recorded && cudaEventElapsedTime(&g_gf_gather_ms, ev[4], g_gf_ev) != cudaSuccess) cudaGetLastError();
   }
   for (int i = 0; i <= DN_PROFILE_STAGES; ++i) cudaEventDestroy(ev[i]);
   return rc;

@@ -261,7 +261,7 @@ int launch_compute_hks(const float* evals, const float* evecs, const float* scal
   if (V <= 0 || S <= 0) return DN_OK;
   if (S <= 16 && K % 32 == 0 && K >= 32 && K <= 256 && (K / 32 <= 4 || K == 256)) {
     int64_t blocks = (V + 31) / 32;       // 8 warps x 4 rows per block iteration
-    const int64_t cap = 148 * 8;          // grid-stride: the coefficient table is built once per warp (4 rows/iteration)
+    const int64_t cap = (int64_t)dn_sm_count() * 8;   // grid-stride: the coefficient table is built once per warp (4 rows/iteration)
     if (blocks > cap) blocks = cap;
     switch (K / 32) {
       case 1: hks_warp_kernel<1><<<(unsigned)blocks, 256, 0, st>>>(evals, evecs, scales, V, S, out); break;

@@ -1,4 +1,4 @@
-// Internal (non-ABI) declarations shared by the SIMT kernels, the tcgen05 kernels and the
+// Internal (non-ABI) declarations shared by the SIMT kernels, the wgmma kernels and the
 // C-ABI glue.  Everything here is device-pointer based; no torch types anywhere in csrc/.
 #pragma once
 #include <cuda_runtime.h>
@@ -33,9 +33,8 @@ struct DnLayer {
   const float* W2;       // optional second block: !w_trans: output rows n >= n_split come from W2[n - n_split]
   int n_split;           //   (stacks [A_re; A_im] without a copy);  w_trans: input rows k >= n_split come from W2[k - n_split]
   const float* prepacked;  // optional: weights already in the tensor-core layout (tc_pack_layers)
-  int pack_fmt;            // layout of `prepacked`: 0 = 16-wide chunks of [tf32 hi | tf32 lo] (round-1 kernels, 3xTF32);
-                           //   1 = 32-wide stages of [tf32 hi | bf16 (hi ; lo)] (rows_chain3_kernel, TF32 + bf16 corrections);
-                           //   2 = 64-wide stages of bf16 (rows_chain16_kernel, DN_ENGINE_BF16)
+  int pack_fmt;            // layout of `prepacked`: 0 = 16-wide K stages of [tf32 hi | tf32 lo] (TF32 engines);
+                           //   2 = 16-wide K stages of bf16 (DN_ENGINE_BF16)
   const float* bias;     // [N] or null
   int relu;
   const float* emul;     // optional elementwise multiplier [V][N] applied after the activation
@@ -51,14 +50,6 @@ struct DnLayer {
   // and 128-row tile t uses matrix tile_group[t] (device array)
   const int32_t* tile_group;
   int64_t group_stride;
-  // complex inner-product epilogue (last layer of a chain only; layers.py:128-130).  The layer computes
-  // [Bre | Bim] = in @ W^T with N/2 columns each for N/2 channels; the output (N/2 wide) is
-  //   tanh(gX * Bre + gY * Bim),  gX = dots_src[:, c], gY = dots_src[:, dots_gy_col + c]   (row stride ld_dots)
-  const float* dots_src;
-  int64_t ld_dots;
-  int dots_gy_col;
-  // weights given as the pair (W = A_re, W2 = A_im) of SpatialGradientFeatures acting on [gX | gY]: see PackJob::rot_C
-  int rot_C, rot_ch0;
   // linear head fused behind the last layer's epilogue (DiffusionNet.last_lin, layers.py:366-370): after bias / residual the
   // N-wide row y is NOT stored (out may be null); head_out[v][o] = head_b[o] + sum_n head_w[o][n] * y[n], o < head_n <= 8,
   // exact fp32 FMAs in the output warps
@@ -96,6 +87,8 @@ int simt_atb_partial_st(const float* A, int64_t lda, int I, const float* B, int6
 int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int accumulate, cudaStream_t st);
 
 // ---- shared small kernels (dn_simt.cu) ----
+// SM count of the current device (cached per device; 1 if it cannot be queried): sizes grids and split-V partials
+int dn_sm_count();
 // S[k][c] = exp(-evals[k]*max(t[c],1e-8)) * sum_p partial[p][k][c]; optionally writes the raw sum
 // (x_spec) and the clamped time back.  s_trans: write S as [c][k].
 int launch_spectral_scale(const float* partial, int P, const float* evals, float* time, int K, int C,
@@ -115,9 +108,6 @@ int launch_grad_spmm_pair(const dn_csr* g, const float* x, int64_t V, int C, flo
 // R-order fused features: feat = tanh(gX*Bre + gY*Bim) from gathers of xd, P, Q (pq = [P|Q], ld 2C or C).
 int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int rotations, int64_t V, int C,
                          float* feat, cudaStream_t st);
-// gxy[v] = [ (gradX @ x)[v] | (gradY @ x)[v] ]  (V x 2C, row-major): the gather of the tensor-core gradient-features
-// route (C = 128 or 256)
-int launch_spmm_gxy(const dn_csr* g, const float* x, int64_t V, int C, float* gxy, cudaStream_t st);
 int launch_features_bwd_local(const dn_csr* g, const float* xd, const float* pq, const float* feat,
                               const float* dfeat, int rotations, int64_t V, int C, float* U /*V x 4C*/,
                               cudaStream_t st);
@@ -130,7 +120,7 @@ int launch_spectral_bwd(const float* gs_partial, int P, const float* evals, cons
                         const float* x_spec, int K, int C, float* dS /*K x C*/, float* grad_time /*+=*/,
                         cudaStream_t st);
 
-// ---- tcgen05 engine (dn_tc.cu) ----
+// ---- wgmma engine (dn_tc.cu) ----
 bool tc_supported_device();
 // Fused chain of up to DN_MAX_LAYERS layers over 128-row tiles; layer 0 reads `src`.
 int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers, int n_layers, int64_t V, int passes /*3 or 1*/,

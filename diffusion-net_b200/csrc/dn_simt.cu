@@ -1,5 +1,5 @@
 // SIMT (FFMA, exact fp32) kernels of the DiffusionNetBlock hot path, and the sparse /
-// elementwise kernels shared by every engine.  sm_100a only.
+// elementwise kernels shared by every engine.  sm_90a.
 //
 // Reference functions restated here (file:line in /root/reference/src/diffusion_net):
 //   to_basis geometry.py:572-583, from_basis geometry.py:586-598,
@@ -426,9 +426,13 @@ __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
 __device__ __forceinline__ void unpack2(unsigned long long v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
-// d = a * b + d on both fp32 halves (sm_100 FFMA2)
+// d = a * b + d on both fp32 halves (two IEEE fp32 FMAs)
 __device__ __forceinline__ void fma2(unsigned long long& d, unsigned long long a, unsigned long long b) {
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(b));
+  float d0, d1, a0, a1, b0, b1;
+  unpack2(d, d0, d1);
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  d = pack2(fmaf(a0, b0, d0), fmaf(a1, b1, d1));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -439,7 +443,7 @@ __device__ __forceinline__ void fma2(unsigned long long& d, unsigned long long a
 //   * a warp issues every neighbour-row load of a batch of NB entries (3 x NB independent 16-byte loads per lane)
 //     before the first FMA; 8 warps walk 8 consecutive rows at a time, so the band structure of a locally ordered
 //     mesh hits L1;
-//   * packed fp32x2 FMAs (fma.rn.f32x2: two IEEE fp32 FMAs per instruction, bit-identical to fmaf).
+//   * fp32 FMAs on pairs of channels (fma2), bit-identical to fmaf per element.
 // Entry order = CSR order and the arithmetic per element is the same fmaf sequence as gather_row: bit-identical output.
 // ---------------------------------------------------------------------------------------------
 constexpr int GB_ROWS = 64;      // rows per CTA
@@ -447,7 +451,7 @@ constexpr int GB_NNZ = 1024;     // staged entries per CTA (entries past it are 
 
 struct __align__(16) GxyEnt { int col; int pad; float gx, gy; };   // (gx, gy) 8-byte aligned: one LDS.64
 
-// one CSR entry of the (x, P, Q) gather: three 16-byte slices of the neighbour's rows, then 12 FFMA2
+// one CSR entry of the (x, P, Q) gather: three 16-byte slices of the neighbour's rows, then 12 paired FMAs (fma2)
 #define DN_FEAT_LOAD(J, ENT)                                                                         \
   const char* pr##J;                                                                                 \
   ulonglong2 x##J, P##J, Q##J = make_ulonglong2(0ull, 0ull);                                         \
@@ -474,7 +478,7 @@ struct __align__(16) GxyEnt { int col; int pad; float gx, gy; };   // (gx, gy) 8
     }                                                                                                \
   }
 
-// (Same staging as spmm_gxy_blk_kernel below: 16-byte entry records, unpredicated full batches -- the first version,
+// (16-byte entry records, unpredicated full batches -- the first version,
 // with per-entry predicates and separate col / value arrays, spent half of its issue slots on bookkeeping.)
 template <bool ROT, int NH>
 __global__ void __launch_bounds__(256, 2)
@@ -553,95 +557,6 @@ spmm_features_blk_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
 }
 #undef DN_FEAT_LOAD
 #undef DN_FEAT_FMA
-
-// The same block gather for the tensor-core gradient-features route: only x_diffuse is gathered (7 x 512 B per
-// vertex instead of 7 x 1.5 KB) and the raw tangent gradients are written out,
-//     gxy[v] = [ sum_j gx_vj x_j | sum_j gy_vj x_j ]                                       (layers.py:216-223)
-// the complex-linear map, the inner product and the tanh follow as a tcgen05 GEMM with a fused epilogue (rows_chain3,
-// has_res == 3).  Entry order = CSR order, fmaf per element (as FFMA2).
-
-
-// One CSR entry of the x-only gather: the neighbour row's 16-byte slice is loaded, then 4 FFMA2 -- gX += gx * x, gY += gy * x
-#define DN_GXY_LOAD(J, ENT)                                                                          \
-  const int4 en##J = *reinterpret_cast<const int4*>(&(ENT));                                         \
-  const ulonglong2 x##J = __ldg(reinterpret_cast<const ulonglong2*>(xb + (int64_t)en##J.x * x_row_bytes));
-#define DN_GXY_FMA(J)                                                                                \
-  {                                                                                                  \
-    const float wx = __int_as_float(en##J.z), wy = __int_as_float(en##J.w);                          \
-    const unsigned long long gx2 = pack2(wx, wx), gy2 = pack2(wy, wy);                               \
-    fma2(gX0, gx2, x##J.x); fma2(gX1, gx2, x##J.y);                                                  \
-    fma2(gY0, gy2, x##J.x); fma2(gY1, gy2, x##J.y);                                                  \
-  }
-
-// The instruction count is what bounds this kernel (ncu: 71 % issue-active in the first version, whose per-entry
-// predicates and two staging arrays cost ~4x the useful instructions): entries are staged as 16-byte records (one
-// broadcast LDS.128 per entry), full batches of 7 run without predicates, and blocks whose entries do not fit the
-// staging buffer take a separate (generic) path.
-template <int NH>
-__global__ void __launch_bounds__(256, 3)
-spmm_gxy_blk_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
-                    const float2* __restrict__ vals, const float* __restrict__ xd, int64_t V, float* __restrict__ gxy) {
-  constexpr int C = 128 * NH;
-  constexpr int64_t x_row_bytes = (int64_t)C * 4;
-  __shared__ int s_rp[GB_ROWS + 1];
-  __shared__ GxyEnt s_e[GB_NNZ];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t base = (int64_t)blockIdx.x * GB_ROWS;
-  const int nrows = (int)((V - base) < GB_ROWS ? (V - base) : GB_ROWS);
-  if ((int)threadIdx.x <= nrows) s_rp[threadIdx.x] = __ldg(rowptr + base + threadIdx.x);
-  __syncthreads();
-  const int e0 = s_rp[0];
-  const int tot = s_rp[nrows] - e0;
-  const bool staged = tot <= GB_NNZ;                              // (block-uniform)
-  if (staged) {
-    for (int i = threadIdx.x; i < tot; i += 256) {
-      const float2 g = __ldg(vals + e0 + i);
-      GxyEnt en;
-      en.col = __ldg(colidx + e0 + i); en.gx = g.x; en.gy = g.y; en.pad = 0;
-      s_e[i] = en;
-    }
-  }
-  __syncthreads();
-#pragma unroll 1
-  for (int rh = warp; rh < nrows * NH; rh += 8) {
-    const int r = rh / NH, h = rh % NH;
-    const char* xb = reinterpret_cast<const char*>(xd) + h * 512 + lane * 16;
-    const int s = s_rp[r] - e0, e = s_rp[r + 1] - e0;
-    unsigned long long gX0 = 0ull, gX1 = 0ull, gY0 = 0ull, gY1 = 0ull;
-    if (staged) {
-      int p = s;
-#pragma unroll 1
-      for (; p + 7 <= e; p += 7) {                                // full batches: seven independent loads, no predicates
-        DN_GXY_LOAD(0, s_e[p]) DN_GXY_LOAD(1, s_e[p + 1]) DN_GXY_LOAD(2, s_e[p + 2]) DN_GXY_LOAD(3, s_e[p + 3])
-        DN_GXY_LOAD(4, s_e[p + 4]) DN_GXY_LOAD(5, s_e[p + 5]) DN_GXY_LOAD(6, s_e[p + 6])
-        DN_GXY_FMA(0) DN_GXY_FMA(1) DN_GXY_FMA(2) DN_GXY_FMA(3) DN_GXY_FMA(4) DN_GXY_FMA(5) DN_GXY_FMA(6)
-      }
-#pragma unroll 1
-      for (; p + 2 <= e; p += 2) {                                // remainder: pairs, then a single entry
-        DN_GXY_LOAD(0, s_e[p]) DN_GXY_LOAD(1, s_e[p + 1])
-        DN_GXY_FMA(0) DN_GXY_FMA(1)
-      }
-      if (p < e) {
-        DN_GXY_LOAD(0, s_e[p])
-        DN_GXY_FMA(0)
-      }
-    } else {
-#pragma unroll 1
-      for (int p = s; p < e; ++p) {                               // (a block with more than GB_NNZ entries)
-        GxyEnt en;
-        const float2 g = __ldg(vals + e0 + p);
-        en.col = __ldg(colidx + e0 + p); en.gx = g.x; en.gy = g.y; en.pad = 0;
-        DN_GXY_LOAD(0, en)
-        DN_GXY_FMA(0)
-      }
-    }
-    char* o = reinterpret_cast<char*>(gxy + (base + r) * (2 * C)) + h * 512 + lane * 16;
-    *reinterpret_cast<ulonglong2*>(o) = make_ulonglong2(gX0, gX1);
-    *reinterpret_cast<ulonglong2*>(o + x_row_bytes) = make_ulonglong2(gY0, gY1);
-  }
-}
-#undef DN_GXY_LOAD
-#undef DN_GXY_FMA
 
 // Patch variant (dn_patches, built once for resident operators): one CTA per patch of graph-adjacent rows.
 // Phase 1 copies the patch's distinct neighbour rows of x_diffuse and [P|Q] into shared memory, coalesced, each row
@@ -870,11 +785,23 @@ int simt_rows_gemm(const DnRowsSrc& src, const DnLayer& L, int64_t V, cudaStream
   return DN_OK;
 }
 
+int dn_sm_count() {
+  static int cache[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); return 1; }
+  if (cache[dev] == 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) { cudaGetLastError(); n = 1; }
+    cache[dev] = n;
+  }
+  return cache[dev];
+}
+
 int simt_atb_partial_st(const float* A, int64_t lda, int I, const float* B, int64_t ldb, int J, const float* scale,
                         int64_t V, float* ws, int64_t ws_floats, int* P_out, cudaStream_t st) {
   const int tiles = ((I + 63) / 64) * ((J + 63) / 64);
   int P = (int)((V + 2047) / 2048);
-  const int maxP = (4 * 148) / tiles > 1 ? (4 * 148) / tiles : 1;
+  const int maxP = (4 * dn_sm_count()) / tiles > 1 ? (4 * dn_sm_count()) / tiles : 1;
   if (P > maxP) P = maxP;
   if (P < 1) P = 1;
   while ((int64_t)P * I * J > ws_floats && P > 1) --P;
@@ -1013,18 +940,6 @@ int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int 
     spmm_features_kernel<true><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, 2 * C, V, C, G, feat);
   else
     spmm_features_kernel<false><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, C, V, C, G, feat);
-  DN_LAUNCH_CHECK();
-  return DN_OK;
-}
-
-int launch_spmm_gxy(const dn_csr* g, const float* x, int64_t V, int C, float* gxy, cudaStream_t st) {
-  if (V <= 0) return DN_OK;
-  if (C != 128 && C != 256) return DN_ERR_UNSUPPORTED;
-  const float2* vals = reinterpret_cast<const float2*>(g->vals);
-  const unsigned ctas = (unsigned)((V + GB_ROWS - 1) / GB_ROWS);
-  // (measured, tools/gf_check.py: streaming stores change nothing, 4 CTAs / SM with 64 registers is 5 % slower)
-  if (C == 128) spmm_gxy_blk_kernel<1><<<ctas, 256, 0, st>>>(g->rowptr, g->colidx, vals, x, V, gxy);
-  else spmm_gxy_blk_kernel<2><<<ctas, 256, 0, st>>>(g->rowptr, g->colidx, vals, x, V, gxy);
   DN_LAUNCH_CHECK();
   return DN_OK;
 }

@@ -1,5 +1,5 @@
-// Inline-PTX wrappers for the Blackwell (sm_100a) features the tensor-core engine uses:
-// mbarrier, bulk TMA copies, tcgen05 (TMEM alloc / MMA / commit / load), proxy fences.
+// Inline-PTX wrappers for the Hopper (sm_90a) features the tensor-core engine uses:
+// mbarrier, bulk TMA copies, proxy fences and warpgroup MMA (wgmma) with the A operand in registers.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,16 +8,6 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-// One lane of a fully-converged warp.  Role loops stay warp-uniform and only the single-thread
-// instructions (tcgen05.mma / commit / TMA issue) are predicated on this, so the compiler keeps
-// descriptors and addresses in uniform registers instead of emitting per-instruction
-// ELECT/BRA.U.ANY "waterfall" loops (measured: ~180 cycles per UTCHMMA issue with `if (lane==0)`).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n.reg .pred P;\nelect.sync _|P, 0xffffffff;\nselp.u32 %0, 1, 0, P;\n}" : "=r"(pred));
-  return pred != 0;
 }
 
 // ---- mbarrier -------------------------------------------------------------------------------
@@ -49,23 +39,23 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
-// one non-blocking probe of the phase parity (the caller falls back to mbar_wait when it fails)
-__device__ __forceinline__ uint32_t mbar_test(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-      : "=r"(done)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return done;
-}
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (UMMA / TMA reads)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// named barrier over `count` threads (a multiple of 32)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// warpgroup register budget hand-off (every warp of the warpgroup executes it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ---- bulk TMA copy global -> shared, completion on an mbarrier ----------------------------------
 __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst_smem, const void* src_gmem, uint32_t bytes, uint32_t bar) {
@@ -74,138 +64,54 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst_smem, const void* src_
                : "memory");
 }
 
-// contiguous global range -> L2 (no smem destination, no completion tracking)
-__device__ __forceinline__ void l2_prefetch_bulk(const void* src_gmem, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src_gmem), "r"(bytes) : "memory");
-}
-
-// ---- tcgen05 ----------------------------------------------------------------------------------
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_result_addr) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_result_addr), "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], tf32 inputs, fp32 accumulate.  One thread issues.
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same, with the A operand read from tensor memory (lane = row, 32-bit column per k element)
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A from tensor memory, 16-bit inputs (bf16 x bf16 -> fp32): K = 16 per instruction, two elements per 32-bit TMEM column
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when every MMA issued so far by this thread has completed
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 16 consecutive fp32 columns of this thread's TMEM lane (lane = 32*(warp%4) + laneid)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// same load without the wait: several loads can be in flight; tmem_ld_wait32 makes their registers valid
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// the registers are in/out operands so that no use of them can be scheduled above the wait
-__device__ __forceinline__ void tmem_ld_wait32(uint32_t* a, uint32_t* b) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(a[0]), "+r"(a[1]), "+r"(a[2]), "+r"(a[3]), "+r"(a[4]), "+r"(a[5]), "+r"(a[6]), "+r"(a[7]),
-                 "+r"(a[8]), "+r"(a[9]), "+r"(a[10]), "+r"(a[11]), "+r"(a[12]), "+r"(a[13]), "+r"(a[14]), "+r"(a[15]),
-                 "+r"(b[0]), "+r"(b[1]), "+r"(b[2]), "+r"(b[3]), "+r"(b[4]), "+r"(b[5]), "+r"(b[6]), "+r"(b[7]),
-                 "+r"(b[8]), "+r"(b[9]), "+r"(b[10]), "+r"(b[11]), "+r"(b[12]), "+r"(b[13]), "+r"(b[14]), "+r"(b[15])
-               :
-               : "memory");
-}
-
-// 16 consecutive fp32 columns of this thread's TMEM lane <- registers
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// shared-memory matrix descriptor, no swizzle, K-major canonical layout:
-//   element (r, k) at  (r%8)*16 + (k%4)*4 + (r/8)*SBO + (k/4)*LBO   [bytes, 4-byte elements]
-// bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=0
+// ---- wgmma ------------------------------------------------------------------------------------
+// shared-memory matrix descriptor, no swizzle, K-major: core matrices of 8 rows x 16 bytes;
+//   LBO = byte distance between core matrices adjacent in K, SBO = between 8-row groups
+// bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout = 0 (no swizzle)
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// instruction descriptor: kind::tf32, fp32 accumulate, both operands K-major
-//   [4,6) c_format=1(F32) | [7,10) a_format=2(TF32) | [10,13) b_format=2 | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ __forceinline__ uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void fence_acc8(float* d) {
+  asm volatile("" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               :: "memory");
 }
 
-// instruction descriptor: kind::f16 with bf16 inputs, fp32 accumulate, both operands K-major
-//   [4,6) c_format=1(F32) | [7,10) a_format=1(BF16) | [10,13) b_format=1(BF16) | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// D[64 x 16] (+)= A[64 x 8] (registers, tf32) * B[8 x 16] (smem descriptor, K-major tf32), fp32 accumulate.
+//   A fragment of lane (g = lane / 4, t = lane % 4) in warp w: a0 (16w+g, t), a1 (16w+g+8, t), a2 (16w+g, t+4),
+//   a3 (16w+g+8, t+4);  D fragment: d[4b + {0,1,2,3}] = (16w+g, 8b+2t), (16w+g, 8b+2t+1), (16w+g+8, 8b+2t), (16w+g+8, 8b+2t+1)
+__device__ __forceinline__ void wgmma_tf32_n16(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+      : "memory");
 }
+// D[64 x 16] (+)= A[64 x 16] (registers, bf16 pairs) * B[16 x 16] (smem descriptor, K-major bf16), fp32 accumulate.
+//   a0 = (16w+g, 2t..2t+1), a1 = (16w+g+8, 2t..2t+1), a2 = (16w+g, 2t+8..2t+9), a3 = (16w+g+8, 2t+8..2t+9)
+__device__ __forceinline__ void wgmma_bf16_n16(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
+
 // two fp32 -> packed bf16x2 (round to nearest even): `lo` in bits [0,16), `hi` in bits [16,32)
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
-}
-
-// A REAL consumer of loaded registers: xor them and branch on the result (never taken in practice).  In-order issue then
-// guarantees every instruction after this one issues after the loads that produced `v...` have returned their data.
-// Needed before releasing a shared-memory slot that was read with ld.shared: mbarrier.arrive runs in a different pipe
-// and can overtake loads whose results nobody has consumed yet, and an empty asm("" :: "f"(x)) "use" leaves no
-// instruction behind for ptxas to keep (measured: rows_chain16_kernel lost whole stages that way).
-__device__ __forceinline__ void consume_loaded(uint32_t d) {
-  asm volatile("{\n.reg .pred p;\nsetp.eq.u32 p, %0, 0x7fedbeef;\n@p trap;\n}" ::"r"(d) : "memory");
 }
 
 // error-compensated split  x ~= hi + lo  with hi, lo exactly representable in TF32
@@ -218,9 +124,8 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   lo = __uint_as_float(l);
 }
 
-// cheaper split for activations: hi = x rounded to TF32 (round-half-up on the magnitude bits: IADD + LOP
-// instead of the 4-instruction cvt.rna emulation); lo = x - hi is exact in fp32 and the MMA reads only its
-// top 19 bits.  Non-finite inputs stay non-finite.
+// cheaper split for activations: hi = x rounded to TF32 (round-half-up on the magnitude bits); lo = x - hi is exact
+// in fp32 and the MMA reads only its top 19 bits.  Non-finite inputs stay non-finite.
 __device__ __forceinline__ void split_tf32_fast(float x, float& hi, float& lo) {
   hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
   lo = x - hi;

@@ -140,7 +140,7 @@ def get_operators(verts, faces, k_eig=128, op_cache_dir=None, normals=None, over
         npz = find_cached_operators(verts, faces, k_eig, op_cache_dir)
     if npz is None:
         raise NotImplementedError(
-            "no usable cache entry for this mesh in {!r}: operator construction is outside the B200 hot path -- "
+            "no usable cache entry for this mesh in {!r}: operator construction is outside the CUDA hot path -- "
             "populate the cache with the reference's get_operators()".format(op_cache_dir))
     return load_operators_npz(npz, k_eig=k_eig, device=device, dtype=verts.dtype)
 

@@ -1,5 +1,5 @@
 """Drop-in mirror of ``diffusion_net.layers`` (reference ``src/diffusion_net/layers.py``) whose
-per-block hot path runs the hand-written sm_100a kernels behind the C-ABI.
+per-block hot path runs the hand-written sm_90a kernels behind the C-ABI.
 
 Same class names, constructor kwargs, forward signatures, exceptions and state_dict keys as the
 reference (SURVEY.md section 8b), so shipped ``.pth`` checkpoints load with ``strict=True`` and
@@ -39,7 +39,7 @@ class LearnedTimeDiffusion(nn.Module):
             return torch.stack([ops.DiffusionFn.apply(x[b], self.diffusion_time, mass[b], evals[b], evecs[b])
                                 for b in range(x.shape[0])], dim=0)
         elif self.method == 'implicit_dense':
-            raise NotImplementedError("diffusion_method='implicit_dense' is outside the B200 hot path "
+            raise NotImplementedError("diffusion_method='implicit_dense' is outside the CUDA hot path "
                                       "(dense Cholesky per channel; use the reference for toy sizes)")
         else:
             raise ValueError("unrecognized method")

@@ -19,9 +19,9 @@ _engine = _ENGINES[os.environ.get("DN_B200_ENGINE", "tc3x")]
 
 
 def set_engine(name: str):
-    """'tc3x' (default: tcgen05, error-compensated 3xTF32, fp32-grade), 'tc1x' (single-pass
+    """'tc3x' (default: wgmma, error-compensated 3xTF32, fp32-grade), 'tc1x' (single-pass
     TF32), 'bf16' (single-pass bf16 tensor-core arithmetic, fp32 tensors in HBM; ~1e-2) or 'simt'
-    (exact fp32 FFMA).  Shapes outside the tcgen05 kernels' envelope always run the exact SIMT kernels."""
+    (exact fp32 FFMA).  Shapes outside the wgmma kernels' envelope always run the exact SIMT kernels."""
     global _engine
     _engine = _ENGINES[name]
 
@@ -258,9 +258,9 @@ class GradOperators:
 
 _prep_cache = {}
 # dn_patches policy on the SECOND use of an operator pair (= the operators are resident): "auto" (default) builds the
-# structure only for poorly ordered meshes, "1" always, "0" never.  Measured on B200 (tools/ab_patch.py, V = 200k,
-# C = 128): the staged gather takes ~206 us whatever the vertex order; the plain gather takes 179 us on a mesh whose
-# order has locality (47 % L1 hits) and 346 us on a randomly permuted one.
+# structure only for poorly ordered meshes, "1" always, "0" never: the staged gather costs about the same whatever the
+# vertex order, while the plain gather is fast on a mesh whose order has locality (L1 hits) and slow on a randomly
+# permuted one.
 auto_patch = os.environ.get("DN_SPMM_PATCH", "auto")
 PATCH_LOCALITY_THRESHOLD = 0.25
 

@@ -1,5 +1,5 @@
 /*
- * diffusion_net_b200 -- C ABI of the B200-native DiffusionNetBlock hot path.
+ * diffusion_net_b200 -- C ABI of the H100-native (sm_90a) DiffusionNetBlock hot path.
  *
  * The reference (nmwsharp/diffusion-net) is pure Python and has no FFI layer; its
  * boundary is the module API of src/diffusion_net/layers.py plus the operator
@@ -18,11 +18,11 @@
  *
  * `engine` selects the arithmetic of the dense contractions:
  *   DN_ENGINE_SIMT  exact fp32 FFMA (debug / gold-on-device, any shape)
- *   DN_ENGINE_TC3X  tcgen05 tensor cores, error-compensated 3xTF32 (fp32-grade,
+ *   DN_ENGINE_TC3X  wgmma tensor cores, error-compensated 3xTF32 (fp32-grade,
  *                   the default product path; <=1e-5 relative vs the reference)
- *   DN_ENGINE_TC1X  tcgen05 single-pass TF32 (fast, ~5e-4 relative)
- *   DN_ENGINE_BF16  tcgen05 single-pass bf16 (kind::f16, fp32 accumulate; ~1e-2 relative; layers up to
- *                   256 wide chain on chip: BASELINE config 3, C_width = 256).  Tensors stay fp32 in HBM.
+ *   DN_ENGINE_TC1X  wgmma single-pass TF32 (fast, ~5e-4 relative)
+ *   DN_ENGINE_BF16  wgmma single-pass bf16 (fp32 accumulate; ~1e-2 relative; layers up to
+ *                   128 wide chain on chip, a 256-wide layer runs as its own launch).  Tensors stay fp32 in HBM.
  */
 #ifndef DIFFUSION_NET_B200_H
 #define DIFFUSION_NET_B200_H
@@ -43,7 +43,7 @@ enum dn_status {
   DN_ERR_INVALID_ARGUMENT = -1, /* null pointer, negative size, mismatched dims   */
   DN_ERR_UNSUPPORTED = -2,      /* shape/engine combination not implemented        */
   DN_ERR_WORKSPACE = -3,        /* workspace too small (see dn_workspace_bytes)    */
-  DN_ERR_NOT_SM100 = -4         /* tensor-core engine requested on a non-sm_100 GPU */
+  DN_ERR_NOT_SM100 = -4         /* tensor-core engine requested on a non-sm_90 GPU */
 };
 
 enum dn_engine { DN_ENGINE_SIMT = 0, DN_ENGINE_TC3X = 1, DN_ENGINE_TC1X = 2, DN_ENGINE_BF16 = 3 };

@@ -127,7 +127,13 @@ def main():
     # gold kept fp32-rounded here to keep the fixture small (adds <=6e-8 relative)
     for k in ("x_diffuse_f64", "out_f64"):
         fx4[k + "_as32"] = r4[k].astype(np.float32)
-    np.savez_compressed(os.path.join(OUT, "block_k128.npz"), **fx4)
+    # stored as three parts (each under 1 MB); tests/conftest.py load_golden merges block_k128.<part>.npz
+    parts = {"ops": ["mass", "evals", "evecs", "g_rows", "g_cols", "gx_vals", "gy_vals"],
+             "params": [k for k in fx4 if k.startswith("p:")],
+             "io": ["x_in", "x_diffuse_f64_as32", "out_f64_as32"]}
+    assert sorted(sum(parts.values(), [])) == sorted(fx4)
+    for part, keys in parts.items():
+        np.savez_compressed(os.path.join(OUT, "block_k128.{}.npz".format(part)), **{k: fx4[k] for k in keys})
 
     # ---- 5. whole net, 2 blocks, all outputs_at modes, batched B=2 ----
     Cin, Cout, Cw, NB = 3, 8, 32, 2
@@ -177,6 +183,9 @@ def main():
                 continue
             sdp = torch.load(os.path.join(d, f), map_location="cpu", weights_only=True)
             man[sub + "/" + f] = {k: list(v.shape) for k, v in sdp.items()}
+            if f == "human_seg_xyz_4x128.pth":     # the strict-load fixture: every tensor, float16 (under 1 MB)
+                np.savez_compressed(os.path.join(OUT, "human_seg_xyz_4x128_f16.npz"),
+                                    **{k: v.numpy().astype(np.float16) for k, v in sdp.items()})
     with open(os.path.join(OUT, "statedict_manifest.json"), "w") as fh:
         json.dump(man, fh, indent=1, sort_keys=True)
     for f in sorted(os.listdir(OUT)):

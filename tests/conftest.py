@@ -11,12 +11,20 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU")
 
 
 def load_golden(name):
-    with np.load(os.path.join(GOLDEN, name + ".npz")) as z:
-        return {k: z[k] for k in z.files}
+    # a fixture too large for one file is stored as parts <name>.<part>.npz and merged here
+    path = os.path.join(GOLDEN, name + ".npz")
+    parts = [path] if os.path.exists(path) else sorted(
+        os.path.join(GOLDEN, f) for f in os.listdir(GOLDEN) if f.startswith(name + ".") and f.endswith(".npz"))
+    assert parts, name
+    out = {}
+    for p in parts:
+        with np.load(p) as z:
+            out.update({k: z[k] for k in z.files})
+    return out
 
 
 def golden_params(fx, dtype=None):

@@ -196,8 +196,8 @@ def test_block_backward_golden(dn, engine, name, kw):
 def test_block_backward_config2_shape_vs_oracle_autograd(dn, engine):
     """BASELINE config 2 shape (human-seg class: V ~ 7k, K = 128, C = 128): forward + backward of one block against
     fp64 autograd through the torch restatement of the reference block (oracle/dn_oracle_torch.py, itself pinned to
-    the live reference by tests/test_oracle.py).  This is the shape the tensor-core backward (rows_chain3 dX layers,
-    split-V tcgen05 weight gradients) is built for.  Tolerances as in the golden backward test."""
+    the live reference by tests/test_oracle.py).  This is the shape the tensor-core backward (rows_chain_kernel dX layers,
+    split-V wgmma weight gradients) is built for.  Tolerances as in the golden backward test."""
     import dn_oracle_torch as T
     dn.set_engine(engine)
     n, m, K, C = 84, 84, 128, 128

@@ -185,7 +185,10 @@ struct HcParams {
 // for every 8-column block b: after the epilogue these values are the next layer's A fragments (columns of a 16-wide
 // K stage: tf32 steps use the permuted weight order of pack_store, bf16 steps the natural one).  NMAX <= 128 chains
 // any number of layers; NMAX = 256 runs a single layer (its accumulator alone takes 128 registers).
-template <int MODE, int NMAX>
+// WIDE: every layer is exactly NMAX wide (so every later layer's K is NMAX too).  Widths and trip counts are then
+// compile-time and each k8 slice of a pass is one m64nNMAXk8 MMA over the whole accumulator; otherwise the layer is
+// covered by N / 16 m64n16 MMAs per slice and pass.
+template <int MODE, int NMAX, bool WIDE>
 __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __grid_constant__ HcParams p) {
   constexpr bool kChain = NMAX <= 128;
   constexpr int NB = NMAX / 16;
@@ -238,53 +241,81 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
     const bool ok0 = r0 < p.V, ok1 = r1 < p.V;
     for (int l = 0; l < L; ++l) {
       const HcLayer& Lr = p.layer[l];
-      const int K = Lr.K, N = Lr.N, nb = N / 16, nst = (K + KC - 1) / KC;
+      const int N = WIDE ? NMAX : Lr.N, nb = N / 16;
+      const int K = (WIDE && l > 0) ? NMAX : Lr.K, nst = (K + KC - 1) / KC;
       const uint32_t lbo = (uint32_t)N * 16;
       int prev = -1;
-      // one K stage: q[0], q[1] = rows (r0, r1) x columns (2t, 2t+1); q[2], q[3] the same 8 columns further
-      auto stage = [&](int c, const float2* q) {
+      // one K stage: q[0], q[1] = rows (r0, r1) x columns (2t, 2t+1); q[2], q[3] the same 8 columns further.  All A
+      // fragments of the stage are formed before wgmma_fence, so the MMAs read registers the fence already covers and
+      // ptxas has no reason to order them.  One commit group per stage, at most two stages in flight -- except in the
+      // full-width TF32 chains: there the accumulator, the activations and two stages of fragments do not fit in the
+      // register budget together (ptxas spills or serializes), so each stage waits for its own MMAs (up to six
+      // full-width MMAs per stage; the other consumer warpgroup keeps the tensor cores busy meanwhile).  `two` marks
+      // a stage whose second k8 slice lies inside K (a literal wherever it is known at compile time).
+      auto stage = [&](int c, const float2* q, bool two) {
         mbar_wait(full + 8 * s, ph);
-        const uint32_t sb = smem_u32(smem + s * STAGE_BYTES);
-        wgmma_fence();
+        uint32_t ah[2][4], al[2][4];
         if (MODE == MODE_BF16) {
-          const uint32_t a[4] = {pack_bf16x2(q[0].x, q[0].y), pack_bf16x2(q[1].x, q[1].y), pack_bf16x2(q[2].x, q[2].y),
-                                 pack_bf16x2(q[3].x, q[3].y)};
-#pragma unroll
-          for (int j = 0; j < NB; ++j)
-            if (j < nb) wgmma_bf16_n16(acc + 8 * j, a, make_desc(sb + j * 256, lbo, 128), c > 0 ? 1u : 0u);
+          ah[0][0] = pack_bf16x2(q[0].x, q[0].y); ah[0][1] = pack_bf16x2(q[1].x, q[1].y);
+          ah[0][2] = pack_bf16x2(q[2].x, q[2].y); ah[0][3] = pack_bf16x2(q[3].x, q[3].y);
         } else {
 #pragma unroll
           for (int ks = 0; ks < 2; ++ks) {
-            if (c * KC + ks * 8 >= K) break;
             const float2 u = q[2 * ks], v = q[2 * ks + 1];
-            uint32_t ah[4], al[4];
             const float x[4] = {u.x, v.x, u.y, v.y};
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               float h, lo;
               split_tf32_fast(x[i], h, lo);
-              ah[i] = __float_as_uint(h);
-              al[i] = __float_as_uint(lo);
+              ah[ks][i] = __float_as_uint(h);
+              al[ks][i] = __float_as_uint(lo);
             }
+          }
+        }
+        const uint32_t sb = smem_u32(smem + s * STAGE_BYTES);
+        wgmma_fence();
+        if (MODE == MODE_BF16) {
+          if constexpr (WIDE) {
+            wgmma_bf16<NMAX>(acc, ah[0], make_desc(sb, lbo, 128), c > 0 ? 1u : 0u);
+          } else {
+#pragma unroll
+            for (int j = 0; j < NB; ++j)
+              if (j < nb) wgmma_bf16_n16(acc + 8 * j, ah[0], make_desc(sb + j * 256, lbo, 128), c > 0 ? 1u : 0u);
+          }
+        } else {
+#pragma unroll
+          for (int ks = 0; ks < 2; ++ks) {
+            if (ks == 1 && !two) break;
             const uint32_t acc0 = (c > 0 || ks > 0) ? 1u : 0u;
             const uint32_t base = sb + ks * 2 * lbo;
-#pragma unroll
-            for (int j = 0; j < NB; ++j) {
-              if (j >= nb) break;
-              const uint64_t dh = make_desc(base + j * 256, lbo, 128);
+            if constexpr (WIDE) {
+              const uint64_t dh = make_desc(base, lbo, 128);
+              const uint32_t* a0 = MODE == MODE_TF32X3 ? al[ks] : ah[ks];
+              wgmma_tf32<NMAX>(acc, a0, dh, acc0);
               if (MODE == MODE_TF32X3) {
-                const uint64_t dl = make_desc(base + KC * N * 4 + j * 256, lbo, 128);
-                wgmma_tf32_n16(acc + 8 * j, al, dh, acc0);
-                wgmma_tf32_n16(acc + 8 * j, ah, dl, 1u);
-                wgmma_tf32_n16(acc + 8 * j, ah, dh, 1u);
-              } else {
-                wgmma_tf32_n16(acc + 8 * j, ah, dh, acc0);
+                wgmma_tf32<NMAX>(acc, ah[ks], make_desc(base + KC * N * 4, lbo, 128), 1u);
+                wgmma_tf32<NMAX>(acc, ah[ks], dh, 1u);
+              }
+            } else {
+#pragma unroll
+              for (int j = 0; j < NB; ++j) {
+                if (j >= nb) break;
+                const uint64_t dh = make_desc(base + j * 256, lbo, 128);
+                if (MODE == MODE_TF32X3) {
+                  const uint64_t dl = make_desc(base + KC * N * 4 + j * 256, lbo, 128);
+                  wgmma_tf32_n16(acc + 8 * j, al[ks], dh, acc0);
+                  wgmma_tf32_n16(acc + 8 * j, ah[ks], dl, 1u);
+                  wgmma_tf32_n16(acc + 8 * j, ah[ks], dh, 1u);
+                } else {
+                  wgmma_tf32_n16(acc + 8 * j, ah[ks], dh, acc0);
+                }
               }
             }
           }
         }
         wgmma_commit();
-        wgmma_wait<1>();                       // the previous stage's MMAs are done: hand its slot back
+        if constexpr (WIDE && MODE != MODE_BF16) wgmma_wait<0>();
+        else wgmma_wait<1>();                  // the previous stage's MMAs are done: hand its slot back
         if (prev >= 0 && lane == 0) mbar_arrive(empty + 8 * prev);
         prev = (int)s;
         if (++s == NST) { s = 0; ph ^= 1; }
@@ -309,10 +340,10 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
         load(0, qa);
         for (int c = 0; c < nst; c += 2) {
           if (c + 1 < nst) load(c + 1, qb);
-          stage(c, qa);
+          stage(c, qa, c * KC + 8 < K);
           if (c + 1 >= nst) break;
           if (c + 2 < nst) load(c + 2, qa);
-          stage(c + 1, qb);
+          stage(c + 1, qb, (c + 1) * KC + 8 < K);
         }
       } else if constexpr (kChain) {
 #pragma unroll
@@ -320,7 +351,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
           if (c >= nst) break;
           const float2 q[4] = {make_float2(act[8 * c], act[8 * c + 1]), make_float2(act[8 * c + 2], act[8 * c + 3]),
                                make_float2(act[8 * c + 4], act[8 * c + 5]), make_float2(act[8 * c + 6], act[8 * c + 7])};
-          stage(c, q);
+          stage(c, q, WIDE || c * KC + 8 < K);
         }
       }
       wgmma_wait<0>();
@@ -333,12 +364,15 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
       const bool head = last && p.head_w != nullptr;
       const float rs0 = (Lr.row_scale && ok0) ? __ldg(Lr.row_scale + r0) : 1.f;
       const float rs1 = (Lr.row_scale && ok1) ? __ldg(Lr.row_scale + r1) : 1.f;
-      float hp0[8], hp1[8];
+      float hp0[kChain ? 1 : 8], hp1[kChain ? 1 : 8];   // head partial sums of a single-layer (256-wide) chain
 #pragma unroll
-      for (int o = 0; o < 8; ++o) hp0[o] = hp1[o] = 0.f;
+      for (int o = 0; o < (kChain ? 1 : 8); ++o) hp0[o] = hp1[o] = 0.f;
+      // the bound is read from the layer even where it is known at compile time: the branch keeps the compiler from
+      // hoisting the epilogue loads of every column block ahead of the first one, which would not fit in registers
+      const int nb_epi = Lr.N / 16;
 #pragma unroll
       for (int j = 0; j < NB; ++j) {
-        if (j >= nb) break;
+        if (j >= nb_epi) break;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int col = 16 * j + 8 * h + 2 * t;
@@ -384,9 +418,9 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
             act[8 * j + 4 * h] = v0.x; act[8 * j + 4 * h + 1] = v0.y;
             act[8 * j + 4 * h + 2] = v1.x; act[8 * j + 4 * h + 3] = v1.y;
           }
-          if (head) {
+          if (!kChain && head) {
 #pragma unroll
-            for (int o = 0; o < 8; ++o) {
+            for (int o = 0; o < (kChain ? 1 : 8); ++o) {
               if (o >= p.head_n) break;
               const float2 w = __ldg(reinterpret_cast<const float2*>(p.head_w + (int64_t)o * N + col));
               hp0[o] = fmaf(w.y, v0.y, fmaf(w.x, v0.x, hp0[o]));
@@ -396,10 +430,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
         }
       }
       if (head) {
-#pragma unroll
-        for (int o = 0; o < 8; ++o) {
-          if (o >= p.head_n) break;
-          float a0 = hp0[o], a1 = hp1[o];
+        auto head_store = [&](int o, float a0, float a1) {
           a0 += __shfl_xor_sync(0xffffffffu, a0, 1);
           a0 += __shfl_xor_sync(0xffffffffu, a0, 2);
           a1 += __shfl_xor_sync(0xffffffffu, a1, 1);
@@ -407,6 +438,32 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
           const float b = p.head_b ? __ldg(p.head_b + o) : 0.f;
           if (t == 0 && ok0) p.head_out[r0 * p.ld_head_out + o] = a0 + b;
           if (t == 0 && ok1) p.head_out[r1 * p.ld_head_out + o] = a1 + b;
+        };
+        if constexpr (kChain) {
+          // the finished rows are in act: one output at a time keeps two partial sums and one weight pair live
+          // (the same summation order as the single-layer form below)
+#pragma unroll 1
+          for (int o = 0; o < p.head_n; ++o) {
+            float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+            for (int j = 0; j < NB; ++j) {
+              if (j >= nb) break;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const float* v = act + 8 * j + 4 * h;
+                const float2 w = __ldg(reinterpret_cast<const float2*>(p.head_w + (int64_t)o * N + 16 * j + 8 * h + 2 * t));
+                a0 = fmaf(w.y, v[1], fmaf(w.x, v[0], a0));
+                a1 = fmaf(w.y, v[3], fmaf(w.x, v[2], a1));
+              }
+            }
+            head_store(o, a0, a1);
+          }
+        } else {
+#pragma unroll
+          for (int o = 0; o < (kChain ? 1 : 8); ++o) {
+            if (o >= p.head_n) break;
+            head_store(o, hp0[o], hp1[o]);
+          }
         }
       }
     }
@@ -418,8 +475,12 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
 //   D = Phi^T (M = K_eig rows: warpgroup 0 rows 0..63, warpgroup 1 rows 64..127) times (m x) (N = C columns); the
 //   reduction runs over v in 16-row chunks.  Warp 8 copies 16 consecutive rows of Phi and of x into a staging ring
 //   with bulk TMA; the A fragments are read from there, B = (m x)^T is written K-major (hi | lo) by all consumers.
-//   The MMA accumulator is folded into an fp32 register sum every TB_FOLD chunks: short accumulation chains keep the
+//   The MMA accumulator is folded into an fp32 sum in shared memory every TB_FOLD chunks: short accumulation chains keep the
 //   tensor core's accumulation below fp32 noise even for V = 200k.
+//   The channel count C = 16 NBC is a compile-time parameter, so every MMA sits on a path ptxas can see is uniform.
+//   C == 128: each k8 slice of a pass is one m64n128k8 MMA; otherwise NBC m64n16 MMAs.  Both warpgroups always
+//   issue their MMAs (a warpgroup whose 64 eigen-rows all lie beyond K multiplies zero A fragments and stores nothing),
+//   so no MMA sits on a path that depends on the warp index.
 // ---------------------------------------------------------------------------------------------
 constexpr int TB_NST = 4;                    // raw staging ring depth
 constexpr int TB_RAW_HALF = KC * 128 * 4;    // 16 rows x up to 128 floats
@@ -427,7 +488,8 @@ constexpr int TB_RAW = 2 * TB_RAW_HALF;      // raw Phi rows + raw x rows
 constexpr int TB_BIMG = KC * 128 * 4;        // one tf32 image of B: up to 128 channels x 16 v
 constexpr int TB_BSTAGE = 2 * TB_BIMG;       // hi | lo
 constexpr int TB_THREADS = 288;              // warps 0..7 consumers (two warpgroups), warp 8 TMA
-constexpr int TB_SMEM = TB_NST * TB_RAW + 2 * TB_BSTAGE + 256;
+constexpr int TB_SUMS = 64 * 256 * 4;        // fp32 fold sums: 64 per consumer thread, [i][thread] (conflict-free)
+constexpr int TB_SMEM = TB_NST * TB_RAW + 2 * TB_BSTAGE + TB_SUMS + 256;
 constexpr int TB_FOLD = 8;
 
 struct TcToBasisParams {
@@ -443,12 +505,13 @@ struct TcToBasisParams {
   const int32_t* cta_rows;   // optional device [2 * grid]: the row range [begin, end) CTA i reduces (mesh batches: a CTA
 };                           //   never crosses a mesh boundary); null = uniform chunks_per_cta * 16 rows per CTA
 
-template <int MODE>
+template <int MODE, int NBC>
 __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_constant__ TcToBasisParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* raw = smem;
   uint8_t* bimg = smem + TB_NST * TB_RAW;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(bimg + 2 * TB_BSTAGE);
+  float* sums = reinterpret_cast<float*>(bimg + 2 * TB_BSTAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(bimg + 2 * TB_BSTAGE + TB_SUMS);
   const uint32_t st_full = smem_u32(bars), st_empty = smem_u32(bars + TB_NST);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -467,7 +530,8 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
     if (re > p.V) re = p.V;
   }
   const int64_t nch = re > rb ? (re - rb + KC - 1) / KC : 0;
-  const int K = p.K, C = p.C;
+  constexpr int C = 16 * NBC;
+  const int K = p.K;
 
   if (warp == 8) {
     if (lane == 0) {
@@ -493,34 +557,33 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
 
   const int g = lane >> 2, t = lane & 3;
   const int m0 = (warp >> 2) * 64 + (warp & 3) * 16 + g;   // eigen-index rows m0, m0 + 8
-  const bool mma_on = (warp >> 2) * 64 < K;
-  const int nb = C / 16;
   const uint32_t lbo = (uint32_t)C * 16;
-  float acc[64], sum[64];
+  // the fold sums live in shared memory: the 64 accumulators, two stages of A fragments and the addressing fit the
+  // kernel's 168 registers, a second register array of 64 would not
+  float acc[64];
+  float* sum = sums + threadIdx.x;
 #pragma unroll
-  for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+  for (int i = 0; i < 64; ++i) sum[256 * i] = 0.f;
 
   for (int64_t c = 0; c < nch; ++c) {
     const uint32_t s = c % TB_NST, ph = (c / TB_NST) & 1;
     const int64_t v0 = rb + c * KC;
     const int nv = (int)((re - v0) < KC ? (re - v0) : KC);
     const int fold = (int)(c % TB_FOLD);
-    if (fold == 0 && c > 0) {              // fold the finished accumulation chain into the register sum
+    if (fold == 0 && c > 0) {              // fold the finished accumulation chain into the sum
       wgmma_wait<0>();
 #pragma unroll
       for (int j = 0; j < 8; ++j) fence_acc8(acc + 8 * j);
-      if (mma_on)
 #pragma unroll
-        for (int i = 0; i < 64; ++i) sum[i] += acc[i];
-    } else {
-      wgmma_wait<1>();                     // this warp's MMAs of chunk c - 2 (the B slot rewritten below) are done
-    }
-    named_bar_sync(1, 256);                // ... and every other warp's
+      for (int i = 0; i < 64; ++i) sum[256 * i] += acc[i];
+    }                                      // (this warp's MMAs of chunk c - 2 are done: waited for in chunk c - 1)
+    named_bar_sync(1, 256);                // every warp's MMAs of chunk c - 2 are done: its B slot is free
     mbar_wait(st_full + 8 * s, ph);
     const float* rphi = reinterpret_cast<const float*>(raw + s * TB_RAW);
     const float* rx = reinterpret_cast<const float*>(raw + s * TB_RAW + TB_RAW_HALF);
     uint8_t* bh = bimg + (c & 1) * TB_BSTAGE;
-    for (int e = threadIdx.x; e < KC * C; e += 256) {
+    for (int e0 = 0; e0 < KC * C; e0 += 256) {   // KC * C is a multiple of 256: the same trip count in every thread
+      const int e = e0 + (int)threadIdx.x;
       const int vv = e / C, cc = e - vv * C;
       float x = 0.f;
       if (vv < nv) {
@@ -533,43 +596,58 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
       *reinterpret_cast<float*>(bh + off) = hi;
       if (MODE == MODE_TF32X3) *reinterpret_cast<float*>(bh + TB_BIMG + off) = lo;
     }
-    float a[2][4];
+    // the A fragment registers are the same in every chunk: the MMAs of chunk c - 1, which read them, must be done
+    // before they are rewritten (they ran while this chunk's B image was built)
+    wgmma_wait<0>();
+    uint32_t ah[2][4], al[2][4];           // A fragments, all formed before wgmma_fence
 #pragma unroll
     for (int ks = 0; ks < 2; ++ks)
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int vv = 8 * ks + t + 4 * (i >> 1), k = m0 + 8 * (i & 1);
-        a[ks][i] = (vv < nv && k < K) ? rphi[vv * K + k] : 0.f;
+        // read unconditionally and select: vv * K + k < 16 * 128 stays inside the staging slot, and a load under a
+        // lane-dependent branch would put the MMA operands on a divergent path
+        const float v = rphi[vv * K + k];
+        float h, lo;
+        split_tf32_fast((vv < nv && k < K) ? v : 0.f, h, lo);
+        ah[ks][i] = __float_as_uint(h);
+        al[ks][i] = __float_as_uint(lo);
       }
     fence_proxy_async();
     __syncwarp();
     if (lane == 0) mbar_arrive(st_empty + 8 * s);
     named_bar_sync(2, 256);                // the B image is complete
-    if (mma_on) {
-      const uint32_t sb = smem_u32(bh);
-      wgmma_fence();
+    const uint32_t sb = smem_u32(bh);
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) {
-        uint32_t ah[4], al[4];
+    for (int ks = 0; ks < 2; ++ks) {
+      fence_frag4(ah[ks]);
+      if (MODE == MODE_TF32X3) fence_frag4(al[ks]);
+    }
+    wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          float h, lo;
-          split_tf32_fast(a[ks][i], h, lo);
-          ah[i] = __float_as_uint(h);
-          al[i] = __float_as_uint(lo);
+    for (int ks = 0; ks < 2; ++ks) {
+      const uint32_t acc0 = (fold > 0 || ks > 0) ? 1u : 0u;
+      if constexpr (NBC == 8) {
+        const uint32_t base = sb + ks * 2 * lbo;
+        const uint64_t dh = make_desc(base, lbo, 128);
+        if (MODE == MODE_TF32X3) {
+          wgmma_tf32_n128(acc, al[ks], dh, acc0);
+          wgmma_tf32_n128(acc, ah[ks], make_desc(base + TB_BIMG, lbo, 128), 1u);
+          wgmma_tf32_n128(acc, ah[ks], dh, 1u);
+        } else {
+          wgmma_tf32_n128(acc, ah[ks], dh, acc0);
         }
-        const uint32_t acc0 = (fold > 0 || ks > 0) ? 1u : 0u;
+      } else {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (j >= nb) break;
+        for (int j = 0; j < NBC; ++j) {
           const uint32_t base = sb + ks * 2 * lbo + j * 256;
           const uint64_t dh = make_desc(base, lbo, 128);
           if (MODE == MODE_TF32X3) {
-            wgmma_tf32_n16(acc + 8 * j, al, dh, acc0);
-            wgmma_tf32_n16(acc + 8 * j, ah, make_desc(base + TB_BIMG, lbo, 128), 1u);
-            wgmma_tf32_n16(acc + 8 * j, ah, dh, 1u);
+            wgmma_tf32_n16(acc + 8 * j, al[ks], dh, acc0);
+            wgmma_tf32_n16(acc + 8 * j, ah[ks], make_desc(base + TB_BIMG, lbo, 128), 1u);
+            wgmma_tf32_n16(acc + 8 * j, ah[ks], dh, 1u);
           } else {
-            wgmma_tf32_n16(acc + 8 * j, ah, dh, acc0);
+            wgmma_tf32_n16(acc + 8 * j, ah[ks], dh, acc0);
           }
         }
       }
@@ -579,18 +657,17 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
   wgmma_wait<0>();
 #pragma unroll
   for (int j = 0; j < 8; ++j) fence_acc8(acc + 8 * j);
-  if (!mma_on) return;
   if (nch > 0)
 #pragma unroll
-    for (int i = 0; i < 64; ++i) sum[i] += acc[i];
+    for (int i = 0; i < 64; ++i) sum[256 * i] += acc[i];
   float* out = p.partial + (int64_t)blockIdx.x * K * p.ldp;
 #pragma unroll
   for (int b = 0; b < 16; ++b) {
     const int col = 8 * b + 2 * t;
     if (col >= C) break;
-    if (m0 < K) *reinterpret_cast<float2*>(out + (int64_t)m0 * p.ldp + col) = make_float2(sum[4 * b], sum[4 * b + 1]);
+    if (m0 < K) *reinterpret_cast<float2*>(out + (int64_t)m0 * p.ldp + col) = make_float2(sum[256 * (4 * b)], sum[256 * (4 * b + 1)]);
     if (m0 + 8 < K)
-      *reinterpret_cast<float2*>(out + (int64_t)(m0 + 8) * p.ldp + col) = make_float2(sum[4 * b + 2], sum[4 * b + 3]);
+      *reinterpret_cast<float2*>(out + (int64_t)(m0 + 8) * p.ldp + col) = make_float2(sum[256 * (4 * b + 2)], sum[256 * (4 * b + 3)]);
   }
 }
 
@@ -603,6 +680,24 @@ DevState g_dev[kMaxDev];
 template <typename F>
 bool set_smem(F* f, int bytes) {
   return cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess;
+}
+// to_basis_kernel<MODE, NBC> for NBC = NBC0 .. 8 (C = 16 .. 128)
+template <int MODE, int NBC0 = 1>
+bool set_to_basis_smem() {
+  if constexpr (NBC0 > 8) return true;
+  else return set_smem(to_basis_kernel<MODE, NBC0>, TB_SMEM) && set_to_basis_smem<MODE, NBC0 + 1>();
+}
+template <int MODE, int NBC0 = 1>
+void launch_to_basis(int nbc, int grid, const TcToBasisParams& p, cudaStream_t st) {
+  if constexpr (NBC0 <= 8) {
+    if (nbc == NBC0) to_basis_kernel<MODE, NBC0><<<grid, TB_THREADS, TB_SMEM, st>>>(p);
+    else launch_to_basis<MODE, NBC0 + 1>(nbc, grid, p, st);
+  }
+}
+template <int MODE>
+bool set_chain_smem() {
+  return set_smem(rows_chain_kernel<MODE, 128, false>, CHAIN_SMEM) && set_smem(rows_chain_kernel<MODE, 128, true>, CHAIN_SMEM) &&
+         set_smem(rows_chain_kernel<MODE, 256, false>, CHAIN_SMEM) && set_smem(rows_chain_kernel<MODE, 256, true>, CHAIN_SMEM);
 }
 
 }  // namespace
@@ -624,13 +719,8 @@ static DevState* cur_dev_state() {
       d.ok = (prop.major == 9 && prop.minor == 0) ? 1 : 0;
       d.sms = prop.multiProcessorCount;
       if (d.ok) {
-        const bool set = set_smem(rows_chain_kernel<MODE_TF32X3, 128>, CHAIN_SMEM) &&
-                         set_smem(rows_chain_kernel<MODE_TF32X3, 256>, CHAIN_SMEM) &&
-                         set_smem(rows_chain_kernel<MODE_TF32, 128>, CHAIN_SMEM) &&
-                         set_smem(rows_chain_kernel<MODE_TF32, 256>, CHAIN_SMEM) &&
-                         set_smem(rows_chain_kernel<MODE_BF16, 128>, CHAIN_SMEM) &&
-                         set_smem(rows_chain_kernel<MODE_BF16, 256>, CHAIN_SMEM) &&
-                         set_smem(to_basis_kernel<MODE_TF32X3>, TB_SMEM) && set_smem(to_basis_kernel<MODE_TF32>, TB_SMEM);
+        const bool set = set_chain_smem<MODE_TF32X3>() && set_chain_smem<MODE_TF32>() && set_chain_smem<MODE_BF16>() &&
+                         set_to_basis_smem<MODE_TF32X3>() && set_to_basis_smem<MODE_TF32>();
         if (!set) {
           cudaGetLastError();
           d.ok = 0;
@@ -740,10 +830,16 @@ int tc_pack_spectral_batched(DnLayer* layer0, int n_meshes, void* ws, int64_t ws
   return DN_OK;
 }
 
+// wide: every layer is exactly 128 wide, or the single layer is 256 wide (full-width MMAs)
 template <int MODE>
-static void launch_chain(const HcParams& p, int nmax, int grid, cudaStream_t st) {
-  if (nmax <= 128) rows_chain_kernel<MODE, 128><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
-  else rows_chain_kernel<MODE, 256><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
+static void launch_chain(const HcParams& p, int nmax, bool wide, int grid, cudaStream_t st) {
+  if (nmax <= 128) {
+    if (wide) rows_chain_kernel<MODE, 128, true><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
+    else rows_chain_kernel<MODE, 128, false><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
+  } else {
+    if (wide) rows_chain_kernel<MODE, 256, true><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
+    else rows_chain_kernel<MODE, 256, false><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
+  }
 }
 
 int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, int64_t V, int passes, void* ws,
@@ -777,7 +873,7 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
   p.V = V;
   p.tile_group = layers[0].tile_group;
   p.group_stride = layers[0].group_stride;
-  int nmax = 0;
+  int nmax = 0, nmin = 1 << 30;
   for (int l = 0; l < n_layers; ++l) {
     const DnLayer& L = layers[l];
     HcLayer& T = p.layer[l];
@@ -785,14 +881,16 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
     T.residual = L.residual; T.ld_res = L.ld_res; T.res_scale = L.res_scale; T.out = L.out; T.ld_out = L.ld_out;
     T.K = L.K; T.N = L.N; T.relu = L.relu;
     if (L.N > nmax) nmax = L.N;
+    if (L.N < nmin) nmin = L.N;
   }
+  const bool wide = nmin == nmax && (nmax == 128 || nmax == 256);
   const DnLayer& Ll = layers[n_layers - 1];
   p.head_w = Ll.head_w; p.head_b = Ll.head_b; p.head_out = Ll.head_out; p.ld_head_out = Ll.ld_head_out; p.head_n = Ll.head_n;
   const int64_t ntiles = (V + TILE_M - 1) / TILE_M;
   const int grid = (int)(ntiles < dv->sms ? ntiles : dv->sms);
-  if (bf16) launch_chain<MODE_BF16>(p, nmax, grid, st);
-  else if (passes == 3) launch_chain<MODE_TF32X3>(p, nmax, grid, st);
-  else launch_chain<MODE_TF32>(p, nmax, grid, st);
+  if (bf16) launch_chain<MODE_BF16>(p, nmax, wide, grid, st);
+  else if (passes == 3) launch_chain<MODE_TF32X3>(p, nmax, wide, grid, st);
+  else launch_chain<MODE_TF32>(p, nmax, wide, grid, st);
   DN_LAUNCH_CHECK();
   return DN_OK;
 }
@@ -831,8 +929,8 @@ int tc_to_basis_partial(const float* values, const float* basis, const float* ma
     grid = (int)((total_chunks + p.chunks_per_cta - 1) / p.chunks_per_cta);
     if (grid < 1) grid = 1;
   }
-  if (passes == 3) to_basis_kernel<MODE_TF32X3><<<grid, TB_THREADS, TB_SMEM, st>>>(p);
-  else to_basis_kernel<MODE_TF32><<<grid, TB_THREADS, TB_SMEM, st>>>(p);
+  if (passes == 3) launch_to_basis<MODE_TF32X3>(C / 16, grid, p, st);
+  else launch_to_basis<MODE_TF32>(C / 16, grid, p, st);
   DN_LAUNCH_CHECK();
   *P_out = grid;
   return DN_OK;

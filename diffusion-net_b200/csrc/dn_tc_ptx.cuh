@@ -84,6 +84,11 @@ __device__ __forceinline__ void fence_acc8(float* d) {
   asm volatile("" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
                :: "memory");
 }
+// pins an A fragment ahead of the next wgmma_fence: without it the compiler may form the fragment (a convert, a
+// subtraction) after the fence, right before its MMA, and ptxas then inserts a warpgroup arrive before every MMA
+__device__ __forceinline__ void fence_frag4(uint32_t* a) {
+  asm volatile("" : "+r"(a[0]), "+r"(a[1]), "+r"(a[2]), "+r"(a[3]) :: "memory");
+}
 
 // D[64 x 16] (+)= A[64 x 8] (registers, tf32) * B[8 x 16] (smem descriptor, K-major tf32), fp32 accumulate.
 //   A fragment of lane (g = lane / 4, t = lane % 4) in warp w: a0 (16w+g, t), a1 (16w+g+8, t), a2 (16w+g, t+4),
@@ -105,6 +110,62 @@ __device__ __forceinline__ void wgmma_bf16_n16(float* d, const uint32_t* a, uint
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
       : "memory");
+}
+
+// Full-width forms: D[64 x N] (+)= A * B[K x N] in one instruction (N = 128 or 256; N / 2 accumulators per lane).  B is
+// the same K-major canonical layout with 8-row groups 128 B apart, so one descriptor at the operand's base covers all N
+// columns, and the D fragment is the n16 fragments laid end to end: d[4b + {0,1,2,3}] belongs to 8-column block b.
+#define DN_ACC8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
+                   "+f"(d[o + 6]), "+f"(d[o + 7])
+#define DN_ACC64 DN_ACC8(0), DN_ACC8(8), DN_ACC8(16), DN_ACC8(24), DN_ACC8(32), DN_ACC8(40), DN_ACC8(48), DN_ACC8(56)
+#define DN_ACC128 DN_ACC64, DN_ACC8(64), DN_ACC8(72), DN_ACC8(80), DN_ACC8(88), DN_ACC8(96), DN_ACC8(104), DN_ACC8(112), \
+                  DN_ACC8(120)
+#define DN_REGS64 \
+  "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15," \
+  "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
+  "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47," \
+  "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+#define DN_REGS128 DN_REGS64 "," \
+  "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79," \
+  "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95," \
+  "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111," \
+  "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+// one wrapper: name, instruction, D register list, operand numbers of A / descriptor / scale-d, trailing immediates
+#define DN_WGMMA_WIDE(NAME, INSTR, REGS, A, DESC, SCALE_D, IMM, ACC)                                                  \
+  __device__ __forceinline__ void NAME(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {         \
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, " SCALE_D ", 0;\n" INSTR " {" REGS "}, {" A "}, " DESC ", p, " \
+                 IMM ";\n}"                                                                                          \
+                 : ACC                                                                                             \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)                        \
+                 : "memory");                                                                                      \
+  }
+DN_WGMMA_WIDE(wgmma_tf32_n128, "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32", DN_REGS64, "%64,%65,%66,%67",
+              "%68", "%69", "1, 1", DN_ACC64)
+DN_WGMMA_WIDE(wgmma_tf32_n256, "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32", DN_REGS128,
+              "%128,%129,%130,%131", "%132", "%133", "1, 1", DN_ACC128)
+DN_WGMMA_WIDE(wgmma_bf16_n128, "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16", DN_REGS64, "%64,%65,%66,%67",
+              "%68", "%69", "1, 1, 0", DN_ACC64)
+DN_WGMMA_WIDE(wgmma_bf16_n256, "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16", DN_REGS128,
+              "%128,%129,%130,%131", "%132", "%133", "1, 1, 0", DN_ACC128)
+#undef DN_WGMMA_WIDE
+#undef DN_REGS128
+#undef DN_REGS64
+#undef DN_ACC128
+#undef DN_ACC64
+#undef DN_ACC8
+
+// one MMA over the whole N-wide accumulator (N = 128 or 256); `accumulate` = 0 starts a new sum (D = A B)
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
+  static_assert(N == 128 || N == 256, "wgmma_tf32: unsupported width");
+  if constexpr (N == 128) wgmma_tf32_n128(d, a, b_desc, accumulate);
+  else wgmma_tf32_n256(d, a, b_desc, accumulate);
+}
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
+  static_assert(N == 128 || N == 256, "wgmma_bf16: unsupported width");
+  if constexpr (N == 128) wgmma_bf16_n128(d, a, b_desc, accumulate);
+  else wgmma_bf16_n256(d, a, b_desc, accumulate);
 }
 
 // two fp32 -> packed bf16x2 (round to nearest even): `lo` in bits [0,16), `hi` in bits [16,32)

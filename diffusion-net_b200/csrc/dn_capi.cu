@@ -24,13 +24,23 @@ struct Bump {
 
 constexpr int64_t kPartialFloats = 16ll << 20;  // 64 MiB split-V partial sums
 
-inline bool use_tc(int engine) { return engine == DN_ENGINE_TC3X || engine == DN_ENGINE_TC1X || engine == DN_ENGINE_BF16; }
-inline int tc_passes(int engine) { return engine == DN_ENGINE_TC1X ? 1 : (engine == DN_ENGINE_BF16 ? DN_PASSES_BF16 : 3); }
+// The engine of one C-ABI call: tensor cores (with their pass count) or the exact SIMT kernels throughout.
+struct Engine {
+  bool tc;
+  int passes;
+};
+
+// A tensor-core engine on a device without the tensor-core kernels is an error (DN_ERR_NOT_SM100): there is no
+// multi-backend dispatch.  Every entry point that dispatches resolves its engine once, before it enqueues any work.
+int resolve(int engine, Engine* e) {
+  e->tc = engine == DN_ENGINE_TC3X || engine == DN_ENGINE_TC1X || engine == DN_ENGINE_BF16;
+  e->passes = engine == DN_ENGINE_TC1X ? 1 : (engine == DN_ENGINE_BF16 ? DN_PASSES_BF16 : 3);
+  return e->tc && !tc_supported_device() ? DN_ERR_NOT_SM100 : DN_OK;
+}
 
 // A tensor-core engine was requested but this contraction is outside the wgmma kernels' envelope and runs the exact
 // fp32 SIMT kernel instead (same result class or better, slower).  Said once per shape on stderr; DN_STRICT_TC=1 turns
-// it into DN_ERR_UNSUPPORTED so that a deployment never runs the slow path unnoticed.  A non-sm_90 device with a
-// tensor-core engine is always an error (DN_ERR_NOT_SM100): there is no multi-backend dispatch.
+// it into DN_ERR_UNSUPPORTED so that a deployment never runs the slow path unnoticed.
 int note_simt_fallback(const char* what, int K, int N) {
   static int strict = -1;
   if (strict < 0) { const char* e = getenv("DN_STRICT_TC"); strict = (e && atoi(e)) ? 1 : 0; }
@@ -45,10 +55,6 @@ int note_simt_fallback(const char* what, int K, int N) {
   }
   return strict ? DN_ERR_UNSUPPORTED : DN_OK;
 }
-#define DN_TC_DEVICE_OR_FAIL(engine)                                              \
-  do {                                                                            \
-    if (use_tc(engine) && !tc_supported_device()) return DN_ERR_NOT_SM100;        \
-  } while (0)
 
 inline DnLayer make_layer(const float* W, int64_t ldw, int w_trans, const float* bias, int relu, int K, int N,
                           float* out, int64_t ld_out) {
@@ -66,59 +72,82 @@ inline DnRowsSrc one_src(const float* p, int width, int64_t ld) {
   return s;
 }
 
-// run a chain of layers; tensor-core engine when it supports the shapes, exact SIMT otherwise.
-// `tmp0/tmp1` are V x maxN ping-pong buffers used only by the unfused SIMT route.
-int run_chain(const DnRowsSrc& src, DnLayer* layers, int n_layers, int64_t V, int engine, float* tmp0,
-              float* tmp1, void* tc_ws, int64_t tc_ws_bytes, cudaStream_t st) {
-  DN_TC_DEVICE_OR_FAIL(engine);
-  const bool tc = use_tc(engine) && tc_supported_device();
-  if (tc && tc_rows_chain_supported(src, layers, n_layers, tc_passes(engine)) == DN_OK) {
-    return tc_rows_chain(src, layers, n_layers, V, tc_passes(engine), tc_ws, tc_ws_bytes, st);
+// One layer on the exact SIMT kernel.  simt_rows_gemm takes every layer but a w_trans one with a second weight block
+// (grad_x = dP A_re + dQ A_im over the sources dP | dQ): that runs as two passes, the second adding the first's output
+// as its residual, which is exact only for a layer without bias or activation.
+int simt_layer(const DnRowsSrc& src, const DnLayer& L, int64_t V, cudaStream_t st) {
+  if (!L.w_trans || !L.W2) return simt_rows_gemm(src, L, V, st);
+  if (src.nsrc != 2 || src.width[0] != L.n_split || L.bias || L.relu || L.emul || L.relu_mask_src || L.row_scale)
+    return DN_ERR_UNSUPPORTED;
+  DnLayer L0 = L;
+  L0.W2 = nullptr; L0.n_split = 0; L0.K = L.n_split;
+  int rc = simt_rows_gemm(one_src(src.ptr[0], src.width[0], src.ld[0]), L0, V, st);
+  if (rc) return rc;
+  DnLayer L1 = L0;
+  L1.W = L.W2; L1.K = L.K - L.n_split; L1.residual = L.out; L1.ld_res = L.ld_out; L1.res_scale = 1.f;
+  return simt_rows_gemm(one_src(src.ptr[1], src.width[1], src.ld[1]), L1, V, st);
+}
+
+// The one way dense layers run.  The chain is one fused tensor-core launch when rows_chain_kernel takes it whole (a
+// chain whose weights the caller packed, the caller planned).  Otherwise it runs layer by layer, each on the tensor-core
+// kernel when its shape allows and on the exact SIMT kernel otherwise; layers without `out` then write two V x N
+// ping-pong buffers carved from ws.  The rest of ws is where the tensor-core kernel packs weights.
+int run_chain(const DnRowsSrc& src, DnLayer* layers, int n_layers, int64_t V, Engine e, Bump ws, cudaStream_t st) {
+  if (e.tc && (layers[0].prepacked || tc_chain_plan(src, layers, n_layers, e.passes) >= 0))
+    return tc_rows_chain(src, layers, n_layers, V, e.passes, ws.base + ws.off, ws.size - ws.off, st);
+  // not fusable as a whole (e.g. a 256-wide layer inside a chain)
+  float* tmp[2] = {nullptr, nullptr};
+  int maxn = 0;
+  bool need_tmp = false;
+  for (int l = 0; l < n_layers; ++l) {
+    if (layers[l].N > maxn) maxn = layers[l].N;
+    need_tmp = need_tmp || !layers[l].out;
   }
-  // not fusable as a whole (e.g. a 256-wide layer inside a chain): layer by layer, each on the
-  // tensor-core kernel when its shape allows, on the exact SIMT kernel otherwise
+  if (need_tmp) {
+    tmp[0] = ws.take(V * maxn);
+    tmp[1] = ws.take(V * maxn);
+    if (!tmp[0] || !tmp[1]) return DN_ERR_WORKSPACE;
+  }
   DnRowsSrc cur = src;
   for (int l = 0; l < n_layers; ++l) {
     DnLayer L = layers[l];
-    float* o = L.out;
-    int64_t ldo = L.ld_out;
-    if (!o) {
-      o = (l & 1) ? tmp1 : tmp0;
-      ldo = L.N;
-      if (!o) return DN_ERR_WORKSPACE;
-    }
-    L.out = o; L.ld_out = ldo;
+    if (!L.out) { L.out = tmp[l & 1]; L.ld_out = L.N; }
     int rc;
-    if (tc && tc_rows_chain_supported(cur, &L, 1, tc_passes(engine)) == DN_OK)
-      rc = tc_rows_chain(cur, &L, 1, V, tc_passes(engine), tc_ws, tc_ws_bytes, st);
-    else {
-      if (use_tc(engine) && (rc = note_simt_fallback("a dense layer", L.K, L.N))) return rc;
-      rc = simt_rows_gemm(cur, L, V, st);
-    }
+    // (a single layer was planned above)
+    if (e.tc && n_layers > 1 && tc_chain_plan(cur, &L, 1, e.passes) >= 0)
+      rc = tc_rows_chain(cur, &L, 1, V, e.passes, ws.base + ws.off, ws.size - ws.off, st);
+    else if (e.tc && (rc = note_simt_fallback("a dense layer", L.K, L.N)))
+      return rc;
+    else
+      rc = simt_layer(cur, L, V, st);
     if (rc) return rc;
-    cur = one_src(o, L.N, ldo);
+    cur = one_src(L.out, L.N, L.ld_out);
   }
   return DN_OK;
 }
 
+// partial[p][k][c] = sum over the rows of split p of basis[v][k] * (mass[v] * values[v][c]), p < *P.  `batch`
+// (optional) is a mesh batch's CTA plan: CTA p reduces rows tb_rows[2p] .. tb_rows[2p + 1], on tensor cores only.
 int to_basis_partials(const float* values, const float* basis, const float* massvec, int64_t V, int K, int C,
-                      float* partial, int64_t partial_floats, int* P, int engine, cudaStream_t st) {
-  if (use_tc(engine) && tc_supported_device() && tc_to_basis_supported(K, C) == DN_OK &&
-      (int64_t)dn_sm_count() * K * C <= partial_floats) {
-    return tc_to_basis_partial(values, basis, massvec, V, K, C, partial, P, tc_passes(engine), st);
-  }
-  // wider than one accumulator set (C_width = 256): 128-column slices, each its own launch into the shared partials
-  if (use_tc(engine) && tc_supported_device() && C > 128 && C % 128 == 0 && tc_to_basis_supported(K, 128) == DN_OK &&
-      (int64_t)dn_sm_count() * K * C <= partial_floats) {
-    for (int c0 = 0; c0 < C; c0 += 128) {
-      const int rc = tc_to_basis_partial(values + c0, basis, massvec, V, K, 128, partial + c0, P, tc_passes(engine), st, C, C);
-      if (rc) return rc;
+                      float* partial, int64_t partial_floats, int* P, Engine e, cudaStream_t st,
+                      const dn_mesh_batch* batch = nullptr) {
+  const int32_t* rows = batch ? batch->tb_rows : nullptr;
+  const int ctas = batch ? batch->n_tb_ctas : dn_sm_count();
+  if (e.tc && (int64_t)ctas * K * C <= partial_floats) {
+    if (tc_to_basis_supported(K, C) == DN_OK)
+      return tc_to_basis_partial(values, basis, massvec, V, K, C, partial, P, e.passes, st, 0, 0, rows, ctas);
+    // wider than one accumulator set (C_width = 256): 128-column slices, each its own launch into the shared partials
+    if (C > 128 && C % 128 == 0 && tc_to_basis_supported(K, 128) == DN_OK) {
+      for (int c0 = 0; c0 < C; c0 += 128) {
+        const int rc = tc_to_basis_partial(values + c0, basis, massvec, V, K, 128, partial + c0, P, e.passes, st, C, C,
+                                           rows, ctas);
+        if (rc) return rc;
+      }
+      return DN_OK;
     }
-    return DN_OK;
   }
-  DN_TC_DEVICE_OR_FAIL(engine);
-  if (use_tc(engine)) { const int rc = note_simt_fallback("to_basis", K, C); if (rc) return rc; }
-  // out[k][c] = sum_v basis[v][k] * (mass[v] * values[v][c])
+  if (batch) return DN_ERR_UNSUPPORTED;   // mesh batches have no SIMT route
+  if (e.tc) { const int rc = note_simt_fallback("to_basis", K, C); if (rc) return rc; }
   return simt_atb_partial_st(basis, K, K, values, C, C, massvec, V, partial, partial_floats, P, st);
 }
 
@@ -126,26 +155,16 @@ int to_basis_partials(const float* values, const float* basis, const float* mass
 // Tensor cores (the split-V to_basis kernel, reference geometry.py:572-583 has the same contraction) when both
 // operands are contiguous and at most 128 wide; the exact SIMT kernel otherwise.
 int atb(const float* A, int64_t lda, int I, const float* B, int64_t ldb, int J, int64_t V, float* out, int64_t ld_out,
-        int accumulate, float* part, int64_t part_floats, int engine, cudaStream_t st) {
-  if (use_tc(engine) && tc_supported_device() && lda == I && ldb == J && tc_to_basis_supported(I, J) == DN_OK &&
+        int accumulate, float* part, int64_t part_floats, Engine e, cudaStream_t st) {
+  if (e.tc && lda == I && ldb == J && tc_to_basis_supported(I, J) == DN_OK &&
       (int64_t)dn_sm_count() * I * J <= part_floats) {
     int P = 0;
-    int rc = tc_to_basis_partial(B, A, nullptr, V, I, J, part, &P, tc_passes(engine), st);
+    int rc = tc_to_basis_partial(B, A, nullptr, V, I, J, part, &P, e.passes, st);
     if (rc == DN_OK) return launch_reduce_partials_ld(part, P, I, J, out, ld_out, accumulate, st);
     if (rc != DN_ERR_UNSUPPORTED) return rc;
   }
-  DN_TC_DEVICE_OR_FAIL(engine);
-  if (use_tc(engine)) { const int rc = note_simt_fallback("a weight gradient", I, J); if (rc) return rc; }
+  if (e.tc) { const int rc = note_simt_fallback("a weight gradient", I, J); if (rc) return rc; }
   return simt_atb(A, lda, I, B, ldb, J, nullptr, V, out, ld_out, accumulate, part, part_floats, st);
-}
-
-// one dense layer on the tensor-core chain kernel when it takes the shape, else the exact SIMT kernel
-int one_layer(const DnRowsSrc& src, DnLayer& L, int64_t V, int engine, void* tc_ws, int64_t tc_ws_bytes, cudaStream_t st) {
-  if (use_tc(engine) && tc_supported_device() && tc_rows_chain_supported(src, &L, 1, tc_passes(engine)) == DN_OK)
-    return tc_rows_chain(src, &L, 1, V, tc_passes(engine), tc_ws, tc_ws_bytes, st);
-  DN_TC_DEVICE_OR_FAIL(engine);
-  if (use_tc(engine)) { const int rc = note_simt_fallback("a dense layer", L.K, L.N); if (rc) return rc; }
-  return simt_rows_gemm(src, L, V, st);
 }
 
 }  // namespace
@@ -299,24 +318,29 @@ int dn_compute_hks(const float* evals, const float* evecs, const float* scales, 
 int dn_to_basis(const float* values, const float* basis, const float* massvec, int64_t V, int K, int C, float* out,
                 void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream) {
   if (!values || !basis || !out || V < 0 || K <= 0 || C <= 0) return DN_ERR_INVALID_ARGUMENT;
+  Engine e;
+  int rc = resolve(engine, &e);
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Bump ws(workspace, ws_bytes);
   const int64_t pf = ws.left_floats() < kPartialFloats ? ws.left_floats() : kPartialFloats;
   float* partial = ws.take(pf);
   if (!partial) return DN_ERR_WORKSPACE;
   int P = 0;
-  int rc = to_basis_partials(values, basis, massvec, V, K, C, partial, pf, &P, engine, st);
-  if (rc) return rc;
+  if ((rc = to_basis_partials(values, basis, massvec, V, K, C, partial, pf, &P, e, st))) return rc;
   return launch_reduce_partials(partial, P, (int64_t)K * C, out, st);
 }
 
 int dn_from_basis(const float* values, const float* basis, const float* row_scale, int64_t V, int K, int C,
                   float* out, void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream) {
   if (!values || !basis || !out || V < 0 || K <= 0 || C <= 0) return DN_ERR_INVALID_ARGUMENT;
+  Engine e;
+  const int rc = resolve(engine, &e);
+  if (rc) return rc;
   DnRowsSrc src = one_src(basis, K, K);
   DnLayer L = make_layer(values, C, /*w_trans=*/1, nullptr, 0, K, C, out, C);
   L.row_scale = row_scale;
-  return run_chain(src, &L, 1, V, engine, nullptr, nullptr, workspace, ws_bytes, (cudaStream_t)stream);
+  return run_chain(src, &L, 1, V, e, Bump(workspace, ws_bytes), (cudaStream_t)stream);
 }
 
 int dn_learned_time_diffusion_fwd(const float* x, const float* mass, const float* evals, const float* evecs,
@@ -324,6 +348,9 @@ int dn_learned_time_diffusion_fwd(const float* x, const float* mass, const float
                                   void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream) {
   if (!x || !mass || !evals || !evecs || !time || !x_diffuse || V < 0 || K <= 0 || C <= 0)
     return DN_ERR_INVALID_ARGUMENT;
+  Engine e;
+  int rc = resolve(engine, &e);
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Bump ws(workspace, ws_bytes);
   float* S = ws.take((int64_t)K * C);
@@ -331,13 +358,12 @@ int dn_learned_time_diffusion_fwd(const float* x, const float* mass, const float
   float* partial = ws.take(pf);
   if (!S || !partial) return DN_ERR_WORKSPACE;
   int P = 0;
-  int rc = to_basis_partials(x, evecs, mass, V, K, C, partial, pf, &P, engine, st);
-  if (rc) return rc;
+  if ((rc = to_basis_partials(x, evecs, mass, V, K, C, partial, pf, &P, e, st))) return rc;
   rc = launch_spectral_scale(partial, P, evals, time, K, C, x_spec_out, S, /*clamp_writeback=*/1, st);
   if (rc) return rc;
   DnRowsSrc src = one_src(evecs, K, K);
   DnLayer L = make_layer(S, C, 1, nullptr, 0, K, C, x_diffuse, C);
-  return run_chain(src, &L, 1, V, engine, nullptr, nullptr, ws.base + ws.off, ws.size - ws.off, st);
+  return run_chain(src, &L, 1, V, e, ws, st);
 }
 
 int dn_learned_time_diffusion_bwd(const float* grad_out, const float* mass, const float* evals, const float* evecs,
@@ -346,6 +372,9 @@ int dn_learned_time_diffusion_bwd(const float* grad_out, const float* mass, cons
                                   dn_stream_t stream) {
   if (!grad_out || !mass || !evals || !evecs || !time || !x_spec || !grad_x || !grad_time)
     return DN_ERR_INVALID_ARGUMENT;
+  Engine e;
+  int rc = resolve(engine, &e);
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Bump ws(workspace, ws_bytes);
   float* dS = ws.take((int64_t)K * C);
@@ -353,8 +382,7 @@ int dn_learned_time_diffusion_bwd(const float* grad_out, const float* mass, cons
   float* partial = ws.take(pf);
   if (!dS || !partial) return DN_ERR_WORKSPACE;
   int P = 0;
-  int rc = to_basis_partials(grad_out, evecs, nullptr, V, K, C, partial, pf, &P, engine, st);
-  if (rc) return rc;
+  if ((rc = to_basis_partials(grad_out, evecs, nullptr, V, K, C, partial, pf, &P, e, st))) return rc;
   if (P > 4) {
     // spectral_bwd walks the partials serially per channel: with the ~132 split-V partials of the tensor-core kernel that
     // took 4.5 ms (V = 7k); sum them first (coalesced, parallel) and hand it one
@@ -369,7 +397,7 @@ int dn_learned_time_diffusion_bwd(const float* grad_out, const float* mass, cons
   DnRowsSrc src = one_src(evecs, K, K);
   DnLayer L = make_layer(dS, C, 1, nullptr, 0, K, C, grad_x, C);
   L.row_scale = mass;
-  return run_chain(src, &L, 1, V, engine, nullptr, nullptr, ws.base + ws.off, ws.size - ws.off, st);
+  return run_chain(src, &L, 1, V, e, ws, st);
 }
 
 int dn_grad_spmm(const dn_csr* grad, const float* x, int64_t V, int C, float* out, dn_stream_t stream) {
@@ -419,6 +447,9 @@ int dn_gradient_features_fwd(const dn_csr* grad, const float* x_diffuse, const f
       C <= 0)
     return DN_ERR_INVALID_ARGUMENT;
   if (C % 4) return DN_ERR_UNSUPPORTED;
+  Engine e;
+  int rc = resolve(engine, &e);
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Bump ws(workspace, ws_bytes);
   const int npq = with_gradient_rotations ? 2 * C : C;
@@ -427,8 +458,7 @@ int dn_gradient_features_fwd(const dn_csr* grad, const float* x_diffuse, const f
   DnRowsSrc src = one_src(x_diffuse, C, C);
   DnLayer L = make_layer(A_re, C, 0, nullptr, 0, C, npq, pq, npq);   // [P|Q] = xd [A_re;A_im]^T
   if (with_gradient_rotations) { L.W2 = A_im; L.n_split = C; }
-  int rc = run_chain(src, &L, 1, V, engine, nullptr, nullptr, ws.base + ws.off, ws.size - ws.off, st);
-  if (rc) return rc;
+  if ((rc = run_chain(src, &L, 1, V, e, ws, st))) return rc;
   return launch_spmm_features(grad, x_diffuse, pq, with_gradient_rotations, V, C, features, st);
 }
 
@@ -441,6 +471,9 @@ int dn_gradient_features_bwd(const dn_csr* grad, const dn_csr* grad_t, const flo
       (with_gradient_rotations && (!A_im || !grad_A_im)))
     return DN_ERR_INVALID_ARGUMENT;
   if (C % 4) return DN_ERR_UNSUPPORTED;
+  Engine e;
+  int rc = resolve(engine, &e);
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   Bump ws(workspace, ws_bytes);
   const int rot = with_gradient_rotations;
@@ -450,39 +483,19 @@ int dn_gradient_features_bwd(const dn_csr* grad, const dn_csr* grad_t, const flo
   float* dQ = rot ? ws.take(V * C) : nullptr;      // kernel's two sources and the weight-gradient kernel's operands
   float* part = ws.take(kPartialFloats / 4);
   if (!U || !dxd || !dP || (rot && !dQ) || !part) return DN_ERR_WORKSPACE;
-  void* tcws = ws.base + ws.off;
-  const int64_t tcws_bytes = ws.size - ws.off;
-  int rc;
   if ((rc = launch_features_bwd_local(grad, x_diffuse, pq, features, grad_features, rot, V, C, U, st))) return rc;
   if ((rc = launch_features_bwd_transpose(grad_t, U, rot, V, C, dxd, dP, dQ, C, st))) return rc;
   // grad_x = dxd + dP A_re (+ dQ A_im): one layer over the sources (dP | dQ) with [A_re ; A_im] stacked along K
-  {
-    DnRowsSrc s;
-    memset(&s, 0, sizeof(s));
-    s.ptr[0] = dP; s.width[0] = C; s.ld[0] = C; s.nsrc = 1;
-    if (rot) { s.ptr[1] = dQ; s.width[1] = C; s.ld[1] = C; s.nsrc = 2; }
-    DnLayer L = make_layer(A_re, C, /*w_trans=*/1, nullptr, 0, rot ? 2 * C : C, C, grad_x, C);
-    if (rot) { L.W2 = A_im; L.n_split = C; }
-    L.residual = dxd; L.ld_res = C;
-    if (use_tc(engine) && tc_supported_device() && tc_rows_chain_supported(s, &L, 1, tc_passes(engine)) == DN_OK) {
-      if ((rc = tc_rows_chain(s, &L, 1, V, tc_passes(engine), tcws, tcws_bytes, st))) return rc;
-    } else {                                       // exact SIMT route: one source at a time
-      DnRowsSrc s0 = one_src(dP, C, C);
-      DnLayer L0 = make_layer(A_re, C, 1, nullptr, 0, C, C, grad_x, C);
-      L0.residual = dxd; L0.ld_res = C;
-      if ((rc = simt_rows_gemm(s0, L0, V, st))) return rc;
-      if (rot) {
-        DnRowsSrc s1 = one_src(dQ, C, C);
-        DnLayer L1 = make_layer(A_im, C, 1, nullptr, 0, C, C, grad_x, C);
-        L1.residual = grad_x; L1.ld_res = C;
-        if ((rc = simt_rows_gemm(s1, L1, V, st))) return rc;
-      }
-    }
-  }
+  DnRowsSrc s = one_src(dP, C, C);
+  if (rot) { s.ptr[1] = dQ; s.width[1] = C; s.ld[1] = C; s.nsrc = 2; }
+  DnLayer L = make_layer(A_re, C, /*w_trans=*/1, nullptr, 0, rot ? 2 * C : C, C, grad_x, C);
+  if (rot) { L.W2 = A_im; L.n_split = C; }
+  L.residual = dxd; L.ld_res = C;
+  if ((rc = run_chain(s, &L, 1, V, e, ws, st))) return rc;
   // grad_A_re[n][k] += sum_v dP[v][n] xd[v][k]   (and grad_A_im from dQ)
-  if ((rc = atb(dP, C, C, x_diffuse, C, C, V, grad_A_re, C, 1, part, kPartialFloats / 4, engine, st))) return rc;
+  if ((rc = atb(dP, C, C, x_diffuse, C, C, V, grad_A_re, C, 1, part, kPartialFloats / 4, e, st))) return rc;
   if (rot)
-    if ((rc = atb(dQ, C, C, x_diffuse, C, C, V, grad_A_im, C, 1, part, kPartialFloats / 4, engine, st))) return rc;
+    if ((rc = atb(dQ, C, C, x_diffuse, C, C, V, grad_A_im, C, 1, part, kPartialFloats / 4, e, st))) return rc;
   return DN_OK;
 }
 
@@ -505,7 +518,6 @@ int dn_mini_mlp_fwd(const float* const* src_host, const int* src_width_host, int
   src.nsrc = nsrc;
   if (k0 != dims_host[0]) return DN_ERR_INVALID_ARGUMENT;
   DnLayer layers[DN_MAX_LAYERS];
-  int maxn = 0;
   for (int l = 0; l < n_layers; ++l) {
     if (!weight_host[l] || dims_host[l + 1] <= 0) return DN_ERR_INVALID_ARGUMENT;
     const bool last = (l + 1 == n_layers);
@@ -514,18 +526,11 @@ int dn_mini_mlp_fwd(const float* const* src_host, const int* src_width_host, int
                            dims_host[l], dims_host[l + 1], o, dims_host[l + 1]);
     if (!last && drop_mask_host) layers[l].emul = drop_mask_host[l];
     if (last && residual) { layers[l].residual = residual; layers[l].ld_res = dims_host[l + 1]; }
-    if (dims_host[l + 1] > maxn) maxn = dims_host[l + 1];
   }
-  Bump ws(workspace, ws_bytes);
-  float *t0 = nullptr, *t1 = nullptr;
-  const bool fused = use_tc(engine) && tc_supported_device() && tc_rows_chain_supported(src, layers, n_layers, tc_passes(engine)) == DN_OK;
-  if (!fused && n_layers > 1) {
-    t0 = ws.take(V * maxn);
-    t1 = ws.take(V * maxn);
-    if (!t0 || !t1) return DN_ERR_WORKSPACE;
-  }
-  return run_chain(src, layers, n_layers, V, engine, t0, t1, ws.base + ws.off, ws.size - ws.off,
-                   (cudaStream_t)stream);
+  Engine e;
+  const int rc = resolve(engine, &e);
+  if (rc) return rc;
+  return run_chain(src, layers, n_layers, V, e, Bump(workspace, ws_bytes), (cudaStream_t)stream);
 }
 
 int dn_mini_mlp_bwd(const float* grad_out, const float* const* src_host, const int* src_width_host, int nsrc,
@@ -537,6 +542,9 @@ int dn_mini_mlp_bwd(const float* grad_out, const float* const* src_host, const i
       n_layers < 1 || n_layers > DN_MAX_LAYERS || (n_layers > 1 && !hidden_host) || !grad_src_host ||
       !grad_weight_host)
     return DN_ERR_INVALID_ARGUMENT;
+  Engine e;
+  int rc = resolve(engine, &e);
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   int maxn = 0;
   for (int l = 0; l <= n_layers; ++l) maxn = dims_host[l] > maxn ? dims_host[l] : maxn;
@@ -545,22 +553,19 @@ int dn_mini_mlp_bwd(const float* grad_out, const float* const* src_host, const i
   float* d1 = ws.take(V * maxn);
   float* part = ws.take(kPartialFloats / 2);
   if (!d0 || !d1 || !part) return DN_ERR_WORKSPACE;
-  void* tcws = ws.base + ws.off;
-  const int64_t tcws_bytes = ws.size - ws.off;
   const float* dz = grad_out;   // gradient w.r.t. the pre-activation of layer l
-  int rc;
   for (int l = n_layers - 1; l >= 0; --l) {
     const int nout = dims_host[l + 1], nin = dims_host[l];
     // weight / bias gradients:  grad_W[n][k] += sum_v dz[v][n] * h_{l-1}[v][k]
     if (l > 0) {
       if ((rc = atb(dz, nout, nout, hidden_host[l - 1], nin, nin, V, grad_weight_host[l], nin, 1, part,
-                    kPartialFloats / 2, engine, st)))
+                    kPartialFloats / 2, e, st)))
         return rc;
     } else {
       int off = 0;
       for (int s = 0; s < nsrc; ++s) {
         if ((rc = atb(dz, nout, nout, src_host[s], src_width_host[s], src_width_host[s], V, grad_weight_host[0] + off,
-                      nin, 1, part, kPartialFloats / 2, engine, st)))
+                      nin, 1, part, kPartialFloats / 2, e, st)))
           return rc;
         off += src_width_host[s];
       }
@@ -574,7 +579,7 @@ int dn_mini_mlp_bwd(const float* grad_out, const float* const* src_host, const i
       DnLayer L = make_layer(weight_host[l], nin, /*w_trans=*/1, nullptr, 0, nout, nin, o, nin);
       L.relu_mask_src = hidden_host[l - 1];
       if (drop_mask_host && drop_mask_host[l - 1]) L.emul = drop_mask_host[l - 1];
-      if ((rc = one_layer(s, L, V, engine, tcws, tcws_bytes, st))) return rc;
+      if ((rc = run_chain(s, &L, 1, V, e, ws, st))) return rc;
       dz = o;
     } else {
       int off = 0;
@@ -582,7 +587,7 @@ int dn_mini_mlp_bwd(const float* grad_out, const float* const* src_host, const i
         if (grad_src_host[q]) {
           DnLayer L = make_layer(weight_host[0] + off, nin, 1, nullptr, 0, nout, src_width_host[q], grad_src_host[q],
                                  src_width_host[q]);
-          if ((rc = one_layer(s, L, V, engine, tcws, tcws_bytes, st))) return rc;
+          if ((rc = run_chain(s, &L, 1, V, e, ws, st))) return rc;
         }
         off += src_width_host[q];
       }
@@ -641,7 +646,6 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
   }
   const int nsrc = p->with_gradient_features ? 3 : 2;
   if (p->mlp_dims_host[0] != nsrc * C) return DN_ERR_INVALID_ARGUMENT;
-  int maxn = 0;
   for (int l = 0; l < nm; ++l) {
     const bool last = (l + 1 == nm);
     if (!p->mlp_weight_host[l] || p->mlp_dims_host[l + 1] <= 0) return DN_ERR_INVALID_ARGUMENT;
@@ -657,9 +661,10 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
         if (!out) Lh.out = nullptr;
       }
     }
-    if (p->mlp_dims_host[l + 1] > maxn) maxn = p->mlp_dims_host[l + 1];
   }
   if (p->mlp_dims_host[nm] != C) return DN_ERR_INVALID_ARGUMENT;
+  Engine e;
+  if ((rc = resolve(engine, &e))) return rc;
   DnRowsSrc src_fb = one_src(evecs, K, K);
   DnRowsSrc src_pq = one_src(xd, C, C);
   DnRowsSrc src_mlp;
@@ -667,106 +672,53 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
   const float* srcs[3] = {x_in, xd, feat};
   for (int q = 0; q < nsrc; ++q) { src_mlp.ptr[q] = srcs[q]; src_mlp.width[q] = C; src_mlp.ld[q] = C; }
   src_mlp.nsrc = nsrc;
-  // one launch packs (hi/lo split + wgmma layout) every weight the tensor-core kernels will stream
-  const bool tc = use_tc(engine) && tc_supported_device();
-  const int passes = tc_passes(engine);
-  const bool front_fused = tc && nfront == 2 && tc_rows_chain_supported(src_fb, &L[0], 2, passes) == DN_OK;
+  // which chains run on tensor cores: from_basis and [P|Q] as one fused chain when it fits, else each layer on its
+  // own; the MiniMLP chain
+  const bool front_fused = e.tc && nfront == 2 && tc_chain_plan(src_fb, &L[0], 2, e.passes) >= 0;
   bool tc_front = front_fused;
-  if (tc && !front_fused) {
-    tc_front = tc_rows_chain_supported(src_fb, &L[0], 1, passes) == DN_OK;
-    for (int l = 1; l < nfront; ++l) tc_front = tc_front && tc_rows_chain_supported(src_pq, &L[l], 1, passes) == DN_OK;
+  if (e.tc && !front_fused) {
+    tc_front = tc_chain_plan(src_fb, &L[0], 1, e.passes) >= 0;
+    for (int l = 1; l < nfront; ++l) tc_front = tc_front && tc_chain_plan(src_pq, &L[l], 1, e.passes) >= 0;
   }
-  const bool tc_mlp = tc && tc_rows_chain_supported(src_mlp, &L[nfront], nm, passes) == DN_OK;
+  const bool tc_mlp = e.tc && tc_chain_plan(src_mlp, &L[nfront], nm, e.passes) >= 0;
   if (head && !tc_mlp) return DN_ERR_UNSUPPORTED;
-  // the spectral multiplier S = exp(-lambda t) * (reduced partial sums) is layer 0's weight: when the tensor-core path
-  // takes the front chain it is formed inside the pack launch (no separate scale kernel, S never round-trips HBM)
-  if (batch && !tc_front) return DN_ERR_UNSUPPORTED;
+  // a batch forms every mesh's spectral multiplier in the pack launch of the tensor-core front chain
+  if (batch && (!tc_front || (V % 128) || batch->n_meshes < 1 || !batch->tile_mesh || !batch->tb_rows ||
+                !batch->mesh_cta_begin || batch->n_tb_ctas < 1))
+    return DN_ERR_UNSUPPORTED;
   // (nothing has been launched up to here: an unsupported head / batch returns before any work is enqueued)
   mark(0);
   // (a1) spectral diffusion: to_basis -> exp(-lambda t) -> from_basis   [layers.py:56-67]
-  if (batch) {
-    // grouped split-V: every CTA reduces a row range inside one mesh
-    if (!use_tc(engine) || !tc_supported_device() || (V % 128) || batch->n_meshes < 1 || !batch->tile_mesh ||
-        !batch->tb_rows || !batch->mesh_cta_begin || batch->n_tb_ctas < 1 || (int64_t)batch->n_tb_ctas * K * C > pf)
-      return DN_ERR_UNSUPPORTED;
-    if (tc_to_basis_supported(K, C) == DN_OK) {
-      if ((rc = tc_to_basis_partial(x_in, evecs, mass, V, K, C, partial, &P, tc_passes(engine), st, 0, 0, batch->tb_rows,
-                                    batch->n_tb_ctas)))
-        return rc;
-    } else if (C > 128 && C % 128 == 0 && tc_to_basis_supported(K, 128) == DN_OK) {
-      for (int c0 = 0; c0 < C; c0 += 128)
-        if ((rc = tc_to_basis_partial(x_in + c0, evecs, mass, V, K, 128, partial + c0, &P, tc_passes(engine), st, C, C,
-                                      batch->tb_rows, batch->n_tb_ctas)))
-          return rc;
-    } else {
-      return DN_ERR_UNSUPPORTED;
-    }
-  } else if ((rc = to_basis_partials(x_in, evecs, mass, V, K, C, partial, pf, &P, engine, st))) {
-    return rc;
-  }
+  if ((rc = to_basis_partials(x_in, evecs, mass, V, K, C, partial, pf, &P, e, st, batch))) return rc;
   mark(1);
   if (!tc_front)
     if ((rc = launch_spectral_scale(partial, P, evals, p->diffusion_time, K, C, nullptr, S, 1, st))) return rc;
   mark(2);
-  if (tc_front) {
-    if (front_fused) tc_choose_pack_fmt(src_fb, &L[0], 2, passes);
-    else {
-      tc_choose_pack_fmt(src_fb, &L[0], 1, passes);
-      for (int l = 1; l < nfront; ++l) tc_choose_pack_fmt(src_pq, &L[l], 1, passes);
-    }
-  }
-  if (tc_mlp) tc_choose_pack_fmt(src_mlp, &L[nfront], nm, passes);
-  if (batch) {
-    // one packed spectral multiplier per mesh (layer 0 of the front chain picks its matrix per tile), then every other
-    // weight of the block in one more launch
-    const int64_t pb0 = tc_chain_ws_bytes(&L[0], 1) * batch->n_meshes;
-    float* pk0 = ws.take(pb0 / 4);
-    if (!pk0) return DN_ERR_WORKSPACE;
-    if ((rc = tc_pack_spectral_batched(&L[0], batch->n_meshes, pk0, pb0, partial, batch->mesh_cta_begin, evals,
-                                       p->diffusion_time, 1, batch->tile_mesh, st)))
-      return rc;
-    const int cnt = (nfront - 1) + (tc_mlp ? nm : 0);
-    if (cnt > 0) {
-      DnLayer* first = (nfront > 1) ? &L[1] : &L[nfront];
-      const int64_t pb = tc_chain_ws_bytes(first, cnt);
-      float* pk = ws.take(pb / 4);
-      if (!pk) return DN_ERR_WORKSPACE;
-      if ((rc = tc_pack_layers(first, cnt, pk, pb, st))) return rc;
-    }
-  } else if (tc_front || tc_mlp) {
+  // one launch packs (hi/lo split + wgmma layout) every weight the tensor-core kernels will stream.  On the front chain
+  // the spectral multiplier S = exp(-lambda t) * (reduced partial sums), layer 0's weight, is formed there (no separate
+  // scale kernel, S never round-trips HBM), one per mesh of a batch.
+  if (tc_front || tc_mlp) {
     DnLayer* first = tc_front ? &L[0] : &L[nfront];
     const int cnt = (tc_front ? nfront : 0) + (tc_mlp ? nm : 0);
-    const int64_t pb = tc_chain_ws_bytes(first, cnt);
+    const TcSpectral sp = {partial, P, evals, p->diffusion_time, batch ? batch->n_meshes : 1,
+                           batch ? batch->mesh_cta_begin : nullptr, batch ? batch->tile_mesh : nullptr};
+    const int64_t pb = tc_chain_ws_bytes(first, cnt, tc_front ? sp.n_meshes : 1);
     float* pk = ws.take(pb / 4);
     if (!pk) return DN_ERR_WORKSPACE;
-    if (tc_front) rc = tc_pack_layers_spectral(first, cnt, pk, pb, partial, P, evals, p->diffusion_time, 1, st);
-    else rc = tc_pack_layers(first, cnt, pk, pb, st);
-    if (rc) return rc;
+    if ((rc = tc_pack_layers(first, cnt, pk, pb, tc_front ? &sp : nullptr, st))) return rc;
   }
   mark(3);
-  float *t0 = nullptr, *t1 = nullptr;
-  if (!tc_mlp && nm > 1) {
-    t0 = ws.take(V * maxn);
-    t1 = ws.take(V * maxn);
-    if (!t0 || !t1) return DN_ERR_WORKSPACE;
-  }
-  void* tcws = ws.base + ws.off;
-  const int64_t tcws_bytes = ws.size - ws.off;
-  // from_basis and [P|Q]: one fused two-layer chain when it fits, else one launch per layer
-  if (front_fused) {
-    if ((rc = run_chain(src_fb, &L[0], 2, V, engine, nullptr, nullptr, tcws, tcws_bytes, st))) return rc;
-  } else {
-    if ((rc = run_chain(src_fb, &L[0], 1, V, engine, nullptr, nullptr, tcws, tcws_bytes, st))) return rc;
-    for (int l = 1; l < nfront; ++l)
-      if ((rc = run_chain(src_pq, &L[l], 1, V, engine, nullptr, nullptr, tcws, tcws_bytes, st))) return rc;
-  }
+  const int n_fused = front_fused ? 2 : 1;
+  if ((rc = run_chain(src_fb, &L[0], n_fused, V, e, ws, st))) return rc;
+  for (int l = n_fused; l < nfront; ++l)
+    if ((rc = run_chain(src_pq, &L[l], 1, V, e, ws, st))) return rc;
   mark(4);
   // (a4+a5) sparse tangent gradient + complex inner product + tanh   [layers.py:216-226,128-130]
   if (p->with_gradient_features) {
     if ((rc = launch_spmm_features(grad, xd, pq, rot, V, C, feat, st))) return rc;
   }
   mark(5);
-  rc = run_chain(src_mlp, &L[nfront], nm, V, engine, t0, t1, tcws, tcws_bytes, st);
+  rc = run_chain(src_mlp, &L[nfront], nm, V, e, ws, st);
   mark(6);
   return rc;
 }

@@ -33,8 +33,8 @@ struct DnLayer {
   const float* W2;       // optional second block: !w_trans: output rows n >= n_split come from W2[n - n_split]
   int n_split;           //   (stacks [A_re; A_im] without a copy);  w_trans: input rows k >= n_split come from W2[k - n_split]
   const float* prepacked;  // optional: weights already in the tensor-core layout (tc_pack_layers)
-  int pack_fmt;            // layout of `prepacked`: 0 = 16-wide K stages of [tf32 hi | tf32 lo] (TF32 engines);
-                           //   2 = 16-wide K stages of bf16 (DN_ENGINE_BF16)
+  int pack_fmt;            // layout of `prepacked` (set by tc_chain_plan): 0 = 16-wide K stages of [tf32 hi | tf32 lo]
+                           //   (TF32 engines); 2 = 16-wide K stages of bf16 (DN_ENGINE_BF16)
   const float* bias;     // [N] or null
   int relu;
   const float* emul;     // optional elementwise multiplier [V][N] applied after the activation
@@ -87,8 +87,6 @@ int simt_atb_partial_st(const float* A, int64_t lda, int I, const float* B, int6
 int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int accumulate, cudaStream_t st);
 
 // ---- shared small kernels (dn_simt.cu) ----
-// SM count of the current device (cached per device; 1 if it cannot be queried): sizes grids and split-V partials
-int dn_sm_count();
 // S[k][c] = exp(-evals[k]*max(t[c],1e-8)) * sum_p partial[p][k][c]; optionally writes the raw sum
 // (x_spec) and the clamped time back.  s_trans: write S as [c][k].
 int launch_spectral_scale(const float* partial, int P, const float* evals, float* time, int K, int C,
@@ -121,15 +119,20 @@ int launch_spectral_bwd(const float* gs_partial, int P, const float* evals, cons
                         cudaStream_t st);
 
 // ---- wgmma engine (dn_tc.cu) ----
+// Per-device table, filled on first use of a device: whether it runs the tensor-core kernels (sm_90, with their
+// >48 KB dynamic shared memory attributes set on it) and its SM count (1 if it cannot be queried), which sizes grids
+// and split-V partials.
 bool tc_supported_device();
-// Fused chain of up to DN_MAX_LAYERS layers over 128-row tiles; layer 0 reads `src`.
-int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers, int n_layers, int64_t V, int passes /*3 or 1*/,
-                  void* ws, int64_t ws_bytes, cudaStream_t st);
+int dn_sm_count();
 // `passes`: 3 = 3xTF32-grade (fp32 parity), 1 = single-pass TF32, DN_PASSES_BF16 = single-pass bf16 (DN_ENGINE_BF16)
 #define DN_PASSES_BF16 16
-int tc_rows_chain_supported(const DnRowsSrc& src, const DnLayer* layers, int n_layers, int passes = 3);
-// packed-weight layout the kernel that will run this chain expects (sets layers[i].pack_fmt; call before tc_pack_layers)
-void tc_choose_pack_fmt(const DnRowsSrc& src, DnLayer* layers, int n_layers, int passes = 3);
+// Whether rows_chain_kernel takes this chain: the packed-weight format it runs it with (also stored in every
+// layers[i].pack_fmt), or DN_ERR_UNSUPPORTED.
+int tc_chain_plan(const DnRowsSrc& src, DnLayer* layers, int n_layers, int passes);
+// Fused chain of up to DN_MAX_LAYERS layers over 128-row tiles; layer 0 reads `src`.  The chain was planned
+// (tc_chain_plan) on a device that runs the tensor-core kernels; layers that are not prepacked are packed into ws.
+int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers, int n_layers, int64_t V, int passes, void* ws,
+                  int64_t ws_bytes, cudaStream_t st);
 // partial[p][k][c] for p < *P_out
 // `values` may be a column slice (row stride ld_values >= C) and a partial a slice of a wider one (row stride ldp):
 // C_width = 256 runs as two 128-column launches into the same [P][K][256] partials.  0 = contiguous (== C).
@@ -137,15 +140,21 @@ int tc_to_basis_partial(const float* values, const float* basis, const float* ma
                         float* partial, int* P_out, int passes, cudaStream_t st, int64_t ld_values = 0, int64_t ldp = 0,
                         const int32_t* cta_rows = nullptr, int n_ctas = 0);
 int tc_to_basis_supported(int K, int C);
-int64_t tc_chain_ws_bytes(const DnLayer* layers, int n_layers);
-// mesh batches: pack S_b = exp(-evals_b t) * (partials of mesh b) for every mesh as layer0's per-mesh weights
-// (ws: n_meshes * tc_chain_ws_bytes(layer0, 1) bytes); sets layer0->prepacked / tile_group / group_stride
-int tc_pack_spectral_batched(DnLayer* layer0, int n_meshes, void* ws, int64_t ws_bytes, const float* partial,
-                             const int32_t* mesh_cta_begin, const float* evals, float* time, int clamp_writeback,
-                             const int32_t* tile_mesh, cudaStream_t st);
-// one launch: pack the weights of n layers into ws and set layers[i].prepacked
-int tc_pack_layers(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, cudaStream_t st);
-// same, with layers[0] (w_trans, K = eigen count, N = channels) replaced by the spectral multiplier
-//   S[k][n] = exp(-evals[k] * max(time[n], 1e-8)) * sum_p partial[p][k][n]    (one launch for scale + pack)
-int tc_pack_layers_spectral(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, const float* partial, int P,
-                            const float* evals, float* time, int clamp_writeback, cudaStream_t st);
+// The spectral multiplier, packed in place of layers[0]'s weight (w_trans, K = eigen count, N = channels):
+//   S_b[k][n] = exp(-evals[b][k] * max(time[n], 1e-8)) * sum_{p in [p0_b, p1_b)} partial[p][k][n]
+// for every mesh b < n_meshes, with [p0_b, p1_b) = [mesh_cta_begin[b], mesh_cta_begin[b + 1]) for a mesh batch (row
+// tile t of layer 0 then streams matrix tile_mesh[t]) and [0, P) without one.  The clamped time is written back.
+struct TcSpectral {
+  const float* partial;
+  int P;
+  const float* evals;              // [n_meshes][K]
+  float* time;
+  int n_meshes;
+  const int32_t* mesh_cta_begin;   // device [n_meshes + 1], null without a batch
+  const int32_t* tile_mesh;        // device, null without a batch
+};
+// bytes tc_pack_layers needs (layer 0 n_meshes times)
+int64_t tc_chain_ws_bytes(const DnLayer* layers, int n_layers, int n_meshes = 1);
+// one launch: pack the weights of n layers (layer 0 the spectral multiplier when sp is given) into ws and set
+// layers[i].prepacked
+int tc_pack_layers(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, const TcSpectral* sp, cudaStream_t st);

@@ -15,7 +15,6 @@
 #include "dn_internal.h"
 #include "dn_tc_ptx.cuh"
 #include <cuda_bf16.h>
-#include <stdlib.h>
 #include <string.h>
 
 namespace {
@@ -51,15 +50,15 @@ struct PackJob {
   int64_t ldw;
   int n_split, w_trans, K, N, blk0, fmt;
 };
+constexpr int kMaxPackJobs = 3 + DN_MAX_LAYERS;   // every dense layer of a block: from_basis, [P|Q] (two at most), MLP
 struct PackJobs {
-  PackJob j[DN_MAX_LAYERS];
+  PackJob j[kMaxPackJobs];
   int n;
-  // optional: job 0's matrix is the spectral multiplier S[k][n] = exp(-evals[k] * max(t[n], 1e-8)) * sum_p partial[p][k][n]
-  // (layers.py:48-49, 62-64), formed here instead of by a separate launch; the clamped time is written back in place
-  const float* sp_partial;
-  const float* sp_evals;
-  float* sp_time;
-  int sp_P, sp_clamp;
+  // optional: job 0's matrix is the spectral multiplier of every mesh (TcSpectral; layers.py:48-49, 62-64), formed here
+  // instead of by a separate launch; sp_blocks blocks per mesh, sp_stride floats between the meshes' packed matrices
+  TcSpectral sp;
+  int sp_blocks;
+  int64_t sp_stride;
 };
 
 __device__ __forceinline__ void pack_store(float* dst, int fmt, int N, int k, int n, float w) {
@@ -81,72 +80,51 @@ __device__ __forceinline__ void pack_store(float* dst, int fmt, int N, int k, in
 
 // all weight matrices of a block forward in one launch (blocks are assigned to jobs by blk0)
 __global__ void pack_weights_kernel(const __grid_constant__ PackJobs jobs) {
-  int ji = 0;
-#pragma unroll
-  for (int i = 1; i < DN_MAX_LAYERS; ++i)
-    if (i < jobs.n && (int)blockIdx.x >= jobs.j[i].blk0) ji = i;
-  const PackJob& J = jobs.j[ji];
-  const int K = J.K, N = J.N;
   int n, k;
   float w;
-  if (ji == 0 && jobs.sp_partial) {
-    // spectral job: a block = 32 consecutive elements (n fastest: coalesced) x 8 slices of the P partial sums
+  if (jobs.sp.partial && (int)blockIdx.x < jobs.sp_blocks * jobs.sp.n_meshes) {
+    // spectral job (job 0, blocks [0, sp_blocks * n_meshes)): a block = 32 consecutive elements (n fastest: coalesced)
+    // of mesh b x 8 slices of its partial sums.  It is most of the launch, so it skips the job search below.
+    const PackJob& J = jobs.j[0];
+    const int K = J.K, N = J.N;
     __shared__ float red[8][33];
+    const int b = jobs.sp.n_meshes > 1 ? (int)blockIdx.x / jobs.sp_blocks : 0;
     const int e = threadIdx.x & 31, sl = threadIdx.x >> 5;
-    const int idx = ((int)blockIdx.x - J.blk0) * 32 + e;
+    const int idx = ((int)blockIdx.x - b * jobs.sp_blocks) * 32 + e;
+    const int p0 = jobs.sp.mesh_cta_begin ? jobs.sp.mesh_cta_begin[b] : 0;
+    const int p1 = jobs.sp.mesh_cta_begin ? jobs.sp.mesh_cta_begin[b + 1] : jobs.sp.P;
     float acc = 0.f;
     if (idx < K * N) {
-      const float* pp = jobs.sp_partial + idx;
+      const float* pp = jobs.sp.partial + idx;
       const int64_t stride = (int64_t)K * N;
-      for (int q = sl; q < jobs.sp_P; q += 8) acc += pp[(int64_t)q * stride];
+      for (int q = p0 + sl; q < p1; q += 8) acc += pp[(int64_t)q * stride];
     }
     red[sl][e] = acc;
     __syncthreads();
     if (sl != 0 || idx >= K * N) return;
     k = idx / N; n = idx % N;
     const float sum = ((red[0][e] + red[1][e]) + (red[2][e] + red[3][e])) + ((red[4][e] + red[5][e]) + (red[6][e] + red[7][e]));
-    const float t = fmaxf(jobs.sp_time[n], 1e-8f);         // torch.clamp(t, min=1e-8)
-    w = expf(-(jobs.sp_evals[k] * t)) * sum;
-    if (jobs.sp_clamp && k == K - 1) jobs.sp_time[n] = t;   // (idempotent for the other readers of t[n])
-  } else {
-    const int idx = ((int)blockIdx.x - J.blk0) * blockDim.x + threadIdx.x;
-    if (idx >= K * N) return;
-    n = idx / K; k = idx % K;
-    if (J.w_trans) w = (J.W2 && k >= J.n_split) ? J.W2[(int64_t)(k - J.n_split) * J.ldw + n] : J.W[(int64_t)k * J.ldw + n];
-    else if (J.W2 && n >= J.n_split) w = J.W2[(int64_t)(n - J.n_split) * J.ldw + k];
-    else w = J.W[(int64_t)n * J.ldw + k];
+    const float t = fmaxf(jobs.sp.time[n], 1e-8f);         // torch.clamp(t, min=1e-8)
+    w = expf(-(jobs.sp.evals[(int64_t)b * K + k] * t)) * sum;
+    pack_store(J.dst + b * jobs.sp_stride, J.fmt, N, k, n, w);
+    // the in-place clamp of the reference, written back by mesh 0 only: every other reader of t[n] in this launch reads
+    // either value (max(t, 1e-8) is idempotent)
+    if (b == 0 && k == K - 1) jobs.sp.time[n] = t;
+    return;
   }
+  int ji = 0;
+#pragma unroll
+  for (int i = 1; i < kMaxPackJobs; ++i)
+    if (i < jobs.n && (int)blockIdx.x >= jobs.j[i].blk0) ji = i;
+  const PackJob& J = jobs.j[ji];
+  const int K = J.K, N = J.N;
+  const int idx = ((int)blockIdx.x - J.blk0) * blockDim.x + threadIdx.x;
+  if (idx >= K * N) return;
+  n = idx / K; k = idx % K;
+  if (J.w_trans) w = (J.W2 && k >= J.n_split) ? J.W2[(int64_t)(k - J.n_split) * J.ldw + n] : J.W[(int64_t)k * J.ldw + n];
+  else if (J.W2 && n >= J.n_split) w = J.W2[(int64_t)(n - J.n_split) * J.ldw + k];
+  else w = J.W[(int64_t)n * J.ldw + k];
   pack_store(J.dst, J.fmt, N, k, n, w);
-}
-
-// mesh batches: the spectral multiplier of every mesh, packed as layer-0 weights of the from_basis chain
-//   S_b[k][n] = exp(-evals[b][k] * max(t[n], 1e-8)) * sum_{p in CTAs of mesh b} partial[p][k][n]     (layers.py:48-49, 62-64)
-// grid (ceil(K*N/32), n_meshes), 256 threads: 32 consecutive elements x 8 slices of the partial sums per block
-__global__ void spectral_pack_batched_kernel(const float* __restrict__ partial, const int32_t* __restrict__ mesh_cta_begin,
-                                             const float* __restrict__ evals, float* time, int K, int N, int fmt,
-                                             float* dst, int64_t dst_stride_floats, int clamp) {
-  __shared__ float red[8][33];
-  const int b = blockIdx.y;
-  const int e = threadIdx.x & 31, sl = threadIdx.x >> 5;
-  const int idx = (int)blockIdx.x * 32 + e;
-  const int p0 = mesh_cta_begin[b], p1 = mesh_cta_begin[b + 1];
-  float acc = 0.f;
-  if (idx < K * N) {
-    const float* pp = partial + idx;
-    const int64_t stride = (int64_t)K * N;
-    for (int q = p0 + sl; q < p1; q += 8) acc += pp[(int64_t)q * stride];
-  }
-  red[sl][e] = acc;
-  __syncthreads();
-  if (sl != 0 || idx >= K * N) return;
-  const int k = idx / N, n = idx % N;
-  const float sum = ((red[0][e] + red[1][e]) + (red[2][e] + red[3][e])) + ((red[4][e] + red[5][e]) + (red[6][e] + red[7][e]));
-  const float t = fmaxf(time[n], 1e-8f);
-  const float w = expf(-(evals[(int64_t)b * K + k] * t)) * sum;
-  pack_store(dst + (int64_t)b * dst_stride_floats, fmt, N, k, n, w);
-  // the in-place clamp of the reference: written back by mesh 0 only, after every reader of t[n] in this launch has at
-  // worst read either value (max(t, 1e-8) is idempotent)
-  if (clamp && b == 0 && k == K - 1) time[n] = t;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -671,10 +649,11 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
   }
 }
 
-// Per-device state: capability, SM count, and whether the >48 KB dynamic shared memory attributes were set on that
-// device (function attributes are per device: a process that drives several GPUs needs them on each one).
+// Per-device table: SM count and capability, read on the first use of the device, and whether the >48 KB dynamic
+// shared memory attributes were set on it, tried on the first use of the tensor-core engine there (function attributes
+// are per device: a process that drives several GPUs needs them on each one).
 constexpr int kMaxDev = 64;
-struct DevState { int tried, ok, sms; };
+struct DevState { int queried, sms, sm90, tc_tried, tc; };
 DevState g_dev[kMaxDev];
 
 template <typename F>
@@ -709,33 +688,36 @@ static DevState* cur_dev_state() {
     return nullptr;
   }
   DevState& d = g_dev[dev];
-  if (!d.tried) {
-    d.tried = 1;
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) {
+  if (!d.queried) {
+    d.queried = 1;
+    int major = 0, minor = 0;
+    if (cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) {
       cudaGetLastError();
-      d.ok = 0;
-    } else {
-      d.ok = (prop.major == 9 && prop.minor == 0) ? 1 : 0;
-      d.sms = prop.multiProcessorCount;
-      if (d.ok) {
-        const bool set = set_chain_smem<MODE_TF32X3>() && set_chain_smem<MODE_TF32>() && set_chain_smem<MODE_BF16>() &&
-                         set_to_basis_smem<MODE_TF32X3>() && set_to_basis_smem<MODE_TF32>();
-        if (!set) {
-          cudaGetLastError();
-          d.ok = 0;
-        }
-      }
+      major = 0;
     }
-    const char* off = getenv("DN_TC_DISABLE");
-    if (off && atoi(off)) d.ok = 0;
+    if (d.sms < 1) d.sms = 1;
+    d.sm90 = major == 9 && minor == 0;
   }
   return &d;
 }
 
+int dn_sm_count() {
+  const DevState* d = cur_dev_state();
+  return d ? d->sms : 1;
+}
+
 bool tc_supported_device() {
   DevState* d = cur_dev_state();
-  return d && d->ok == 1;
+  if (!d || !d->sm90) return false;
+  if (!d->tc_tried) {
+    d->tc_tried = 1;
+    d->tc = set_chain_smem<MODE_TF32X3>() && set_chain_smem<MODE_TF32>() && set_chain_smem<MODE_BF16>() &&
+            set_to_basis_smem<MODE_TF32X3>() && set_to_basis_smem<MODE_TF32>();
+    if (!d->tc) cudaGetLastError();
+  }
+  return d->tc;
 }
 
 static bool aligned8(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 7) == 0; }
@@ -766,33 +748,26 @@ static int chain_supported(const DnRowsSrc& src, const DnLayer* layers, int n_la
   return DN_OK;
 }
 
-int tc_rows_chain_supported(const DnRowsSrc& src, const DnLayer* layers, int n_layers, int passes) {
-  if (passes == DN_PASSES_BF16 && chain_supported(src, layers, n_layers, true) == DN_OK) return DN_OK;
-  return chain_supported(src, layers, n_layers, false);
-}
-
-void tc_choose_pack_fmt(const DnRowsSrc& src, DnLayer* layers, int n_layers, int passes) {
-  const int fmt = (passes == DN_PASSES_BF16 && chain_supported(src, layers, n_layers, true) == DN_OK) ? 2 : 0;
+int tc_chain_plan(const DnRowsSrc& src, DnLayer* layers, int n_layers, int passes) {
+  int fmt;
+  if (passes == DN_PASSES_BF16 && chain_supported(src, layers, n_layers, true) == DN_OK) fmt = 2;
+  else if (chain_supported(src, layers, n_layers, false) == DN_OK) fmt = 0;
+  else return DN_ERR_UNSUPPORTED;
   for (int l = 0; l < n_layers; ++l) layers[l].pack_fmt = fmt;
+  return fmt;
 }
 
-int64_t tc_chain_ws_bytes(const DnLayer* layers, int n_layers) {
-  int64_t b = 0;
+int64_t tc_chain_ws_bytes(const DnLayer* layers, int n_layers, int n_meshes) {
+  int64_t b = (n_meshes - 1) * packed_bytes(layers[0].K, layers[0].N);
   for (int l = 0; l < n_layers; ++l) b += packed_bytes(layers[l].K, layers[l].N);
   return b;
 }
 
-int tc_pack_layers(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, cudaStream_t st) {
-  return tc_pack_layers_spectral(layers, n_layers, ws, ws_bytes, nullptr, 0, nullptr, nullptr, 0, st);
-}
-
-int tc_pack_layers_spectral(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, const float* partial, int P,
-                            const float* evals, float* time, int clamp_writeback, cudaStream_t st) {
-  if (n_layers < 1 || n_layers > DN_MAX_LAYERS) return DN_ERR_INVALID_ARGUMENT;
-  if (tc_chain_ws_bytes(layers, n_layers) > ws_bytes || !ws) return DN_ERR_WORKSPACE;
+int tc_pack_layers(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, const TcSpectral* sp, cudaStream_t st) {
+  if (n_layers < 1 || n_layers > kMaxPackJobs || (sp && sp->n_meshes < 1)) return DN_ERR_INVALID_ARGUMENT;
+  if (tc_chain_ws_bytes(layers, n_layers, sp ? sp->n_meshes : 1) > ws_bytes || !ws) return DN_ERR_WORKSPACE;
   PackJobs jobs;
   memset(&jobs, 0, sizeof(jobs));
-  jobs.sp_partial = partial; jobs.sp_P = P; jobs.sp_evals = evals; jobs.sp_time = time; jobs.sp_clamp = clamp_writeback;
   jobs.n = n_layers;
   char* wp = static_cast<char*>(ws);
   int blocks = 0;
@@ -803,30 +778,21 @@ int tc_pack_layers_spectral(DnLayer* layers, int n_layers, void* ws, int64_t ws_
     J.fmt = L.pack_fmt;
     J.dst = reinterpret_cast<float*>(wp);
     J.blk0 = blocks;
-    blocks += (l == 0 && partial) ? (L.K * L.N + 31) / 32 : (L.K * L.N + 255) / 256;
     L.prepacked = J.dst;
-    wp += packed_bytes(L.K, L.N);
+    if (l == 0 && sp) {
+      jobs.sp = *sp;
+      jobs.sp_blocks = (L.K * L.N + 31) / 32;
+      jobs.sp_stride = packed_bytes(L.K, L.N) / 4;
+      blocks += jobs.sp_blocks * sp->n_meshes;
+      wp += packed_bytes(L.K, L.N) * sp->n_meshes;
+      if (sp->tile_mesh) { L.tile_group = sp->tile_mesh; L.group_stride = jobs.sp_stride; }
+    } else {
+      blocks += (L.K * L.N + 255) / 256;
+      wp += packed_bytes(L.K, L.N);
+    }
   }
   pack_weights_kernel<<<blocks, 256, 0, st>>>(jobs);
   DN_LAUNCH_CHECK();
-  return DN_OK;
-}
-
-int tc_pack_spectral_batched(DnLayer* layer0, int n_meshes, void* ws, int64_t ws_bytes, const float* partial,
-                             const int32_t* mesh_cta_begin, const float* evals, float* time, int clamp_writeback,
-                             const int32_t* tile_mesh, cudaStream_t st) {
-  if (!layer0 || n_meshes < 1 || !ws || !partial || !mesh_cta_begin || !evals || !time || !tile_mesh)
-    return DN_ERR_INVALID_ARGUMENT;
-  const int64_t per = tc_chain_ws_bytes(layer0, 1);
-  if (per * n_meshes > ws_bytes) return DN_ERR_WORKSPACE;
-  const int K = layer0->K, N = layer0->N;
-  dim3 grid((unsigned)((K * N + 31) / 32), (unsigned)n_meshes);
-  spectral_pack_batched_kernel<<<grid, 256, 0, st>>>(partial, mesh_cta_begin, evals, time, K, N, layer0->pack_fmt,
-                                                     static_cast<float*>(ws), per / 4, clamp_writeback);
-  DN_LAUNCH_CHECK();
-  layer0->prepacked = static_cast<float*>(ws);
-  layer0->tile_group = tile_mesh;
-  layer0->group_stride = per / 4;
   return DN_OK;
 }
 
@@ -845,8 +811,6 @@ static void launch_chain(const HcParams& p, int nmax, bool wide, int grid, cudaS
 int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, int64_t V, int passes, void* ws,
                   int64_t ws_bytes, cudaStream_t st) {
   if (V <= 0) return DN_OK;
-  DevState* dv = cur_dev_state();
-  if (!dv || dv->ok != 1) return DN_ERR_NOT_SM100;
   if (n_layers < 1 || n_layers > DN_MAX_LAYERS) return DN_ERR_INVALID_ARGUMENT;
   DnLayer layers[DN_MAX_LAYERS];
   bool packed = true;
@@ -855,16 +819,12 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
     packed = packed && layers[l].prepacked != nullptr;
   }
   if (!packed) {
-    tc_choose_pack_fmt(src, layers, n_layers, passes);
-    int rc = tc_pack_layers(layers, n_layers, ws, ws_bytes, st);
+    int rc = tc_pack_layers(layers, n_layers, ws, ws_bytes, nullptr, st);
     if (rc) return rc;
   }
   // bf16 engine: bf16 MMAs when the shapes fit them (weights packed as bf16), single-pass TF32 otherwise
   const bool bf16 = passes == DN_PASSES_BF16 && layers[0].pack_fmt == 2;
   if (passes == DN_PASSES_BF16 && !bf16) passes = 1;
-  if (chain_supported(src, layers, n_layers, bf16) != DN_OK) return DN_ERR_UNSUPPORTED;
-  for (int l = 0; l < n_layers; ++l)
-    if (layers[l].pack_fmt != (bf16 ? 2 : 0)) return DN_ERR_INVALID_ARGUMENT;
   if (V >= (1ll << 31) - 256) return DN_ERR_UNSUPPORTED;
   HcParams p;
   memset(&p, 0, sizeof(p));
@@ -887,7 +847,8 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
   const DnLayer& Ll = layers[n_layers - 1];
   p.head_w = Ll.head_w; p.head_b = Ll.head_b; p.head_out = Ll.head_out; p.ld_head_out = Ll.ld_head_out; p.head_n = Ll.head_n;
   const int64_t ntiles = (V + TILE_M - 1) / TILE_M;
-  const int grid = (int)(ntiles < dv->sms ? ntiles : dv->sms);
+  const int sms = dn_sm_count();
+  const int grid = (int)(ntiles < sms ? ntiles : sms);
   if (bf16) launch_chain<MODE_BF16>(p, nmax, wide, grid, st);
   else if (passes == 3) launch_chain<MODE_TF32X3>(p, nmax, wide, grid, st);
   else launch_chain<MODE_TF32>(p, nmax, wide, grid, st);
@@ -904,8 +865,6 @@ int tc_to_basis_supported(int K, int C) {
 int tc_to_basis_partial(const float* values, const float* basis, const float* massvec, int64_t V, int K, int C,
                         float* partial, int* P_out, int passes, cudaStream_t st, int64_t ld_values, int64_t ldp,
                         const int32_t* cta_rows, int n_ctas) {
-  DevState* dv = cur_dev_state();
-  if (!dv || dv->ok != 1) return DN_ERR_NOT_SM100;
   if (tc_to_basis_supported(K, C) != DN_OK) return DN_ERR_UNSUPPORTED;
   if (ld_values <= 0) ld_values = C;
   if (ldp <= 0) ldp = C;
@@ -922,7 +881,7 @@ int tc_to_basis_partial(const float* values, const float* basis, const float* ma
     grid = n_ctas;
   } else {
     const int64_t total_chunks = (V + KC - 1) / KC;
-    grid = dv->sms;
+    grid = dn_sm_count();
     if (total_chunks < grid) grid = (int)(total_chunks > 0 ? total_chunks : 1);
     p.chunks_per_cta = (total_chunks + grid - 1) / grid;
     if (p.chunks_per_cta < 1) p.chunks_per_cta = 1;

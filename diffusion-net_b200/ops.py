@@ -187,7 +187,7 @@ class GradOperators:
         rows in shared memory once.  Worth its one-off cost (a D2H of the pattern, the clustering, an H2D) only for
         operators that stay resident, so ``prepare_operators`` calls it on the SECOND use of the same tensors.
         Default 32 rows / 72 distinct source rows per patch: 72 x (C + 2C) floats = 108 KiB of shared memory at
-        C = 128, two CTAs per SM (measured best of the shapes tried, tools/ab_patch.py)."""
+        C = 128, two CTAs per SM (measured best of the shapes tried)."""
         if getattr(self, "_patches", None) is not None or self.nnz == 0:
             return self
         import numpy as np
@@ -260,7 +260,7 @@ _prep_cache = {}
 # dn_patches policy on the SECOND use of an operator pair (= the operators are resident): "auto" (default) builds the
 # structure only for poorly ordered meshes, "1" always, "0" never: the staged gather costs about the same whatever the
 # vertex order, while the plain gather is fast on a mesh whose order has locality (L1 hits) and slow on a randomly
-# permuted one.
+# permuted one.  The library runs the patched gather whenever a dn_csr carries patches, so this is the only switch.
 auto_patch = os.environ.get("DN_SPMM_PATCH", "auto")
 PATCH_LOCALITY_THRESHOLD = 0.25
 

@@ -437,6 +437,33 @@ def test_forward_batch_equals_per_mesh(dn, engine, C):
         dn.set_engine("tc3x")
 
 
+def test_block_with_seven_mlp_layers(dn):
+    """The deepest MiniMLP a block takes besides 8 layers (mlp_hidden_dims of length 6): with from_basis and [P|Q] its
+    weights are 9 matrices, packed in one launch.  Inference on one mesh and on a two-mesh batch vs the fp64 oracle."""
+    dn.set_engine("tc3x")
+    C, K = 64, 64
+    torch.manual_seed(0)
+    blk = dn.DiffusionNetBlock(C_width=C, mlp_hidden_dims=[C] * 6, dropout=False)
+    with torch.no_grad():
+        blk.diffusion.diffusion_time.uniform_(1e-3, 0.3)
+    blk = blk.cuda().eval()
+    params = {k: v.detach().cpu() for k, v in blk.state_dict().items()}
+    cases = [_structural_case(dn, n, m, K, C, seed=i) for i, (n, m) in enumerate([(20, 30), (13, 17)])]
+    golds = [_oracle_block(ops_t, params, x) for ops_t, _, x in cases]
+    with torch.no_grad():
+        ops_t, _, x = cases[0]
+        mass, L, evals, evecs, gradX, gradY = ops_t
+        out = blk(x.unsqueeze(0), mass.unsqueeze(0), None, evals.unsqueeze(0), evecs.unsqueeze(0), [gradX], [gradY])
+        assert O.rel_err(out[0].cpu().numpy(), golds[0]) < TOL["tc3x"]
+        mb = dn.MeshBatch([dict(mass=o[0], evals=o[2], evecs=o[3], gradX=o[4], gradY=o[5]) for o, _, _ in cases])
+        A_re, A_im = blk.gradient_features.weights()
+        lins = blk.mlp.linears()
+        y = dn.batch.block_forward_batched_raw(mb, mb.pack([x for _, _, x in cases]), blk.diffusion.diffusion_time, A_re,
+                                               A_im, [l.weight for l in lins], [l.bias for l in lins], True)
+    for o, gold in zip(mb.unpack(y), golds):
+        assert O.rel_err(o.cpu().numpy(), gold) < TOL["tc3x"]
+
+
 def test_build_grad_on_device_vs_reference(dn):
     """SURVEY 8f-4: dn_build_grad (edge_tangent_vectors + build_grad, geometry.py:198-273) against the gradX / gradY the
     live reference produced (tests/golden/geom_small.npz) and against the oracle restatement on a larger mesh."""

@@ -108,6 +108,10 @@ SIGNATURES = {
                              C.POINTER(dn_head), _L, _I, _I, _P, _P, _L, _I, _P]),
     "dn_block_fwd_batched": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),
                                   _L, _I, _I, _P, _P, _L, _I, _P]),
+    "dn_learned_time_diffusion_fwd_batched": (_I, [_P, _P, _P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P, _P,
+                                                   _L, _I, _P]),
+    "dn_learned_time_diffusion_bwd_batched": (_I, [_P, _P, _P, _P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P,
+                                                   _P, _L, _I, _P]),
 }
 
 _lib = None

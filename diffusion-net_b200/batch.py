@@ -19,7 +19,8 @@ from . import _lib, ops
 
 class MeshBatch:
     """``items``: dicts with mass (V), evals (K), evecs (V,K), gradX, gradY (sparse COO (V,V) or a prepared
-    ``ops.GradOperators`` under 'gradX') -- the reference's operator tuple per mesh.  Build once, reuse every step."""
+    ``ops.GradOperators`` under 'gradX') -- the reference's operator tuple per mesh -- and optionally faces (F,3) /
+    edges (E,2) for ``DiffusionNet.forward_batch`` with outputs_at 'faces' / 'edges'.  Build once, reuse every step."""
 
     def __init__(self, items, device=None):
         lib = _lib.load()
@@ -85,9 +86,21 @@ class MeshBatch:
         self._cta_begin = torch.from_numpy(cta_begin).to(dev)
         self.desc = _lib.dn_mesh_batch(B, n_ctas, self._tile_mesh.data_ptr(), self._tb_rows.data_ptr(),
                                        self._cta_begin.data_ptr())
+        # elements for outputs_at 'faces' / 'edges', vertex ids offset to batch rows (None unless every item has them)
+        self.faces, self.edges, self._elem_counts = None, None, {}
+        for name in ("faces", "edges"):
+            if all(it.get(name) is not None for it in items):
+                els = [torch.as_tensor(it[name]).to(device=dev, dtype=torch.int64) for it in items]
+                setattr(self, name, torch.cat([e + r0 for e, r0 in zip(els, self.row_begin)], 0))
+                self._elem_counts[name] = [int(e.shape[0]) for e in els]
+
+    def elem_counts(self, name):
+        """Number of 'faces' or 'edges' of every mesh (the split of the batch's element outputs)."""
+        return self._elem_counts[name]
 
     def pack(self, xs):
-        """List of per-mesh (V_b, C) features -> one (V, C) tensor in the batch layout (padding rows zero)."""
+        """List of per-mesh (V_b, C) features -> one (V, C) tensor in the batch layout (padding rows zero).
+        Differentiable: gradients reach every x_b."""
         Cc = xs[0].shape[-1]
         out = torch.zeros(self.V, Cc, dtype=torch.float32, device=self.device)
         for b, x in enumerate(xs):

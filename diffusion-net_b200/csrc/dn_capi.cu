@@ -167,6 +167,41 @@ int atb(const float* A, int64_t lda, int I, const float* B, int64_t ldb, int J, 
   return simt_atb(A, lda, I, B, ldb, J, nullptr, V, out, ld_out, accumulate, part, part_floats, st);
 }
 
+// Plan and scratch of a spectral diffusion over a mesh batch (dn_learned_time_diffusion_{fwd,bwd}_batched): grouped
+// to_basis partials -> one pack launch forming every mesh's multiplier -> the from_basis chain picking its matrix per
+// tile.  The envelope is dn_block_fwd_batched's (tensor-core engine, V a multiple of 128, a planned batch, a from_basis
+// layer the fused chain takes); everything is checked and carved before any work is enqueued.
+struct BatchedSpectral {
+  Engine e;
+  DnRowsSrc src;       // evecs
+  DnLayer L;           // from_basis, packed once per mesh by tc_pack_layers
+  float* partial;      // [n_tb_ctas][K][C]
+  int64_t pf;
+  float* packed;
+  int64_t packed_bytes;
+  float* sums;         // [n_meshes][K][C]
+};
+
+int batched_spectral_plan(const dn_mesh_batch* batch, const float* evecs, int64_t V, int K, int C, int engine,
+                          float* out, Bump& ws, BatchedSpectral* b) {
+  int rc = resolve(engine, &b->e);
+  if (rc) return rc;
+  if (!b->e.tc || (V % 128) || batch->n_meshes < 1 || !batch->tile_mesh || !batch->tb_rows || !batch->mesh_cta_begin ||
+      batch->n_tb_ctas < 1)
+    return DN_ERR_UNSUPPORTED;
+  const bool tb = tc_to_basis_supported(K, C) == DN_OK ||
+                  (C > 128 && C % 128 == 0 && tc_to_basis_supported(K, 128) == DN_OK);
+  b->src = one_src(evecs, K, K);
+  b->L = make_layer(nullptr, C, 1, nullptr, 0, K, C, out, C);
+  if (!tb || tc_chain_plan(b->src, &b->L, 1, b->e.passes) < 0) return DN_ERR_UNSUPPORTED;
+  b->pf = (int64_t)batch->n_tb_ctas * K * C;
+  b->packed_bytes = tc_chain_ws_bytes(&b->L, 1, batch->n_meshes);
+  b->partial = ws.take(b->pf);
+  b->packed = ws.take(b->packed_bytes / 4);
+  b->sums = ws.take((int64_t)batch->n_meshes * K * C);
+  return (b->partial && b->packed && b->sums) ? DN_OK : DN_ERR_WORKSPACE;
+}
+
 }  // namespace
 
 long long g_dn_launches = 0;
@@ -398,6 +433,50 @@ int dn_learned_time_diffusion_bwd(const float* grad_out, const float* mass, cons
   DnLayer L = make_layer(dS, C, 1, nullptr, 0, K, C, grad_x, C);
   L.row_scale = mass;
   return run_chain(src, &L, 1, V, e, ws, st);
+}
+
+int dn_learned_time_diffusion_fwd_batched(const float* x, const float* mass, const float* evals, const float* evecs,
+                                          float* time, const dn_mesh_batch* batch, int64_t V, int K, int C,
+                                          float* x_diffuse, float* x_spec_out, void* workspace, int64_t ws_bytes,
+                                          int engine, dn_stream_t stream) {
+  if (!x || !mass || !evals || !evecs || !time || !batch || !x_diffuse || V < 0 || K <= 0 || C <= 0)
+    return DN_ERR_INVALID_ARGUMENT;
+  Bump ws(workspace, ws_bytes);
+  BatchedSpectral b;
+  int rc = batched_spectral_plan(batch, evecs, V, K, C, engine, x_diffuse, ws, &b);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  int P = 0;
+  if ((rc = to_basis_partials(x, evecs, mass, V, K, C, b.partial, b.pf, &P, b.e, st, batch))) return rc;
+  // S_b = exp(-lambda_b t) * (Phi_b^T M_b x_b), packed per mesh; the unscaled sums go to x_spec_out, the clamp to time
+  const TcSpectral sp = {b.partial, P, evals, time, batch->n_meshes, batch->mesh_cta_begin, batch->tile_mesh,
+                         x_spec_out, /*no_clamp_writeback=*/0};
+  if ((rc = tc_pack_layers(&b.L, 1, b.packed, b.packed_bytes, &sp, st))) return rc;
+  return run_chain(b.src, &b.L, 1, V, b.e, ws, st);
+}
+
+int dn_learned_time_diffusion_bwd_batched(const float* grad_out, const float* mass, const float* evals,
+                                          const float* evecs, const float* time, const float* x_spec,
+                                          const dn_mesh_batch* batch, int64_t V, int K, int C, float* grad_x,
+                                          float* grad_time, void* workspace, int64_t ws_bytes, int engine,
+                                          dn_stream_t stream) {
+  if (!grad_out || !mass || !evals || !evecs || !time || !x_spec || !batch || !grad_x || !grad_time || V < 0 ||
+      K <= 0 || C <= 0)
+    return DN_ERR_INVALID_ARGUMENT;
+  Bump ws(workspace, ws_bytes);
+  BatchedSpectral b;
+  int rc = batched_spectral_plan(batch, evecs, V, K, C, engine, grad_x, ws, &b);
+  if (rc) return rc;
+  b.L.row_scale = mass;
+  cudaStream_t st = (cudaStream_t)stream;
+  int P = 0;
+  if ((rc = to_basis_partials(grad_out, evecs, nullptr, V, K, C, b.partial, b.pf, &P, b.e, st, batch))) return rc;
+  // G_b = Phi_b^T g_b to b.sums and dS_b = exp(-lambda_b t) * G_b packed per mesh; time is only read
+  const TcSpectral sp = {b.partial, P, evals, const_cast<float*>(time), batch->n_meshes, batch->mesh_cta_begin,
+                         batch->tile_mesh, b.sums, /*no_clamp_writeback=*/1};
+  if ((rc = tc_pack_layers(&b.L, 1, b.packed, b.packed_bytes, &sp, st))) return rc;
+  if ((rc = run_chain(b.src, &b.L, 1, V, b.e, ws, st))) return rc;                // grad_x = M Phi_b dS_b
+  return launch_spectral_time_grad_batched(b.sums, x_spec, evals, time, batch->n_meshes, K, C, grad_time, st);
 }
 
 int dn_grad_spmm(const dn_csr* grad, const float* x, int64_t V, int C, float* out, dn_stream_t stream) {

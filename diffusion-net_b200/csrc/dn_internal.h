@@ -117,6 +117,10 @@ int launch_complex_dots_tanh(const float* g01, const float* b01, int64_t V, int 
 int launch_spectral_bwd(const float* gs_partial, int P, const float* evals, const float* time,
                         const float* x_spec, int K, int C, float* dS /*K x C*/, float* grad_time /*+=*/,
                         cudaStream_t st);
+// Time gradient of a mesh batch: grad_time[c] += sum_b sum_k G[b][k][c] * (-evals[b][k]) * E * x_spec[b][k][c] with
+// E = exp(-evals[b][k] * max(time[c], 1e-8)).  Fixed summation order, no atomics: deterministic.
+int launch_spectral_time_grad_batched(const float* G, const float* x_spec, const float* evals, const float* time,
+                                      int n_meshes, int K, int C, float* grad_time, cudaStream_t st);
 
 // ---- wgmma engine (dn_tc.cu) ----
 // Per-device table, filled on first use of a device: whether it runs the tensor-core kernels (sm_90, with their
@@ -143,7 +147,8 @@ int tc_to_basis_supported(int K, int C);
 // The spectral multiplier, packed in place of layers[0]'s weight (w_trans, K = eigen count, N = channels):
 //   S_b[k][n] = exp(-evals[b][k] * max(time[n], 1e-8)) * sum_{p in [p0_b, p1_b)} partial[p][k][n]
 // for every mesh b < n_meshes, with [p0_b, p1_b) = [mesh_cta_begin[b], mesh_cta_begin[b + 1]) for a mesh batch (row
-// tile t of layer 0 then streams matrix tile_mesh[t]) and [0, P) without one.  The clamped time is written back.
+// tile t of layer 0 then streams matrix tile_mesh[t]) and [0, P) without one.  The clamped time is written back unless
+// no_clamp_writeback is set (the backward pass reads a saved copy of the clamped time).
 struct TcSpectral {
   const float* partial;
   int P;
@@ -152,6 +157,8 @@ struct TcSpectral {
   int n_meshes;
   const int32_t* mesh_cta_begin;   // device [n_meshes + 1], null without a batch
   const int32_t* tile_mesh;        // device, null without a batch
+  float* sum_out;                  // optional [n_meshes][K][N]: the reduced partial sums before the exp(-lambda t) scale
+  int no_clamp_writeback;
 };
 // bytes tc_pack_layers needs (layer 0 n_meshes times)
 int64_t tc_chain_ws_bytes(const DnLayer* layers, int n_layers, int n_meshes = 1);

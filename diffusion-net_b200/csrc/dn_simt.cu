@@ -312,6 +312,32 @@ __global__ void spectral_bwd_kernel(const float* __restrict__ partial, int P, co
   grad_time[c] += dt;
 }
 
+// the same time gradient over a mesh batch: G, x_spec [n_meshes][K][C], evals [n_meshes][K].  Block (32, 16): 32
+// consecutive channels (coalesced) x 16 slices of the n_meshes * K eigenpairs, combined in a fixed order.
+__global__ void spectral_time_grad_batched_kernel(const float* __restrict__ G, const float* __restrict__ x_spec,
+                                                  const float* __restrict__ evals, const float* __restrict__ time,
+                                                  int rows, int C, float* __restrict__ grad_time) {
+  __shared__ float red[16][33];
+  const int c = blockIdx.x * 32 + threadIdx.x;
+  float dt = 0.f;
+  if (c < C) {
+    const float t = fmaxf(time[c], 1e-8f);
+    for (int r = threadIdx.y; r < rows; r += 16) {   // r = b * K + k
+      const int64_t idx = (int64_t)r * C + c;
+      const float lam = evals[r];
+      const float e = expf(-(lam * t));
+      dt += G[idx] * (-lam) * e * x_spec[idx];
+    }
+  }
+  red[threadIdx.y][threadIdx.x] = dt;
+  __syncthreads();
+  if (threadIdx.y != 0 || c >= C) return;
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) s += red[i][threadIdx.x];
+  grad_time[c] += s;
+}
+
 // ---------------------------------------------------------------------------------------------
 // sparse kernels
 // ---------------------------------------------------------------------------------------------
@@ -849,6 +875,14 @@ int launch_reduce_partials_ld(const float* partial, int P, int rows, int cols, f
 int launch_spectral_bwd(const float* gs_partial, int P, const float* evals, const float* time, const float* x_spec,
                         int K, int C, float* dS, float* grad_time, cudaStream_t st) {
   spectral_bwd_kernel<<<(C + 63) / 64, 64, 0, st>>>(gs_partial, P, evals, time, x_spec, K, C, dS, grad_time);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
+int launch_spectral_time_grad_batched(const float* G, const float* x_spec, const float* evals, const float* time,
+                                      int n_meshes, int K, int C, float* grad_time, cudaStream_t st) {
+  spectral_time_grad_batched_kernel<<<(C + 31) / 32, dim3(32, 16), 0, st>>>(G, x_spec, evals, time, n_meshes * K, C,
+                                                                           grad_time);
   DN_LAUNCH_CHECK();
   return DN_OK;
 }

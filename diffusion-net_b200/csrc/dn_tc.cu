@@ -107,9 +107,10 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackJobs jobs) {
     const float t = fmaxf(jobs.sp.time[n], 1e-8f);         // torch.clamp(t, min=1e-8)
     w = expf(-(jobs.sp.evals[(int64_t)b * K + k] * t)) * sum;
     pack_store(J.dst + b * jobs.sp_stride, J.fmt, N, k, n, w);
+    if (jobs.sp.sum_out) jobs.sp.sum_out[(int64_t)b * K * N + idx] = sum;
     // the in-place clamp of the reference, written back by mesh 0 only: every other reader of t[n] in this launch reads
     // either value (max(t, 1e-8) is idempotent)
-    if (b == 0 && k == K - 1) jobs.sp.time[n] = t;
+    if (b == 0 && k == K - 1 && !jobs.sp.no_clamp_writeback) jobs.sp.time[n] = t;
     return;
   }
   int ji = 0;

@@ -168,6 +168,17 @@ class DiffusionNetBlock(nn.Module):
             srcs.append(ops.GradFeaturesFn.apply(x_diffuse, A_re, A_im, gops))
         return self.mlp.forward_sources(srcs, residual=x_in)   # layers.py:229-239
 
+    def _forward_batch(self, batch, x_in):
+        """Differentiable block over every mesh of a ``batch.MeshBatch`` (x_in in the batch layout): the per-mesh
+        spectral diffusion runs grouped (ops.BatchedDiffusionFn); the gradient features run on the block-diagonal CSR
+        and the MiniMLP row-wise, each once over the whole range.  Padding rows never reach a real row."""
+        x_diffuse = ops.BatchedDiffusionFn.apply(x_in, self.diffusion.diffusion_time, batch)
+        srcs = [x_in, x_diffuse]
+        if self.with_gradient_features:
+            A_re, A_im = self.gradient_features.weights()
+            srcs.append(ops.GradFeaturesFn.apply(x_diffuse, A_re, A_im, batch.gops))
+        return self.mlp.forward_sources(srcs, residual=x_in)
+
     def forward(self, x_in, mass, L, evals, evecs, gradX, gradY, head=None):
         """Reference signature (layers.py:200); ``head=(weight, bias)`` is this package's extension: a linear head fused
         behind the block in inference (returns the head's output; raises ops.HeadNotFused when it cannot be fused)."""
@@ -239,28 +250,61 @@ class DiffusionNet(nn.Module):
         return torch.stack([ops.mlp_apply([x[b]], [lin.weight], [lin.bias]) for b in range(B)], 0)
 
     def forward_batch(self, batch, xs):
-        """Inference over a ``batch.MeshBatch`` of independent meshes in ONE launch sequence (BASELINE config 4): the
+        """The net over a ``batch.MeshBatch`` of independent meshes in ONE launch sequence (BASELINE config 4): the
         reference's per-mesh loop (layers.py:217-222, 366-401) with every stage of every block launched once over all
-        meshes (``dn_block_fwd_batched``).  ``xs``: list of per-mesh (V_b, C_in) features, or one tensor already in the
-        batch layout.  Returns the list of per-mesh outputs (views into one tensor); 'vertices' and 'global_mean'
-        outputs only.  Equal to ``[self(x_b, mass_b, ...) for b]`` (tests/test_gpu_parity.py)."""
-        from . import batch as _batch
-        if self.outputs_at not in ('vertices', 'global_mean'):
-            raise ValueError("forward_batch supports outputs_at 'vertices' and 'global_mean'")
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise RuntimeError("forward_batch is an inference path: call it under torch.no_grad()")
+        meshes.  ``xs``: list of per-mesh (V_b, C_in) features, or one tensor already in the batch layout.  Returns the
+        list of per-mesh outputs.  Equal to ``[self(x_b, mass_b, ...) for b]`` (tests/test_gpu_parity.py).
+
+        Inference runs the fused block (``dn_block_fwd_batched``).  When autograd is needed or dropout is active the
+        blocks run differentiably (``DiffusionNetBlock._forward_batch``): sum or average the per-mesh losses and the
+        gradients are the per-mesh gradients accumulated, input gradients reaching each ``x_b``.  Dropout masks are
+        drawn over the whole batch layout, one draw per hidden layer per block.  'faces' / 'edges' outputs need the
+        batch items to carry ``faces`` / ``edges``."""
         if self.diffusion_method != 'spectral':
             raise NotImplementedError("forward_batch: spectral diffusion only")
+        elems = None
+        if self.outputs_at in ('edges', 'faces'):
+            elems = batch.faces if self.outputs_at == 'faces' else batch.edges
+            if elems is None:
+                raise ValueError("forward_batch with outputs_at='{0}' needs '{0}' in every MeshBatch item".format(
+                    self.outputs_at))
         x = xs if torch.is_tensor(xs) else batch.pack(xs)
         if x.shape[-1] != self.C_in:
             raise ValueError("DiffusionNet was constructed with C_in={}, but x_in has last dim={}".format(
                 self.C_in, x.shape[-1]))
+        needs_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))
+        dropout = any(blk.training and blk.dropout for blk in self.blocks)
+        if needs_grad or dropout:
+            x = ops.mlp_apply([x], [self.first_lin.weight], [self.first_lin.bias])
+            for blk in self.blocks:
+                x = blk._forward_batch(batch, x)
+            x = ops.mlp_apply([x], [self.last_lin.weight], [self.last_lin.bias])
+        else:
+            x = self._forward_batch_fused(batch, x)
+        if elems is not None:
+            # mean of the per-vertex outputs over each element's corners (as in forward), one gather for the batch
+            y = x[elems.view(-1)].view(elems.shape + (x.shape[-1],)).mean(dim=1)
+            outs = list(torch.split(y, batch.elem_counts(self.outputs_at)))
+        else:
+            outs = batch.unpack(x)
+        if self.outputs_at == 'global_mean':
+            res = []
+            for b, o in enumerate(outs):
+                m = batch.mass[batch.row_begin[b]:batch.row_begin[b] + batch.n_rows[b]]
+                res.append((o * (m / m.sum()).unsqueeze(-1)).sum(dim=-2))
+            outs = res
+        if self.last_activation != None:
+            outs = [self.last_activation(o) for o in outs]
+        return outs
+
+    def _forward_batch_fused(self, batch, x):
+        """Inference route of forward_batch: one dn_block_fwd_batched per block, last_lin fused behind the last one when
+        it can be.  Returns the (V, C_out) output in the batch layout."""
+        from . import batch as _batch
         x = ops.mlp_apply([x], [self.first_lin.weight], [self.first_lin.bias])
         fuse_head = FUSE_HEAD and ops.head_fusable(self.C_out)
         head_done = False
         for i_b, blk in enumerate(self.blocks):
-            if blk.training and blk.dropout:
-                raise RuntimeError("forward_batch: eval mode only (dropout)")
             A_re = A_im = None
             if blk.with_gradient_features:
                 A_re, A_im = blk.gradient_features.weights()
@@ -277,16 +321,7 @@ class DiffusionNet(nn.Module):
             x = _batch.block_forward_batched_raw(*args)
         if not head_done:
             x = ops.mlp_apply([x], [self.last_lin.weight], [self.last_lin.bias])
-        outs = batch.unpack(x)
-        if self.outputs_at == 'global_mean':
-            res = []
-            for b, o in enumerate(outs):
-                m = batch.mass[batch.row_begin[b]:batch.row_begin[b] + batch.n_rows[b]]
-                res.append((o * (m / m.sum()).unsqueeze(-1)).sum(dim=-2))
-            outs = res
-        if self.last_activation != None:
-            outs = [self.last_activation(o) for o in outs]
-        return outs
+        return x
 
     def forward(self, x_in, mass, L=None, evals=None, evecs=None, gradX=None, gradY=None, edges=None, faces=None):
         """[N,C] or [B,N,C] in, [N,C_out] or [B,N,C_out] out (reference layers.py:314-407)."""

@@ -595,6 +595,56 @@ class DiffusionFn(torch.autograd.Function):
         return gx, gt, None, None, None
 
 
+def batched_diffusion_workspace_extra(n_meshes, K, C_):
+    """Workspace bytes the batched diffusion calls need on top of dn_workspace_bytes: one packed K x C multiplier and
+    one fp32 K x C sum per mesh (include/diffusion_net_b200.h)."""
+    return int(n_meshes) * (8 * C_ * ((K + 15) // 16 * 16) + 4 * K * C_ + 512)
+
+
+class BatchedDiffusionFn(torch.autograd.Function):
+    """layers.py:44-67 spectral LearnedTimeDiffusion over every mesh of a ``batch.MeshBatch`` at once (x in the batch
+    layout).  Forward 3 launches, backward 4, whatever the mesh count; no SIMT route (the call raises)."""
+
+    @staticmethod
+    @_device_guard
+    def forward(ctx, x, time, batch):
+        lib = _lib.load()
+        x = _f32c(x)
+        V, Cc = x.shape
+        K, B = batch.K, batch.n_meshes
+        if V != batch.V:
+            raise ValueError("x is not in this batch's layout ({} rows, expected {})".format(V, batch.V))
+        xd = torch.empty_like(x)
+        x_spec = torch.empty(B, K, Cc, dtype=torch.float32, device=x.device)
+        ws = workspace(V, K, Cc, x.device, extra=batched_diffusion_workspace_extra(B, K, Cc))
+        # the kernel clamps `time` in place, as the reference does on the Parameter (layers.py:48-49)
+        _lib.check(lib.dn_learned_time_diffusion_fwd_batched(
+            x.data_ptr(), batch.mass.data_ptr(), batch.evals.data_ptr(), batch.evecs.data_ptr(), time.data_ptr(),
+            C.byref(batch.desc), V, K, Cc, xd.data_ptr(), x_spec.data_ptr(), ws.data_ptr(), ws.numel(), _engine,
+            _stream()), "dn_learned_time_diffusion_fwd_batched")
+        ctx.batch = batch
+        ctx.save_for_backward(time.detach().clone(), x_spec)
+        return xd
+
+    @staticmethod
+    @_device_guard
+    def backward(ctx, g):
+        lib = _lib.load()
+        time, x_spec = ctx.saved_tensors
+        batch = ctx.batch
+        g = _f32c(g)
+        V, Cc = g.shape
+        K, B = batch.K, batch.n_meshes
+        gx = torch.empty_like(g)
+        gt = torch.zeros_like(time)
+        ws = workspace(V, K, Cc, g.device, extra=batched_diffusion_workspace_extra(B, K, Cc))
+        _lib.check(lib.dn_learned_time_diffusion_bwd_batched(
+            g.data_ptr(), batch.mass.data_ptr(), batch.evals.data_ptr(), batch.evecs.data_ptr(), time.data_ptr(),
+            x_spec.data_ptr(), C.byref(batch.desc), V, K, Cc, gx.data_ptr(), gt.data_ptr(), ws.data_ptr(), ws.numel(),
+            _engine, _stream()), "dn_learned_time_diffusion_bwd_batched")
+        return gx, gt, None
+
+
 class GradFeaturesFn(torch.autograd.Function):
     """layers.py:216-226: sparse tangent gradient + SpatialGradientFeatures, fused."""
 

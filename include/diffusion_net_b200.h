@@ -264,6 +264,27 @@ int dn_block_fwd_batched(const float* x_in, const float* mass, const float* eval
                          const dn_csr* grad, const dn_block_params* params, const dn_mesh_batch* batch, int64_t V,
                          int K, int C, float* out, void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream);
 
+/* dn_learned_time_diffusion_fwd / _bwd over a batch laid out as above, for training over many small meshes in one
+ * launch sequence (3 launches forward, 4 backward, whatever the mesh count; C = 256 adds one to_basis launch to each).
+ * evals is (n_meshes, K); x_spec (n_meshes, K, C) holds each mesh's unscaled coefficients Phi_b^T M_b x_b.
+ *   fwd: time (C) is clamped in place (layers.py:48-49); x_diffuse is 0 on padding rows; x_spec_out optional.
+ *   bwd: grad_x = M * Phi_b (exp(-lambda_b t) * Phi_b^T g_b) on the rows of mesh b and exactly 0 on padding rows;
+ *        grad_time[c] += sum_b sum_k G_b[k][c] * (-lambda_bk) * exp(-lambda_bk t_c) * x_spec_b[k][c], G_b = Phi_b^T g_b,
+ *        in a fixed summation order (deterministic).  `time` is the clamped time the forward left; it is only read.
+ * Same envelope as dn_block_fwd_batched: tensor-core engines only, V % 128 == 0, and a from_basis layer the fused chain
+ * takes; anything else (the SIMT engine included: batches have no SIMT route) is DN_ERR_UNSUPPORTED before any work is
+ * enqueued.  Workspace: dn_workspace_bytes(V, K, C) plus, per mesh, one packed K x C matrix and one fp32 K x C sum:
+ * n_meshes * (8 * C * (K rounded up to 16) + 4 * K * C + 512) bytes. */
+int dn_learned_time_diffusion_fwd_batched(const float* x, const float* mass, const float* evals, const float* evecs,
+                                          float* time, const dn_mesh_batch* batch, int64_t V, int K, int C,
+                                          float* x_diffuse, float* x_spec_out, void* workspace, int64_t ws_bytes,
+                                          int engine, dn_stream_t stream);
+int dn_learned_time_diffusion_bwd_batched(const float* grad_out, const float* mass, const float* evals,
+                                          const float* evecs, const float* time, const float* x_spec,
+                                          const dn_mesh_batch* batch, int64_t V, int K, int C, float* grad_x,
+                                          float* grad_time, void* workspace, int64_t ws_bytes, int engine,
+                                          dn_stream_t stream);
+
 /* Linear head fused behind a block (SURVEY.md 8f-1): `DiffusionNet.last_lin` (layers.py:366-370 -- the nn.Linear applied
  * to the last block's output) computed in the epilogue of that block's MiniMLP chain, in exact fp32, so that the
  * C_width-wide block output is never written: out_head[v][o] = bias[o] + sum_c weight[o][c] * block_out[v][c]. */

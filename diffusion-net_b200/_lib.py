@@ -14,7 +14,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libdiffusion_net_b200.so")
-SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_tc.cu", "dn_capi.cu"]
+SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_eig.cu", "dn_tc.cu", "dn_capi.cu"]
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "diffusion_net_b200.h")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -72,7 +72,7 @@ class dn_head(C.Structure):
     _fields_ = [("weight", C.c_void_p), ("bias", C.c_void_p), ("n_out", C.c_int32), ("out", C.c_void_p), ("ld_out", C.c_int64)]
 
 
-_P, _I, _L = C.c_void_p, C.c_int, C.c_int64
+_P, _I, _L, _D = C.c_void_p, C.c_int, C.c_int64, C.c_double
 _PP = C.POINTER(C.c_void_p)
 _IP = C.POINTER(C.c_int)
 
@@ -103,6 +103,13 @@ SIGNATURES = {
     "dn_block_fwd_profile": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), _L, _I, _I, _P, _P, _L,
                                   _I, _P, C.POINTER(C.c_float)]),
     "dn_build_grad": (_I, [_P, _P, _P, _P, _L, _L, _P, _P, _P, _P, _L, _P]),
+    "dn_mesh_laplacian": (_I, [_P, _P, _L, _L, _D, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P]),
+    "dn_vertex_frames": (_I, [_P, _P, _L, _L, _P, _P, _P, _P, _P, _L, _P]),
+    "dn_eig_filter": (_I, [_P, _P, _P, _P, _L, _I, _P, _P, _L, _D, _D, _D, _P, _P]),
+    "dn_eig_gram": (_I, [_P, _L, _P, _L, _L, _I, _I, _P, _P, _L, _P]),
+    "dn_eig_rotate": (_I, [_P, _L, _P, _L, _L, _I, _I, _D, _P, _L, _P]),
+    "dn_eig_residual_norms": (_I, [_P, _L, _P, _L, _P, _L, _I, _P, _P, _L, _P]),
+    "dn_eig_finalize": (_I, [_P, _L, _P, _I, _P, _L, _P, _P, _L, _P]),
     "dn_mesh_batch_plan": (_I, [_I, _P, _I, _P, _P, _P, _P]),
     "dn_block_fwd_ex": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),
                              C.POINTER(dn_head), _L, _I, _I, _P, _P, _L, _I, _P]),

@@ -343,6 +343,72 @@ int dn_build_grad(const float* verts, const float* frames, const float* edge_tan
                            (cudaStream_t)stream);
 }
 
+int dn_mesh_laplacian(const double* verts, const int64_t* faces, int64_t F, int64_t V, double eps, int32_t* rowptr_out,
+                      int32_t* colidx_out, double* L_vals_out, double* mass_out, double* A_vals_out, double* A_diag_out,
+                      double* bound_out, int32_t* nan_out, void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  if (V < 0 || F < 0 || !rowptr_out || !bound_out || !nan_out || (F > 0 && (!faces || !verts)) ||
+      (V > 0 && (!colidx_out || !L_vals_out || !mass_out)))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (6 * F + V >= (1ll << 31) || V >= (1ll << 31) - 1) return DN_ERR_UNSUPPORTED;
+  if (V > 0 && (!workspace || ws_bytes < mesh_laplacian_ws_bytes(F, V))) return DN_ERR_WORKSPACE;
+  return launch_mesh_laplacian(verts, faces, F, V, eps, rowptr_out, colidx_out, L_vals_out, mass_out, A_vals_out,
+                               A_diag_out, bound_out, nan_out, workspace, (cudaStream_t)stream);
+}
+
+int dn_vertex_frames(const double* verts, const int64_t* faces, int64_t F, int64_t V, const double* normals_in,
+                     double* normals_out, double* frames_out, int32_t* n_bad_out, void* workspace, int64_t ws_bytes,
+                     dn_stream_t stream) {
+  if (V < 0 || F < 0 || !n_bad_out || (V > 0 && !frames_out) ||
+      (!normals_in && V > 0 && (!normals_out || (F > 0 && (!faces || !verts)))))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (3 * F >= (1ll << 31) || V >= (1ll << 31) - 1) return DN_ERR_UNSUPPORTED;
+  if (!normals_in && V > 0 && (!workspace || ws_bytes < vertex_frames_ws_bytes(F, V))) return DN_ERR_WORKSPACE;
+  return launch_vertex_frames(verts, faces, F, V, normals_in, normals_out, frames_out, n_bad_out, workspace,
+                              (cudaStream_t)stream);
+}
+
+int dn_eig_filter(const int32_t* rowptr, const int32_t* colidx, const double* A_vals, const double* A_diag, int64_t V,
+                  int n, const double* Y, const double* Y_prev, int64_t ld, double alpha, double beta, double gamma,
+                  double* Y_out, dn_stream_t stream) {
+  if (V < 0 || n < 0 || ld < n || (V > 0 && n > 0 && (!rowptr || !colidx || !A_vals || !A_diag || !Y || !Y_out)) ||
+      (Y_out && (Y_out == Y || Y_out == Y_prev)))
+    return DN_ERR_INVALID_ARGUMENT;
+  return launch_eig_filter(rowptr, colidx, A_vals, A_diag, V, n, Y, Y_prev, ld, alpha, beta, gamma, Y_out,
+                           (cudaStream_t)stream);
+}
+
+int dn_eig_gram(const double* X, int64_t ldx, const double* Y, int64_t ldy, int64_t V, int m, int n, double* out,
+                void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  if (V < 0 || m < 0 || n < 0 || ldx < m || ldy < n || (m > 0 && n > 0 && (!out || (V > 0 && (!X || !Y)))))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (m > 0 && n > 0 && V > 0 && (!workspace || ws_bytes < eig_gram_ws_bytes(V, m, n))) return DN_ERR_WORKSPACE;
+  return launch_eig_gram(X, ldx, Y, ldy, V, m, n, out, (double*)workspace, (cudaStream_t)stream);
+}
+
+int dn_eig_rotate(const double* X, int64_t ldx, const double* C, int64_t ldc, int64_t V, int kd, int n, double beta,
+                  double* Z, int64_t ldz, dn_stream_t stream) {
+  if (V < 0 || kd < 0 || n < 0 || ldx < kd || ldc < n || ldz < n || (V > 0 && n > 0 && (!Z || (kd > 0 && (!X || !C)))) ||
+      (Z && Z == X))
+    return DN_ERR_INVALID_ARGUMENT;
+  return launch_eig_rotate(X, ldx, C, ldc, V, kd, n, beta, Z, ldz, (cudaStream_t)stream);
+}
+
+int dn_eig_residual_norms(const double* W, int64_t ldw, const double* Q, int64_t ldq, const double* theta, int64_t V,
+                          int n, double* out, void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  if (V < 0 || n < 0 || ldw < n || ldq < n || (n > 0 && (!out || !theta || (V > 0 && (!W || !Q)))))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (n > 0 && V > 0 && (!workspace || ws_bytes < eig_resid_ws_bytes(V, n))) return DN_ERR_WORKSPACE;
+  return launch_eig_residual_norms(W, ldw, Q, ldq, theta, V, n, out, (double*)workspace, (cudaStream_t)stream);
+}
+
+int dn_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass, int64_t V, double* out,
+                    void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  if (V < 0 || k < 0 || (V > 0 && k > 0 && (!Y || !cols || !mass || !out)))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (V > 0 && k > 0 && (!workspace || ws_bytes < 8ll * k)) return DN_ERR_WORKSPACE;
+  return launch_eig_finalize(Y, ldy, cols, k, mass, V, out, (double*)workspace, (cudaStream_t)stream);
+}
+
 int dn_compute_hks(const float* evals, const float* evecs, const float* scales, int64_t V, int K, int S, float* out,
                    dn_stream_t stream) {
   if (V < 0 || K <= 0 || S < 0 || ((V > 0 && S > 0) && (!evals || !evecs || !scales || !out)))

@@ -3,6 +3,7 @@
 //   * CSC (the reference's on-disk operator cache, geometry.py:548-568) -> device CSR, i.e. a sparse transpose
 // Both are HBM-bound index/streaming work: plain coalesced SIMT, no tensor cores.
 #include "dn_internal.h"
+#include <type_traits>
 
 namespace {
 
@@ -90,9 +91,11 @@ __global__ void hks_generic_kernel(const float* __restrict__ evals, const float*
 }
 
 // ---------------------------------------------------------------------------------------------
-// sparse transpose of the shared-pattern CSR (int32 indices, interleaved (x, y) values)
+// sparse transpose of the shared-pattern CSR (int32 indices, interleaved (x, y) values); the count / scan / row-sort
+// kernels also build the mesh Laplacian and the vertex -> face incidence below
 // ---------------------------------------------------------------------------------------------
-__global__ void tr_count_kernel(const int32_t* __restrict__ colidx, int64_t nnz, int32_t* __restrict__ cnt) {
+template <typename I>
+__global__ void tr_count_kernel(const I* __restrict__ colidx, int64_t nnz, int32_t* __restrict__ cnt) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p < nnz) atomicAdd(cnt + colidx[p] + 1, 1);
 }
@@ -135,24 +138,40 @@ __global__ void tr_fill_kernel(const int32_t* __restrict__ rowptr, const int32_t
   }
 }
 
+// Row payloads of the sort below.  Ties (equal column) are ordered by value_less so that rows filled by atomics in
+// arbitrary order come out in one deterministic order; the transposes never have ties (their input has unique entries).
+struct NoVal {};                      // keys only (vertex -> face incidence)
+struct LapVal { double w, a; };       // one directed half of a face corner: cotan weight w and a sixth of the face area
+__device__ __forceinline__ bool value_less(const float2&, const float2&) { return false; }
+__device__ __forceinline__ bool value_less(const LapVal& x, const LapVal& y) {
+  return x.w < y.w || (x.w == y.w && x.a < y.a);
+}
+
 // the atomics above land entries of one output row in arbitrary order: sort each row by column (rows are short --
 // vertex degree + 1 on meshes, 31 on point clouds -- so one thread per row with an insertion sort)
+template <typename T>
 __global__ void tr_sort_rows_kernel(const int32_t* __restrict__ rowptr_t, int64_t V, int32_t* __restrict__ colidx_t,
-                                    float2* __restrict__ vals_t) {
+                                    T* __restrict__ vals_t) {
   const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= V) return;
   const int s = rowptr_t[row], e = rowptr_t[row + 1];
   for (int i = s + 1; i < e; ++i) {
     const int32_t ck = colidx_t[i];
-    const float2 vk = vals_t[i];
+    T vk{};
+    if constexpr (!std::is_same<T, NoVal>::value) vk = vals_t[i];
+    auto after = [&](int j) {             // entry j sorts after the one being inserted
+      if (colidx_t[j] != ck) return colidx_t[j] > ck;
+      if constexpr (std::is_same<T, NoVal>::value) return false;
+      else return value_less(vk, vals_t[j]);
+    };
     int j = i - 1;
-    while (j >= s && colidx_t[j] > ck) {
+    while (j >= s && after(j)) {
       colidx_t[j + 1] = colidx_t[j];
-      vals_t[j + 1] = vals_t[j];
+      if constexpr (!std::is_same<T, NoVal>::value) vals_t[j + 1] = vals_t[j];
       --j;
     }
     colidx_t[j + 1] = ck;
-    vals_t[j + 1] = vk;
+    if constexpr (!std::is_same<T, NoVal>::value) vals_t[j + 1] = vk;
   }
 }
 
@@ -229,6 +248,189 @@ __global__ void bg_solve_kernel(const int32_t* __restrict__ rowptr, const int32_
   if (self >= 0) vals[self] = make_float2((float)(-sx), (float)(-sy));
 }
 
+// ---------------------------------------------------------------------------------------------
+// Mesh Laplacian and lumped mass (reference geometry.py:322-329): the cotan Laplacian with cot = (u.v) / (|u x v| +
+// denom_eps) per face corner, L_jk = -1/2 sum cot, L_jj = -sum_k L_jk, and the barycentric vertex areas.  fp64.
+// Pattern as scipy's coo -> csc of the reference: the diagonal of every vertex a face references plus both directions
+// of every face edge, duplicates summed, explicit zeros kept.  Each corner's weight is computed once and scattered to
+// (j, k) and (k, j) together with a sixth of the face area (every vertex of a face receives two such halves); rows are
+// sorted by (column, value) so that every sum runs in one fixed order and L is exactly symmetric.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ double3 ld3(const double* p, int64_t i) { return make_double3(p[3 * i], p[3 * i + 1], p[3 * i + 2]); }
+__device__ __forceinline__ double3 sub3(double3 a, double3 b) { return make_double3(a.x - b.x, a.y - b.y, a.z - b.z); }
+__device__ __forceinline__ double dot3(double3 a, double3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+__device__ __forceinline__ double3 cross3(double3 a, double3 b) {
+  return make_double3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x);
+}
+__device__ __forceinline__ double norm3(double3 a) { return sqrt(dot3(a, a)); }
+
+__device__ __forceinline__ bool face_ok(const int64_t* f, int64_t V) {
+  return f[0] >= 0 && f[0] < V && f[1] >= 0 && f[1] < V && f[2] >= 0 && f[2] < V;
+}
+
+// per face: 2 directed entries per corner whose opposite edge has two distinct ends; marks referenced vertices
+__global__ void lap_count_kernel(const int64_t* __restrict__ faces, int64_t F, int64_t V, int32_t* __restrict__ cnt,
+                                 int32_t* __restrict__ ref) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F || !face_ok(faces + 3 * f, V)) return;
+  const int64_t* t = faces + 3 * f;
+  for (int c = 0; c < 3; ++c) {
+    const int64_t i = t[c], j = t[(c + 1) % 3], k = t[(c + 2) % 3];
+    ref[i] = 1;
+    if (j != k) { atomicAdd(cnt + j + 1, 1); atomicAdd(cnt + k + 1, 1); }
+  }
+}
+
+// A corner whose opposite edge is a single vertex (a face with a repeated index) adds -w, -w, +w, +w to that vertex's
+// diagonal in the reference, i.e. nothing, and its face has zero area: it is skipped.
+__global__ void lap_fill_kernel(const double* __restrict__ verts, const int64_t* __restrict__ faces, int64_t F, int64_t V,
+                                double denom_eps, const int32_t* __restrict__ rawptr, int32_t* __restrict__ cursor,
+                                int32_t* __restrict__ rawcol, LapVal* __restrict__ rawval) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F || !face_ok(faces + 3 * f, V)) return;
+  const int64_t* t = faces + 3 * f;
+  const double3 p0 = ld3(verts, t[0]);
+  const double area6 = 0.5 * norm3(cross3(sub3(ld3(verts, t[1]), p0), sub3(ld3(verts, t[2]), p0))) / 6.0;
+  for (int c = 0; c < 3; ++c) {
+    const int64_t i = t[c], j = t[(c + 1) % 3], k = t[(c + 2) % 3];
+    if (j == k) continue;
+    const double3 pi = ld3(verts, i), u = sub3(ld3(verts, j), pi), v = sub3(ld3(verts, k), pi);
+    const double w = 0.5 * (dot3(u, v) / (norm3(cross3(u, v)) + denom_eps));
+    int dst = rawptr[j] + atomicAdd(cursor + j, 1);
+    rawcol[dst] = (int32_t)k;
+    rawval[dst] = LapVal{w, area6};
+    dst = rawptr[k] + atomicAdd(cursor + k, 1);
+    rawcol[dst] = (int32_t)j;
+    rawval[dst] = LapVal{w, area6};
+  }
+}
+
+// per row (sorted): number of distinct columns + the diagonal -> cnt[v + 1]; the vertex area (before the eps shift)
+__global__ void lap_rows_kernel(const int32_t* __restrict__ rawptr, const int32_t* __restrict__ rawcol,
+                                const LapVal* __restrict__ rawval, const int32_t* __restrict__ ref, int64_t V,
+                                int32_t* __restrict__ cnt, double* __restrict__ area) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  const int s = rawptr[v], e = rawptr[v + 1];
+  int n = ref[v] ? 1 : 0;
+  double a = 0.0;
+  for (int p = s; p < e; ++p) {
+    if (p == s || rawcol[p] != rawcol[p - 1]) ++n;
+    a += rawval[p].a;
+  }
+  cnt[v + 1] = n;
+  area[v] = a;
+}
+
+// mass += eps * mean(mass), one block, fixed summation order
+__global__ void __launch_bounds__(1024) lap_mass_shift_kernel(double* __restrict__ mass, int64_t V, double eps) {
+  __shared__ double part[1024];
+  const int t = threadIdx.x;
+  double s = 0.0;
+  for (int64_t i = t; i < V; i += 1024) s += mass[i];
+  part[t] = s;
+  __syncthreads();
+  for (int o = 512; o > 0; o >>= 1) {
+    if (t < o) part[t] += part[t + o];
+    __syncthreads();
+  }
+  const double shift = eps * (part[0] / (double)V);
+  for (int64_t i = t; i < V; i += 1024) mass[i] += shift;
+}
+
+// Merge the sorted raw row into the final CSR row (diagonal at its column position), and the operator the eigensolver
+// runs on, A = M^-1/2 (L + eps I) M^-1/2, as A_vals (same pattern: d_v d_k L_vk) + A_diag (eps / m_v).  Row bound of
+// Gershgorin's theorem -> max into bound_bits; NaN counts -> nan_out[0] (L rows) and nan_out[1] (mass entries).
+__global__ void lap_emit_kernel(const int32_t* __restrict__ rawptr, const int32_t* __restrict__ rawcol,
+                                const LapVal* __restrict__ rawval, const int32_t* __restrict__ ref,
+                                const double* __restrict__ mass, int64_t V, double eps, const int32_t* __restrict__ rowptr,
+                                int32_t* __restrict__ colidx, double* __restrict__ lvals, double* __restrict__ avals,
+                                double* __restrict__ adiag, unsigned long long* __restrict__ bound_bits,
+                                int32_t* __restrict__ nan_out) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  const int s = rawptr[v], e = rawptr[v + 1];
+  const double dv = 1.0 / sqrt(mass[v]);
+  double diag = 0.0;
+  for (int p = s; p < e; ++p) diag += rawval[p].w;
+  int out = rowptr[v];
+  bool diag_done = !ref[v], bad = false;
+  double rowsum = 0.0;
+  const double shift = eps * dv * dv;
+  auto emit = [&](int32_t col, double l) {
+    colidx[out] = col;
+    lvals[out] = l;
+    const double a = (dv * (col == v ? dv : 1.0 / sqrt(mass[col]))) * l;   // d_v d_k commutes: A is symmetric too
+    if (avals) avals[out] = a;
+    rowsum += fabs(col == v ? a + shift : a);
+    bad |= isnan(l);
+    ++out;
+  };
+  for (int p = s; p < e;) {
+    const int32_t col = rawcol[p];
+    double w = 0.0;
+    for (; p < e && rawcol[p] == col; ++p) w += rawval[p].w;
+    if (!diag_done && col > v) { emit((int32_t)v, diag); diag_done = true; }
+    emit(col, -w);
+  }
+  if (!diag_done) emit((int32_t)v, diag);
+  if (!ref[v]) rowsum += fabs(shift);
+  if (adiag) adiag[v] = shift;
+  if (bad) atomicAdd(nan_out, 1);
+  if (isnan(mass[v])) atomicAdd(nan_out + 1, 1);
+  if (!isnan(rowsum)) atomicMax(bound_bits, (unsigned long long)__double_as_longlong(rowsum));   // >= 0: bits order as values
+}
+
+// ---------------------------------------------------------------------------------------------
+// Vertex normals and tangent frames (reference geometry.py:101-177).  Unit face normals (divide-eps 1e-6) summed per
+// vertex in face order over the vertex -> face incidence (count / scan / fill / sort), then normalised without eps: a
+// vertex no face with a nonzero normal touches gets NaN and is counted (the host applies the reference's remedy).
+// Frames: basis candidate e_x unless |n.e_x| >= 0.9 (then e_y), projected to the tangent plane, normalised
+// (divide-eps 1e-6), basisY = n x basisX.
+// ---------------------------------------------------------------------------------------------
+__global__ void vf_fill_kernel(const int64_t* __restrict__ faces, int64_t F, const int32_t* __restrict__ rowptr,
+                               int32_t* __restrict__ cursor, int32_t* __restrict__ inc) {
+  const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= 3 * F) return;
+  const int64_t v = faces[s];
+  inc[rowptr[v] + atomicAdd(cursor + v, 1)] = (int32_t)(s / 3);
+}
+
+__global__ void vf_normals_kernel(const double* __restrict__ verts, const int64_t* __restrict__ faces,
+                                  const int32_t* __restrict__ rowptr, const int32_t* __restrict__ inc, int64_t V,
+                                  double* __restrict__ normals, int32_t* __restrict__ n_bad) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  double3 n = make_double3(0.0, 0.0, 0.0);
+  for (int p = rowptr[v]; p < rowptr[v + 1]; ++p) {
+    const int64_t* t = faces + 3 * (int64_t)inc[p];
+    const double3 p0 = ld3(verts, t[0]);
+    const double3 r = cross3(sub3(ld3(verts, t[1]), p0), sub3(ld3(verts, t[2]), p0));
+    const double d = norm3(r) + 1e-6;
+    n.x += r.x / d; n.y += r.y / d; n.z += r.z / d;
+  }
+  const double l = norm3(n);
+  n.x /= l; n.y /= l; n.z /= l;
+  normals[3 * v] = n.x; normals[3 * v + 1] = n.y; normals[3 * v + 2] = n.z;
+  if (isnan(n.x) || isnan(n.y) || isnan(n.z)) atomicAdd(n_bad, 1);
+}
+
+__global__ void vf_frames_kernel(const double* __restrict__ normals, int64_t V, double* __restrict__ frames) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  const double3 n = ld3(normals, v);
+  double3 b = fabs(n.x) < 0.9 ? make_double3(1.0, 0.0, 0.0) : make_double3(0.0, 1.0, 0.0);
+  const double d = dot3(b, n);
+  b = make_double3(b.x - n.x * d, b.y - n.y * d, b.z - n.z * d);
+  const double l = norm3(b) + 1e-6;
+  b = make_double3(b.x / l, b.y / l, b.z / l);
+  const double3 y = cross3(n, b);
+  double* o = frames + 9 * v;
+  o[0] = b.x; o[1] = b.y; o[2] = b.z;
+  o[3] = y.x; o[4] = y.y; o[5] = y.z;
+  o[6] = n.x; o[7] = n.y; o[8] = n.z;
+}
+
 }  // namespace
 
 int launch_build_grad(const float* verts, const float* frames, const float* edge_tangent, const int64_t* edges, int64_t E,
@@ -252,6 +454,92 @@ int launch_build_grad(const float* verts, const float* frames, const float* edge
   tr_sort_rows_kernel<<<vb, 256, 0, st>>>(rowptr, V, colidx, reinterpret_cast<float2*>(vals));
   DN_LAUNCH_CHECK();
   bg_solve_kernel<<<vb, 256, 0, st>>>(rowptr, colidx, V, reinterpret_cast<float2*>(vals));
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
+namespace {
+template <typename T>
+T* carve(char*& p, int64_t count) {
+  T* r = reinterpret_cast<T*>(p);
+  p += (count * (int64_t)sizeof(T) + 255) / 256 * 256;
+  return r;
+}
+}  // namespace
+
+int64_t mesh_laplacian_ws_bytes(int64_t F, int64_t V) { return 120 * F + 12 * V + 2048; }
+int64_t vertex_frames_ws_bytes(int64_t F, int64_t V) { return 12 * F + 8 * V + 1024; }
+
+int launch_mesh_laplacian(const double* verts, const int64_t* faces, int64_t F, int64_t V, double eps, int32_t* rowptr,
+                          int32_t* colidx, double* lvals, double* mass, double* avals, double* adiag, double* bound,
+                          int32_t* nan_out, void* ws, cudaStream_t st) {
+  DN_CUDA_TRY(cudaMemsetAsync(rowptr, 0, sizeof(int32_t) * (V + 1), st));
+  DN_CUDA_TRY(cudaMemsetAsync(bound, 0, sizeof(double), st));
+  DN_CUDA_TRY(cudaMemsetAsync(nan_out, 0, 2 * sizeof(int32_t), st));
+  if (V <= 0) return DN_OK;
+  char* p = static_cast<char*>(ws);
+  int32_t* rawcol = carve<int32_t>(p, 6 * F);
+  LapVal* rawval = carve<LapVal>(p, 6 * F);
+  int32_t* rawptr = carve<int32_t>(p, V + 1);
+  int32_t* cursor = carve<int32_t>(p, V);
+  int32_t* ref = carve<int32_t>(p, V);
+  DN_CUDA_TRY(cudaMemsetAsync(rawptr, 0, sizeof(int32_t) * (V + 1), st));
+  DN_CUDA_TRY(cudaMemsetAsync(cursor, 0, sizeof(int32_t) * V, st));
+  DN_CUDA_TRY(cudaMemsetAsync(ref, 0, sizeof(int32_t) * V, st));
+  const unsigned vb = (unsigned)((V + 255) / 256), fb = (unsigned)((F + 255) / 256);
+  if (F > 0) {
+    lap_count_kernel<<<fb, 256, 0, st>>>(faces, F, V, rawptr, ref);
+    DN_LAUNCH_CHECK();
+  }
+  tr_scan_kernel<<<1, 1024, 0, st>>>(rawptr, V + 1);
+  DN_LAUNCH_CHECK();
+  if (F > 0) {
+    lap_fill_kernel<<<fb, 256, 0, st>>>(verts, faces, F, V, 1e-10, rawptr, cursor, rawcol, rawval);
+    DN_LAUNCH_CHECK();
+  }
+  tr_sort_rows_kernel<<<vb, 256, 0, st>>>(rawptr, V, rawcol, rawval);
+  DN_LAUNCH_CHECK();
+  lap_rows_kernel<<<vb, 256, 0, st>>>(rawptr, rawcol, rawval, ref, V, rowptr, mass);
+  DN_LAUNCH_CHECK();
+  tr_scan_kernel<<<1, 1024, 0, st>>>(rowptr, V + 1);
+  DN_LAUNCH_CHECK();
+  lap_mass_shift_kernel<<<1, 1024, 0, st>>>(mass, V, eps);
+  DN_LAUNCH_CHECK();
+  lap_emit_kernel<<<vb, 256, 0, st>>>(rawptr, rawcol, rawval, ref, mass, V, eps, rowptr, colidx, lvals, avals, adiag,
+                                      reinterpret_cast<unsigned long long*>(bound), nan_out);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
+int launch_vertex_frames(const double* verts, const int64_t* faces, int64_t F, int64_t V, const double* normals_in,
+                         double* normals_out, double* frames, int32_t* n_bad, void* ws, cudaStream_t st) {
+  DN_CUDA_TRY(cudaMemsetAsync(n_bad, 0, sizeof(int32_t), st));
+  if (V <= 0) return DN_OK;
+  const unsigned vb = (unsigned)((V + 255) / 256);
+  if (!normals_in) {
+    char* p = static_cast<char*>(ws);
+    int32_t* rowptr = carve<int32_t>(p, V + 1);
+    int32_t* cursor = carve<int32_t>(p, V);
+    int32_t* inc = carve<int32_t>(p, 3 * F);
+    DN_CUDA_TRY(cudaMemsetAsync(rowptr, 0, sizeof(int32_t) * (V + 1), st));
+    DN_CUDA_TRY(cudaMemsetAsync(cursor, 0, sizeof(int32_t) * V, st));
+    if (F > 0) {
+      tr_count_kernel<<<(unsigned)((3 * F + 255) / 256), 256, 0, st>>>(faces, 3 * F, rowptr);
+      DN_LAUNCH_CHECK();
+    }
+    tr_scan_kernel<<<1, 1024, 0, st>>>(rowptr, V + 1);
+    DN_LAUNCH_CHECK();
+    if (F > 0) {
+      vf_fill_kernel<<<(unsigned)((3 * F + 255) / 256), 256, 0, st>>>(faces, F, rowptr, cursor, inc);
+      DN_LAUNCH_CHECK();
+    }
+    tr_sort_rows_kernel<<<vb, 256, 0, st>>>(rowptr, V, inc, static_cast<NoVal*>(nullptr));
+    DN_LAUNCH_CHECK();
+    vf_normals_kernel<<<vb, 256, 0, st>>>(verts, faces, rowptr, inc, V, normals_out, n_bad);
+    DN_LAUNCH_CHECK();
+    normals_in = normals_out;
+  }
+  vf_frames_kernel<<<vb, 256, 0, st>>>(normals_in, V, frames);
   DN_LAUNCH_CHECK();
   return DN_OK;
 }

@@ -102,6 +102,27 @@ int launch_build_grad(const float* verts, const float* frames, const float* edge
                       int64_t V, int32_t* rowptr, int32_t* colidx, float* vals, int32_t* cursor, cudaStream_t st);
 int launch_csr_transpose(const dn_csr* in, int64_t V, int32_t* rowptr_t, int32_t* colidx_t, float* vals_t,
                          int32_t* cursor, cudaStream_t st);
+// mesh operators (dn_geom.cu) and the eigensolver's kernels (dn_eig.cu); fp64
+int64_t mesh_laplacian_ws_bytes(int64_t F, int64_t V);
+int64_t vertex_frames_ws_bytes(int64_t F, int64_t V);
+int launch_mesh_laplacian(const double* verts, const int64_t* faces, int64_t F, int64_t V, double eps, int32_t* rowptr,
+                          int32_t* colidx, double* lvals, double* mass, double* avals, double* adiag, double* bound,
+                          int32_t* nan_out, void* ws, cudaStream_t st);
+int launch_vertex_frames(const double* verts, const int64_t* faces, int64_t F, int64_t V, const double* normals_in,
+                         double* normals_out, double* frames, int32_t* n_bad, void* ws, cudaStream_t st);
+int64_t eig_gram_ws_bytes(int64_t V, int m, int n);
+int64_t eig_resid_ws_bytes(int64_t V, int n);
+int launch_eig_filter(const int32_t* rowptr, const int32_t* colidx, const double* avals, const double* adiag, int64_t V,
+                      int n, const double* Y, const double* Yp, int64_t ld, double alpha, double beta, double gamma,
+                      double* out, cudaStream_t st);
+int launch_eig_gram(const double* X, int64_t ldx, const double* Y, int64_t ldy, int64_t V, int m, int n, double* out,
+                    double* ws, cudaStream_t st);
+int launch_eig_rotate(const double* X, int64_t ldx, const double* Cm, int64_t ldc, int64_t V, int kd, int n, double beta,
+                      double* Z, int64_t ldz, cudaStream_t st);
+int launch_eig_residual_norms(const double* W, int64_t ldw, const double* Q, int64_t ldq, const double* theta, int64_t V,
+                              int n, double* out, double* ws, cudaStream_t st);
+int launch_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass, int64_t V,
+                        double* out, double* sign_ws, cudaStream_t st);
 int launch_grad_spmm_pair(const dn_csr* g, const float* x, int64_t V, int C, float* out_vc2, cudaStream_t st);
 // R-order fused features: feat = tanh(gX*Bre + gY*Bim) from gathers of xd, P, Q (pq = [P|Q], ld 2C or C).
 int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int rotations, int64_t V, int C,

@@ -1,6 +1,7 @@
 """The pieces of the reference's ``geometry`` module that sit either side of the block: ``to_basis`` / ``from_basis``
-(geometry.py:572-598), heat-kernel-signature features (geometry.py:600-633) and the READ side of the operator
-cache (geometry.py:426-519) -- all with the reference signatures, all running the hand-written kernels.
+(geometry.py:572-598), heat-kernel-signature features (geometry.py:600-633), the operator cache (geometry.py:426-568)
+and operator construction for triangle meshes (geometry.py:101-392) -- all with the reference signatures, all running
+the hand-written kernels.
 Batched (B,V,*) or single-mesh (V,*) inputs, as the reference accepts."""
 from __future__ import annotations
 
@@ -51,7 +52,7 @@ def compute_hks_autoscale(evals, evecs, count):
 
 
 # ------------------------------------------------------------------------------------------------
-# operator cache -> device  (the read side of geometry.py:426-519; construction itself is out of scope)
+# operator cache <-> device  (geometry.py:426-568; a miss is built by compute_operators on request)
 # ------------------------------------------------------------------------------------------------
 def hash_arrays(arrs):
     """utils.py:71-76 -- the cache file name is sha1(verts bytes, faces bytes)."""
@@ -126,11 +127,57 @@ def find_cached_operators(verts, faces, k_eig, op_cache_dir):
         return npz
 
 
-def get_operators(verts, faces, k_eig=128, op_cache_dir=None, normals=None, overwrite_cache=False, device=None):
-    """``geometry.get_operators`` (geometry.py:426) for a POPULATED cache: same arguments, same file naming, same
-    returned tuple.  ``device`` (extra) places the operators directly on a GPU; default = ``verts.device``.
-    Building operators (robust-laplacian / eigsh / build_grad, geometry.py:275-393) is out of this framework's
-    scope (SURVEY.md 8f item 4): a cache miss raises instead of computing."""
+def find_cache_bucket(verts, faces, op_cache_dir):
+    """The file the reference's ``get_operators`` writes a freshly computed entry to (geometry.py:447-533): the first
+    ``<sha1>_<i>.npz`` that is absent, unreadable or holds this very mesh (a stale entry -- too few eigenpairs, no
+    ``L_data``, or ``overwrite_cache`` -- is rewritten in place); buckets holding other meshes are skipped."""
+    verts_np, faces_np = _to_np(verts), _to_np(faces)
+    key = hash_arrays((verts_np, faces_np))
+    i = 0
+    while True:
+        path = os.path.join(op_cache_dir, "{}_{}.npz".format(key, i))
+        try:
+            npz = np.load(path, allow_pickle=True)
+            same = np.array_equal(verts_np, npz["verts"]) and np.array_equal(faces_np, npz["faces"])
+        except FileNotFoundError:
+            return path
+        except Exception:                # geometry.py:529-532: an unreadable entry is replaced
+            return path
+        if same:
+            return path
+        i += 1                           # hash collision (geometry.py:470-473)
+
+
+def write_operators_npz(path, verts, faces, k_eig, operators, grad_ops):
+    """The ``np.savez`` of geometry.py:539-568 for a tuple returned by ``compute_operators``: fp32 data, int32 index
+    arrays, the sparse matrices as CSC.  L is exactly symmetric, so its CSC arrays are its CSR arrays; the CSC of
+    gradX / gradY is the transposed device CSR of ``grad_ops`` (``dn_csr_transpose``)."""
+    frames, mass, L, evals, evecs, gradX, gradY = operators
+    f32 = np.float32
+    np_ = lambda t: t.detach().cpu().numpy()
+    V = int(mass.shape[0])
+    Lc = L.coalesce()
+    rows = np_(Lc.indices()[0])
+    L_indptr = np.searchsorted(rows, np.arange(V + 1)).astype(np.int32)
+    g = grad_ops
+    _, rt, ct, vt = g.csr_t
+    vt = np_(vt[:2 * g.nnz]).reshape(-1, 2)
+    gx_ptr, gx_idx = np_(rt).astype(np.int32), np_(ct[:g.nnz]).astype(np.int32)
+    shape = np.array((V, V), dtype=np.int64)
+    np.savez(path, verts=_to_np(verts).astype(f32), frames=np_(frames).astype(f32), faces=_to_np(faces), k_eig=k_eig,
+             mass=np_(mass).astype(f32), L_data=np_(Lc.values()).astype(f32), L_indices=np_(Lc.indices()[1]).astype(np.int32),
+             L_indptr=L_indptr, L_shape=shape, evals=np_(evals).astype(f32), evecs=np_(evecs).astype(f32),
+             gradX_data=vt[:, 0].astype(f32), gradX_indices=gx_idx, gradX_indptr=gx_ptr, gradX_shape=shape,
+             gradY_data=vt[:, 1].astype(f32), gradY_indices=gx_idx, gradY_indptr=gx_ptr, gradY_shape=shape)
+
+
+def get_operators(verts, faces, k_eig=128, op_cache_dir=None, normals=None, overwrite_cache=False, device=None,
+                  compute_missing=False):
+    """``geometry.get_operators`` (geometry.py:426): same arguments, same file naming, same returned tuple.  ``device``
+    (extra) places the operators directly on a GPU; default = ``verts.device``.
+    On a cache miss (or with ``overwrite_cache``) this raises unless ``compute_missing=True``; then the operators are
+    built on the GPU by ``compute_operators`` and, with an ``op_cache_dir``, written to the bucket the reference would
+    write (``find_cache_bucket``), in its file format.  The computed tuple is returned; the next call is a hit."""
     verts_np = _to_np(verts)
     if np.isnan(verts_np).any():
         raise RuntimeError("tried to construct operators from NaN verts")
@@ -139,16 +186,170 @@ def get_operators(verts, faces, k_eig=128, op_cache_dir=None, normals=None, over
     if op_cache_dir is not None and not overwrite_cache:
         npz = find_cached_operators(verts, faces, k_eig, op_cache_dir)
     if npz is None:
-        raise NotImplementedError(
-            "no usable cache entry for this mesh in {!r}: operator construction is outside the CUDA hot path -- "
-            "populate the cache with the reference's get_operators()".format(op_cache_dir))
+        if not compute_missing:
+            raise NotImplementedError(
+                "no usable cache entry for this mesh in {!r}: populate the cache with the reference's get_operators(), "
+                "or pass compute_missing=True to build the operators on the GPU".format(op_cache_dir))
+        out, g = _compute_operators(verts, faces, k_eig, normals, device, None)
+        if op_cache_dir is not None:
+            os.makedirs(op_cache_dir, exist_ok=True)
+            write_operators_npz(find_cache_bucket(verts, faces, op_cache_dir), verts, faces, k_eig, out, g)
+        return out
     return load_operators_npz(npz, k_eig=k_eig, device=device, dtype=verts.dtype)
 
 
-def get_all_operators(verts_list, faces_list, k_eig, op_cache_dir=None, normals=None, device=None):
-    """geometry.py:395-424: seven parallel lists."""
-    outs = [get_operators(v, f, k_eig, op_cache_dir, device=device) for v, f in zip(verts_list, faces_list)]
+def get_all_operators(verts_list, faces_list, k_eig, op_cache_dir=None, normals=None, device=None,
+                      compute_missing=False):
+    """geometry.py:395-424: seven parallel lists; ``normals[i]`` goes with mesh i."""
+    outs = [get_operators(v, f, k_eig, op_cache_dir, normals=None if normals is None else normals[i], device=device,
+                          compute_missing=compute_missing)
+            for i, (v, f) in enumerate(zip(verts_list, faces_list))]
     return tuple([o[i] for o in outs] for i in range(7))
+
+
+# ------------------------------------------------------------------------------------------------
+# operator construction for triangle meshes (geometry.py:276-392) on the GPU
+# ------------------------------------------------------------------------------------------------
+EPS = 1e-8          # geometry.py:308: mass shift (times the mean) and eigenproblem shift
+
+
+def _vertex_frames(v64, f64, normals, dtype, verts):
+    """geometry.py:101-177 for meshes: (V,3,3) fp64 frames from dn_vertex_frames, with the reference's remedy for NaN
+    normals (geometry.py:128-141: wiggle the bad vertices with RandomState(777) and recompute; if still NaN, random
+    normals from the same seed).  Normals are rounded to ``dtype`` before the frames are built, as the reference
+    converts them (geometry.py:144)."""
+    lib = _lib_load()
+    V, F = int(v64.shape[0]), int(f64.shape[0])
+    dev = v64.device
+    frames = torch.empty(V, 3, 3, dtype=torch.float64, device=dev)
+    nbad = torch.zeros(1, dtype=torch.int32, device=dev)
+    if normals is None:
+        nrm = torch.empty(V, 3, dtype=torch.float64, device=dev)
+        ws = torch.empty(12 * F + 8 * V + 1024, dtype=torch.uint8, device=dev)
+        call = lambda v: _lib_check(lib.dn_vertex_frames(v.data_ptr(), f64.data_ptr(), F, V, None, nrm.data_ptr(),
+                                                         frames.data_ptr(), nbad.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                         ops._stream()), "dn_vertex_frames")
+        call(v64)
+        if int(nbad.item()) > 0:
+            verts_np = _to_np(verts)
+            bad = torch.isnan(nrm).any(dim=1, keepdim=True).cpu().numpy()
+            bbox = np.amax(verts_np, axis=0) - np.amin(verts_np, axis=0)
+            wiggle = (np.random.RandomState(seed=777).rand(*verts_np.shape) - 0.5) * (np.linalg.norm(bbox) * 1e-4)
+            call(torch.from_numpy(np.ascontiguousarray(verts_np + bad * wiggle, dtype=np.float64)).to(dev))
+            if int(nbad.item()) > 0:
+                bad = torch.isnan(nrm).any(dim=1).cpu().numpy()
+                rnd = (np.random.RandomState(seed=777).rand(*verts_np.shape) - 0.5)[bad, :]
+                rnd = rnd / np.linalg.norm(rnd, axis=-1)[:, None]
+                nrm[torch.from_numpy(bad).to(dev)] = torch.from_numpy(rnd).to(dev)
+        normals = nrm
+    n_in = normals.to(device=dev, dtype=dtype).to(torch.float64).contiguous()
+    _lib_check(lib.dn_vertex_frames(None, None, F, V, n_in.data_ptr(), None, frames.data_ptr(), nbad.data_ptr(), None,
+                                    0, ops._stream()), "dn_vertex_frames")
+    return frames
+
+
+def mesh_laplacian(v64, f64, eps=EPS):
+    """dn_mesh_laplacian: ``(rowptr, colidx, L_vals, mass, A_vals, A_diag, bound)`` on the device (fp64 values, int32
+    indices), the reference's cotan Laplacian and lumped mass (geometry.py:322-329) and the operator the eigensolver
+    runs on.  Raises the reference's RuntimeError on a NaN Laplacian or mass (geometry.py:326-329)."""
+    lib = _lib_load()
+    V, F = int(v64.shape[0]), int(f64.shape[0])
+    dev = v64.device
+    cap = max(6 * F + V, 1)
+    rowptr = torch.empty(V + 1, dtype=torch.int32, device=dev)
+    colidx = torch.empty(cap, dtype=torch.int32, device=dev)
+    lvals = torch.empty(cap, dtype=torch.float64, device=dev)
+    avals = torch.empty(cap, dtype=torch.float64, device=dev)
+    mass = torch.empty(V, dtype=torch.float64, device=dev)
+    adiag = torch.empty(V, dtype=torch.float64, device=dev)
+    bound = torch.empty(1, dtype=torch.float64, device=dev)
+    nan = torch.empty(2, dtype=torch.int32, device=dev)
+    ws = torch.empty(120 * F + 12 * V + 2048, dtype=torch.uint8, device=dev)
+    _lib_check(lib.dn_mesh_laplacian(v64.data_ptr(), f64.data_ptr(), F, V, eps, rowptr.data_ptr(), colidx.data_ptr(),
+                                     lvals.data_ptr(), mass.data_ptr(), avals.data_ptr(), adiag.data_ptr(),
+                                     bound.data_ptr(), nan.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()),
+               "dn_mesh_laplacian")
+    nan_l, nan_m = nan.tolist()
+    if nan_l:
+        raise RuntimeError("NaN Laplace matrix")
+    if nan_m:
+        raise RuntimeError("NaN mass matrix")
+    nnz = int(rowptr[-1].item())
+    return rowptr, colidx[:nnz], lvals[:nnz], mass, avals[:nnz], adiag, float(bound.item())
+
+
+def _lib_load():
+    from . import _lib
+    return _lib.load()
+
+
+def _lib_check(code, what):
+    from . import _lib
+    _lib.check(code, what)
+
+
+def compute_operators(verts, faces, k_eig, normals=None, device=None, stats=None):
+    """``geometry.compute_operators`` (geometry.py:276-392) for triangle meshes, on the GPU: returns
+    ``(frames, mass, L, evals, evecs, gradX, gradY)`` resident on ``device`` (default ``verts.device``), each in the
+    dtype of ``verts``; L, gradX and gradY are coalesced COO tensors, and (for fp32) gradX / gradY are registered
+    against their prepared CSR so the first forward does no conversion.
+
+    Frames, Laplacian, mass and the eigenpairs are computed in fp64 by the library's kernels (``eigen`` has the
+    solver: the k_eig lowest pairs of ``(L + 1e-8 I, M)``, the problem of the reference's ``eigsh(..., sigma=1e-8)``,
+    ascending, clipped at 0, sign-fixed so that each eigenvector's largest-magnitude entry is positive).  L is rounded
+    to fp32 on the way out as the reference's ``sparse_np_to_torch`` does.  gradX / gradY come from ``dn_build_grad``,
+    which is fp32: for fp64 ``verts`` they are still fp32-grade.  Deterministic: two calls give bitwise-equal results.
+
+    Raises RuntimeError for a CPU device or a NaN Laplacian / mass, NotImplementedError for a point cloud (empty
+    ``faces``), ValueError("failed to compute eigendecomp ...") if the eigensolver does not converge.  ``stats``
+    (dict, optional) receives per-stage times in ms and the solver's counters."""
+    return _compute_operators(verts, faces, k_eig, normals, device, stats)[0]
+
+
+def _compute_operators(verts, faces, k_eig, normals, device, stats):
+    """compute_operators, also returning the ``ops.GradOperators`` of (gradX, gradY)."""
+    from . import eigen
+    device = torch.device(device) if device is not None else verts.device
+    if device.type != "cuda":
+        raise RuntimeError("diffusion_net_b200 keeps operators on CUDA devices only (no CPU path); got {}".format(device))
+    if faces.numel() == 0:
+        raise NotImplementedError("point clouds need robust_laplacian.point_cloud_laplacian and a KNN graph; only "
+                                  "triangle meshes are supported")
+    dtype = verts.dtype
+    with torch.cuda.device(device):
+        ev = []
+        mark = lambda: ev.append(torch.cuda.Event(enable_timing=True)) or ev[-1].record()
+        mark()
+        v64 = torch.as_tensor(verts).detach().to(device=device, dtype=torch.float64).contiguous()
+        f64 = torch.as_tensor(faces).detach().to(device=device, dtype=torch.int64).reshape(-1, 3).contiguous()
+        V = int(v64.shape[0])
+        if int(f64.min()) < 0 or int(f64.max()) >= V:
+            raise ValueError("faces index vertices outside [0, {})".format(V))
+        frames = _vertex_frames(v64, f64, normals, dtype, verts)
+        mark()
+        rowptr, colidx, lvals, mass, avals, adiag, bound = mesh_laplacian(v64, f64)
+        mark()
+        op = eigen.LaplaceOperator(V, rowptr, colidx, avals, adiag, mass, bound)
+        est = {} if stats is not None else None
+        evals, evecs = eigen.lowest_eigenpairs(op, int(k_eig), stats=est)
+        mark()
+        rows = torch.repeat_interleave(torch.arange(V, device=device), (rowptr[1:] - rowptr[:-1]).long(),
+                                       output_size=int(colidx.numel()))
+        idx = torch.stack((rows, colidx.long()), 0)
+        g = build_grad_operators(v64.to(torch.float32), frames.to(torch.float32), idx)
+        mark()
+        if dtype == torch.float32:
+            gradX, gradY = g.to_sparse_coo()
+            ops.register_prepared(gradX, gradY, g)
+        else:
+            gradX, gradY = (t.to(dtype) for t in g.to_sparse_coo())
+        L = torch.sparse_coo_tensor(idx, lvals.to(torch.float32).to(dtype), (V, V), is_coalesced=True)
+        out = (frames.to(dtype), mass.to(dtype), L, evals.to(dtype), evecs.to(dtype), gradX, gradY)
+        if stats is not None:
+            torch.cuda.synchronize(device)
+            ms = [a.elapsed_time(b) for a, b in zip(ev[:-1], ev[1:])]
+            stats.update(frames_ms=ms[0], laplacian_ms=ms[1], eig_ms=ms[2], build_grad_ms=ms[3], **est)
+    return out, g
 
 
 # ------------------------------------------------------------------------------------------------

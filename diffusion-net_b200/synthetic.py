@@ -39,6 +39,65 @@ def torus_mesh(n, m, seed=0, jit=0.25, R=1.0, r=0.4):
     return torch.from_numpy(verts), torch.from_numpy(faces)
 
 
+def patch_mesh(n, m, seed=0, jit=0.25, height=0.15):
+    """n x m jittered open grid patch (a disk-like mesh with a boundary) over [0, 1] x [0, m/n], with a smooth height
+    field; vertex id = i*m + j; V = n*m, F = 2(n-1)(m-1)."""
+    rs = np.random.RandomState(seed)
+    ii, jj = np.meshgrid(np.arange(n), np.arange(m), indexing="ij")
+    h = 1.0 / (n - 1)
+    x = (ii + jit * (rs.rand(n, m) - 0.5) * (ii > 0) * (ii < n - 1)) * h
+    y = (jj + jit * (rs.rand(n, m) - 0.5) * (jj > 0) * (jj < m - 1)) * h
+    z = height * np.sin(2.1 * x + 0.3) * np.cos(3.3 * y - 0.2)
+    verts = np.stack((x, y, z), axis=-1).reshape(-1, 3).astype(np.float32)
+    a, b = ii[:-1, :-1], jj[:-1, :-1]
+    vid = lambda p, q: p * m + q
+    f1 = np.stack((vid(a, b), vid(a + 1, b), vid(a + 1, b + 1)), axis=-1).reshape(-1, 3)
+    f2 = np.stack((vid(a, b), vid(a + 1, b + 1), vid(a, b + 1)), axis=-1).reshape(-1, 3)
+    return torch.from_numpy(verts), torch.from_numpy(np.concatenate((f1, f2), 0).astype(np.int64))
+
+
+def icosphere_mesh(subdiv, seed=0, jit=0.1, bump=0.08):
+    """Genus-0 test mesh: a subdivided icosahedron (V = 10 * 4**subdiv + 2) whose vertices are jittered tangentially
+    (by ``jit`` of the edge length) and pushed radially by a few smooth bumps of relative height ``bump``.  A sphere's
+    Laplace-Beltrami eigenvalues come in clusters of 2l + 1; the perturbation splits each only slightly, so the mesh
+    has wide near-degenerate clusters."""
+    t = (1.0 + 5 ** 0.5) / 2.0
+    v = [(-1, t, 0), (1, t, 0), (-1, -t, 0), (1, -t, 0), (0, -1, t), (0, 1, t), (0, -1, -t), (0, 1, -t),
+         (t, 0, -1), (t, 0, 1), (-t, 0, -1), (-t, 0, 1)]
+    f = [(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2), (10, 7, 6),
+         (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11), (6, 2, 10),
+         (8, 6, 7), (9, 8, 1)]
+    verts = [np.array(p, dtype=np.float64) / np.linalg.norm(p) for p in v]
+    faces = f
+    for _ in range(subdiv):
+        mid = {}
+
+        def midpoint(a, b):
+            key = (min(a, b), max(a, b))
+            if key not in mid:
+                p = verts[a] + verts[b]
+                verts.append(p / np.linalg.norm(p))
+                mid[key] = len(verts) - 1
+            return mid[key]
+        nf = []
+        for a, b, c in faces:
+            ab, bc, ca = midpoint(a, b), midpoint(b, c), midpoint(c, a)
+            nf += [(a, ab, ca), (b, bc, ab), (c, ca, bc), (ab, bc, ca)]
+        faces = nf
+    P = np.array(verts)
+    rs = np.random.RandomState(seed)
+    h = 1.1 / (2 ** subdiv)                                       # about one edge length on the unit sphere
+    d = rs.randn(*P.shape) * jit * h
+    d -= (d * P).sum(1, keepdims=True) * P                        # tangential jitter
+    P = P + d
+    P /= np.linalg.norm(P, axis=1, keepdims=True)
+    centres = rs.randn(5, 3)
+    centres /= np.linalg.norm(centres, axis=1, keepdims=True)
+    r = 1.0 + bump * np.exp(-8.0 * (1.0 - P @ centres.T)).sum(1)
+    P = P * r[:, None]
+    return torch.from_numpy(P.astype(np.float32)), torch.from_numpy(np.array(faces, dtype=np.int64))
+
+
 def torus_pattern(n, m):
     """(rows, cols) int64, row-sorted then col-sorted: self + 6 torus-grid
     neighbours, the pattern the cotan Laplacian / gradient matrices share."""

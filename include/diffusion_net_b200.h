@@ -234,6 +234,50 @@ int dn_build_grad(const float* verts, const float* frames, const float* edge_tan
                   int64_t V, int32_t* rowptr_out, int32_t* colidx_out, float* vals_out, void* workspace,
                   int64_t ws_bytes, dn_stream_t stream);
 
+/* ---- operator construction for triangle meshes (geometry.py:276-392 compute_operators) --------------------------
+ * The calls below are fp64 (double) throughout; `faces` is (F, 3) int64 with every index in [0, V).  They are the
+ * steps of geometry.compute_operators: Laplacian + mass, frames, then the eigensolver's kernels, then dn_build_grad
+ * on the Laplacian's pattern.  None synchronises. */
+
+/* geometry.py:322-329 for meshes: the cotan Laplacian (cot = u.v / (|u x v| + 1e-10) per face corner) as int32 CSR with
+ * sorted columns, the pattern of the reference's `L` (the diagonal of every referenced vertex and both directions of
+ * every face edge, duplicates summed, explicit zeros kept; exactly symmetric), and the lumped mass (barycentric areas
+ * + eps * mean).  Capacity of colidx_out / L_vals_out / A_vals_out: 6 F + V; the count is rowptr_out[V].
+ * A_vals_out (optional, same pattern) and A_diag_out (optional, V) describe A = M^-1/2 (L + eps I) M^-1/2 =
+ * A_vals + diag(A_diag); bound_out (1) receives Gershgorin's upper bound on A's spectrum; nan_out (2) the number of
+ * rows of L holding a NaN and of NaN mass entries.  Deterministic.  workspace: 120 F + 12 V + 2048 bytes. */
+int dn_mesh_laplacian(const double* verts, const int64_t* faces, int64_t F, int64_t V, double eps, int32_t* rowptr_out,
+                      int32_t* colidx_out, double* L_vals_out, double* mass_out, double* A_vals_out, double* A_diag_out,
+                      double* bound_out, int32_t* nan_out, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
+/* geometry.py:101-177 for meshes.  normals_in NULL: unit face normals (divide-eps 1e-6) summed per vertex in face order
+ * and normalised into normals_out (V, 3); a vertex whose normal is NaN (no face with a nonzero normal) is counted in
+ * n_bad_out (1) -- the caller applies the reference's remedy and calls again.  normals_in given: used as they are.
+ * frames_out (V, 3, 3): rows basisX, basisY, normal.  workspace (only without normals_in): 12 F + 8 V + 1024 bytes. */
+int dn_vertex_frames(const double* verts, const int64_t* faces, int64_t F, int64_t V, const double* normals_in,
+                     double* normals_out, double* frames_out, int32_t* n_bad_out, void* workspace, int64_t ws_bytes,
+                     dn_stream_t stream);
+
+/* Eigensolver kernels on row-major V x n fp64 blocks with leading dimension ld (>= n).
+ * dn_eig_filter: one step of the scaled Chebyshev recurrence, Y_out = alpha (A Y) + beta Y + gamma Y_prev with A from
+ *   dn_mesh_laplacian (Y_prev may be NULL).  Y_out must not alias Y or Y_prev.
+ * dn_eig_gram: out (m x n, dense) = X^T Y; split-V partial sums in a fixed order.  workspace: 512 m n bytes.
+ * dn_eig_rotate: Z = beta Z + X C, X (V x kd), C (kd x n, ldc); Z must not alias X.  beta = 0 does not read Z.
+ * dn_eig_residual_norms: out[c] = || W[:, c] - theta[c] Q[:, c] ||_2.  workspace: 512 n bytes.
+ * dn_eig_finalize: out (V x k, dense) = s_i M^-1/2 Y[:, cols[i]], s_i = +-1 making the largest-magnitude entry of each
+ *   column positive (lowest row on ties).  workspace: 8 k bytes. */
+int dn_eig_filter(const int32_t* rowptr, const int32_t* colidx, const double* A_vals, const double* A_diag, int64_t V,
+                  int n, const double* Y, const double* Y_prev, int64_t ld, double alpha, double beta, double gamma,
+                  double* Y_out, dn_stream_t stream);
+int dn_eig_gram(const double* X, int64_t ldx, const double* Y, int64_t ldy, int64_t V, int m, int n, double* out,
+                void* workspace, int64_t ws_bytes, dn_stream_t stream);
+int dn_eig_rotate(const double* X, int64_t ldx, const double* C, int64_t ldc, int64_t V, int kd, int n, double beta,
+                  double* Z, int64_t ldz, dn_stream_t stream);
+int dn_eig_residual_norms(const double* W, int64_t ldw, const double* Q, int64_t ldq, const double* theta, int64_t V,
+                          int n, double* out, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+int dn_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass, int64_t V, double* out,
+                    void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
 /* ---- batches of independent meshes in one launch sequence (BASELINE config 4; SURVEY.md 8e) -------------------
  * The reference loops over the batch dimension with one set of operators per mesh (layers.py:217-222; a DataLoader
  * of batch_size None in every experiment).  Here a batch is ONE vertex range: mesh b occupies rows

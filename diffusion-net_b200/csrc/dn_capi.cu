@@ -409,6 +409,41 @@ int dn_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, co
   return launch_eig_finalize(Y, ldy, cols, k, mass, V, out, (double*)workspace, (cudaStream_t)stream);
 }
 
+int64_t dn_implicit_diffusion_workspace_bytes(int64_t V, int C) {
+  if (V < 0 || C <= 0) return -1;
+  return implicit_ws_bytes(V, C);
+}
+
+static int implicit_check(const dn_csr* L, const float* mass, const float* time, const float* rhs, int64_t V, int C,
+                          double rtol, int max_iter, const float* out, const double* status, const void* workspace,
+                          int64_t ws_bytes) {
+  if (!L || V < 0 || C <= 0 || L->nnz < 0 || !(rtol >= 0.0) || max_iter < 1 || !time || !status ||
+      (V > 0 && (!L->rowptr || !mass || !rhs || !out || (L->nnz > 0 && (!L->colidx || !L->vals)))))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (C > 256 || L->nnz >= (1ll << 31) || V >= (1ll << 31) - 1) return DN_ERR_UNSUPPORTED;
+  if (!workspace || ws_bytes < implicit_ws_bytes(V, C)) return DN_ERR_WORKSPACE;
+  return DN_OK;
+}
+
+int dn_implicit_diffusion_fwd(const dn_csr* L, const float* x, const float* mass, float* time, int64_t V, int C,
+                              double rtol, int max_iter, float* x_diffuse, double* status, void* workspace,
+                              int64_t ws_bytes, dn_stream_t stream) {
+  const int rc = implicit_check(L, mass, time, x, V, C, rtol, max_iter, x_diffuse, status, workspace, ws_bytes);
+  if (rc != DN_OK) return rc;
+  return launch_implicit_diffusion(L, mass, time, x, nullptr, V, C, rtol, max_iter, 0, x_diffuse, nullptr, status,
+                                   workspace, (cudaStream_t)stream);
+}
+
+int dn_implicit_diffusion_bwd(const dn_csr* L, const float* grad_out, const float* mass, const float* time,
+                              const float* x_diffuse, int64_t V, int C, double rtol, int max_iter, float* grad_x,
+                              float* grad_time, double* status, void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  const int rc = implicit_check(L, mass, time, grad_out, V, C, rtol, max_iter, grad_x, status, workspace, ws_bytes);
+  if (rc != DN_OK) return rc;
+  if (!grad_time || (V > 0 && !x_diffuse)) return DN_ERR_INVALID_ARGUMENT;
+  return launch_implicit_diffusion(L, mass, const_cast<float*>(time), grad_out, x_diffuse, V, C, rtol, max_iter, 1,
+                                   grad_x, grad_time, status, workspace, (cudaStream_t)stream);
+}
+
 int dn_compute_hks(const float* evals, const float* evecs, const float* scales, int64_t V, int K, int S, float* out,
                    dn_stream_t stream) {
   if (V < 0 || K <= 0 || S < 0 || ((V > 0 && S > 0) && (!evals || !evecs || !scales || !out)))

@@ -123,6 +123,11 @@ int launch_eig_residual_norms(const double* W, int64_t ldw, const double* Q, int
                               int n, double* out, double* ws, cudaStream_t st);
 int launch_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass, int64_t V,
                         double* out, double* sign_ws, cudaStream_t st);
+// implicit diffusion (dn_implicit.cu): one cooperative block-PCG solve of (M + diag(t) (x) L) Y = b, fp64 state
+int64_t implicit_ws_bytes(int64_t V, int C);
+int launch_implicit_diffusion(const dn_csr* L, const float* mass, float* time, const float* rhs, const float* y,
+                              int64_t V, int C, double rtol, int max_iter, int backward, float* out, float* grad_time,
+                              double* status, void* ws, cudaStream_t st);
 int launch_grad_spmm_pair(const dn_csr* g, const float* x, int64_t V, int C, float* out_vc2, cudaStream_t st);
 // R-order fused features: feat = tanh(gX*Bre + gY*Bim) from gathers of xd, P, Q (pq = [P|Q], ld 2C or C).
 int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int rotations, int64_t V, int C,

@@ -16,8 +16,17 @@ import torch
 from . import ops
 
 
+def _refuse_implicit(net):
+    """Implicit diffusion reads its convergence status on the host after every solve: it cannot be captured."""
+    from .layers import LearnedTimeDiffusion
+    if any(isinstance(m, LearnedTimeDiffusion) and m.method != 'spectral' for m in net.modules()):
+        raise NotImplementedError("CUDA-graph capture supports spectral diffusion only; this net uses "
+                                  "diffusion_method='implicit_dense' (run it eagerly)")
+
+
 class GraphedNet:
     def __init__(self, net, n_streams=4):
+        _refuse_implicit(net)
         self.net = net
         self.device = next(net.parameters()).device
         self.streams = [torch.cuda.Stream(device=self.device) for _ in range(n_streams)]
@@ -68,6 +77,7 @@ class GraphedBatch:
     views of the static output buffer (overwritten by the next call).  Inference only."""
 
     def __init__(self, net, batch):
+        _refuse_implicit(net)
         self.net, self.batch = net, batch
         self.device = batch.device
         ops.pin_workspaces = True
@@ -109,6 +119,7 @@ class GraphedTrainStep:
     plumbing, see layers.MiniMLP)."""
 
     def __init__(self, net, loss_fn, inputs, warmup=3):
+        _refuse_implicit(net)
         self.net, self.loss_fn, self.inputs = net, loss_fn, inputs
         dev = next(net.parameters()).device
         ops.pin_workspaces = True

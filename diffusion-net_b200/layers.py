@@ -16,8 +16,10 @@ from . import ops
 class LearnedTimeDiffusion(nn.Module):
     """Per-channel learned-time heat diffusion (reference layers.py:17-90).
 
-    ``spectral``: ``evecs @ (exp(-evals t^T) * (evecs^T (mass * x)))``.  ``implicit_dense`` (a dense
-    O(C V^3) Cholesky solve, toy sizes only) is outside the accelerated path and not provided."""
+    ``spectral``: ``evecs @ (exp(-evals t^T) * (evecs^T (mass * x)))``.  ``implicit_dense``: per channel
+    ``(M + t_c L)^-1 M x_c``, which the reference forms as a dense (B, C, V, V) Cholesky; here a sparse fp64 block
+    conjugate-gradient solve on L's CSR (ops.ImplicitDiffusionFn), exact at any size and needing no eigenbasis
+    (evals / evecs may be None).  L: sparse (V, V) for 2-D x, (B, V, V) for 3-D x, or a list of per-mesh Laplacians."""
 
     def __init__(self, C_inout, method='spectral'):
         super(LearnedTimeDiffusion, self).__init__()
@@ -39,8 +41,14 @@ class LearnedTimeDiffusion(nn.Module):
             return torch.stack([ops.DiffusionFn.apply(x[b], self.diffusion_time, mass[b], evals[b], evecs[b])
                                 for b in range(x.shape[0])], dim=0)
         elif self.method == 'implicit_dense':
-            raise NotImplementedError("diffusion_method='implicit_dense' is outside the CUDA hot path "
-                                      "(dense Cholesky per channel; use the reference for toy sizes)")
+            ops._require_cuda(x, mass, self.diffusion_time)
+            # the clamp of layers.py:48-49 happens inside the kernel, in place on the Parameter's storage
+            if x.dim() == 2:
+                lap = ops.prepare_laplacians(L, 1)[0]
+                return ops.ImplicitDiffusionFn.apply(x, self.diffusion_time, mass, lap)
+            laps = ops.prepare_laplacians(L, x.shape[0])
+            return torch.stack([ops.ImplicitDiffusionFn.apply(x[b], self.diffusion_time, mass[b], laps[b])
+                                for b in range(x.shape[0])], dim=0)
         else:
             raise ValueError("unrecognized method")
 
@@ -151,7 +159,7 @@ class DiffusionNetBlock(nn.Module):
             self.MLP_C += self.C_width
         self.mlp = MiniMLP([self.MLP_C] + self.mlp_hidden_dims + [self.C_width], dropout=self.dropout)
 
-    def _forward_mesh(self, x_in, mass, evals, evecs, gops, fused, head=None):
+    def _forward_mesh(self, x_in, mass, evals, evecs, gops, fused, head=None, lap=None):
         A_re = A_im = None
         if self.with_gradient_features:
             A_re, A_im = self.gradient_features.weights()
@@ -162,7 +170,7 @@ class DiffusionNetBlock(nn.Module):
                                          self.with_gradient_features, head=head)
         if head is not None:
             raise ops.HeadNotFused()
-        x_diffuse = self.diffusion(x_in, None, mass, evals, evecs)
+        x_diffuse = self.diffusion(x_in, lap, mass, evals, evecs)
         srcs = [x_in, x_diffuse]
         if self.with_gradient_features:
             srcs.append(ops.GradFeaturesFn.apply(x_diffuse, A_re, A_im, gops))
@@ -188,8 +196,12 @@ class DiffusionNetBlock(nn.Module):
                 "Tensor has wrong shape = {}. Last dim shape should have number of channels = {}".format(
                     x_in.shape, self.C_width))
         ops._require_cuda(x_in, mass, evals, evecs)
-        if self.diffusion.method != 'spectral':
+        implicit = self.diffusion.method == 'implicit_dense'
+        if self.diffusion.method not in ('spectral', 'implicit_dense'):
             self.diffusion(x_in, L, mass, evals, evecs)   # raises like the reference would route
+        # implicit: the eigenbasis is not used (k_eig = 0 gives None or empty evals / evecs); L's CSR, once per mesh
+        laps = ops.prepare_laplacians(L, B) if implicit else [None] * B
+        pick = lambda t, b: None if t is None else t[b]
         gops = [None] * B
         if self.with_gradient_features:
             if isinstance(gradX, (list, tuple)):           # pre-split per-mesh operators
@@ -202,10 +214,12 @@ class DiffusionNetBlock(nn.Module):
                 gops = ops.prepare_operators_batched(gradX, gradY)
         params_need_grad = any(p.requires_grad for p in self.parameters())
         needs_grad = torch.is_grad_enabled() and (x_in.requires_grad or params_need_grad)
-        fused = (not needs_grad) and self.mlp._fused_ok and not (self.training and self.dropout)
+        # the fused inference block is spectral: an implicit block runs the composed path (solve, features, MiniMLP)
+        fused = (not implicit) and (not needs_grad) and self.mlp._fused_ok and not (self.training and self.dropout)
         if head is not None and not fused:
             raise ops.HeadNotFused()
-        outs = [self._forward_mesh(x_in[b], mass[b], evals[b], evecs[b], gops[b], fused, head) for b in range(B)]
+        outs = [self._forward_mesh(x_in[b], mass[b], pick(evals, b), pick(evecs, b), gops[b], fused, head, laps[b])
+                for b in range(B)]
         return torch.stack(outs, dim=0)
 
 
@@ -339,6 +353,7 @@ class DiffusionNet(nn.Module):
             if evecs != None: evecs = evecs.unsqueeze(0)
             # sparse operators stay un-batched: wrapping them in 1-element lists keeps the user's
             # tensor objects (and the CSR prepared from them) alive across blocks and epochs
+            if L is not None: L = [L]
             if gradX != None: gradX = [gradX]
             if gradY != None: gradY = [gradY]
             if edges != None: edges = edges.unsqueeze(0)

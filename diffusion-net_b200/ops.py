@@ -341,6 +341,69 @@ def prepare_operators_batched(gradX, gradY):
     return ops
 
 
+class LaplacianCSR:
+    """The cotan Laplacian of one mesh as the dn_csr the implicit diffusion solves with (built once per mesh)."""
+
+    def __init__(self, L):
+        _require_cuda(L)
+        if not L.is_sparse or L.dim() != 2 or L.shape[0] != L.shape[1]:
+            raise ValueError("L must be a square sparse COO matrix (V, V), as get_operators returns it")
+        Lc = L if L.is_coalesced() else L.coalesce()
+        self.V, self.device = int(Lc.shape[0]), Lc.device
+        idx = Lc.indices()
+        self.nnz = int(idx.shape[1])
+        vals = _f32c(Lc.values())
+        lib = _lib.load()
+        rowptr = torch.empty(self.V + 1, dtype=torch.int32, device=self.device)
+        colidx = torch.empty(max(self.nnz, 1), dtype=torch.int32, device=self.device)
+        cv = torch.empty(2 * max(self.nnz, 1), dtype=torch.float32, device=self.device)
+        rows, cols = idx[0].contiguous(), idx[1].contiguous()
+        with _on(vals):
+            _lib.check(lib.dn_csr_from_coo(rows.data_ptr(), cols.data_ptr(), vals.data_ptr(), None, self.nnz, self.V,
+                                           rowptr.data_ptr(), colidx.data_ptr(), cv.data_ptr(), _stream()),
+                       "dn_csr_from_coo")
+        self.csr = (_lib.dn_csr(rowptr.data_ptr(), colidx.data_ptr(), cv.data_ptr(), self.nnz), rowptr, colidx, cv)
+
+
+def prepare_laplacian(L):
+    """Memoised like ``prepare_operators``: the CSR of the user's sparse ``L`` (coalesced COO (V, V) as get_operators
+    returns it, or a (B, V, V) stack, giving a list) is built once per tensor and reused across blocks and epochs while
+    the tensor lives and is not modified in place."""
+    key = (id(L), "laplacian")
+    hit = _prep_cache.get(key)
+    if hit is not None:
+        rl, _, ver, lap = hit
+        if rl() is L and ver == (L._version, L._version):
+            return lap
+    if isinstance(L, torch.Tensor) and L.is_sparse and L.dim() == 3:
+        lap = [LaplacianCSR(L[b]) for b in range(L.shape[0])]
+    else:
+        lap = LaplacianCSR(L)
+    _sweep_prep_cache()
+    _prep_cache[key] = (weakref.ref(L), weakref.ref(L), (L._version, L._version), lap)
+    _evict_when_dead(key, L)
+    return lap
+
+
+def prepare_laplacians(L, B):
+    """Per-mesh LaplacianCSRs for a batch of B meshes from what a caller may pass as ``L``: a (B, V, V) sparse stack, a
+    (V, V) sparse matrix (B = 1), a list of those (``DiffusionNet.forward`` wraps a 2-D call's L this way), or already
+    prepared LaplacianCSRs."""
+    if L is None:
+        raise ValueError("diffusion_method='implicit_dense' needs the Laplacian L")
+    if isinstance(L, (list, tuple)):
+        out = [l if isinstance(l, LaplacianCSR) else prepare_laplacian(l) for l in L]
+    elif isinstance(L, LaplacianCSR):
+        out = [L]
+    else:
+        _require_cuda(L)
+        out = prepare_laplacian(L)
+        out = out if isinstance(out, list) else [out]
+    if len(out) != B:
+        raise ValueError("got {} Laplacians for a batch of {} meshes".format(len(out), B))
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # thin wrappers (no autograd)
 # ------------------------------------------------------------------------------------------------
@@ -593,6 +656,66 @@ class DiffusionFn(torch.autograd.Function):
                                                      gx.data_ptr(), gt.data_ptr(), ws.data_ptr(), ws.numel(),
                                                      _engine, _stream()), "dn_learned_time_diffusion_bwd")
         return gx, gt, None, None, None
+
+
+IMPLICIT_RTOL = 1e-8        # stop column c once ||r_c|| <= IMPLICIT_RTOL ||b_c|| (fp64 residual)
+IMPLICIT_MAX_ITER = 20000   # a 200k-vertex mesh at t ~ 1 needs a few thousand iterations
+implicit_last_status = None  # host copy of the last solve's status (iterations per column, residuals; see the header)
+
+
+def _implicit_call(what, fn, V, Cc, device, args, outs):
+    """Run one dn_implicit_diffusion_* call (``args`` before rtol / max_iter, ``outs`` after) and raise if a column did
+    not converge: one host read of the device status per solve."""
+    status = torch.empty(2 + 2 * Cc, dtype=torch.float64, device=device)
+    ws = torch.empty(int(_lib.load().dn_implicit_diffusion_workspace_bytes(V, Cc)), dtype=torch.uint8, device=device)
+    _lib.check(fn(*args, float(IMPLICIT_RTOL), int(IMPLICIT_MAX_ITER), *outs, status.data_ptr(), ws.data_ptr(),
+                  ws.numel(), _stream()), what)
+    global implicit_last_status
+    st = implicit_last_status = status.cpu()
+    if st[0] > 0:
+        raise RuntimeError("diffusion_net_b200 {}: {} of {} columns did not converge in {} iterations (worst relative "
+                           "residual {:.3e}, tolerance {:.1e})".format(what, int(st[0]), Cc, IMPLICIT_MAX_ITER,
+                                                                      float(st[2 + Cc:].max()), IMPLICIT_RTOL))
+    return st
+
+
+class ImplicitDiffusionFn(torch.autograd.Function):
+    """layers.py:69-84 implicit LearnedTimeDiffusion on one mesh: y_c = (M + t_c L)^-1 M x_c by a fp64 block
+    Jacobi-PCG (dn_implicit_diffusion_fwd / _bwd).  ``lap`` is the mesh's LaplacianCSR (prepare_laplacian).  The kernel
+    clamps ``time`` in place, as the reference does on the Parameter (layers.py:48-49)."""
+
+    @staticmethod
+    @_device_guard
+    def forward(ctx, x, time, mass, lap):
+        lib = _lib.load()
+        x, mass = _f32c(x), _f32c(mass)
+        if time.dtype != torch.float32 or not time.is_contiguous():
+            raise RuntimeError("diffusion_time must be a contiguous float32 tensor")
+        V, Cc = x.shape
+        if lap.V != V or mass.shape != (V,) or time.shape != (Cc,):
+            raise ValueError("implicit diffusion: x {}, mass {}, time {} and L ({}x{}) do not agree".format(
+                tuple(x.shape), tuple(mass.shape), tuple(time.shape), lap.V, lap.V))
+        y = torch.empty_like(x)
+        _implicit_call("dn_implicit_diffusion_fwd", lib.dn_implicit_diffusion_fwd, V, Cc, x.device,
+                       (C.byref(lap.csr[0]), x.data_ptr(), mass.data_ptr(), time.data_ptr(), V, Cc),
+                       (y.data_ptr(),))
+        ctx.lap = lap
+        ctx.save_for_backward(mass, time.detach().clone(), y)
+        return y
+
+    @staticmethod
+    @_device_guard
+    def backward(ctx, g):
+        lib = _lib.load()
+        mass, time, y = ctx.saved_tensors
+        g = _f32c(g)
+        V, Cc = g.shape
+        gx = torch.empty_like(g)
+        gt = torch.zeros_like(time)
+        _implicit_call("dn_implicit_diffusion_bwd", lib.dn_implicit_diffusion_bwd, V, Cc, g.device,
+                       (C.byref(ctx.lap.csr[0]), g.data_ptr(), mass.data_ptr(), time.data_ptr(), y.data_ptr(), V, Cc),
+                       (gx.data_ptr(), gt.data_ptr()))
+        return gx, gt, None, None
 
 
 def batched_diffusion_workspace_extra(n_meshes, K, C_):

@@ -278,6 +278,33 @@ int dn_eig_residual_norms(const double* W, int64_t ldw, const double* Q, int64_t
 int dn_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass, int64_t V, double* out,
                     void* workspace, int64_t ws_bytes, dn_stream_t stream);
 
+/* ---- implicit diffusion (layers.py:69-84, method='implicit_dense') -------------------------------------------------
+ * Per channel c: x_diffuse[:, c] = (M + t_c L)^-1 M x[:, c], solved at any size by a Jacobi-preconditioned block
+ * conjugate gradient over the C columns (preconditioner m_v + t_c L_vv), with each column's own step lengths, instead of
+ * the reference's dense (B, C, V, V) Cholesky.  `L` is the cotan Laplacian as a dn_csr built by dn_csr_from_coo with
+ * vy = NULL (the gy half is ignored); it is used as given (symmetric positive semi-definite, as get_operators returns
+ * it) and promoted to fp64 like `mass`.  The solver state and every reduction are fp64 SIMT on every device: there is
+ * no `engine` argument.  One cooperative launch per call; reductions run in a fixed order without atomics, so results
+ * are bitwise reproducible on a given device.  C <= 256 (DN_ERR_UNSUPPORTED above).
+ *
+ * Convergence is decided on the device, per column: column c stops (its solution is final) once
+ * ||r_c||_2 <= rtol ||b_c||_2 (b = M x forward, b = grad_out backward).  `status` (device, 2 + 2C doubles) receives
+ * [0] the number of columns that did not converge within max_iter iterations, [1] the largest iteration count,
+ * [2 + c] the iterations of column c, [2 + C + c] its final ||r_c|| / ||b_c|| (0 when b_c = 0).  When [0] > 0 the
+ * outputs are not written (grad_time is not accumulated); the caller reads `status` to find out.
+ *   fwd: time (C) is clamped in place (layers.py:48-49) whether or not the solve converges, as the reference clamps
+ *        before solving.
+ *   bwd: with A_c = M + t_c L and w_c = A_c^-1 grad_out[:, c]: grad_x = M w, grad_time[c] += -sum_v w[v][c] (L x_diffuse)[v][c]
+ *        (ACCUMULATED, fixed order).  `time` is the clamped time the forward left; `x_diffuse` the forward's output.
+ * Workspace: dn_implicit_diffusion_workspace_bytes(V, C) (about 32 V C bytes). */
+int64_t dn_implicit_diffusion_workspace_bytes(int64_t V, int C);
+int dn_implicit_diffusion_fwd(const dn_csr* L, const float* x, const float* mass, float* time, int64_t V, int C,
+                              double rtol, int max_iter, float* x_diffuse, double* status, void* workspace,
+                              int64_t ws_bytes, dn_stream_t stream);
+int dn_implicit_diffusion_bwd(const dn_csr* L, const float* grad_out, const float* mass, const float* time,
+                              const float* x_diffuse, int64_t V, int C, double rtol, int max_iter, float* grad_x,
+                              float* grad_time, double* status, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
 /* ---- batches of independent meshes in one launch sequence (BASELINE config 4; SURVEY.md 8e) -------------------
  * The reference loops over the batch dimension with one set of operators per mesh (layers.py:217-222; a DataLoader
  * of batch_size None in every experiment).  Here a batch is ONE vertex range: mesh b occupies rows

@@ -751,7 +751,7 @@ int dn_mini_mlp_bwd(const float* grad_out, const float* const* src_host, const i
       }
     }
     if (grad_bias_host && grad_bias_host[l])
-      if ((rc = simt_colsum(dz, nout, nout, V, grad_bias_host[l], 1, st))) return rc;
+      if ((rc = simt_colsum(dz, nout, nout, V, grad_bias_host[l], 1, part, kPartialFloats / 2, st))) return rc;
     // input gradient:  dz_{l-1} = (dz_l W_l) * 1[h_{l-1} > 0] (* dropout mask)
     DnRowsSrc s = one_src(dz, nout, nout);
     if (l > 0) {

@@ -84,7 +84,10 @@ int simt_atb(const float* A, int64_t lda, int I, const float* B, int64_t ldb, in
              cudaStream_t st);
 int simt_atb_partial_st(const float* A, int64_t lda, int I, const float* B, int64_t ldb, int J, const float* scale,
                         int64_t V, float* ws, int64_t ws_floats, int* P_out, cudaStream_t st);
-int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int accumulate, cudaStream_t st);
+// out[n] (+)= sum_v A[v][n] in a fixed order (bias gradients): one partial row per row slice in ws, then the slices
+// summed in slice order.  Deterministic: no atomics.
+int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int accumulate, float* ws,
+                int64_t ws_floats, cudaStream_t st);
 
 // ---- shared small kernels (dn_simt.cu) ----
 // S[k][c] = exp(-evals[k]*max(t[c],1e-8)) * sum_p partial[p][k][c]; optionally writes the raw sum

@@ -241,24 +241,24 @@ __global__ void reduce_partials_kernel(const float* __restrict__ partial, int P,
   out[idx] = s;
 }
 
-__global__ void colsum_kernel(const float* __restrict__ A, int64_t lda, int N, int64_t V, float* __restrict__ out) {
-  // block (32, 8): 256 rows per block, 32 columns
+// partial[p][n] = sum over the rows of slice p of A[v][n].  Block (32, 8): 32 columns x 8 row lanes, combined in a
+// fixed order, so the sum does not depend on scheduling.
+__global__ void colsum_partial_kernel(const float* __restrict__ A, int64_t lda, int N, int64_t V,
+                                      int64_t rows_per_split, float* __restrict__ partial) {
   __shared__ float red[8][33];
   const int n = blockIdx.y * 32 + threadIdx.x;
-  const int64_t v0 = (int64_t)blockIdx.x * 256;
+  const int64_t vbeg = (int64_t)blockIdx.x * rows_per_split;
+  const int64_t vend = min(V, vbeg + rows_per_split);
   float s = 0.f;
   if (n < N)
-    for (int r = threadIdx.y; r < 256; r += 8) {
-      const int64_t v = v0 + r;
-      if (v < V) s += __ldg(A + v * lda + n);
-    }
+    for (int64_t v = vbeg + threadIdx.y; v < vend; v += 8) s += __ldg(A + v * lda + n);
   red[threadIdx.y][threadIdx.x] = s;
   __syncthreads();
   if (threadIdx.y == 0 && n < N) {
     float tot = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) tot += red[i][threadIdx.x];
-    atomicAdd(out + n, tot);
+    partial[(int64_t)blockIdx.x * N + n] = tot;
   }
 }
 
@@ -841,13 +841,24 @@ int simt_atb(const float* A, int64_t lda, int I, const float* B, int64_t ldb, in
   return DN_OK;
 }
 
-int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int accumulate, cudaStream_t st) {
-  if (!accumulate) DN_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * N, st));
-  if (V <= 0) return DN_OK;
-  dim3 grid((unsigned)((V + 255) / 256), (unsigned)((N + 31) / 32));
-  colsum_kernel<<<grid, dim3(32, 8), 0, st>>>(A, lda, N, V, out);
+int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int accumulate, float* ws,
+                int64_t ws_floats, cudaStream_t st) {
+  if (V <= 0) {
+    if (!accumulate) DN_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * N, st));
+    return DN_OK;
+  }
+  // slices of >= 2048 rows, at most 4 CTAs per SM over the column tiles and never more than ws holds
+  const int tiles = (N + 31) / 32;
+  int P = (int)((V + 2047) / 2048);
+  const int maxP = (4 * dn_sm_count()) / tiles > 1 ? (4 * dn_sm_count()) / tiles : 1;
+  if (P > maxP) P = maxP;
+  while ((int64_t)P * N > ws_floats && P > 1) --P;
+  if ((int64_t)P * N > ws_floats) return DN_ERR_WORKSPACE;
+  const int64_t rps = (V + P - 1) / P;
+  P = (int)((V + rps - 1) / rps);
+  colsum_partial_kernel<<<dim3(P, tiles), dim3(32, 8), 0, st>>>(A, lda, N, V, rps, ws);
   DN_LAUNCH_CHECK();
-  return DN_OK;
+  return launch_reduce_partials_ld(ws, P, 1, N, out, N, accumulate, st);
 }
 
 int launch_spectral_scale(const float* partial, int P, const float* evals, float* time, int K, int C,

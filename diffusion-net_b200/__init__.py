@@ -7,9 +7,11 @@ the dense contractions; ``_lib.build`` compiles the in-tree C-ABI library.
 """
 __version__ = "0.1.0"
 
-from . import _lib, ops, geometry, layers, synthetic, streaming, dist, graphs, batch  # noqa: F401,E402
+from . import _lib, ops, geometry, layers, synthetic, streaming, dist, graphs, batch, fmaps  # noqa: F401,E402
 from .layers import (DiffusionNet, DiffusionNetBlock, LearnedTimeDiffusion,  # noqa: F401,E402
                      SpatialGradientFeatures, MiniMLP)
+from .fmaps import (FunctionalMapCorrespondenceWithDiffusionNetFeatures, compute_correspondence,  # noqa: F401,E402
+                    pointwise_map)
 from .geometry import to_basis, from_basis  # noqa: F401,E402
 from .ops import set_engine, get_engine, prepare_operators  # noqa: F401,E402
 from .batch import MeshBatch  # noqa: F401,E402

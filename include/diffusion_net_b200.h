@@ -305,6 +305,39 @@ int dn_implicit_diffusion_bwd(const dn_csr* L, const float* grad_out, const floa
                               const float* x_diffuse, int64_t V, int C, double rtol, int max_iter, float* grad_x,
                               float* grad_time, double* status, void* workspace, int64_t ws_bytes, dn_stream_t stream);
 
+/* ---- functional maps (experiments/functional_correspondence/fmaps_model.py:11-40) ----------------------------------
+ * A = F_hat, B = G_hat (n x d, the spectral features of shapes x and y), D[i][j] = (evals_x[j] - evals_y[i])^2.  Row i of
+ * the functional map C (n x n) solves
+ *   S_i c_i = A b_i,   S_i = A A^T + lambda diag(D[i, :]),   b_i = B[i, :]^T,   C[i, :] = c_i^T.
+ * One CTA per row forms A A^T and A b_i in fp64 from the exactly promoted fp32 inputs (each a sum over d in increasing
+ * order), adds the regulariser, factors S_i by an fp64 Cholesky in shared memory and writes the solution in fp32.
+ * 1 <= n <= 128 (DN_ERR_UNSUPPORTED above, before any work is enqueued), any d >= 1, lambda >= 0.  There is no
+ * `engine` argument: the arithmetic is fp64 SIMT on every device.
+ * A row whose S_i has a non-positive (or NaN) pivot is written as NaN and the call goes on: nothing is read back on the
+ * host, so the call can be captured in a CUDA graph.  (The reference's torch.inverse raises on a singular system.)
+ *   fwd: 1 launch.
+ *   bwd: 2 launches.  With g_i = grad_C[i, :]^T and w_i = S_i^-1 g_i (S_i re-factored, c_i re-solved in fp64):
+ *        grad_B = W A,  grad_A = W^T B - sum_i (w_i c_i^T + c_i w_i^T) A  (W has rows w_i^T), OVERWRITTEN, every sum in a
+ *        fixed order without atomics (two calls give bitwise-equal results).  No gradient reaches the eigenvalues or
+ *        lambda.  Workspace: 16 n^2 bytes.  Rows of a singular S_i make the gradients NaN. */
+int dn_fmap_solve_fwd(const float* A, const float* B, const float* evals_x, const float* evals_y, int n, int d,
+                      double lambda, float* C, dn_stream_t stream);
+int dn_fmap_solve_bwd(const float* A, const float* B, const float* evals_x, const float* evals_y, int n, int d,
+                      double lambda, const float* grad_C, float* grad_A, float* grad_B, void* workspace,
+                      int64_t ws_bytes, dn_stream_t stream);
+
+/* Exact 1-nearest neighbour (geometry.find_knn(source, target, k=1), functional_correspondence.py:194-196):
+ * out_index[s] = argmin_t sum_k (source[s][k] - target[t][k])^2 over the rows of target (Vt x n), n <= 128
+ * (DN_ERR_UNSUPPORTED above, and for Vt >= 2^31).  The distance of each pair is one fp32 FMA chain over k in increasing
+ * order, in the difference form (no |q|^2 + |t|^2 - 2 q.t expansion, no tensor cores); the Vs x Vt distance matrix is
+ * never formed.  Ties go to the lowest target index; a source row whose distances are all NaN or +inf gets index 0.  The
+ * result is deterministic and does not depend on the device.  1 launch, or 2 when Vs is too small to fill the GPU and
+ * the targets are split into ranges; the workspace (dn_nearest_neighbor_workspace_bytes, 0 when not split) holds the
+ * per-range partials. */
+int64_t dn_nearest_neighbor_workspace_bytes(int64_t Vs, int64_t Vt, int n);
+int dn_nearest_neighbor(const float* source, int64_t Vs, const float* target, int64_t Vt, int n, int64_t* out_index,
+                        void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
 /* ---- batches of independent meshes in one launch sequence (BASELINE config 4; SURVEY.md 8e) -------------------
  * The reference loops over the batch dimension with one set of operators per mesh (layers.py:217-222; a DataLoader
  * of batch_size None in every experiment).  Here a batch is ONE vertex range: mesh b occupies rows

@@ -156,13 +156,14 @@ def lowest_eigenpairs(op, k, seed=0, stats=None):
     Eigenvector signs: the largest-magnitude entry of every column is positive (lowest vertex index on ties).
     Deterministic: a seeded start block and fixed-order reductions, so two calls give bitwise-equal results.
     ``stats`` (dict, optional) receives iterations, total filter degree, block size and stage times (ms).
-    Raises ValueError("failed to compute eigendecomp ...") if the iteration cap is reached."""
+    Raises ValueError("failed to compute eigendecomp ...") if the iteration cap is reached, and for k >= V, where the
+    reference's ``eigsh(..., sigma=eps)`` refuses (k must be below the matrix order) and it ends in that error."""
     V = op.V
     dev = op.mass.device
     if k <= 0:
         return (torch.zeros(0, dtype=torch.float64, device=dev), torch.zeros(V, 0, dtype=torch.float64, device=dev))
-    if k > V:
-        raise ValueError("failed to compute eigendecomp: k_eig = {} exceeds the vertex count {}".format(k, V))
+    if k >= V:
+        raise ValueError("failed to compute eigendecomp: k_eig = {} is not below the vertex count {}".format(k, V))
     B = block_size(V, k)
     s = _Solver(op, k, B, seed)
     t0 = _event()

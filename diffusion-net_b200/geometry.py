@@ -301,7 +301,9 @@ def compute_operators(verts, faces, k_eig, normals=None, device=None, stats=None
     which is fp32: for fp64 ``verts`` they are still fp32-grade.  Deterministic: two calls give bitwise-equal results.
 
     Raises RuntimeError for a CPU device or a NaN Laplacian / mass, NotImplementedError for a point cloud (empty
-    ``faces``), ValueError("failed to compute eigendecomp ...") if the eigensolver does not converge.  ``stats``
+    ``faces``), ValueError for faces outside [0, V), ValueError("failed to compute eigendecomp ...") if the
+    eigensolver does not converge or k_eig >= V (the reference's ``eigsh`` refuses k >= V and, after its retries,
+    raises that error).  ``stats``
     (dict, optional) receives per-stage times in ms and the solver's counters."""
     return _compute_operators(verts, faces, k_eig, normals, device, stats)[0]
 
@@ -363,17 +365,34 @@ def edge_tangent_vectors(verts, frames, edges):
     return torch.stack(((edge_vecs * basisX).sum(-1), (edge_vecs * basisY).sum(-1)), dim=-1)
 
 
+def _check_edges(edges, V, edge_tangent):
+    """The reference's loop raises IndexError on a tail outside [0, V) and reads one tangent row per edge: refuse bad
+    ``edges`` / ``edge_tangent`` on the host instead of letting the kernels drop or over-read them (one host sync)."""
+    if edges.dim() != 2 or edges.shape[0] != 2:
+        raise ValueError("edges must have shape (2, E), got {}".format(tuple(edges.shape)))
+    E = int(edges.shape[1])
+    if E > 0:
+        lo, hi = (int(x) for x in torch.aminmax(edges))
+        if lo < 0 or hi >= V:
+            raise IndexError("edges index vertices outside [0, {}): min {}, max {}".format(V, lo, hi))
+    if edge_tangent is not None and tuple(edge_tangent.shape) != (E, 2):
+        raise ValueError("edge_tangent must have shape ({}, 2), got {}".format(E, tuple(edge_tangent.shape)))
+
+
 def build_grad_operators(verts, frames, edges, edge_tangent=None):
     """``edge_tangent_vectors`` + ``build_grad`` (reference geometry.py:198-273) on the GPU, straight into the prepared
     shared-pattern CSR the layers consume: returns ``ops.GradOperators`` standing for the (gradX, gradY) pair
     (``.to_sparse_coo()`` gives the two coalesced COO tensors the reference returns).  ``edges``: (2,E) integer tensor
-    as in the reference (for meshes: the Laplacian's sparsity pattern, geometry.py:374-376).  One host sync (the entry
-    count); fp64 2x2 solves like numpy; 1e-6-grade agreement with the reference (tests/test_gpu_parity.py)."""
+    as in the reference (for meshes: the Laplacian's sparsity pattern, geometry.py:374-376).  Two host syncs (the edge
+    range check and the entry count); fp64 2x2 solves like numpy; 1e-6-grade agreement with the reference
+    (tests/test_gpu_parity.py).  Raises IndexError for edges outside [0, V), ValueError for an ``edge_tangent`` that is
+    not (E, 2)."""
     import ctypes as C
     from . import _lib
+    V = int(verts.shape[0])
+    _check_edges(edges, V, edge_tangent)
     ops._require_cuda(verts)
     dev = verts.device
-    V = int(verts.shape[0])
     edges = edges.to(device=dev, dtype=torch.int64).contiguous()
     E = int(edges.shape[1])
     verts = verts.to(torch.float32).contiguous()
@@ -393,13 +412,17 @@ def build_grad_operators(verts, frames, edges, edge_tangent=None):
 
 def build_grad(verts, edges, edge_tangent_vectors):
     """Drop-in for the reference's ``build_grad`` (geometry.py:209-273): numpy / torch in, scipy complex CSC (V,V) out,
-    computed by ``dn_build_grad`` on the current CUDA device instead of the per-vertex Python loop."""
+    computed by ``dn_build_grad`` on the current CUDA device instead of the per-vertex Python loop.  Raises IndexError
+    for edges outside [0, V), ValueError for tangent vectors that are not (E, 2)."""
     import scipy.sparse
-    dev = torch.device("cuda", torch.cuda.current_device())
     V = int(verts.shape[0])
-    as_t = lambda a, dt: (a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))).to(device=dev, dtype=dt)
-    g = build_grad_operators(torch.empty(V, 3, device=dev), torch.empty(V, 3, 3, device=dev), as_t(edges, torch.int64),
-                             edge_tangent=as_t(edge_tangent_vectors, torch.float32))
+    as_t = lambda a: a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))
+    edges, edge_tangent_vectors = as_t(edges), as_t(edge_tangent_vectors)
+    _check_edges(edges, V, edge_tangent_vectors)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    g = build_grad_operators(torch.empty(V, 3, device=dev), torch.empty(V, 3, 3, device=dev),
+                             edges.to(device=dev, dtype=torch.int64),
+                             edge_tangent=edge_tangent_vectors.to(device=dev, dtype=torch.float32))
     rowptr, colidx, vals = g.to_host_csr()
     vals = np.asarray(vals, dtype=np.float64)
     data = vals[:, 0] + 1j * vals[:, 1]

@@ -111,6 +111,9 @@ int run_chain(const DnRowsSrc& src, DnLayer* layers, int n_layers, int64_t V, En
   DnRowsSrc cur = src;
   for (int l = 0; l < n_layers; ++l) {
     DnLayer L = layers[l];
+    // a sibling reads the same input as the layer before it: its own output must not overwrite that input
+    if (L.sibling && (l == 0 || !L.out)) return DN_ERR_UNSUPPORTED;
+    L.sibling = 0;
     if (!L.out) { L.out = tmp[l & 1]; L.ld_out = L.N; }
     int rc;
     // (a single layer was planned above)
@@ -121,7 +124,7 @@ int run_chain(const DnRowsSrc& src, DnLayer* layers, int n_layers, int64_t V, En
     else
       rc = simt_layer(cur, L, V, st);
     if (rc) return rc;
-    cur = one_src(L.out, L.N, L.ld_out);
+    if (!(l + 1 < n_layers && layers[l + 1].sibling)) cur = one_src(L.out, L.N, L.ld_out);
   }
   return DN_OK;
 }
@@ -807,16 +810,21 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
   // every dense layer of the block: [0] from_basis, [1] (a5, commuted) [P|Q] = x_diffuse [A_re;A_im]^T,
   // [2..] cat -> MiniMLP -> + x_in  [layers.py:229-239]
   const int nm = p->n_mlp_layers;
+  Engine e;
+  if ((rc = resolve(engine, &e))) return rc;
   DnLayer L[3 + DN_MAX_LAYERS];
   L[0] = make_layer(S, C, 1, nullptr, 0, K, C, xd, C);
   int nfront = 1;
   // gradient features, commuted route: [P|Q] = x_diffuse [A_re; A_im]^T as a dense layer in front of one CSR gather of
   // x, P and Q that forms tanh(gX * Bre + gY * Bim) (layers.py:117-130)
   if (p->with_gradient_features) {
-    if (rot && npq > 256) {
-      // [P|Q] wider than one tensor-core layer (C_width = 256): P and Q are separate layers writing the two halves
+    if (rot && (npq > 256 || (e.tc && npq > 128))) {
+      // [P|Q] wider than one tensor-core layer (C_width = 256), or wider than a layer inside a chain (C_width = 128):
+      // P and Q are separate layers writing the two halves.  At C_width = 128 they join from_basis in one chain, Q
+      // as P's sibling (both read x_diffuse from the registers from_basis left it in)
       L[1] = make_layer(p->A_re, C, 0, nullptr, 0, C, C, pq, npq);
       L[2] = make_layer(p->A_im, C, 0, nullptr, 0, C, C, pq + C, npq);
+      L[2].sibling = 1;
       nfront = 3;
     } else {
       L[1] = make_layer(p->A_re, C, 0, nullptr, 0, C, npq, pq, npq);
@@ -843,8 +851,6 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
     }
   }
   if (p->mlp_dims_host[nm] != C) return DN_ERR_INVALID_ARGUMENT;
-  Engine e;
-  if ((rc = resolve(engine, &e))) return rc;
   DnRowsSrc src_fb = one_src(evecs, K, K);
   DnRowsSrc src_pq = one_src(xd, C, C);
   DnRowsSrc src_mlp;
@@ -852,9 +858,10 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
   const float* srcs[3] = {x_in, xd, feat};
   for (int q = 0; q < nsrc; ++q) { src_mlp.ptr[q] = srcs[q]; src_mlp.width[q] = C; src_mlp.ld[q] = C; }
   src_mlp.nsrc = nsrc;
-  // which chains run on tensor cores: from_basis and [P|Q] as one fused chain when it fits, else each layer on its
-  // own; the MiniMLP chain
-  const bool front_fused = e.tc && nfront == 2 && tc_chain_plan(src_fb, &L[0], 2, e.passes) >= 0;
+  // which chains run on tensor cores: from_basis and [P|Q] (or P, Q) as one fused chain when it fits, else each layer
+  // on its own (Q then reads x_diffuse from HBM like P); the MiniMLP chain
+  const bool front_fused = e.tc && nfront > 1 && tc_chain_plan(src_fb, &L[0], nfront, e.passes) >= 0;
+  if (!front_fused && nfront == 3) L[2].sibling = 0;
   bool tc_front = front_fused;
   if (e.tc && !front_fused) {
     tc_front = tc_chain_plan(src_fb, &L[0], 1, e.passes) >= 0;
@@ -888,7 +895,7 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
     if ((rc = tc_pack_layers(first, cnt, pk, pb, tc_front ? &sp : nullptr, st))) return rc;
   }
   mark(3);
-  const int n_fused = front_fused ? 2 : 1;
+  const int n_fused = front_fused ? nfront : 1;
   if ((rc = run_chain(src_fb, &L[0], n_fused, V, e, ws, st))) return rc;
   for (int l = n_fused; l < nfront; ++l)
     if ((rc = run_chain(src_pq, &L[l], 1, V, e, ws, st))) return rc;

@@ -50,6 +50,9 @@ struct DnLayer {
   // and 128-row tile t uses matrix tile_group[t] (device array)
   const int32_t* tile_group;
   int64_t group_stride;
+  // inside a fused chain (layer 2 or later): this layer reads the input of the layer before it instead of that layer's
+  // output (P and Q of the gradient features both read x_diffuse)
+  int sibling;
   // linear head fused behind the last layer's epilogue (DiffusionNet.last_lin, layers.py:366-370): after bias / residual the
   // N-wide row y is NOT stored (out may be null); head_out[v][o] = head_b[o] + sum_n head_w[o][n] * y[n], o < head_n <= 8,
   // exact fp32 FMAs in the output warps
@@ -160,7 +163,8 @@ int dn_sm_count();
 // `passes`: 3 = 3xTF32-grade (fp32 parity), 1 = single-pass TF32, DN_PASSES_BF16 = single-pass bf16 (DN_ENGINE_BF16)
 #define DN_PASSES_BF16 16
 // Whether rows_chain_kernel takes this chain: the packed-weight format it runs it with (also stored in every
-// layers[i].pack_fmt), or DN_ERR_UNSUPPORTED.
+// layers[i].pack_fmt), or DN_ERR_UNSUPPORTED.  Layer 0's sources are copied with 2-D TMA: each must be 16-byte
+// aligned with a row stride that is a multiple of 4 floats.
 int tc_chain_plan(const DnRowsSrc& src, DnLayer* layers, int n_layers, int passes);
 // Fused chain of up to DN_MAX_LAYERS layers over 128-row tiles; layer 0 reads `src`.  The chain was planned
 // (tc_chain_plan) on a device that runs the tensor-core kernels; layers that are not prepacked are packed into ws.

@@ -10,10 +10,13 @@
 //
 // Data movement: weights are pre-split and pre-laid-out in the wgmma canonical (no-swizzle, K-major) layout by a
 // small pack kernel and streamed per 16-wide K stage with bulk TMA copies (cp.async.bulk + mbarrier complete_tx).
-// Activations never pass through shared memory: the A operand of every MMA comes from registers, loaded from HBM for
-// the first layer of a chain and taken straight from the previous layer's accumulator fragment for the others.
+// The A operand of every MMA is in registers.  For the first layer of a chain it is read from a shared-memory ring
+// that a second producer lane fills from HBM with 2-D tiled TMA copies (8 columns x 128 rows per copy), running ahead
+// of the consumers across layers and tiles; every later layer's A is the previous layer's accumulator fragment.
 #include "dn_internal.h"
 #include "dn_tc_ptx.cuh"
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_bf16.h>
 #include <string.h>
 
@@ -25,8 +28,12 @@ constexpr int KC = 16;                          // k-elements per weight stage
 constexpr int TILE_M = 128;                     // vertex rows per tile: two consumer warpgroups of 64 rows
 constexpr int NST = 4;                          // weight stages in flight
 constexpr int STAGE_BYTES = KC * 256 * 8;       // 32 KiB: tf32 hi | lo images of a 256-wide layer
-constexpr int CHAIN_THREADS = 384;              // warpgroups 0, 1: consumers; warpgroup 2: weight producer (one lane)
-constexpr int CHAIN_SMEM = NST * STAGE_BYTES + 256;
+constexpr int CHAIN_THREADS = 384;              // warpgroups 0, 1: consumers; warpgroup 2: producers (two lanes)
+// first-layer activations: 16-column x 128-row fp32 stages, each two 8-column boxes of [128 rows][8 floats]
+constexpr int A_BOX_BYTES = 8 * TILE_M * 4;     // 4 KiB
+constexpr int A_STAGE_BYTES = 2 * A_BOX_BYTES;
+constexpr int A_NST = 8;                        // activation stages in flight (64 KiB per SM)
+constexpr int CHAIN_SMEM = NST * STAGE_BYTES + A_NST * A_STAGE_BYTES + 256;
 
 enum { MODE_TF32 = 1, MODE_TF32X3 = 3, MODE_BF16 = DN_PASSES_BF16 };
 
@@ -142,10 +149,11 @@ struct HcLayer {
   float res_scale;
   float* out;
   int64_t ld_out;
-  int K, N, relu;
+  int K, N, relu, sibling;
 };
 
 struct HcParams {
+  CUtensorMap amap[DN_MAX_SRC];   // layer 0's sources: fp32 [V rows][width], 8 x 128 boxes, rows >= V zero-filled
   DnRowsSrc src;
   HcLayer layer[DN_MAX_LAYERS];
   int n_layers;
@@ -160,7 +168,15 @@ struct HcParams {
 };
 
 // Both consumer warpgroups own 64 rows of the tile each and share the weight stages; one lane of warpgroup 2 streams
-// the stages with bulk TMA (that warpgroup hands its registers to the consumers with setmaxnreg).  Per lane, the accumulator of an N-wide layer holds rows (16w+g, 16w+g+8) x columns (8b+2t, 8b+2t+1)
+// the stages with bulk TMA (that warpgroup hands its registers to the consumers with setmaxnreg).  A second lane
+// (warp 9) copies layer 0's activations of every tile into an A_NST-deep ring of 16-column stages with 2-D TMA: box h
+// of a stage holds columns 8h .. 8h+7 as [128 rows][8 floats], so the 32 bytes a row contributes are contiguous and a
+// half-warp's float2 reads (rows g = 0..3 of its warp, columns 2t, 2t+1) cover 128 consecutive bytes: every bank once,
+// no conflict and no swizzle.  A stage whose columns lie in two sources (widths that are multiples of 8, not of 16)
+// is two boxes from two tensor maps.  Consumers read their fragments, issue the stage's MMAs and release the slot
+// (a proxy fence, then one arrival per warp); the producer meanwhile runs ahead into the next tile's first layer while the consumers are
+// in the epilogue and the later layers.
+// Per lane, the accumulator of an N-wide layer holds rows (16w+g, 16w+g+8) x columns (8b+2t, 8b+2t+1)
 // for every 8-column block b: after the epilogue these values are the next layer's A fragments (columns of a 16-wide
 // K stage: tf32 steps use the permuted weight order of pack_store, bf16 steps the natural one).  NMAX <= 128 chains
 // any number of layers; NMAX = 256 runs a single layer (its accumulator alone takes 128 registers).
@@ -172,11 +188,14 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
   constexpr bool kChain = NMAX <= 128;
   constexpr int NB = NMAX / 16;
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NST * STAGE_BYTES);
+  uint8_t* aring = smem + NST * STAGE_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(aring + A_NST * A_STAGE_BYTES);
   const uint32_t full = smem_u32(bars), empty = smem_u32(bars + NST);
+  const uint32_t afull = smem_u32(bars + 2 * NST), aempty = smem_u32(bars + 2 * NST + A_NST);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < NST; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 8); }
+    for (int i = 0; i < A_NST; ++i) { mbar_init(afull + 8 * i, 1); mbar_init(aempty + 8 * i, 8); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -184,8 +203,26 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
   const int64_t ntiles = (p.V + TILE_M - 1) / TILE_M;
 
   if (warp >= 8) {
-    // ===================== weight producer =====================
     setmaxnreg_dec<40>();
+    if (warp == 9 && lane == 0) {
+      // ===================== layer-0 activation producer =====================
+      const int K0 = p.layer[0].K, nst0 = (K0 + KC - 1) / KC;
+      uint32_t s = 0, ph = 0;
+      for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
+        for (int c = 0; c < nst0; ++c) {
+          const int nbox = c * KC + 8 < K0 ? 2 : 1;   // a half stage (K % 16 == 8) is one box
+          mbar_wait(aempty + 8 * s, ph ^ 1);
+          mbar_arrive_expect_tx(afull + 8 * s, (uint32_t)(nbox * A_BOX_BYTES));
+          for (int h = 0; h < nbox; ++h) {
+            int kc = c * KC + 8 * h, sidx = 0;
+            while (sidx + 1 < p.src.nsrc && kc >= p.src.width[sidx]) { kc -= p.src.width[sidx]; ++sidx; }
+            tma_tile_2d_g2s(smem_u32(aring + s * A_STAGE_BYTES + h * A_BOX_BYTES), &p.amap[sidx], kc,
+                            (int)(tile * TILE_M), afull + 8 * s);
+          }
+          if (++s == A_NST) { s = 0; ph ^= 1; }
+        }
+    }
+    // ===================== weight producer =====================
     if (warp == 8 && lane == 0) {
       uint32_t s = 0, ph = 0;
       for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
@@ -213,7 +250,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
   const int rloc = (warp >> 2) * 64 + (warp & 3) * 16 + g;
   float acc[NB * 8];
   float act[kChain ? NB * 8 : 1];
-  uint32_t s = 0, ph = 0;
+  uint32_t s = 0, ph = 0, as = 0, aph = 0;
 
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int64_t r0 = tile * TILE_M + rloc, r1 = r0 + 8;
@@ -301,28 +338,25 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
       };
 
       if (l == 0) {
-        auto load = [&](int c, float2* q) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            int kc = c * KC + 8 * h;
-            q[2 * h] = q[2 * h + 1] = make_float2(0.f, 0.f);
-            if (kc >= K) continue;
-            int sidx = 0;
-            while (sidx + 1 < p.src.nsrc && kc >= p.src.width[sidx]) { kc -= p.src.width[sidx]; ++sidx; }
-            const float* b = p.src.ptr[sidx] + kc + 2 * t;
-            const int64_t ld = p.src.ld[sidx];
-            if (ok0) q[2 * h] = __ldg(reinterpret_cast<const float2*>(b + r0 * ld));
-            if (ok1) q[2 * h + 1] = __ldg(reinterpret_cast<const float2*>(b + r1 * ld));
+        for (int c = 0; c < nst; ++c) {
+          const bool two = c * KC + 8 < K;
+          mbar_wait(afull + 8 * as, aph);
+          const float* a = reinterpret_cast<const float*>(aring + as * A_STAGE_BYTES) + rloc * 8 + 2 * t;
+          float2 q[4];
+          q[0] = *reinterpret_cast<const float2*>(a);
+          q[1] = *reinterpret_cast<const float2*>(a + 64);
+          q[2] = q[3] = make_float2(0.f, 0.f);
+          if (two) {
+            q[2] = *reinterpret_cast<const float2*>(a + A_BOX_BYTES / 4);
+            q[3] = *reinterpret_cast<const float2*>(a + A_BOX_BYTES / 4 + 64);
           }
-        };
-        float2 qa[4], qb[4];
-        load(0, qa);
-        for (int c = 0; c < nst; c += 2) {
-          if (c + 1 < nst) load(c + 1, qb);
-          stage(c, qa, c * KC + 8 < K);
-          if (c + 1 >= nst) break;
-          if (c + 2 < nst) load(c + 2, qa);
-          stage(c + 1, qb, (c + 1) * KC + 8 < K);
+          stage(c, q, two);
+          // the slot is handed back once the stage's fragments are formed from the loaded values, behind a proxy fence:
+          // the producer's next TMA write to it (async proxy) must not overtake these generic-proxy reads
+          fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(aempty + 8 * as);
+          if (++as == A_NST) { as = 0; aph ^= 1; }
         }
       } else if constexpr (kChain) {
 #pragma unroll
@@ -341,6 +375,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
       // ---- epilogue (the operation order of simt_rows_gemm)
       const bool last = l + 1 == L;
       const bool head = last && p.head_w != nullptr;
+      const bool keep_act = !last && p.layer[l + 1].sibling;   // the next layer reads this layer's input again
       const float rs0 = (Lr.row_scale && ok0) ? __ldg(Lr.row_scale + r0) : 1.f;
       const float rs1 = (Lr.row_scale && ok1) ? __ldg(Lr.row_scale + r1) : 1.f;
       float hp0[kChain ? 1 : 8], hp1[kChain ? 1 : 8];   // head partial sums of a single-layer (256-wide) chain
@@ -394,8 +429,10 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
             if (ok1) *reinterpret_cast<float2*>(Lr.out + r1 * Lr.ld_out + col) = v1;
           }
           if constexpr (kChain) {
-            act[8 * j + 4 * h] = v0.x; act[8 * j + 4 * h + 1] = v0.y;
-            act[8 * j + 4 * h + 2] = v1.x; act[8 * j + 4 * h + 3] = v1.y;
+            if (!keep_act) {
+              act[8 * j + 4 * h] = v0.x; act[8 * j + 4 * h + 1] = v0.y;
+              act[8 * j + 4 * h + 2] = v1.x; act[8 * j + 4 * h + 3] = v1.y;
+            }
           }
           if (!kChain && head) {
 #pragma unroll
@@ -680,6 +717,21 @@ bool set_chain_smem() {
          set_smem(rows_chain_kernel<MODE, 256, false>, CHAIN_SMEM) && set_smem(rows_chain_kernel<MODE, 256, true>, CHAIN_SMEM);
 }
 
+// cuTensorMapEncodeTiled from the driver the runtime already loaded (no link dependency on libcuda); null if absent
+PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
+  static const PFN_cuTensorMapEncodeTiled_v12000 fn = [] {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &f, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess) {
+      cudaGetLastError();
+      f = nullptr;
+    }
+    return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
+  }();
+  return fn;
+}
+
 }  // namespace
 
 static DevState* cur_dev_state() {
@@ -714,22 +766,25 @@ bool tc_supported_device() {
   if (!d || !d->sm90) return false;
   if (!d->tc_tried) {
     d->tc_tried = 1;
-    d->tc = set_chain_smem<MODE_TF32X3>() && set_chain_smem<MODE_TF32>() && set_chain_smem<MODE_BF16>() &&
-            set_to_basis_smem<MODE_TF32X3>() && set_to_basis_smem<MODE_TF32>();
+    d->tc = tensor_map_encoder() != nullptr && set_chain_smem<MODE_TF32X3>() && set_chain_smem<MODE_TF32>() &&
+            set_chain_smem<MODE_BF16>() && set_to_basis_smem<MODE_TF32X3>() && set_to_basis_smem<MODE_TF32>();
     if (!d->tc) cudaGetLastError();
   }
   return d->tc;
 }
 
 static bool aligned8(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 7) == 0; }
+static bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
-// shapes rows_chain_kernel takes (bf16: 16-wide K steps; tf32: 8-wide)
+// shapes rows_chain_kernel takes (bf16: 16-wide K steps; tf32: 8-wide).  Layer 0's sources are TMA tensor maps: base
+// 16-byte aligned, row stride a multiple of 16 bytes.
 static int chain_supported(const DnRowsSrc& src, const DnLayer* layers, int n_layers, bool bf16) {
   const int ks = bf16 ? 16 : 8;
   if (n_layers < 1 || n_layers > DN_MAX_LAYERS) return DN_ERR_UNSUPPORTED;
   int k0 = 0;
   for (int s = 0; s < src.nsrc; ++s) {
-    if (src.width[s] % ks || src.ld[s] % 2 || !aligned8(src.ptr[s])) return DN_ERR_UNSUPPORTED;
+    if (src.width[s] % ks || src.ld[s] % 4 || src.ld[s] < src.width[s] || !aligned16(src.ptr[s]))
+      return DN_ERR_UNSUPPORTED;
     k0 += src.width[s];
   }
   if (k0 != layers[0].K) return DN_ERR_UNSUPPORTED;
@@ -737,7 +792,9 @@ static int chain_supported(const DnRowsSrc& src, const DnLayer* layers, int n_la
     const DnLayer& L = layers[l];
     const bool last = l + 1 == n_layers;
     if (L.K % ks || L.K < ks || L.N % 16 || L.N < 16 || L.N > (n_layers > 1 ? 128 : 256)) return DN_ERR_UNSUPPORTED;
-    if (l > 0 && (L.K != layers[l - 1].N || L.tile_group)) return DN_ERR_UNSUPPORTED;
+    // a sibling reads the input of the layer before it, which must itself be a chain layer (not layer 0's sources)
+    if (L.sibling && l < 2) return DN_ERR_UNSUPPORTED;
+    if (l > 0 && (L.K != (L.sibling ? layers[l - 1].K : layers[l - 1].N) || L.tile_group)) return DN_ERR_UNSUPPORTED;
     if (L.emul && !aligned8(L.emul)) return DN_ERR_UNSUPPORTED;
     if (L.relu_mask_src && !aligned8(L.relu_mask_src)) return DN_ERR_UNSUPPORTED;
     if (L.residual && (L.ld_res % 2 || !aligned8(L.residual))) return DN_ERR_UNSUPPORTED;
@@ -834,13 +891,25 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
   p.V = V;
   p.tile_group = layers[0].tile_group;
   p.group_stride = layers[0].group_stride;
+  // one tensor map per source of layer 0 (encoded on the host; a captured graph keeps them with the launch)
+  const PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
+  if (!encode) return DN_ERR_UNSUPPORTED;
+  for (int s = 0; s < src.nsrc; ++s) {
+    const cuuint64_t dims[2] = {(cuuint64_t)src.width[s], (cuuint64_t)V};
+    const cuuint64_t strides[1] = {(cuuint64_t)src.ld[s] * 4};
+    const cuuint32_t box[2] = {8, TILE_M}, estr[2] = {1, 1};
+    if (encode(&p.amap[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(src.ptr[s]), dims, strides, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+      return DN_ERR_UNSUPPORTED;
+  }
   int nmax = 0, nmin = 1 << 30;
   for (int l = 0; l < n_layers; ++l) {
     const DnLayer& L = layers[l];
     HcLayer& T = p.layer[l];
     T.wpack = L.prepacked; T.bias = L.bias; T.emul = L.emul; T.relu_mask = L.relu_mask_src; T.row_scale = L.row_scale;
     T.residual = L.residual; T.ld_res = L.ld_res; T.res_scale = L.res_scale; T.out = L.out; T.ld_out = L.ld_out;
-    T.K = L.K; T.N = L.N; T.relu = L.relu;
+    T.K = L.K; T.N = L.N; T.relu = L.relu; T.sibling = L.sibling;
     if (L.N > nmax) nmax = L.N;
     if (L.N < nmin) nmin = L.N;
   }

@@ -1,5 +1,5 @@
 // Inline-PTX wrappers for the Hopper (sm_90a) features the tensor-core engine uses:
-// mbarrier, bulk TMA copies, proxy fences and warpgroup MMA (wgmma) with the A operand in registers.
+// mbarrier, bulk and tiled TMA copies, proxy fences and warpgroup MMA (wgmma) with the A operand in registers.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -62,6 +62,15 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst_smem, const void* src_
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
                "l"(src_gmem), "r"(bytes), "r"(bar)
                : "memory");
+}
+// 2-D tiled TMA copy of the box at (column c0, row c1) of the tensor map `tmap` (a __grid_constant__ kernel parameter)
+// into shared memory; elements outside the tensor are zero-filled and still counted in the transaction bytes
+__device__ __forceinline__ void tma_tile_2d_g2s(uint32_t dst_smem, const void* tmap, int c0, int c1, uint32_t bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+          dst_smem),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(bar)
+      : "memory");
 }
 
 // ---- wgmma ------------------------------------------------------------------------------------

@@ -629,7 +629,6 @@ int dn_gradient_features_fwd(const dn_csr* grad, const float* x_diffuse, const f
   if (!grad || !grad->rowptr || !x_diffuse || !A_re || (with_gradient_rotations && !A_im) || !features || V < 0 ||
       C <= 0)
     return DN_ERR_INVALID_ARGUMENT;
-  if (C % 4) return DN_ERR_UNSUPPORTED;
   Engine e;
   int rc = resolve(engine, &e);
   if (rc) return rc;
@@ -653,7 +652,6 @@ int dn_gradient_features_bwd(const dn_csr* grad, const dn_csr* grad_t, const flo
   if (!grad || !grad_t || !grad_features || !x_diffuse || !pq || !features || !A_re || !grad_x || !grad_A_re ||
       (with_gradient_rotations && (!A_im || !grad_A_im)))
     return DN_ERR_INVALID_ARGUMENT;
-  if (C % 4) return DN_ERR_UNSUPPORTED;
   Engine e;
   int rc = resolve(engine, &e);
   if (rc) return rc;
@@ -688,7 +686,7 @@ int dn_mini_mlp_fwd(const float* const* src_host, const int* src_width_host, int
                     float* const* hidden_out_host, float* out, void* workspace, int64_t ws_bytes, int engine,
                     dn_stream_t stream) {
   if (!src_host || !src_width_host || nsrc < 1 || nsrc > DN_MAX_SRC || !weight_host || !dims_host || n_layers < 1 ||
-      n_layers > DN_MAX_LAYERS || !out || V < 0)
+      !out || V < 0)
     return DN_ERR_INVALID_ARGUMENT;
   DnRowsSrc src;
   memset(&src, 0, sizeof(src));
@@ -700,7 +698,8 @@ int dn_mini_mlp_fwd(const float* const* src_host, const int* src_width_host, int
   }
   src.nsrc = nsrc;
   if (k0 != dims_host[0]) return DN_ERR_INVALID_ARGUMENT;
-  DnLayer layers[DN_MAX_LAYERS];
+  // a MiniMLP deeper than one fused chain (DN_MAX_LAYERS) runs layer by layer in run_chain
+  std::vector<DnLayer> layers(n_layers);
   for (int l = 0; l < n_layers; ++l) {
     if (!weight_host[l] || dims_host[l + 1] <= 0) return DN_ERR_INVALID_ARGUMENT;
     const bool last = (l + 1 == n_layers);
@@ -713,7 +712,7 @@ int dn_mini_mlp_fwd(const float* const* src_host, const int* src_width_host, int
   Engine e;
   const int rc = resolve(engine, &e);
   if (rc) return rc;
-  return run_chain(src, layers, n_layers, V, e, Bump(workspace, ws_bytes), (cudaStream_t)stream);
+  return run_chain(src, layers.data(), n_layers, V, e, Bump(workspace, ws_bytes), (cudaStream_t)stream);
 }
 
 int dn_mini_mlp_bwd(const float* grad_out, const float* const* src_host, const int* src_width_host, int nsrc,
@@ -722,7 +721,7 @@ int dn_mini_mlp_bwd(const float* grad_out, const float* const* src_host, const i
                     float* const* grad_src_host, float* const* grad_weight_host, float* const* grad_bias_host,
                     void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream) {
   if (!grad_out || !src_host || !src_width_host || nsrc < 1 || nsrc > DN_MAX_SRC || !weight_host || !dims_host ||
-      n_layers < 1 || n_layers > DN_MAX_LAYERS || (n_layers > 1 && !hidden_host) || !grad_src_host ||
+      n_layers < 1 || (n_layers > 1 && !hidden_host) || !grad_src_host ||
       !grad_weight_host)
     return DN_ERR_INVALID_ARGUMENT;
   Engine e;
@@ -791,9 +790,8 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
     return DN_ERR_INVALID_ARGUMENT;
   if (p->with_gradient_features && (!grad || !grad->rowptr || !p->A_re || (p->with_gradient_rotations && !p->A_im)))
     return DN_ERR_INVALID_ARGUMENT;
-  if (p->n_mlp_layers < 1 || p->n_mlp_layers > DN_MAX_LAYERS || !p->mlp_weight_host || !p->mlp_dims_host)
+  if (p->n_mlp_layers < 1 || !p->mlp_weight_host || !p->mlp_dims_host)
     return DN_ERR_INVALID_ARGUMENT;
-  if (p->with_gradient_features && (C % 4)) return DN_ERR_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   Bump ws(workspace, ws_bytes);
   const int rot = p->with_gradient_rotations;
@@ -812,7 +810,8 @@ static int block_fwd_impl(const float* x_in, const float* mass, const float* eva
   const int nm = p->n_mlp_layers;
   Engine e;
   if ((rc = resolve(engine, &e))) return rc;
-  DnLayer L[3 + DN_MAX_LAYERS];
+  // a MiniMLP deeper than one fused chain (DN_MAX_LAYERS) is not a tensor-core chain: run_chain runs it layer by layer
+  std::vector<DnLayer> L(3 + nm);
   L[0] = make_layer(S, C, 1, nullptr, 0, K, C, xd, C);
   int nfront = 1;
   // gradient features, commuted route: [P|Q] = x_diffuse [A_re; A_im]^T as a dense layer in front of one CSR gather of

@@ -443,6 +443,50 @@ __global__ void __launch_bounds__(256) spmm_features_kernel(const int32_t* __res
   }
 }
 
+// Scalar-lane forms of the features kernels for C % 4 != 0 (no float4 row access): one thread per (row, channel), the
+// same per-element operation order as gather_row and the float4 kernels.
+struct Acc1 {
+  float gX, gY, bre, bim;
+};
+
+template <bool ROT>
+__device__ __forceinline__ Acc1 gather_row_scalar(const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
+                                                  const float* __restrict__ xd, const float* __restrict__ pq,
+                                                  int ld_pq, int C, int s, int e, int c) {
+  Acc1 a = {0.f, 0.f, 0.f, 0.f};
+  for (int p = s; p < e; ++p) {
+    const int64_t col = __ldg(colidx + p);
+    const float2 g = __ldg(vals + p);
+    const float x = __ldg(xd + col * C + c);
+    const float P = __ldg(pq + col * ld_pq + c);
+    a.gX = fmaf(g.x, x, a.gX);
+    a.gY = fmaf(g.y, x, a.gY);
+    a.bre = fmaf(g.x, P, a.bre);
+    a.bim = fmaf(g.y, P, a.bim);
+    if (ROT) {
+      const float Q = __ldg(pq + col * ld_pq + C + c);
+      a.bre = fmaf(-g.y, Q, a.bre);
+      a.bim = fmaf(g.x, Q, a.bim);
+    }
+  }
+  return a;
+}
+
+template <bool ROT>
+__global__ void __launch_bounds__(256) spmm_features_scalar_kernel(const int32_t* __restrict__ rowptr,
+                                                                   const int32_t* __restrict__ colidx,
+                                                                   const float2* __restrict__ vals,
+                                                                   const float* __restrict__ xd,
+                                                                   const float* __restrict__ pq, int ld_pq, int64_t V,
+                                                                   int C, float* __restrict__ feat) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= V * C) return;
+  const int64_t row = idx / C;
+  const int c = (int)(idx - row * C);
+  const Acc1 a = gather_row_scalar<ROT>(colidx, vals, xd, pq, ld_pq, C, __ldg(rowptr + row), __ldg(rowptr + row + 1), c);
+  feat[row * C + c] = feat_tanh(fmaf(a.gX, a.bre, a.gY * a.bim));
+}
+
 __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
   unsigned long long r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -757,6 +801,51 @@ __global__ void __launch_bounds__(256) features_bwd_transpose_kernel(
   }
 }
 
+// scalar-lane forms of the two kernels above (C % 4 != 0)
+template <bool ROT>
+__global__ void __launch_bounds__(256) features_bwd_local_scalar_kernel(
+    const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
+    const float* __restrict__ xd, const float* __restrict__ pq, int ld_pq, const float* __restrict__ feat,
+    const float* __restrict__ dfeat, int64_t V, int C, float* __restrict__ U) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= V * C) return;
+  const int64_t row = idx / C;
+  const int c = (int)(idx - row * C);
+  const Acc1 a = gather_row_scalar<ROT>(colidx, vals, xd, pq, ld_pq, C, __ldg(rowptr + row), __ldg(rowptr + row + 1), c);
+  const float f = __ldg(feat + row * C + c);
+  const float dd = __ldg(dfeat + row * C + c) * (1.f - f * f);
+  float* u = U + row * 4 * C + c;
+  u[0] = dd * a.bre;
+  u[C] = dd * a.bim;
+  u[2 * C] = dd * a.gX;
+  u[3 * C] = dd * a.gY;
+}
+
+template <bool ROT>
+__global__ void __launch_bounds__(256) features_bwd_transpose_scalar_kernel(
+    const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
+    const float* __restrict__ U, int64_t V, int C, float* __restrict__ dxd, float* __restrict__ dP,
+    float* __restrict__ dQ, int64_t ld_pq) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= V * C) return;
+  const int64_t row = idx / C;
+  const int c = (int)(idx - row * C);
+  const int s = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
+  float ax = 0.f, ap = 0.f, aq = 0.f;
+  for (int p = s; p < e; ++p) {
+    const int64_t i = __ldg(colidx + p);
+    const float2 g = __ldg(vals + p);
+    const float* u = U + i * 4 * C + c;
+    const float u1 = __ldg(u), u2 = __ldg(u + C), u3 = __ldg(u + 2 * C), u4 = __ldg(u + 3 * C);
+    ax += g.x * u1 + g.y * u2;
+    ap += g.x * u3 + g.y * u4;
+    if (ROT) aq += g.x * u4 - g.y * u3;
+  }
+  dxd[row * C + c] = ax;
+  dP[row * ld_pq + c] = ap;
+  if (ROT) dQ[row * ld_pq + c] = aq;
+}
+
 __global__ void deinterleave_vc2_kernel(const float2* __restrict__ vc2, int64_t V, int C, float* __restrict__ g01) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= V * C) return;
@@ -921,7 +1010,14 @@ int launch_grad_spmm_pair(const dn_csr* g, const float* x, int64_t V, int C, flo
 int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int rotations, int64_t V, int C,
                          float* feat, cudaStream_t st) {
   if (V <= 0) return DN_OK;
-  if (C % 4) return DN_ERR_UNSUPPORTED;
+  const float2* vals = reinterpret_cast<const float2*>(g->vals);
+  if (C % 4) {   // no float4 row access: one thread per (row, channel)
+    const unsigned blocks = (unsigned)((V * C + 255) / 256);
+    if (rotations) spmm_features_scalar_kernel<true><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, 2 * C, V, C, feat);
+    else spmm_features_scalar_kernel<false><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, C, V, C, feat);
+    DN_LAUNCH_CHECK();
+    return DN_OK;
+  }
   // the patched kernel when the host built patches for this operator (bit-identical to the plain kernel, both ROT
   // variants).  C == 128 only: that is the shape validated on the GPU; the phase-2 shuffles also assume every lane owns
   // a float4 of the row (C/4 a multiple of 32)
@@ -944,7 +1040,6 @@ int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int 
       return DN_OK;
     }
   }
-  const float2* vals = reinterpret_cast<const float2*>(g->vals);
   if (C == 128 || C == 256) {
     const unsigned ctas = (unsigned)((V + GB_ROWS - 1) / GB_ROWS);
     const int ld = rotations ? 2 * C : C;
@@ -970,11 +1065,19 @@ int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int 
 int launch_features_bwd_local(const dn_csr* g, const float* xd, const float* pq, const float* feat,
                               const float* dfeat, int rotations, int64_t V, int C, float* U, cudaStream_t st) {
   if (V <= 0) return DN_OK;
-  if (C % 4) return DN_ERR_UNSUPPORTED;
+  const float2* vals = reinterpret_cast<const float2*>(g->vals);
+  if (C % 4) {
+    const unsigned sb = (unsigned)((V * C + 255) / 256);
+    if (rotations)
+      features_bwd_local_scalar_kernel<true><<<sb, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, 2 * C, feat, dfeat, V, C, U);
+    else
+      features_bwd_local_scalar_kernel<false><<<sb, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, C, feat, dfeat, V, C, U);
+    DN_LAUNCH_CHECK();
+    return DN_OK;
+  }
   const int G = pick_group(C);
   const int64_t warps = (V + (32 / G) - 1) / (32 / G);
   const unsigned blocks = (unsigned)((warps * 32 + 255) / 256);
-  const float2* vals = reinterpret_cast<const float2*>(g->vals);
   if (rotations)
     features_bwd_local_kernel<true><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, 2 * C, feat, dfeat,
                                                              V, C, G, U);
@@ -988,11 +1091,19 @@ int launch_features_bwd_local(const dn_csr* g, const float* xd, const float* pq,
 int launch_features_bwd_transpose(const dn_csr* gt, const float* U, int rotations, int64_t V, int C, float* dxd,
                                   float* dP, float* dQ, int64_t ld_pq, cudaStream_t st) {
   if (V <= 0) return DN_OK;
-  if (C % 4) return DN_ERR_UNSUPPORTED;
+  const float2* vals = reinterpret_cast<const float2*>(gt->vals);
+  if (C % 4) {
+    const unsigned sb = (unsigned)((V * C + 255) / 256);
+    if (rotations)
+      features_bwd_transpose_scalar_kernel<true><<<sb, 256, 0, st>>>(gt->rowptr, gt->colidx, vals, U, V, C, dxd, dP, dQ, ld_pq);
+    else
+      features_bwd_transpose_scalar_kernel<false><<<sb, 256, 0, st>>>(gt->rowptr, gt->colidx, vals, U, V, C, dxd, dP, dQ, ld_pq);
+    DN_LAUNCH_CHECK();
+    return DN_OK;
+  }
   const int G = pick_group(C);
   const int64_t warps = (V + (32 / G) - 1) / (32 / G);
   const unsigned blocks = (unsigned)((warps * 32 + 255) / 256);
-  const float2* vals = reinterpret_cast<const float2*>(gt->vals);
   if (rotations)
     features_bwd_transpose_kernel<true><<<blocks, 256, 0, st>>>(gt->rowptr, gt->colidx, vals, U, V, C, G, dxd, dP, dQ, ld_pq);
   else

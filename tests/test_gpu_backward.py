@@ -427,17 +427,23 @@ BLOCK_CASES = {   # name: (n, m, K, C, block keyword arguments)
     "tiny": (5, 10, 40, 16, {}),
     "full": (400, 500, 128, 128, {}),
     "config2": (84, 84, 128, 128, {}),
+    # C % 4 != 0: the scalar-lane feature gather and its two backward kernels
+    "c1": (20, 25, 64, 1, {}), "c3": (20, 25, 64, 3, {}), "c6": (20, 25, 64, 6, {}), "c30": (20, 25, 64, 30, {}),
+    # a MiniMLP deeper than one fused chain (8 layers): layer by layer, forward and backward
+    "mlp9": (20, 25, 64, 64, {"mlp_hidden_dims": [64] * 8}), "mlp12": (20, 25, 64, 64, {"mlp_hidden_dims": [64] * 11}),
 }
 
 
 def _block_run(dn, engine, name, chk, floor=False):
     n, m, K, C, kw = BLOCK_CASES[name]
+    kw = dict(kw)
+    hid = kw.pop("mlp_hidden_dims", [C, C])
     V = n * m
     mass, L, evals, evecs, gX, gY = dn.synthetic.structural_operators(n, m, K, seed=5, device="cuda")
-    params = dn.synthetic.block_weights(C, seed=5, **kw)
+    params = dn.synthetic.block_weights(C, seed=5, mlp_hidden_dims=hid, **kw)
     g = _gen(21)
     x, R = torch.randn(V, C, generator=g), torch.randn(V, C, generator=g)
-    blk = dn.DiffusionNetBlock(C_width=C, mlp_hidden_dims=[C, C], dropout=False, **kw)
+    blk = dn.DiffusionNetBlock(C_width=C, mlp_hidden_dims=hid, dropout=False, **kw)
     blk.load_state_dict(params, strict=True)
     blk = blk.cuda().train()
     xg = x.cuda().unsqueeze(0).requires_grad_(True)
@@ -467,6 +473,15 @@ def _block_run(dn, engine, name, chk, floor=False):
     chk("grad_x", xg.grad[0], x64.grad[0], tol[1], f32[1].grad[0] if floor else None)
     for pname, p_ in blk.named_parameters():
         assert p_.grad is not None, pname
+        if C == 1 and pname.endswith("A_im.weight"):
+            # one channel: g0 b_re + g1 b_im = A_re (g0^2 + g1^2), A_im cancels and its gradient is 0 in exact arithmetic;
+            # ours is rounding, held to the bound relative to A_re's gradient
+            scale = prm[pname.replace("A_im", "A_re")].grad.abs().max().item()
+            err = (p_.grad.detach().cpu().double() - prm[pname].grad).abs().max().item() / scale
+            print("[measured] {} grad {} err={:.3e} (of max|grad A_re|)".format(chk.label, pname, err))
+            if not err < tol[2]:
+                chk.misses.append("grad {}: {:.3e} >= {:.1e}".format(pname, err, tol[2]))
+            continue
         chk("grad " + pname, p_.grad, prm[pname].grad, tol[2], f32[2][pname].grad if floor else None)
 
 

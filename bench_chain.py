@@ -1,10 +1,11 @@
-"""Per-chain timing of the fused row-chain kernel (rows_chain_kernel) at the headline block's shapes.
+"""Per-chain timing of the fused row-chain kernel (rows_chain_kernel), and of to_basis, at the headline block's shapes.
 
 Each chain is called alone through its C-ABI entry point, tc3x, K = C = 128:
 
   from_basis   dn_from_basis,   evecs (V, 128) -> (V, 128)
   pq           dn_mini_mlp_fwd, one 128 -> 256 layer (the [P|Q] shape of the gradient features)
   mlp          dn_mini_mlp_fwd, cat(3 x (V, 128)) -> 128 -> 128 with ReLU, biases and the residual (the MiniMLP)
+  to_basis     dn_to_basis,     evecs^T (mass * x): the split-V to_basis kernel and its partial reduction
 
 A call is the weight-pack launch (a few microseconds) plus the chain launch; it is timed with CUDA events over
 --iters calls after --warmup calls.  Bytes and TF32 MMA operations come from the shapes (3 MMA passes in tc3x); the
@@ -45,6 +46,8 @@ def chain_model(name, V):
         layers, rows_in, rows_out = [(K, C)], K, C
     elif name == "pq":
         layers, rows_in, rows_out = [(C, 2 * C)], C, 2 * C
+    elif name == "to_basis":  # evecs, x and mass in; a K x C result (no weights)
+        return 4 * V * (K + C + 1), 2 * V * K * C * PASSES, 0
     else:  # mlp: 3 sources + residual in, C out
         layers, rows_in, rows_out = [(3 * C, C), (C, C), (C, C)], 4 * C, C
     hbm = 4 * V * (rows_in + rows_out)
@@ -127,7 +130,14 @@ def main():
         def call_mlp():
             _lib.check(lib.dn_mini_mlp_fwd(*mlp_args, ws.data_ptr(), ws.numel(), eng, st), "dn_mini_mlp_fwd")
 
-        for name, fn in (("from_basis", call_fb), ("pq", call_pq), ("mlp", call_mlp)):
+        mass = torch.rand(V, device=dev, generator=g) + 0.5
+        out_kc = torch.empty(K, C, device=dev)
+
+        def call_tb():
+            _lib.check(lib.dn_to_basis(x.data_ptr(), evecs.data_ptr(), mass.data_ptr(), V, K, C, out_kc.data_ptr(),
+                                       ws.data_ptr(), ws.numel(), eng, st), "dn_to_basis")
+
+        for name, fn in (("from_basis", call_fb), ("pq", call_pq), ("mlp", call_mlp), ("to_basis", call_tb)):
             ms = timed(fn, args.iters, args.warmup)
             hbm, flops, l2w = chain_model(name, V)
             rows.append({

@@ -26,16 +26,27 @@ using namespace tc;
 
 constexpr int KC = 16;                          // k-elements per weight stage
 constexpr int TILE_M = 128;                     // vertex rows per tile: two consumer warpgroups of 64 rows
-constexpr int NST = 4;                          // weight stages in flight
-constexpr int STAGE_BYTES = KC * 256 * 8;       // 32 KiB: tf32 hi | lo images of a 256-wide layer
+constexpr int W_RING_BYTES = 128 * 1024;        // weight ring: as many stages of the instantiation's width as fit
+constexpr int W_NST_MAX = 8;                    // ... but no deeper than this
 constexpr int CHAIN_THREADS = 384;              // warpgroups 0, 1: consumers; warpgroup 2: producers (two lanes)
 // first-layer activations: 16-column x 128-row fp32 stages, each two 8-column boxes of [128 rows][8 floats]
 constexpr int A_BOX_BYTES = 8 * TILE_M * 4;     // 4 KiB
 constexpr int A_STAGE_BYTES = 2 * A_BOX_BYTES;
 constexpr int A_NST = 8;                        // activation stages in flight (64 KiB per SM)
-constexpr int CHAIN_SMEM = NST * STAGE_BYTES + A_NST * A_STAGE_BYTES + 256;
 
 enum { MODE_TF32 = 1, MODE_TF32X3 = 3, MODE_BF16 = DN_PASSES_BF16 };
+
+// Weight ring of rows_chain_kernel<MODE, NMAX>: a slot holds one K stage of an NMAX-wide layer as the producer streams
+// it (tf32x3: hi | lo images, 8 bytes per weight; tf32: hi, 4; bf16: 2).  At NMAX = 128 / 256: tc3x 8 slots of 16 KiB /
+// 4 of 32 KiB; tc1x 8 of 8 KiB / 8 of 16 KiB; bf16 8 of 4 KiB / 8 of 8 KiB.  (With 16 slots for the narrower stages,
+// repeated bf16 mesh-batch forwards once gave differing bits; the cause was not found, so the depth stays at 8.)
+template <int MODE, int NMAX>
+struct ChainRing {
+  static constexpr int STAGE = KC * NMAX * (MODE == MODE_TF32X3 ? 8 : MODE == MODE_TF32 ? 4 : 2);
+  static constexpr int NST = W_RING_BYTES / STAGE < W_NST_MAX ? W_RING_BYTES / STAGE : W_NST_MAX;
+  static constexpr int BARS = 8 * (2 * NST + 2 * A_NST);   // full / empty of both rings
+  static constexpr int SMEM = NST * STAGE + A_NST * A_STAGE_BYTES + BARS;
+};
 
 // bytes of one packed K stage of an N-wide layer: tf32 hi image (KC * N * 4) then lo image; bf16 uses the first quarter
 __host__ __device__ __forceinline__ int64_t stage_stride(int N) { return (int64_t)KC * N * 8; }
@@ -174,8 +185,9 @@ struct HcParams {
 // half-warp's float2 reads (rows g = 0..3 of its warp, columns 2t, 2t+1) cover 128 consecutive bytes: every bank once,
 // no conflict and no swizzle.  A stage whose columns lie in two sources (widths that are multiples of 8, not of 16)
 // is two boxes from two tensor maps.  Consumers read their fragments, issue the stage's MMAs and release the slot
-// (a proxy fence, then one arrival per warp); the producer meanwhile runs ahead into the next tile's first layer while the consumers are
-// in the epilogue and the later layers.
+// (a proxy fence, then one arrival per warp); the producer meanwhile runs ahead into the next tile's first layer while
+// the consumers are in the epilogue and the later layers.  The weight ring (ChainRing) is as deep as the
+// instantiation's stage width allows.
 // Per lane, the accumulator of an N-wide layer holds rows (16w+g, 16w+g+8) x columns (8b+2t, 8b+2t+1)
 // for every 8-column block b: after the epilogue these values are the next layer's A fragments (columns of a 16-wide
 // K stage: tf32 steps use the permuted weight order of pack_store, bf16 steps the natural one).  NMAX <= 128 chains
@@ -187,6 +199,7 @@ template <int MODE, int NMAX, bool WIDE>
 __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __grid_constant__ HcParams p) {
   constexpr bool kChain = NMAX <= 128;
   constexpr int NB = NMAX / 16;
+  constexpr int NST = ChainRing<MODE, NMAX>::NST, STAGE_BYTES = ChainRing<MODE, NMAX>::STAGE;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* aring = smem + NST * STAGE_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(aring + A_NST * A_STAGE_BYTES);
@@ -268,6 +281,8 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
       // register budget together (ptxas spills or serializes), so each stage waits for its own MMAs (up to six
       // full-width MMAs per stage; the other consumer warpgroup keeps the tensor cores busy meanwhile).  `two` marks
       // a stage whose second k8 slice lies inside K (a literal wherever it is known at compile time).
+      // Weight slots: where a stage waits for its own MMAs (wait<0>) it hands its slot back right there; under wait<1>
+      // the previous stage's slot is handed back once that stage's MMAs are done.
       auto stage = [&](int c, const float2* q, bool two) {
         mbar_wait(full + 8 * s, ph);
         uint32_t ah[2][4], al[2][4];
@@ -330,10 +345,14 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
           }
         }
         wgmma_commit();
-        if constexpr (WIDE && MODE != MODE_BF16) wgmma_wait<0>();
-        else wgmma_wait<1>();                  // the previous stage's MMAs are done: hand its slot back
-        if (prev >= 0 && lane == 0) mbar_arrive(empty + 8 * prev);
-        prev = (int)s;
+        if constexpr (WIDE && MODE != MODE_BF16) {
+          wgmma_wait<0>();                     // this stage's MMAs are done: hand its own slot back
+          if (lane == 0) mbar_arrive(empty + 8 * s);
+        } else {
+          wgmma_wait<1>();                     // the previous stage's MMAs are done: hand its slot back
+          if (prev >= 0 && lane == 0) mbar_arrive(empty + 8 * prev);
+          prev = (int)s;
+        }
         if (++s == NST) { s = 0; ph ^= 1; }
       };
 
@@ -351,8 +370,10 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
             q[3] = *reinterpret_cast<const float2*>(a + A_BOX_BYTES / 4 + 64);
           }
           stage(c, q, two);
-          // the slot is handed back once the stage's fragments are formed from the loaded values, behind a proxy fence:
-          // the producer's next TMA write to it (async proxy) must not overtake these generic-proxy reads
+          // the slot is handed back once the stage's fragments are formed from the loaded values and its MMAs issued,
+          // behind a proxy fence: the producer's next TMA write to it (async proxy) must not overtake these
+          // generic-proxy reads.  (Handing it back before the MMAs, even behind the same fence, made two identical
+          // bf16 forwards differ.)
           fence_proxy_async();
           __syncwarp();
           if (lane == 0) mbar_arrive(aempty + 8 * as);
@@ -593,19 +614,31 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
 #pragma unroll
       for (int i = 0; i < 64; ++i) sum[256 * i] += acc[i];
     }                                      // (this warp's MMAs of chunk c - 2 are done: waited for in chunk c - 1)
+    // B image: element i of this thread is e = 256 i + thread (KC * C = 256 NBC elements).  Every load is issued
+    // before any is used: the mass values (global) before the two waits below, so their latency overlaps them, and the
+    // x values (staging ring) as one batch.  Loaded one element at a time behind a branch, each global round trip came
+    // in series with the next.  Rows >= nv read a valid row and are then replaced by zero.
+    float mv[NBC], xv[NBC];
+    if (p.mass) {
+#pragma unroll
+      for (int i = 0; i < NBC; ++i) {
+        const int vv = (256 * i + (int)threadIdx.x) / C;
+        mv[i] = __ldg(p.mass + v0 + (vv < nv ? vv : nv - 1));
+      }
+    }
     named_bar_sync(1, 256);                // every warp's MMAs of chunk c - 2 are done: its B slot is free
     mbar_wait(st_full + 8 * s, ph);
     const float* rphi = reinterpret_cast<const float*>(raw + s * TB_RAW);
     const float* rx = reinterpret_cast<const float*>(raw + s * TB_RAW + TB_RAW_HALF);
     uint8_t* bh = bimg + (c & 1) * TB_BSTAGE;
-    for (int e0 = 0; e0 < KC * C; e0 += 256) {   // KC * C is a multiple of 256: the same trip count in every thread
-      const int e = e0 + (int)threadIdx.x;
+#pragma unroll
+    for (int i = 0; i < NBC; ++i) xv[i] = rx[256 * i + (int)threadIdx.x];   // row vv, channel cc: vv * C + cc = e
+#pragma unroll
+    for (int i = 0; i < NBC; ++i) {
+      const int e = 256 * i + (int)threadIdx.x;
       const int vv = e / C, cc = e - vv * C;
       float x = 0.f;
-      if (vv < nv) {
-        x = rx[vv * C + cc];
-        if (p.mass) x *= __ldg(p.mass + v0 + vv);           // (values * massvec), geometry.py:583
-      }
+      if (vv < nv) x = p.mass ? xv[i] * mv[i] : xv[i];     // (values * massvec), geometry.py:583
       float hi, lo;
       split_tf32_fast(x, hi, lo);
       const uint32_t off = (vv >> 2) * C * 16 + (cc >> 3) * 128 + (cc & 7) * 16 + (vv & 3) * 4;
@@ -713,8 +746,9 @@ void launch_to_basis(int nbc, int grid, const TcToBasisParams& p, cudaStream_t s
 }
 template <int MODE>
 bool set_chain_smem() {
-  return set_smem(rows_chain_kernel<MODE, 128, false>, CHAIN_SMEM) && set_smem(rows_chain_kernel<MODE, 128, true>, CHAIN_SMEM) &&
-         set_smem(rows_chain_kernel<MODE, 256, false>, CHAIN_SMEM) && set_smem(rows_chain_kernel<MODE, 256, true>, CHAIN_SMEM);
+  constexpr int s128 = ChainRing<MODE, 128>::SMEM, s256 = ChainRing<MODE, 256>::SMEM;
+  return set_smem(rows_chain_kernel<MODE, 128, false>, s128) && set_smem(rows_chain_kernel<MODE, 128, true>, s128) &&
+         set_smem(rows_chain_kernel<MODE, 256, false>, s256) && set_smem(rows_chain_kernel<MODE, 256, true>, s256);
 }
 
 // cuTensorMapEncodeTiled from the driver the runtime already loaded (no link dependency on libcuda); null if absent
@@ -857,12 +891,13 @@ int tc_pack_layers(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, co
 // wide: every layer is exactly 128 wide, or the single layer is 256 wide (full-width MMAs)
 template <int MODE>
 static void launch_chain(const HcParams& p, int nmax, bool wide, int grid, cudaStream_t st) {
+  constexpr int s128 = ChainRing<MODE, 128>::SMEM, s256 = ChainRing<MODE, 256>::SMEM;
   if (nmax <= 128) {
-    if (wide) rows_chain_kernel<MODE, 128, true><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
-    else rows_chain_kernel<MODE, 128, false><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
+    if (wide) rows_chain_kernel<MODE, 128, true><<<grid, CHAIN_THREADS, s128, st>>>(p);
+    else rows_chain_kernel<MODE, 128, false><<<grid, CHAIN_THREADS, s128, st>>>(p);
   } else {
-    if (wide) rows_chain_kernel<MODE, 256, true><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
-    else rows_chain_kernel<MODE, 256, false><<<grid, CHAIN_THREADS, CHAIN_SMEM, st>>>(p);
+    if (wide) rows_chain_kernel<MODE, 256, true><<<grid, CHAIN_THREADS, s256, st>>>(p);
+    else rows_chain_kernel<MODE, 256, false><<<grid, CHAIN_THREADS, s256, st>>>(p);
   }
 }
 

@@ -45,7 +45,9 @@ struct ChainRing {
   static constexpr int STAGE = KC * NMAX * (MODE == MODE_TF32X3 ? 8 : MODE == MODE_TF32 ? 4 : 2);
   static constexpr int NST = W_RING_BYTES / STAGE < W_NST_MAX ? W_RING_BYTES / STAGE : W_NST_MAX;
   static constexpr int BARS = 8 * (2 * NST + 2 * A_NST);   // full / empty of both rings
-  static constexpr int SMEM = NST * STAGE + A_NST * A_STAGE_BYTES + BARS;
+  // every layer's bias, staged once per CTA (NMAX = 256 chains run a single layer)
+  static constexpr int BIAS = (NMAX <= 128 ? DN_MAX_LAYERS : 1) * NMAX * 4;
+  static constexpr int SMEM = NST * STAGE + A_NST * A_STAGE_BYTES + BIAS + BARS;
 };
 
 // bytes of one packed K stage of an N-wide layer: tf32 hi image (KC * N * 4) then lo image; bf16 uses the first quarter
@@ -202,7 +204,8 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
   constexpr int NST = ChainRing<MODE, NMAX>::NST, STAGE_BYTES = ChainRing<MODE, NMAX>::STAGE;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* aring = smem + NST * STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(aring + A_NST * A_STAGE_BYTES);
+  float* sbias = reinterpret_cast<float*>(aring + A_NST * A_STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(aring + A_NST * A_STAGE_BYTES + ChainRing<MODE, NMAX>::BIAS);
   const uint32_t full = smem_u32(bars), empty = smem_u32(bars + NST);
   const uint32_t afull = smem_u32(bars + 2 * NST), aempty = smem_u32(bars + 2 * NST + A_NST);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -259,6 +262,15 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
 
   // ===================== consumers =====================
   setmaxnreg_inc<232>();
+  // The biases go to shared memory once per CTA.  Read from global memory in the epilogue they were one round trip per
+  // column block (the epilogue's loads are kept in series, see below), and the residual and output traffic of the
+  // tiles evicts them from L1: the two hidden-layer epilogues of the MiniMLP took about 10,000 cycles each that way.
+  for (int l = 0; l < L; ++l) {
+    const HcLayer& Lr = p.layer[l];
+    if (!Lr.bias) continue;
+    for (int n = threadIdx.x; n < Lr.N; n += 256) sbias[l * NMAX + n] = __ldg(Lr.bias + n);
+  }
+  named_bar_sync(1, 256);                     // the consumers' copies are done (the producers do not take part)
   const int g = lane >> 2, t = lane & 3;
   const int rloc = (warp >> 2) * 64 + (warp & 3) * 16 + g;
   float acc[NB * 8];
@@ -274,6 +286,22 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
       const int K = (WIDE && l > 0) ? NMAX : Lr.K, nst = (K + KC - 1) / KC;
       const uint32_t lbo = (uint32_t)N * 16;
       int prev = -1;
+      // The epilogue reads the rows' residual, emul and relu-mask values from global memory one column block after the
+      // other (their loads cannot all be in flight at once: the registers do not fit), so each is a round trip.  Asking
+      // L2 for those rows now, while this layer's MMAs run, makes every one of those round trips an L2 hit.  The four
+      // lanes that share a row pair ask for one 128-byte line each of every 512 bytes; lane 0 also for the row's end.
+      auto prefetch_rows = [&](const float* base, int64_t ld) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!(h ? ok1 : ok0)) continue;
+          const char* row = reinterpret_cast<const char*>(base + (h ? r1 : r0) * ld);
+          for (int b = 128 * t; b < N * 4; b += 512) prefetch_l2(row + b);
+          if (t == 0) prefetch_l2(row + N * 4 - 4);
+        }
+      };
+      if (Lr.residual) prefetch_rows(Lr.residual, Lr.ld_res);
+      if (Lr.emul) prefetch_rows(Lr.emul, N);
+      if (Lr.relu_mask) prefetch_rows(Lr.relu_mask, N);
       // one K stage: q[0], q[1] = rows (r0, r1) x columns (2t, 2t+1); q[2], q[3] the same 8 columns further.  All A
       // fragments of the stage are formed before wgmma_fence, so the MMAs read registers the fence already covers and
       // ptxas has no reason to order them.  One commit group per stage, at most two stages in flight -- except in the
@@ -414,7 +442,8 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
           float* d = acc + 8 * j + 4 * h;
           float2 v0 = make_float2(d[0], d[1]), v1 = make_float2(d[2], d[3]);
           if (Lr.bias) {
-            const float b0 = __ldg(Lr.bias + col), b1 = __ldg(Lr.bias + col + 1);
+            const float2 b = *reinterpret_cast<const float2*>(sbias + l * NMAX + col);
+            const float b0 = b.x, b1 = b.y;
             v0.x += b0; v0.y += b1; v1.x += b0; v1.y += b1;
           }
           if (Lr.relu) {

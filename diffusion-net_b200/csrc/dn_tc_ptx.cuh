@@ -46,6 +46,10 @@ __device__ __forceinline__ void fence_barrier_init() {
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// brings the 128-byte line holding `p` into L2 (a hint: no register, no completion to wait for)
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
 // named barrier over `count` threads (a multiple of 32)
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");

@@ -68,6 +68,12 @@ class dn_mesh_batch(C.Structure):
                 ("mesh_cta_begin", C.c_void_p)]
 
 
+class dn_eig_batch(C.Structure):
+    _fields_ = [("n_meshes", C.c_int32), ("n_tiles", C.c_int32), ("n_slices", C.c_int32), ("row_begin", C.c_void_p),
+                ("tile_mesh", C.c_void_p), ("tile_begin", C.c_void_p), ("slice_mesh", C.c_void_p),
+                ("slice_begin", C.c_void_p)]
+
+
 class dn_head(C.Structure):
     _fields_ = [("weight", C.c_void_p), ("bias", C.c_void_p), ("n_out", C.c_int32), ("out", C.c_void_p), ("ld_out", C.c_int64)]
 
@@ -110,6 +116,12 @@ SIGNATURES = {
     "dn_eig_rotate": (_I, [_P, _L, _P, _L, _L, _I, _I, _D, _P, _L, _P]),
     "dn_eig_residual_norms": (_I, [_P, _L, _P, _L, _P, _L, _I, _P, _P, _L, _P]),
     "dn_eig_finalize": (_I, [_P, _L, _P, _I, _P, _L, _P, _P, _L, _P]),
+    "dn_mesh_laplacian_batched": (_I, [_P, _P, _L, _L, _I, _P, _D, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P]),
+    "dn_eig_filter_batched": (_I, [_P, _P, _P, _P, C.POINTER(dn_eig_batch), _I, _P, _P, _L, _P, _P, _P, _P, _P, _P]),
+    "dn_eig_gram_batched": (_I, [_P, _L, _P, _L, C.POINTER(dn_eig_batch), _I, _I, _P, _P, _P, _L, _P]),
+    "dn_eig_rotate_batched": (_I, [_P, _L, _P, C.POINTER(dn_eig_batch), _I, _I, _D, _P, _P, _L, _P]),
+    "dn_eig_residual_norms_batched": (_I, [_P, _L, _P, _L, _P, C.POINTER(dn_eig_batch), _I, _P, _P, _P, _L, _P]),
+    "dn_eig_finalize_batched": (_I, [_P, _L, _P, _I, _P, C.POINTER(dn_eig_batch), _P, _P, _L, _P]),
     "dn_implicit_diffusion_workspace_bytes": (_L, [_L, _I]),
     "dn_implicit_diffusion_fwd": (_I, [C.POINTER(dn_csr), _P, _P, _P, _L, _I, _D, _I, _P, _P, _P, _L, _P]),
     "dn_implicit_diffusion_bwd": (_I, [C.POINTER(dn_csr), _P, _P, _P, _P, _L, _I, _D, _I, _P, _P, _P, _P, _L, _P]),

@@ -412,6 +412,78 @@ int dn_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, co
   return launch_eig_finalize(Y, ldy, cols, k, mass, V, out, (double*)workspace, (cudaStream_t)stream);
 }
 
+int dn_mesh_laplacian_batched(const double* verts, const int64_t* faces, int64_t F, int64_t V, int n_meshes,
+                              const int32_t* row_begin, double eps, int32_t* rowptr_out, int32_t* colidx_out,
+                              double* L_vals_out, double* mass_out, double* A_vals_out, double* A_diag_out,
+                              double* bound_out, int32_t* nan_out, void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  if (V < 0 || F < 0 || n_meshes < 0 || !rowptr_out || (n_meshes > 0 && (!row_begin || !bound_out || !nan_out)) ||
+      (F > 0 && (!faces || !verts)) || (V > 0 && (n_meshes == 0 || !colidx_out || !L_vals_out || !mass_out)))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (6 * F + V >= (1ll << 31) || V >= (1ll << 31) - 1) return DN_ERR_UNSUPPORTED;
+  if (V > 0 && (!workspace || ws_bytes < mesh_laplacian_ws_bytes(F, V))) return DN_ERR_WORKSPACE;
+  return launch_mesh_laplacian_batched(verts, faces, F, V, n_meshes, row_begin, eps, rowptr_out, colidx_out, L_vals_out,
+                                       mass_out, A_vals_out, A_diag_out, bound_out, nan_out, workspace,
+                                       (cudaStream_t)stream);
+}
+
+static bool eig_batch_ok(const dn_eig_batch* bt) {
+  return bt && bt->n_meshes >= 0 && bt->n_tiles >= 0 && bt->n_slices >= 0 && bt->n_slices <= 65535 &&
+         (bt->n_meshes == 0 || (bt->n_meshes <= 65535 && bt->row_begin && bt->tile_begin && bt->slice_begin)) &&
+         (bt->n_tiles == 0 || bt->tile_mesh) && (bt->n_slices == 0 || bt->slice_mesh);
+}
+
+int dn_eig_filter_batched(const int32_t* rowptr, const int32_t* colidx, const double* A_vals, const double* A_diag,
+                          const dn_eig_batch* batch, int n, const double* Y, const double* Y_prev, int64_t ld,
+                          const double* alpha, const double* beta, const double* gamma, const int32_t* active,
+                          double* Y_out, dn_stream_t stream) {
+  if (!eig_batch_ok(batch) || n < 0 || ld < n ||
+      (batch->n_tiles > 0 && n > 0 && (!rowptr || !colidx || !A_vals || !A_diag || !Y || !Y_out || !alpha || !beta || !gamma)) ||
+      (Y_out && (Y_out == Y || Y_out == Y_prev)))
+    return DN_ERR_INVALID_ARGUMENT;
+  if ((int64_t)batch->n_tiles * 8 >= (1ll << 31)) return DN_ERR_UNSUPPORTED;
+  return launch_eig_filter_batched(rowptr, colidx, A_vals, A_diag, batch, n, Y, Y_prev, ld, alpha, beta, gamma, active,
+                                   Y_out, (cudaStream_t)stream);
+}
+
+int dn_eig_gram_batched(const double* X, int64_t ldx, const double* Y, int64_t ldy, const dn_eig_batch* batch, int m, int n,
+                        const int32_t* active, double* out, void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  if (!eig_batch_ok(batch) || m < 0 || n < 0 || ldx < m || ldy < n ||
+      (m > 0 && n > 0 && batch->n_meshes > 0 && (!out || (batch->n_tiles > 0 && (!X || !Y)))))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (m > 0 && n > 0 && batch->n_slices > 0 && (!workspace || ws_bytes < eig_gram_batched_ws_bytes(batch->n_slices, m, n)))
+    return DN_ERR_WORKSPACE;
+  return launch_eig_gram_batched(X, ldx, Y, ldy, batch, m, n, active, out, (double*)workspace, (cudaStream_t)stream);
+}
+
+int dn_eig_rotate_batched(const double* X, int64_t ldx, const double* C, const dn_eig_batch* batch, int kd, int n,
+                          double beta, const int32_t* active, double* Z, int64_t ldz, dn_stream_t stream) {
+  if (!eig_batch_ok(batch) || kd < 0 || n < 0 || ldx < kd || ldz < n ||
+      (batch->n_tiles > 0 && n > 0 && (!Z || (kd > 0 && (!X || !C)))) || (Z && Z == X))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (batch->n_tiles > 65535) return DN_ERR_UNSUPPORTED;
+  return launch_eig_rotate_batched(X, ldx, C, batch, kd, n, beta, active, Z, ldz, (cudaStream_t)stream);
+}
+
+int dn_eig_residual_norms_batched(const double* W, int64_t ldw, const double* Q, int64_t ldq, const double* theta,
+                                  const dn_eig_batch* batch, int n, const int32_t* active, double* out, void* workspace,
+                                  int64_t ws_bytes, dn_stream_t stream) {
+  if (!eig_batch_ok(batch) || n < 0 || ldw < n || ldq < n ||
+      (n > 0 && batch->n_meshes > 0 && (!out || !theta || (batch->n_tiles > 0 && (!W || !Q)))))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (n > 0 && batch->n_slices > 0 && (!workspace || ws_bytes < eig_resid_batched_ws_bytes(batch->n_slices, n)))
+    return DN_ERR_WORKSPACE;
+  return launch_eig_residual_norms_batched(W, ldw, Q, ldq, theta, batch, n, active, out, (double*)workspace,
+                                           (cudaStream_t)stream);
+}
+
+int dn_eig_finalize_batched(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass,
+                            const dn_eig_batch* batch, double* out, void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  if (!eig_batch_ok(batch) || k < 0 || (batch->n_tiles > 0 && k > 0 && (!Y || !cols || !mass || !out)))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (batch->n_tiles > 0 && k > 0 && (!workspace || ws_bytes < 8ll * batch->n_meshes * k)) return DN_ERR_WORKSPACE;
+  return launch_eig_finalize_batched(Y, ldy, cols, k, mass, batch, out, (double*)workspace, (cudaStream_t)stream);
+}
+
 int64_t dn_implicit_diffusion_workspace_bytes(int64_t V, int C) {
   if (V < 0 || C <= 0) return -1;
   return implicit_ws_bytes(V, C);

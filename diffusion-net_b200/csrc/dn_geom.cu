@@ -322,10 +322,16 @@ __global__ void lap_rows_kernel(const int32_t* __restrict__ rawptr, const int32_
   area[v] = a;
 }
 
-// mass += eps * mean(mass), one block, fixed summation order
-__global__ void __launch_bounds__(1024) lap_mass_shift_kernel(double* __restrict__ mass, int64_t V, double eps) {
+// mass += eps * mean(mass) per mesh, one block each, fixed summation order; block b owns rows [row_begin[b],
+// row_begin[b + 1]) (all V rows without row_begin)
+__global__ void __launch_bounds__(1024) lap_mass_shift_kernel(double* __restrict__ mass, const int32_t* __restrict__ row_begin,
+                                                              int64_t V, double eps) {
   __shared__ double part[1024];
   const int t = threadIdx.x;
+  if (row_begin) {
+    mass += row_begin[blockIdx.x];
+    V = row_begin[blockIdx.x + 1] - row_begin[blockIdx.x];
+  }
   double s = 0.0;
   for (int64_t i = t; i < V; i += 1024) s += mass[i];
   part[t] = s;
@@ -340,15 +346,25 @@ __global__ void __launch_bounds__(1024) lap_mass_shift_kernel(double* __restrict
 
 // Merge the sorted raw row into the final CSR row (diagonal at its column position), and the operator the eigensolver
 // runs on, A = M^-1/2 (L + eps I) M^-1/2, as A_vals (same pattern: d_v d_k L_vk) + A_diag (eps / m_v).  Row bound of
-// Gershgorin's theorem -> max into bound_bits; NaN counts -> nan_out[0] (L rows) and nan_out[1] (mass entries).
+// Gershgorin's theorem -> max into bound_bits; NaN counts -> nan_out[0] (L rows) and nan_out[1] (mass entries).  With
+// row_begin (n_meshes + 1 row offsets of a batch of meshes) the bound and the NaN counts are kept per mesh.
 __global__ void lap_emit_kernel(const int32_t* __restrict__ rawptr, const int32_t* __restrict__ rawcol,
                                 const LapVal* __restrict__ rawval, const int32_t* __restrict__ ref,
                                 const double* __restrict__ mass, int64_t V, double eps, const int32_t* __restrict__ rowptr,
                                 int32_t* __restrict__ colidx, double* __restrict__ lvals, double* __restrict__ avals,
                                 double* __restrict__ adiag, unsigned long long* __restrict__ bound_bits,
-                                int32_t* __restrict__ nan_out) {
+                                int32_t* __restrict__ nan_out, int n_meshes, const int32_t* __restrict__ row_begin) {
   const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= V) return;
+  if (row_begin) {                      // the vertex's mesh b: bound_bits[b], nan_out[2 b .. 2 b + 1]
+    int lo = 0, hi = n_meshes - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (row_begin[mid] <= v) lo = mid; else hi = mid - 1;
+    }
+    bound_bits += lo;
+    nan_out += 2 * lo;
+  }
   const int s = rawptr[v], e = rawptr[v + 1];
   const double dv = 1.0 / sqrt(mass[v]);
   double diag = 0.0;
@@ -470,12 +486,15 @@ T* carve(char*& p, int64_t count) {
 int64_t mesh_laplacian_ws_bytes(int64_t F, int64_t V) { return 120 * F + 12 * V + 2048; }
 int64_t vertex_frames_ws_bytes(int64_t F, int64_t V) { return 12 * F + 8 * V + 1024; }
 
-int launch_mesh_laplacian(const double* verts, const int64_t* faces, int64_t F, int64_t V, double eps, int32_t* rowptr,
-                          int32_t* colidx, double* lvals, double* mass, double* avals, double* adiag, double* bound,
-                          int32_t* nan_out, void* ws, cudaStream_t st) {
+// row_begin == nullptr: one mesh.  Otherwise the union of n_meshes meshes (faces index the union's rows): every kernel but
+// the mass shift and the emit is per face or per row and runs on the union unchanged.
+static int mesh_laplacian_impl(const double* verts, const int64_t* faces, int64_t F, int64_t V, int n_meshes,
+                               const int32_t* row_begin, double eps, int32_t* rowptr, int32_t* colidx, double* lvals,
+                               double* mass, double* avals, double* adiag, double* bound, int32_t* nan_out, void* ws,
+                               cudaStream_t st) {
   DN_CUDA_TRY(cudaMemsetAsync(rowptr, 0, sizeof(int32_t) * (V + 1), st));
-  DN_CUDA_TRY(cudaMemsetAsync(bound, 0, sizeof(double), st));
-  DN_CUDA_TRY(cudaMemsetAsync(nan_out, 0, 2 * sizeof(int32_t), st));
+  DN_CUDA_TRY(cudaMemsetAsync(bound, 0, sizeof(double) * n_meshes, st));
+  DN_CUDA_TRY(cudaMemsetAsync(nan_out, 0, 2 * sizeof(int32_t) * n_meshes, st));
   if (V <= 0) return DN_OK;
   char* p = static_cast<char*>(ws);
   int32_t* rawcol = carve<int32_t>(p, 6 * F);
@@ -503,12 +522,28 @@ int launch_mesh_laplacian(const double* verts, const int64_t* faces, int64_t F, 
   DN_LAUNCH_CHECK();
   tr_scan_kernel<<<1, 1024, 0, st>>>(rowptr, V + 1);
   DN_LAUNCH_CHECK();
-  lap_mass_shift_kernel<<<1, 1024, 0, st>>>(mass, V, eps);
+  lap_mass_shift_kernel<<<(unsigned)n_meshes, 1024, 0, st>>>(mass, row_begin, V, eps);
   DN_LAUNCH_CHECK();
   lap_emit_kernel<<<vb, 256, 0, st>>>(rawptr, rawcol, rawval, ref, mass, V, eps, rowptr, colidx, lvals, avals, adiag,
-                                      reinterpret_cast<unsigned long long*>(bound), nan_out);
+                                      reinterpret_cast<unsigned long long*>(bound), nan_out, n_meshes, row_begin);
   DN_LAUNCH_CHECK();
   return DN_OK;
+}
+
+int launch_mesh_laplacian(const double* verts, const int64_t* faces, int64_t F, int64_t V, double eps, int32_t* rowptr,
+                          int32_t* colidx, double* lvals, double* mass, double* avals, double* adiag, double* bound,
+                          int32_t* nan_out, void* ws, cudaStream_t st) {
+  return mesh_laplacian_impl(verts, faces, F, V, 1, nullptr, eps, rowptr, colidx, lvals, mass, avals, adiag, bound, nan_out,
+                             ws, st);
+}
+
+int launch_mesh_laplacian_batched(const double* verts, const int64_t* faces, int64_t F, int64_t V, int n_meshes,
+                                  const int32_t* row_begin, double eps, int32_t* rowptr, int32_t* colidx, double* lvals,
+                                  double* mass, double* avals, double* adiag, double* bound, int32_t* nan_out, void* ws,
+                                  cudaStream_t st) {
+  if (n_meshes <= 0) return DN_OK;
+  return mesh_laplacian_impl(verts, faces, F, V, n_meshes, row_begin, eps, rowptr, colidx, lvals, mass, avals, adiag, bound,
+                             nan_out, ws, st);
 }
 
 int launch_vertex_frames(const double* verts, const int64_t* faces, int64_t F, int64_t V, const double* normals_in,

@@ -129,6 +129,26 @@ int launch_eig_residual_norms(const double* W, int64_t ldw, const double* Q, int
                               int n, double* out, double* ws, cudaStream_t st);
 int launch_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass, int64_t V,
                         double* out, double* sign_ws, cudaStream_t st);
+// the same over a batch of meshes laid out by dn_eig_batch (a mesh with active[b] == 0 is skipped; active may be null)
+int launch_mesh_laplacian_batched(const double* verts, const int64_t* faces, int64_t F, int64_t V, int n_meshes,
+                                  const int32_t* row_begin, double eps, int32_t* rowptr, int32_t* colidx, double* lvals,
+                                  double* mass, double* avals, double* adiag, double* bound, int32_t* nan_out, void* ws,
+                                  cudaStream_t st);
+int64_t eig_gram_batched_ws_bytes(int n_slices, int m, int n);
+int64_t eig_resid_batched_ws_bytes(int n_slices, int n);
+int launch_eig_filter_batched(const int32_t* rowptr, const int32_t* colidx, const double* avals, const double* adiag,
+                              const dn_eig_batch* bt, int n, const double* Y, const double* Yp, int64_t ld,
+                              const double* alpha, const double* beta, const double* gamma, const int32_t* active,
+                              double* out, cudaStream_t st);
+int launch_eig_gram_batched(const double* X, int64_t ldx, const double* Y, int64_t ldy, const dn_eig_batch* bt, int m, int n,
+                            const int32_t* active, double* out, double* ws, cudaStream_t st);
+int launch_eig_rotate_batched(const double* X, int64_t ldx, const double* Cm, const dn_eig_batch* bt, int kd, int n,
+                              double beta, const int32_t* active, double* Z, int64_t ldz, cudaStream_t st);
+int launch_eig_residual_norms_batched(const double* W, int64_t ldw, const double* Q, int64_t ldq, const double* theta,
+                                      const dn_eig_batch* bt, int n, const int32_t* active, double* out, double* ws,
+                                      cudaStream_t st);
+int launch_eig_finalize_batched(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass,
+                                const dn_eig_batch* bt, double* out, double* sign_ws, cudaStream_t st);
 // implicit diffusion (dn_implicit.cu): one cooperative block-PCG solve of (M + diag(t) (x) L) Y = b, fp64 state
 int64_t implicit_ws_bytes(int64_t V, int C);
 int launch_implicit_diffusion(const dn_csr* L, const float* mass, float* time, const float* rhs, const float* y,

@@ -234,3 +234,274 @@ def lowest_eigenpairs(op, k, seed=0, stats=None):
                      filter_ms=sum(a.elapsed_time(b) for a, b in filter_ms),
                      rr_ms=sum(a.elapsed_time(b) for a, b in rr_ms))
     return evals, evecs
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the same iteration for a batch of small meshes, as one launch sequence
+# ----------------------------------------------------------------------------------------------------------------------
+TILE_ROWS, SLICE_ROWS = 64, 1024        # DN_EIG_TILE_ROWS, DN_EIG_SLICE_ROWS of the header
+
+
+class BatchPlan:
+    """``dn_eig_batch`` for meshes of ``Vs`` vertices laid out one after the other: the struct and its device arrays."""
+
+    def __init__(self, Vs, device):
+        import numpy as np
+        Vs = np.asarray(Vs, dtype=np.int64)
+        n = len(Vs)
+        begin = lambda c: np.concatenate(([0], np.cumsum(c)))
+        tiles, slices = -(-Vs // TILE_ROWS), -(-Vs // SLICE_ROWS)
+        self.row_begin = begin(Vs)
+        if self.row_begin[-1] >= 2 ** 31 - 1:
+            raise ValueError("a batch of {} rows exceeds the int32 row index".format(int(self.row_begin[-1])))
+        parts = [self.row_begin, np.repeat(np.arange(n), tiles), begin(tiles), np.repeat(np.arange(n), slices), begin(slices)]
+        offs = begin([len(p) for p in parts])
+        self.arrays = torch.from_numpy(np.concatenate(parts).astype(np.int32)).to(device)   # kept alive next to the struct
+        ptr = [self.arrays.data_ptr() + 4 * int(o) for o in offs[:5]]
+        self.n, self.V, self.n_slices = n, int(self.row_begin[-1]), int(slices.sum())
+        self.struct = _lib.dn_eig_batch(n, int(tiles.sum()), self.n_slices, *ptr)
+
+
+class _BatchSolver:
+    """_Solver's kernels on the concatenated V x B blocks of the meshes of a batch (full blocks: nothing is locked)."""
+
+    def __init__(self, ops_, k, B, seed):
+        import ctypes
+        self.k, self.B, self.n = k, B, len(ops_)
+        self.lib = _lib.load()
+        dev = self.dev = ops_[0].mass.device
+        f64 = torch.float64
+        self.plan = BatchPlan([op.V for op in ops_], dev)
+        self.bt = ctypes.byref(self.plan.struct)
+        V, rb = self.plan.V, self.plan.row_begin
+        # one block-diagonal CSR with batch-global columns
+        nz = [0]
+        for op in ops_:
+            nz.append(nz[-1] + int(op.colidx.numel()))
+        self.rowptr = torch.cat([op.rowptr[:-1] + nz[b] for b, op in enumerate(ops_)] +
+                                [torch.tensor([nz[-1]], dtype=torch.int32, device=dev)]).to(torch.int32)
+        self.colidx = torch.cat([op.colidx + int(rb[b]) for b, op in enumerate(ops_)]).to(torch.int32)
+        self.avals = torch.cat([op.avals for op in ops_])
+        self.adiag = torch.cat([op.adiag for op in ops_])
+        self.mass = torch.cat([op.mass for op in ops_])
+        # every mesh starts from the block lowest_eigenpairs would start from: its start does not depend on the batch
+        self.Q = torch.empty(V, B, device=dev, dtype=f64)
+        gen = torch.Generator(device=dev)
+        for b, op in enumerate(ops_):
+            gen.manual_seed(seed)
+            self.Q[int(rb[b]):int(rb[b + 1])] = torch.randn(op.V, B, generator=gen, device=dev, dtype=f64)
+        self.T = [torch.empty(V, B, device=dev, dtype=f64) for _ in range(2)]
+        self.W = torch.empty(V, B, device=dev, dtype=f64)
+        self.W2 = torch.empty(V, B, device=dev, dtype=f64)
+        self.ws = torch.empty(max(8 * self.plan.n_slices * B * B, 8 * self.n * B, 4096), dtype=torch.uint8, device=dev)
+        self.active = torch.ones(self.n, dtype=torch.int32, device=dev)
+        self.act = torch.arange(self.n, device=dev)                  # indices of the active meshes
+        self.G = torch.zeros(self.n, B, B, dtype=f64, device=dev)    # Gram / rotation stacks, all meshes
+        self.Cm = torch.zeros(self.n, B, B, dtype=f64, device=dev)
+        self.eye = torch.eye(B, dtype=f64, device=dev)
+        self.unit = torch.tensor([[1.0] * self.n, [0.0] * self.n, [0.0] * self.n], dtype=f64, device=dev)
+        self.steps = 0
+        self.dense_ev = []
+
+    def set_active(self, flags):
+        self.active = torch.tensor([int(f) for f in flags], dtype=torch.int32, device=self.dev)
+        self.act = torch.tensor([b for b, f in enumerate(flags) if f], dtype=torch.int64, device=self.dev)
+
+    def filt(self, src, prev, dst, coef):
+        """coef: (3, n) device rows alpha, beta, gamma"""
+        _check(self.lib.dn_eig_filter_batched(self.rowptr.data_ptr(), self.colidx.data_ptr(), self.avals.data_ptr(),
+                                              self.adiag.data_ptr(), self.bt, self.B, src.data_ptr(),
+                                              prev.data_ptr() if prev is not None else None, self.B, coef[0].data_ptr(),
+                                              coef[1].data_ptr(), coef[2].data_ptr(), self.active.data_ptr(),
+                                              dst.data_ptr(), ops._stream()), "dn_eig_filter_batched")
+
+    def gram(self, X, Y):
+        _check(self.lib.dn_eig_gram_batched(X.data_ptr(), self.B, Y.data_ptr(), self.B, self.bt, self.B, self.B,
+                                            self.active.data_ptr(), self.G.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
+                                            ops._stream()), "dn_eig_gram_batched")
+        G = self.G[self.act]
+        return 0.5 * (G + G.transpose(1, 2))
+
+    def rotate(self, X, Cm, Z):
+        _check(self.lib.dn_eig_rotate_batched(X.data_ptr(), self.B, Cm.data_ptr(), self.bt, self.B, self.B, 0.0,
+                                              self.active.data_ptr(), Z.data_ptr(), self.B, ops._stream()),
+               "dn_eig_rotate_batched")
+
+    def _dense(self, fn):
+        a = _event()
+        r = fn()
+        self.dense_ev.append((a, _event()))
+        return r
+
+    def chebyshev(self, degree, lo, cut, hi):
+        """_Solver.chebyshev with every mesh's own (lo, cut, hi): the coefficients of all steps go up in one copy."""
+        import numpy as np
+        e, c = (hi - cut) / 2.0, (hi + cut) / 2.0
+        sigma = e / (lo - c)
+        sigma1 = sigma
+        coef = np.zeros((degree, 3, self.n))
+        coef[0, 0], coef[0, 1] = sigma1 / e, -c * sigma1 / e
+        for d in range(1, degree):
+            sigma2 = 1.0 / (2.0 / sigma1 - sigma)
+            a = 2.0 * sigma2 / e
+            coef[d] = a, -c * a, -sigma * sigma2
+            sigma = sigma2
+        coef = torch.from_numpy(coef).to(self.dev)
+        bufs = [self.Q, self.T[0], self.T[1]]
+        prev, cur = 0, 1
+        self.filt(bufs[prev], None, bufs[cur], coef[0])
+        for d in range(1, degree):
+            nxt = 3 - prev - cur
+            self.filt(bufs[cur], bufs[prev], bufs[nxt], coef[d])
+            prev, cur = cur, nxt
+        self.steps += degree
+        return bufs[cur]
+
+    def orthonormalize(self, Y):
+        """CholQR2 per mesh on (n_active, B, B) stacks; SVQB for exactly the meshes whose Cholesky fails (one host read
+        of the info vector per pass)."""
+        for _ in range(2):
+            G = self.gram(Y, Y)
+
+            def dense():
+                R, info = torch.linalg.cholesky_ex(G, upper=True)
+                bad = torch.nonzero(info).flatten()                  # host read
+                R[bad] = self.eye
+                Cm = torch.linalg.solve_triangular(R, self.eye.expand_as(R), upper=True)
+                if bad.numel():
+                    Gb = G[bad]
+                    d = Gb.diagonal(dim1=1, dim2=2).clamp_min(1e-300).rsqrt()
+                    S, U = torch.linalg.eigh(d[:, :, None] * Gb * d[:, None, :])
+                    S = torch.maximum(S, S.max(dim=1, keepdim=True).values * 1e-15)
+                    Cm[bad] = d[:, :, None] * U * S.rsqrt()[:, None, :]
+                self.Cm[self.act] = Cm
+            self._dense(dense)
+            Z = next(b for b in (self.T[0], self.T[1], self.W2) if b is not Y)
+            self.rotate(Y, self.Cm, Z)
+            Y = Z
+        return Y
+
+    def rayleigh_ritz(self, Z, theta_all, res_all):
+        """Ritz vectors of the active meshes into Q, A times them into W2; their rows of theta_all / res_all updated."""
+        self.filt(Z, None, self.W, self.unit)
+        H = self.gram(Z, self.W)
+
+        def dense():
+            theta, U = torch.linalg.eigh(H)
+            self.Cm[self.act] = U
+            theta_all[self.act] = theta
+        self._dense(dense)
+        self.rotate(Z, self.Cm, self.Q)
+        self.rotate(self.W, self.Cm, self.W2)
+        _check(self.lib.dn_eig_residual_norms_batched(self.W2.data_ptr(), self.B, self.Q.data_ptr(), self.B,
+                                                      theta_all.data_ptr(), self.bt, self.B, self.active.data_ptr(),
+                                                      res_all.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
+                                                      ops._stream()), "dn_eig_residual_norms_batched")
+
+
+def lowest_eigenpairs_batch(ops_, k, seed=0, stats=None, first=0):
+    """``lowest_eigenpairs`` for a list of ``LaplaceOperator`` (the meshes of one dataset, a few hundred to some ten
+    thousand vertices each): a list of its ``(evals, evecs)`` pairs, in order.
+
+    The meshes whose block has the full width ``B = k + guard`` are iterated together on their concatenated rows: each
+    filter step, Gram matrix, rotation and residual is one launch over all of them (dn_eig_*_batched), the B x B dense
+    steps are batched ``torch.linalg`` calls on an (n_active, B, B) stack, and the host reads the Ritz values and
+    residuals of all meshes in one copy per outer iteration (plus the Cholesky info vector of each of the two
+    orthonormalisation passes).  Same constants and the same per-mesh convergence test as ``lowest_eigenpairs``; what
+    differs: nothing is locked (every active mesh iterates its full block -- at these sizes the filter is the cheap
+    part, and ragged widths would need a launch per width), and one filter degree per outer iteration serves the whole
+    batch, the largest any active mesh asks for (each mesh keeps its own damped interval [cut_b, bound_b]; the scaled
+    recurrence makes a higher degree than needed harmless).  A converged mesh turns inactive: its Ritz vectors stay
+    where they are and no later launch touches its rows.  A mesh's start block, tile and slice cuts are its own, so
+    every kernel gives it the bits it would get alone; only the shared degree ties it to its batch, which moves its
+    eigenpairs within the solver's tolerance.  Two calls on the same list give bitwise-equal results.
+
+    A mesh with ``V < k + guard`` (a narrower block) is solved by ``lowest_eigenpairs``; ``k >= V`` raises its
+    ValueError, prefixed with ``mesh {i}: `` like every other per-mesh failure (i counts from ``first``, the index of
+    ``ops_[0]`` in the caller's list).
+    ``stats`` (dict, optional) receives iterations, filter_steps, block, n_stacked and filter / Rayleigh-Ritz / dense
+    ``torch.linalg`` times in ms (the dense time is part of the Rayleigh-Ritz time)."""
+    import numpy as np
+    n, k = len(ops_), int(k)
+    for i, op in enumerate(ops_):
+        if 0 < k and k >= op.V:
+            raise ValueError("mesh {}: failed to compute eigendecomp: k_eig = {} is not below the vertex count {}"
+                             .format(first + i, k, op.V))
+    out = [None] * n
+    if k <= 0:
+        return [lowest_eigenpairs(op, k, seed=seed) for op in ops_]
+    B = k + max(16, k // 4)
+    stack = [i for i, op in enumerate(ops_) if op.V >= B]
+    for i, op in enumerate(ops_):
+        if op.V < B:
+            try:
+                out[i] = lowest_eigenpairs(op, k, seed=seed)
+            except ValueError as e:
+                raise ValueError("mesh {}: {}".format(first + i, e)) from None
+    it, s = 0, None
+    if stack:
+        sops = [ops_[i] for i in stack]
+        m = len(sops)
+        s = _BatchSolver(sops, k, B, seed)
+        dev = s.dev
+        bound = np.array([op.bound for op in sops])
+        theta_all = torch.zeros(m, B, dtype=torch.float64, device=dev)
+        res_all = torch.zeros(m, B, dtype=torch.float64, device=dev)
+        t0 = _event()
+        s.rayleigh_ritz(s.orthonormalize(s.Q), theta_all, res_all)
+        rr_ev, filter_ev = [(t0, _event())], []
+        active = np.ones(m, dtype=bool)
+        while True:
+            host = torch.stack((theta_all, res_all)).cpu().numpy()      # the outer iteration's one read of both
+            th, res = host[0], host[1]
+            tol = np.maximum(RES_TOL * np.abs(th[:, k - 1]), RES_FLOOR * bound)
+            active &= ~(res[:, :k] <= tol[:, None]).all(axis=1)
+            if not active.any():
+                break
+            who = [stack[b] for b in np.nonzero(active)[0]]
+            if it >= MAX_ITERATIONS:
+                raise ValueError("mesh {}: failed to compute eigendecomp: {} filter iterations ({} steps) did not reach "
+                                 "residual {:.1e}".format(first + who[0], it, s.steps, tol[active][0]))
+            cut, lo = th[:, -1].copy(), th[:, 0].copy()
+            if (cut[active] >= bound[active]).any():
+                b = int(np.nonzero(active & (cut >= bound))[0][0])
+                raise ValueError("mesh {}: failed to compute eigendecomp: the block's Ritz values reach the spectral bound"
+                                 .format(first + stack[b]))
+            cut[~active], lo[~active] = 0.5 * bound[~active], 0.0       # placeholders: inactive rows are not touched
+            e, c = (bound - cut) / 2.0, (bound + cut) / 2.0
+            need = MIN_DEGREE
+            for b in np.nonzero(active)[0]:
+                for i in range(k):
+                    r = res[b, i]
+                    if r > tol[b]:
+                        t = abs((th[b, i] - c[b]) / e[b])
+                        if t > 1.0 + 1e-12:
+                            need = max(need, math.ceil(math.acosh(r / tol[b]) / math.acosh(t)))
+                        else:
+                            need = MAX_DEGREE
+            degree = min(max(need, MIN_DEGREE), MAX_DEGREE)
+            s.set_active(active)
+            f0 = _event()
+            Y = s.chebyshev(degree, lo, cut, bound)
+            f1 = _event()
+            s.rayleigh_ritz(s.orthonormalize(Y), theta_all, res_all)
+            rr_ev.append((f1, _event()))
+            filter_ev.append((f0, f1))
+            it += 1
+        # eigh returns every mesh's Ritz values ascending and nothing was locked: the k lowest are the first k columns
+        cols = torch.arange(k, dtype=torch.int32, device=dev).repeat(m, 1).contiguous()
+        evecs = torch.empty(s.plan.V, k, dtype=torch.float64, device=dev)
+        _check(s.lib.dn_eig_finalize_batched(s.Q.data_ptr(), B, cols.data_ptr(), k, s.mass.data_ptr(), s.bt,
+                                             evecs.data_ptr(), s.ws.data_ptr(), s.ws.numel(), ops._stream()),
+               "dn_eig_finalize_batched")
+        evals = theta_all[:, :k].clamp_min(0.0)
+        rb = s.plan.row_begin
+        for b, i in enumerate(stack):
+            out[i] = (evals[b], evecs[int(rb[b]):int(rb[b + 1])])
+    if stats is not None:
+        stats.update(iterations=it, filter_steps=s.steps if s else 0, block=B, n_stacked=len(stack))
+        if s:
+            torch.cuda.synchronize(s.dev)
+            ms = lambda evs: sum(a.elapsed_time(b) for a, b in evs)
+            stats.update(filter_ms=ms(filter_ev), rr_ms=ms(rr_ev), dense_ms=ms(s.dense_ev))
+    return out

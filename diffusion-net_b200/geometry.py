@@ -199,11 +199,35 @@ def get_operators(verts, faces, k_eig=128, op_cache_dir=None, normals=None, over
 
 
 def get_all_operators(verts_list, faces_list, k_eig, op_cache_dir=None, normals=None, device=None,
-                      compute_missing=False):
-    """geometry.py:395-424: seven parallel lists; ``normals[i]`` goes with mesh i."""
-    outs = [get_operators(v, f, k_eig, op_cache_dir, normals=None if normals is None else normals[i], device=device,
-                          compute_missing=compute_missing)
-            for i, (v, f) in enumerate(zip(verts_list, faces_list))]
+                      compute_missing=False, batch_misses=False):
+    """geometry.py:395-424: seven parallel lists; ``normals[i]`` goes with mesh i.
+    ``batch_misses`` (extra, with ``compute_missing``): the meshes without a usable cache entry are built together by
+    ``compute_operators_batch`` -- one launch sequence per group of small meshes instead of one eigensolve after the
+    other -- and written to the same buckets in the same format; hits are read as without it."""
+    if not (batch_misses and compute_missing):
+        outs = [get_operators(v, f, k_eig, op_cache_dir, normals=None if normals is None else normals[i], device=device,
+                              compute_missing=compute_missing)
+                for i, (v, f) in enumerate(zip(verts_list, faces_list))]
+        return tuple([o[i] for o in outs] for i in range(7))
+    outs, misses = [None] * len(verts_list), []
+    for i, (v, f) in enumerate(zip(verts_list, faces_list)):
+        if np.isnan(_to_np(v)).any():
+            raise RuntimeError("tried to construct operators from NaN verts")
+        npz = find_cached_operators(v, f, k_eig, op_cache_dir) if op_cache_dir is not None else None
+        if npz is None:
+            misses.append(i)
+        else:
+            outs[i] = load_operators_npz(npz, k_eig=k_eig, device=torch.device(device) if device is not None else v.device,
+                                         dtype=v.dtype)
+    if misses:
+        built = _compute_operators_batch([verts_list[i] for i in misses], [faces_list[i] for i in misses], k_eig,
+                                         None if normals is None else [normals[i] for i in misses], device, None, None)
+        for i, (out, g) in zip(misses, built):
+            outs[i] = out
+            if op_cache_dir is not None:
+                os.makedirs(op_cache_dir, exist_ok=True)
+                write_operators_npz(find_cache_bucket(verts_list[i], faces_list[i], op_cache_dir), verts_list[i],
+                                    faces_list[i], k_eig, out, g)
     return tuple([o[i] for o in outs] for i in range(7))
 
 
@@ -352,6 +376,187 @@ def _compute_operators(verts, faces, k_eig, normals, device, stats):
             ms = [a.elapsed_time(b) for a, b in zip(ev[:-1], ev[1:])]
             stats.update(frames_ms=ms[0], laplacian_ms=ms[1], eig_ms=ms[2], build_grad_ms=ms[3], **est)
     return out, g
+
+
+# ------------------------------------------------------------------------------------------------
+# the same for a dataset of small meshes: one launch sequence per group of meshes
+# ------------------------------------------------------------------------------------------------
+def batch_groups(n_rows, max_rows):
+    """Consecutive index ranges ``[(i0, i1), ...]`` covering ``range(len(n_rows))`` in order: each group takes meshes
+    while its vertex total stays within ``max_rows`` (a single mesh above ``max_rows`` is a group of its own)."""
+    groups, i0, total = [], 0, 0
+    for i, v in enumerate(n_rows):
+        if i > i0 and total + v > max_rows:
+            groups.append((i0, i))
+            i0, total = i, 0
+        total += v
+    if len(n_rows) > i0:
+        groups.append((i0, len(n_rows)))
+    return groups
+
+
+def compute_operators_batch(verts_list, faces_list, k_eig, normals=None, device=None, max_rows=None, stats=None):
+    """``compute_operators`` for a list of triangle meshes (a dataset of small meshes, a few hundred to some ten
+    thousand vertices each): a list of its seven-tuples, in order, same dtypes and placement, gradX / gradY registered
+    against their prepared CSR.  The meshes of a group are laid out as one disjoint union: frames, Laplacian + mass and
+    ``build_grad`` run once on the union (``dn_mesh_laplacian_batched``; the frame and gradient kernels are per vertex
+    and work on a union as they are), and ``eigen.lowest_eigenpairs_batch`` iterates all meshes together.
+
+    frames, mass, L, gradX and gradY of every mesh are bitwise what ``compute_operators`` returns for it alone; evals /
+    evecs come from a different iteration (no locking, one filter degree for the meshes of a group) and agree to the
+    solver's tolerance, with it and between two different lists.  Two calls on the same list give bitwise-equal results.
+
+    ``normals`` is a list (entries may be None).  All meshes share one dtype.  ``max_rows`` caps the vertex total of a
+    group (default: what fits a third of the free device memory, at five V x B fp64 blocks, the eigenvectors and the
+    Laplacian's workspace per vertex); a longer list is processed group by group.  Errors are ``compute_operators``'
+    own, prefixed with ``mesh {i}: ``.  ``stats`` (dict, optional) receives the stage times in ms summed over the
+    groups (``laplacian_ms`` includes the upload and the face range check, ``split_ms`` is the cutting of the union
+    into per-mesh tensors), the number of groups and the solver's counters per group (``eig``)."""
+    return [o for o, _ in _compute_operators_batch(verts_list, faces_list, k_eig, normals, device, max_rows, stats)]
+
+
+def _compute_operators_batch(verts_list, faces_list, k_eig, normals, device, max_rows, stats):
+    """compute_operators_batch, returning (tuple, ops.GradOperators) per mesh."""
+    n = len(verts_list)
+    if n == 0:
+        return []
+    device = torch.device(device) if device is not None else verts_list[0].device
+    if device.type != "cuda":
+        raise RuntimeError("diffusion_net_b200 keeps operators on CUDA devices only (no CPU path); got {}".format(device))
+    dtype = verts_list[0].dtype
+    for i, (v, f) in enumerate(zip(verts_list, faces_list)):
+        if f.numel() == 0:
+            raise NotImplementedError("mesh {}: point clouds need robust_laplacian.point_cloud_laplacian and a KNN graph; "
+                                      "only triangle meshes are supported".format(i))
+        if v.dtype != dtype:
+            raise ValueError("mesh {}: the meshes of one call share a dtype ({} after {})".format(i, v.dtype, dtype))
+    k_eig = int(k_eig)
+    Vs = [int(v.shape[0]) for v in verts_list]
+    if max_rows is None:
+        B = k_eig + max(16, k_eig // 4)
+        with torch.cuda.device(device):
+            max_rows = max(torch.cuda.mem_get_info()[0] // 3 // (5 * 8 * B + 8 * k_eig + 2048), 1)
+    out = []
+    groups = batch_groups(Vs, int(max_rows))
+    if stats is not None:
+        stats.update(groups=len(groups), frames_ms=0.0, laplacian_ms=0.0, eig_ms=0.0, build_grad_ms=0.0, split_ms=0.0, eig=[])
+    with torch.cuda.device(device):
+        for i0, i1 in groups:
+            out += _compute_group(verts_list[i0:i1], faces_list[i0:i1], k_eig,
+                                  [None] * (i1 - i0) if normals is None else list(normals[i0:i1]), device, dtype, i0, stats)
+    return out
+
+
+def _compute_group(verts_list, faces_list, k_eig, normals, device, dtype, first, stats):
+    from . import eigen
+    lib = _lib_load()
+    n = len(verts_list)
+    ev = []
+    mark = lambda: ev.append(torch.cuda.Event(enable_timing=True)) or ev[-1].record()
+    mark()
+    Vs = [int(v.shape[0]) for v in verts_list]
+    rb = np.concatenate(([0], np.cumsum(Vs)))
+    V = int(rb[-1])
+    v64s = [torch.as_tensor(v).detach().to(device=device, dtype=torch.float64).contiguous() for v in verts_list]
+    f64s = [torch.as_tensor(f).detach().to(device=device, dtype=torch.int64).reshape(-1, 3) for f in faces_list]
+    lohi = torch.stack([torch.stack(torch.aminmax(f)) for f in f64s]).cpu().numpy()      # one read for the range check
+    for b in range(n):
+        if lohi[b, 0] < 0 or lohi[b, 1] >= Vs[b]:
+            raise ValueError("mesh {}: faces index vertices outside [0, {})".format(first + b, Vs[b]))
+    v64 = torch.cat(v64s)
+    f64 = torch.cat([f + int(rb[b]) for b, f in enumerate(f64s)]).contiguous()
+    F = int(f64.shape[0])
+    row_begin = torch.from_numpy(rb.astype(np.int32)).to(device)
+    # Laplacian + mass of the union, (mass shift, bound, NaN flags) per mesh
+    cap = max(6 * F + V, 1)
+    rowptr = torch.empty(V + 1, dtype=torch.int32, device=device)
+    colidx = torch.empty(cap, dtype=torch.int32, device=device)
+    lvals = torch.empty(cap, dtype=torch.float64, device=device)
+    avals = torch.empty(cap, dtype=torch.float64, device=device)
+    mass = torch.empty(V, dtype=torch.float64, device=device)
+    adiag = torch.empty(V, dtype=torch.float64, device=device)
+    bound = torch.empty(n, dtype=torch.float64, device=device)
+    nan = torch.empty(n, 2, dtype=torch.int32, device=device)
+    ws = torch.empty(120 * F + 12 * V + 2048, dtype=torch.uint8, device=device)
+    _lib_check(lib.dn_mesh_laplacian_batched(v64.data_ptr(), f64.data_ptr(), F, V, n, row_begin.data_ptr(), EPS,
+                                             rowptr.data_ptr(), colidx.data_ptr(), lvals.data_ptr(), mass.data_ptr(),
+                                             avals.data_ptr(), adiag.data_ptr(), bound.data_ptr(), nan.data_ptr(),
+                                             ws.data_ptr(), ws.numel(), ops._stream()), "dn_mesh_laplacian_batched")
+    del ws
+    host = torch.cat((bound, nan.flatten().double(), rowptr[row_begin.long()].double())).cpu().numpy()
+    bound_h, nan_h, nzb = host[:n], host[n:3 * n].reshape(n, 2), host[3 * n:].astype(np.int64)
+    for b in range(n):
+        if nan_h[b, 0]:
+            raise RuntimeError("mesh {}: NaN Laplace matrix".format(first + b))
+        if nan_h[b, 1]:
+            raise RuntimeError("mesh {}: NaN mass matrix".format(first + b))
+    nnz = int(nzb[-1])
+    colidx, lvals, avals = colidx[:nnz], lvals[:nnz], avals[:nnz]
+    mark()
+    # frames of the union; a mesh with a NaN normal takes compute_operators' own route (its remedy is a host step)
+    frames = torch.empty(V, 3, 3, dtype=torch.float64, device=device)
+    nbad = torch.zeros(1, dtype=torch.int32, device=device)
+    nrm = torch.empty(V, 3, dtype=torch.float64, device=device)
+    ws = torch.empty(12 * F + 8 * V + 1024, dtype=torch.uint8, device=device)
+    _lib_check(lib.dn_vertex_frames(v64.data_ptr(), f64.data_ptr(), F, V, None, nrm.data_ptr(), frames.data_ptr(),
+                                    nbad.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()), "dn_vertex_frames")
+    redo = []
+    if int(nbad.item()) > 0:
+        bad_rows = torch.isnan(nrm).any(dim=1).cpu().numpy()
+        redo = [b for b in range(n) if normals[b] is None and bad_rows[rb[b]:rb[b + 1]].any()]
+    for b, nb in enumerate(normals):
+        if nb is not None:
+            nrm[rb[b]:rb[b + 1]] = nb.to(device=device, dtype=torch.float64)
+    n_in = nrm.to(dtype).to(torch.float64).contiguous()
+    _lib_check(lib.dn_vertex_frames(None, None, F, V, n_in.data_ptr(), None, frames.data_ptr(), nbad.data_ptr(), None, 0,
+                                    ops._stream()), "dn_vertex_frames")
+    for b in redo:
+        frames[rb[b]:rb[b + 1]] = _vertex_frames(v64s[b], f64s[b].contiguous(), None, dtype, verts_list[b])
+    mark()
+    # per-mesh views of the union's CSR with local indices, and the eigenpairs
+    rows = torch.repeat_interleave(torch.arange(V, device=device), (rowptr[1:] - rowptr[:-1]).long(), output_size=nnz)
+    off = torch.repeat_interleave(row_begin[:-1].long(), torch.from_numpy(np.diff(nzb)).to(device), output_size=nnz)
+    col_local = (colidx.long() - off).to(torch.int32)
+    lops = []
+    for b in range(n):
+        r0, r1, p0, p1 = int(rb[b]), int(rb[b + 1]), int(nzb[b]), int(nzb[b + 1])
+        lops.append(eigen.LaplaceOperator(Vs[b], rowptr[r0:r1 + 1] - p0, col_local[p0:p1], avals[p0:p1], adiag[r0:r1],
+                                          mass[r0:r1], bound_h[b]))
+    est = {} if stats is not None else None
+    pairs = eigen.lowest_eigenpairs_batch(lops, k_eig, stats=est, first=first)
+    mark()
+    # build_grad on the union's pattern (one entry more than L's in the row of a vertex no face references)
+    g = build_grad_operators(v64.to(torch.float32), frames.to(torch.float32), torch.stack((rows, colidx.long()), 0))
+    _, grp, gci, gvals = g.csr
+    gnzb = grp[row_begin.long()].cpu().numpy().astype(np.int64)
+    goff = torch.repeat_interleave(row_begin[:-1].long(), torch.from_numpy(np.diff(gnzb)).to(device), output_size=g.nnz)
+    gcol_local = (gci[:g.nnz].long() - goff).to(torch.int32)
+    gv = gvals[:2 * g.nnz].view(-1, 2)
+    mark()
+    out = []
+    lvals32 = lvals.to(torch.float32).to(dtype)
+    rows_local = rows - off
+    for b in range(n):
+        r0, r1, p0, p1 = int(rb[b]), int(rb[b + 1]), int(nzb[b]), int(nzb[b + 1])
+        q0, q1 = int(gnzb[b]), int(gnzb[b + 1])
+        gb = ops.GradOperators.from_csr(Vs[b], grp[r0:r1 + 1] - q0, gcol_local[q0:q1], gv[q0:q1].clone())
+        if dtype == torch.float32:
+            gradX, gradY = gb.to_sparse_coo()
+            ops.register_prepared(gradX, gradY, gb)
+        else:
+            gradX, gradY = (t.to(dtype) for t in gb.to_sparse_coo())
+        idx = torch.stack((rows_local[p0:p1], col_local[p0:p1].long()), 0)
+        L = torch.sparse_coo_tensor(idx, lvals32[p0:p1].clone(), (Vs[b], Vs[b]), is_coalesced=True)
+        evals, evecs = pairs[b]
+        out.append(((frames[r0:r1].to(dtype), mass[r0:r1].to(dtype), L, evals.to(dtype), evecs.to(dtype), gradX, gradY), gb))
+    mark()
+    if stats is not None:
+        torch.cuda.synchronize(device)
+        ms = [a.elapsed_time(b) for a, b in zip(ev[:-1], ev[1:])]
+        for key, t in zip(("laplacian_ms", "frames_ms", "eig_ms", "build_grad_ms", "split_ms"), ms):
+            stats[key] += t
+        stats["eig"].append(est)
+    return out
 
 
 # ------------------------------------------------------------------------------------------------

@@ -278,6 +278,62 @@ int dn_eig_residual_norms(const double* W, int64_t ldw, const double* Q, int64_t
 int dn_eig_finalize(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass, int64_t V, double* out,
                     void* workspace, int64_t ws_bytes, dn_stream_t stream);
 
+/* ---- the same for a batch of small meshes, as one launch sequence ---------------------------------------------------
+ * Mesh b owns rows [row_begin[b], row_begin[b + 1]) of every V x n block (V = row_begin[n_meshes]), of mass / A_diag
+ * and of one block-diagonal CSR whose column indices are batch-global.  Inside each mesh, starting at its first row,
+ * rows are cut into tiles of DN_EIG_TILE_ROWS (what one CTA of a row-parallel kernel owns) and into slices of
+ * DN_EIG_SLICE_ROWS (what one partial sum of a reduction over rows covers); the partial sums of a mesh are added in
+ * slice order.  So no tile or slice spans two meshes, and a mesh's results do not depend on which other meshes share the
+ * batch or on its position in it.  All arrays are device int32, built by the caller; the kernels trust them. */
+#define DN_EIG_TILE_ROWS 64
+#define DN_EIG_SLICE_ROWS 1024
+typedef struct dn_eig_batch {
+  int32_t n_meshes;
+  int32_t n_tiles;                /* sum over meshes of ceil(V_b / DN_EIG_TILE_ROWS)                    */
+  int32_t n_slices;               /* sum over meshes of ceil(V_b / DN_EIG_SLICE_ROWS)                   */
+  const int32_t* row_begin;       /* [n_meshes + 1]                                                     */
+  const int32_t* tile_mesh;       /* [n_tiles]: mesh of every tile                                      */
+  const int32_t* tile_begin;      /* [n_meshes + 1]: the tiles of mesh b are [begin[b], begin[b + 1])   */
+  const int32_t* slice_mesh;      /* [n_slices]                                                         */
+  const int32_t* slice_begin;     /* [n_meshes + 1]                                                     */
+} dn_eig_batch;
+
+/* dn_mesh_laplacian on the union of n_meshes meshes: `verts` (V, 3) is their concatenation, `faces` (F, 3) index the
+ * union (each mesh's faces offset by its row_begin, every face inside its own mesh -- the caller checks), row_begin is
+ * device int32 [n_meshes + 1].  The outputs are the union's (block-diagonal CSR, batch-global columns), and the rows of
+ * every mesh are bitwise what dn_mesh_laplacian gives for that mesh alone: the mass shift eps * mean(mass_b),
+ * bound_out[b] and nan_out[2 b], nan_out[2 b + 1] are kept per mesh (bound_out: n_meshes doubles, nan_out: 2 n_meshes
+ * ints).  Capacities and workspace as for dn_mesh_laplacian with the union's F and V. */
+int dn_mesh_laplacian_batched(const double* verts, const int64_t* faces, int64_t F, int64_t V, int n_meshes,
+                              const int32_t* row_begin, double eps, int32_t* rowptr_out, int32_t* colidx_out,
+                              double* L_vals_out, double* mass_out, double* A_vals_out, double* A_diag_out,
+                              double* bound_out, int32_t* nan_out, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
+/* The eigensolver's kernels over such a batch; blocks are row-major V x n with leading dimension ld as above.
+ * `active` (device int32 [n_meshes], may be NULL = all): nothing of a mesh with active[b] == 0 is read or written, in
+ * the blocks or in the per-mesh outputs.  Reductions use no atomics: results are bitwise reproducible.
+ * filter: Y_out = alpha[b] (A Y) + beta[b] Y + gamma[b] Y_prev on the rows of mesh b; alpha, beta, gamma are device
+ *   arrays of n_meshes doubles; Y_prev may be NULL; Y_out must not alias Y or Y_prev.
+ * gram: out[b] (m x n, dense; out is (n_meshes, m, n)) = X_b^T Y_b.  workspace: 8 n_slices m n bytes.
+ * rotate: Z_b = beta Z_b + X_b C[b], X (V x kd), C (n_meshes, kd, n) dense; Z must not alias X.
+ * residual_norms: out[b][c] = || W_b[:, c] - theta[b][c] Q_b[:, c] ||_2; theta and out are (n_meshes, n).
+ *   workspace: 8 n_slices n bytes.
+ * finalize: out (V x k, dense) rows of mesh b = s_bi M^-1/2 Y_b[:, cols[b][i]], cols (n_meshes, k) device int32, with
+ *   dn_eig_finalize's sign rule inside each mesh.  workspace: 8 n_meshes k bytes. */
+int dn_eig_filter_batched(const int32_t* rowptr, const int32_t* colidx, const double* A_vals, const double* A_diag,
+                          const dn_eig_batch* batch, int n, const double* Y, const double* Y_prev, int64_t ld,
+                          const double* alpha, const double* beta, const double* gamma, const int32_t* active,
+                          double* Y_out, dn_stream_t stream);
+int dn_eig_gram_batched(const double* X, int64_t ldx, const double* Y, int64_t ldy, const dn_eig_batch* batch, int m, int n,
+                        const int32_t* active, double* out, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+int dn_eig_rotate_batched(const double* X, int64_t ldx, const double* C, const dn_eig_batch* batch, int kd, int n,
+                          double beta, const int32_t* active, double* Z, int64_t ldz, dn_stream_t stream);
+int dn_eig_residual_norms_batched(const double* W, int64_t ldw, const double* Q, int64_t ldq, const double* theta,
+                                  const dn_eig_batch* batch, int n, const int32_t* active, double* out, void* workspace,
+                                  int64_t ws_bytes, dn_stream_t stream);
+int dn_eig_finalize_batched(const double* Y, int64_t ldy, const int32_t* cols, int k, const double* mass,
+                            const dn_eig_batch* batch, double* out, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
 /* ---- implicit diffusion (layers.py:69-84, method='implicit_dense') -------------------------------------------------
  * Per channel c: x_diffuse[:, c] = (M + t_c L)^-1 M x[:, c], solved at any size by a Jacobi-preconditioned block
  * conjugate gradient over the C columns (preconditioner m_v + t_c L_vv), with each column's own step lengths, instead of

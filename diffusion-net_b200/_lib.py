@@ -14,7 +14,8 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libdiffusion_net_b200.so")
-SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_eig.cu", "dn_implicit.cu", "dn_fmap.cu", "dn_tc.cu", "dn_capi.cu"]
+SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_eig.cu", "dn_implicit.cu", "dn_fmap.cu", "dn_fmap_batch.cu", "dn_tc.cu",
+           "dn_capi.cu"]
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "diffusion_net_b200.h")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -138,6 +139,13 @@ SIGNATURES = {
                                                    _L, _I, _P]),
     "dn_learned_time_diffusion_bwd_batched": (_I, [_P, _P, _P, _P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P,
                                                    _P, _L, _I, _P]),
+    "dn_to_basis_batched": (_I, [_P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P, _L, _I, _P]),
+    "dn_from_basis_batched": (_I, [_P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P, _L, _I, _P]),
+    "dn_fmap_solve_batched_workspace_bytes": (_L, [_I, _I, _I]),
+    "dn_fmap_solve_fwd_batched": (_I, [_P, _L, _P, _L, _I, _P, _P, _I, _I, _I, _D, _P, _P]),
+    "dn_fmap_solve_bwd_batched": (_I, [_P, _L, _P, _L, _I, _P, _P, _I, _P, _P, _I, _I, _D, _P, _P, _P, _L, _P]),
+    "dn_fmap_pointwise_map_batched_workspace_bytes": (_L, [_I, _I, _P, _P, _P, _P, _I]),
+    "dn_fmap_pointwise_map_batched": (_I, [_P, _I, _P, _L, _P, _P, _I, _P, _P, _I, _P, _P, _L, _P]),
 }
 
 _lib = None

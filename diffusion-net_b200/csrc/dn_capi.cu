@@ -655,6 +655,45 @@ int dn_learned_time_diffusion_bwd_batched(const float* grad_out, const float* ma
   return launch_spectral_time_grad_batched(b.sums, x_spec, evals, time, batch->n_meshes, K, C, grad_time, st);
 }
 
+int dn_to_basis_batched(const float* values, const float* basis, const float* mass, const dn_mesh_batch* batch,
+                        int64_t V, int K, int C, float* out, void* workspace, int64_t ws_bytes, int engine,
+                        dn_stream_t stream) {
+  if (!values || !basis || !batch || !out || V < 0 || K <= 0 || C <= 0) return DN_ERR_INVALID_ARGUMENT;
+  Bump ws(workspace, ws_bytes);
+  BatchedSpectral b;
+  // the batch envelope and scratch of the spectral diffusion; its from_basis chain (checked on `values`, a V x C array
+  // like its output) is not run here
+  int rc = batched_spectral_plan(batch, basis, V, K, C, engine, const_cast<float*>(values), ws, &b);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  int P = 0;
+  if ((rc = to_basis_partials(values, basis, mass, V, K, C, b.partial, b.pf, &P, b.e, st, batch))) return rc;
+  return launch_reduce_mesh_partials(b.partial, batch->mesh_cta_begin, batch->n_meshes, (int64_t)K * C, out, st);
+}
+
+int dn_from_basis_batched(const float* values, const float* basis, const float* row_scale, const dn_mesh_batch* batch,
+                          int64_t V, int K, int C, float* out, void* workspace, int64_t ws_bytes, int engine,
+                          dn_stream_t stream) {
+  if (!values || !basis || !batch || !out || V < 0 || K <= 0 || C <= 0) return DN_ERR_INVALID_ARGUMENT;
+  Bump ws(workspace, ws_bytes);
+  BatchedSpectral b;
+  int rc = batched_spectral_plan(batch, basis, V, K, C, engine, out, ws, &b);
+  if (rc) return rc;
+  b.L.row_scale = row_scale;
+  cudaStream_t st = (cudaStream_t)stream;
+  // every mesh's G_b packed as it is, in one launch; the chain then picks G_b per 128-row tile
+  TcSpectral sp;
+  memset(&sp, 0, sizeof(sp));
+  sp.partial = values;
+  sp.P = batch->n_meshes;
+  sp.n_meshes = batch->n_meshes;
+  sp.tile_mesh = batch->tile_mesh;
+  sp.no_clamp_writeback = 1;
+  sp.plain = 1;
+  if ((rc = tc_pack_layers(&b.L, 1, b.packed, b.packed_bytes, &sp, st))) return rc;
+  return run_chain(b.src, &b.L, 1, V, b.e, ws, st);
+}
+
 int dn_grad_spmm(const dn_csr* grad, const float* x, int64_t V, int C, float* out, dn_stream_t stream) {
   if (!grad || !grad->rowptr || !x || !out || V < 0 || C <= 0) return DN_ERR_INVALID_ARGUMENT;
   return launch_grad_spmm_pair(grad, x, V, C, out, (cudaStream_t)stream);

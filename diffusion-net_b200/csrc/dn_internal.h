@@ -98,6 +98,9 @@ int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int a
 int launch_spectral_scale(const float* partial, int P, const float* evals, float* time, int K, int C,
                           float* x_spec_out, float* S_out, int clamp_writeback, cudaStream_t st);
 int launch_reduce_partials(const float* partial, int P, int64_t n, float* out, cudaStream_t st);
+// out[b] = sum over the to_basis CTAs of mesh b of a mesh batch's partials (n floats each), in CTA order
+int launch_reduce_mesh_partials(const float* partial, const int32_t* mesh_cta_begin, int n_meshes, int64_t n, float* out,
+                                cudaStream_t st);
 int launch_reduce_partials_ld(const float* partial, int P, int rows, int cols, float* out, int64_t ld_out,
                               int accumulate, cudaStream_t st);
 int launch_csr_from_coo(const int64_t* rows, const int64_t* cols, const float* vx, const float* vy,
@@ -212,6 +215,9 @@ struct TcSpectral {
   const int32_t* tile_mesh;        // device, null without a batch
   float* sum_out;                  // optional [n_meshes][K][N]: the reduced partial sums before the exp(-lambda t) scale
   int no_clamp_writeback;
+  // plain: `partial` is (n_meshes, K, N) and mesh b's matrix is partial[b] as it is (no sum, no scale; evals, time,
+  // mesh_cta_begin and sum_out are not read)
+  int plain;
 };
 // bytes tc_pack_layers needs (layer 0 n_meshes times)
 int64_t tc_chain_ws_bytes(const DnLayer* layers, int n_layers, int n_meshes = 1);

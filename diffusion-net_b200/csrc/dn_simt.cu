@@ -241,6 +241,17 @@ __global__ void reduce_partials_kernel(const float* __restrict__ partial, int P,
   out[idx] = s;
 }
 
+// out[b][i] = sum over the CTAs p of mesh b (mesh_cta_begin) of partial[p][i], in CTA order from 0
+__global__ void reduce_mesh_partials_kernel(const float* __restrict__ partial, const int32_t* __restrict__ mesh_cta_begin,
+                                            int64_t n, float* __restrict__ out) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int b = blockIdx.y;
+  if (idx >= n) return;
+  float s = 0.f;
+  for (int p = mesh_cta_begin[b]; p < mesh_cta_begin[b + 1]; ++p) s += partial[(int64_t)p * n + idx];
+  out[(int64_t)b * n + idx] = s;
+}
+
 // partial[p][n] = sum over the rows of slice p of A[v][n].  Block (32, 8): 32 columns x 8 row lanes, combined in a
 // fixed order, so the sum does not depend on scheduling.
 __global__ void colsum_partial_kernel(const float* __restrict__ A, int64_t lda, int N, int64_t V,
@@ -960,6 +971,15 @@ int launch_spectral_scale(const float* partial, int P, const float* evals, float
 
 int launch_reduce_partials(const float* partial, int P, int64_t n, float* out, cudaStream_t st) {
   reduce_partials_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(partial, P, n, out);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
+int launch_reduce_mesh_partials(const float* partial, const int32_t* mesh_cta_begin, int n_meshes, int64_t n, float* out,
+                                cudaStream_t st) {
+  reduce_mesh_partials_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)n_meshes), 256, 0, st>>>(partial,
+                                                                                                    mesh_cta_begin, n,
+                                                                                                    out);
   DN_LAUNCH_CHECK();
   return DN_OK;
 }

@@ -111,6 +111,11 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackJobs jobs) {
     const int b = jobs.sp.n_meshes > 1 ? (int)blockIdx.x / jobs.sp_blocks : 0;
     const int e = threadIdx.x & 31, sl = threadIdx.x >> 5;
     const int idx = ((int)blockIdx.x - b * jobs.sp_blocks) * 32 + e;
+    if (jobs.sp.plain) {
+      if (sl != 0 || idx >= K * N) return;
+      pack_store(J.dst + b * jobs.sp_stride, J.fmt, N, idx / N, idx % N, jobs.sp.partial[(int64_t)b * K * N + idx]);
+      return;
+    }
     const int p0 = jobs.sp.mesh_cta_begin ? jobs.sp.mesh_cta_begin[b] : 0;
     const int p1 = jobs.sp.mesh_cta_begin ? jobs.sp.mesh_cta_begin[b + 1] : jobs.sp.P;
     float acc = 0.f;

@@ -10,6 +10,10 @@ evaluation's pointwise map (``functional_correspondence.py:194-196``) on the GPU
   dense ``evecs.t()[:n_fmap] @ torch.diag(mass)`` (a V x V matrix) is never formed.
 * ``pointwise_map`` / ``nearest_neighbor``: the vertex-to-vertex map by an exact fp32 nearest-neighbour search
   (``dn_nearest_neighbor``), instead of the reference's host KD-tree.
+* ``PairBatch`` / ``forward_pairs`` / ``pointwise_map_batch``: the same over many shape pairs in one launch sequence
+  (the training and evaluation loops of functional_correspondence.py): features once per shape (``forward_batch``),
+  one batched projection, one batched solve, and the pointwise maps of all pairs, each pair's result what the per-pair
+  calls give.
 """
 from __future__ import annotations
 
@@ -154,6 +158,24 @@ class FunctionalMapCorrespondenceWithDiffusionNetFeatures(nn.Module):
         C_pred = fmap_solve(A, B, evals1[:n], evals2[:n], self.lambda_param).unsqueeze(0)
         return C_pred, feat1, feat2
 
+    def forward_pairs(self, pair_batch, xs):
+        """Every pair of a ``PairBatch`` in one launch sequence: (C_pred (P, n, n), feats), C_pred[p] what
+        ``forward(shape_{x_p}, shape_{y_p})`` gives for that pair and feats the list of per-shape features.  ``xs``: the
+        per-shape inputs (verts or HKS, per ``input_features``) as a list, or one tensor in the batch layout.  The
+        features run once per shape through ``feature_extractor.forward_batch``'s route, so in training mode a shape
+        used by several pairs gets ONE dropout mask per step (the reference draws one per forward call); then
+        ``project_batched`` and ``fmap_solve_batched``.  The loss over all pairs backpropagates through each shape's
+        features once, with the per-pair gradients summed in a fixed order."""
+        n = self.n_fmap
+        if pair_batch.n != n:
+            raise ValueError("forward_pairs: the pair batch was built for n_fmap = {}, the model uses {}".format(
+                pair_batch.n, n))
+        mb = pair_batch.mesh_batch
+        feat = self.feature_extractor._forward_batch_layout(mb, xs)
+        F_hat = project_batched(feat, pair_batch)
+        C_pred = fmap_solve_batched(F_hat, pair_batch.evals, pair_batch.pairs, n, self.lambda_param)
+        return C_pred, mb.unpack(feat)
+
 
 # ------------------------------------------------------------------------------------------------
 # pointwise map
@@ -208,3 +230,221 @@ def pointwise_map(C, evecs_x, evecs_y, n_fmap=30):
         ct = ops._f32c(Cm[:n, :n].t().contiguous())
         target = _apply_basis_exact(ct, ops._f32c(evecs_x[:, :n].contiguous()))
         return nearest_neighbor(evecs_y[:, :n].contiguous(), target)
+
+
+# ------------------------------------------------------------------------------------------------
+# pair batches: the head over many shape pairs in one launch sequence
+# ------------------------------------------------------------------------------------------------
+MAX_PAIRS = 65535        # grid-y limit of the batched solve
+MAX_SHAPES = 1024        # dn_mesh_batch_plan gives every mesh at least one of its 1024 to_basis CTAs
+
+
+class PairList:
+    """Ordered pairs (x_p, y_p) of indices into ``n_shapes`` shapes, on the device, with the shape -> (pair, role) CSR the
+    batched solve's backward sums over: entries 2 p + role (role 0 = x, 1 = y), each shape's in increasing order
+    (increasing p, the x role of a self-pair before its y role).  Built once per pair batch."""
+
+    def __init__(self, pairs, n_shapes, device):
+        self.pairs = [(int(a), int(b)) for a, b in pairs]
+        self.n_shapes = S = int(n_shapes)
+        self.n_pairs = P = len(self.pairs)
+        if P == 0:
+            raise ValueError("a pair batch needs at least one pair")
+        if P > MAX_PAIRS:
+            raise ValueError("a pair batch takes at most {} pairs, got {}".format(MAX_PAIRS, P))
+        for p, (a, b) in enumerate(self.pairs):
+            if not (0 <= a < S and 0 <= b < S):
+                raise ValueError("pair {} = ({}, {}) indexes a shape outside [0, {})".format(p, a, b, S))
+        self.role_begin, self.role_list = role_csr(self.pairs, S)
+        i32 = dict(dtype=torch.int32, device=device)
+        self.pair_x_host = [a for a, _ in self.pairs]
+        self.pair_y_host = [b for _, b in self.pairs]
+        self.pair_x = torch.tensor(self.pair_x_host, **i32)
+        self.pair_y = torch.tensor(self.pair_y_host, **i32)
+        self._role_begin = torch.tensor(self.role_begin, **i32)
+        self._role_list = torch.tensor(self.role_list, **i32)
+
+
+def role_csr(pairs, n_shapes):
+    """(begin [S + 1], entries [2 P]) of the shape -> (pair, role) lists: shape s owns entries[begin[s]:begin[s + 1]],
+    each 2 p + role (role 0 = x, 1 = y) in increasing order."""
+    lists = [[] for _ in range(n_shapes)]
+    for p, (a, b) in enumerate(pairs):
+        lists[a].append(2 * p)
+        lists[b].append(2 * p + 1)
+    begin, entries = [0], []
+    for lst in lists:
+        entries.extend(lst)          # already increasing: p grows, and 2p precedes 2p + 1
+        begin.append(len(entries))
+    return begin, entries
+
+
+class PairBatch:
+    """S shapes and P ordered pairs of them for ``forward_pairs`` / ``pointwise_map_batch``.  ``items`` are
+    ``batch.MeshBatch`` items (mass, evals, evecs, gradX, gradY, optional faces), all with the same K >= n_fmap;
+    ``pairs`` a list of (i, j).  Self-pairs, repeated shapes and shapes in no pair are allowed.  Builds once: the
+    MeshBatch, the (V, n rounded up to 8) projection basis in its layout (the first n eigenvectors, then zero columns:
+    32 columns at n = 30, as in the single-pair path), the (S, n) eigenvalue stack, and the device pair arrays with
+    their role CSR."""
+
+    def __init__(self, items, pairs, n_fmap=30):
+        from .batch import MeshBatch
+        n = int(n_fmap)
+        S = len(items)
+        if S < 1:
+            raise ValueError("PairBatch needs at least one shape")
+        if S > MAX_SHAPES:
+            raise ValueError("PairBatch: {} shapes exceed the {} the mesh-batch planner takes".format(S, MAX_SHAPES))
+        pairs = list(pairs)
+        if not pairs:
+            raise ValueError("PairBatch needs at least one pair")
+        for p, (a, b) in enumerate(pairs):
+            if not (0 <= int(a) < S and 0 <= int(b) < S):
+                raise ValueError("PairBatch: pair {} = ({}, {}) indexes a shape outside [0, {})".format(p, a, b, S))
+        _check_n(n, "PairBatch")
+        if n < 1:
+            raise ValueError("PairBatch: n_fmap must be at least 1, got {}".format(n))
+        K = min(int(it["evals"].shape[0]) for it in items)
+        if K < n:
+            raise ValueError("PairBatch: K = {} eigenpairs is fewer than n_fmap = {}".format(K, n))
+        self.n, self.n_shapes, self.n_pairs = n, S, len(pairs)
+        self.mesh_batch = mb = MeshBatch(items)
+        self.device = mb.device
+        self.pairs = PairList(pairs, S, mb.device)
+        self.kp = kp = (n + 7) // 8 * 8
+        self.basis = torch.zeros(mb.V, kp, dtype=torch.float32, device=mb.device)
+        self.basis[:, :n] = mb.evecs[:, :n]
+        self.evals = mb.evals[:, :n].contiguous()
+        self.row_begin_host = mb.row_begin[:-1]
+        self.n_rows_host = mb.n_rows
+
+
+def _spectral_ws(pb, Cc):
+    mb = pb.mesh_batch
+    return ops.workspace(mb.V, pb.kp, Cc, mb.device, extra=ops.batched_diffusion_workspace_extra(mb.n_meshes, pb.kp, Cc))
+
+
+class ProjectBatchedFn(torch.autograd.Function):
+    """(S, kp, C) spectral features Phi_s^T M_s F_s of every shape of a PairBatch from the (V, C) per-vertex features in
+    its batch layout (dn_to_basis_batched); backward M_s Phi_s G_s (dn_from_basis_batched), 0 on padding rows.  Two
+    launches each way, whatever S is; tensor-core engines only."""
+
+    @staticmethod
+    @ops._device_guard
+    def forward(ctx, feat, pb):
+        mb = pb.mesh_batch
+        feat = ops._f32c(feat)
+        if feat.dim() != 2 or feat.shape[0] != mb.V:
+            raise ValueError("project_batched: features {} are not in the pair batch's layout ({} rows)".format(
+                tuple(feat.shape), mb.V))
+        Cc = feat.shape[1]
+        out = torch.empty(mb.n_meshes, pb.kp, Cc, dtype=torch.float32, device=feat.device)
+        ws = _spectral_ws(pb, Cc)
+        _lib.check(_lib.load().dn_to_basis_batched(feat.data_ptr(), pb.basis.data_ptr(), mb.mass.data_ptr(),
+                                                   C.byref(mb.desc), mb.V, pb.kp, Cc, out.data_ptr(), ws.data_ptr(),
+                                                   ws.numel(), ops._engine, ops._stream()), "dn_to_basis_batched")
+        ctx.pb = pb
+        return out
+
+    @staticmethod
+    @ops._device_guard
+    def backward(ctx, g):
+        pb = ctx.pb
+        mb = pb.mesh_batch
+        g = ops._f32c(g)
+        Cc = g.shape[2]
+        gx = torch.empty(mb.V, Cc, dtype=torch.float32, device=g.device)
+        ws = _spectral_ws(pb, Cc)
+        _lib.check(_lib.load().dn_from_basis_batched(g.data_ptr(), pb.basis.data_ptr(), mb.mass.data_ptr(),
+                                                     C.byref(mb.desc), mb.V, pb.kp, Cc, gx.data_ptr(), ws.data_ptr(),
+                                                     ws.numel(), ops._engine, ops._stream()), "dn_from_basis_batched")
+        return gx, None
+
+
+def project_batched(feat, pair_batch):
+    """(S, kp, C): every shape's spectral features from ``feat`` (V, C) in ``pair_batch``'s layout; rows n .. kp - 1 are
+    zero (zero basis columns).  Differentiable in ``feat``."""
+    ops._require_cuda(feat)
+    return ProjectBatchedFn.apply(feat, pair_batch)
+
+
+class FmapSolveBatchedFn(torch.autograd.Function):
+    """The functional-map solve of every pair of a PairList: C (P, n, n), C[p] = FmapSolveFn's C for A = F_hat[x_p][:n],
+    B = F_hat[y_p][:n] and the shapes' first n eigenvalues, bitwise.  One launch forward, three backward
+    (dn_fmap_solve_{fwd,bwd}_batched); the gradient of a shape is the per-pair gradients summed in a fixed order."""
+
+    @staticmethod
+    @ops._device_guard
+    def forward(ctx, F_hat, evals, pairs, n, lambda_param):
+        F_hat, evals = ops._f32c(F_hat), ops._f32c(evals)
+        if F_hat.dim() != 3 or F_hat.shape[0] != pairs.n_shapes or F_hat.shape[1] < n or evals.dim() != 2 or \
+                evals.shape[0] != pairs.n_shapes or evals.shape[1] < n:
+            raise ValueError("fmap_solve_batched: F_hat {} must be (S, >= n, d) and evals {} (S, >= n) for S = {}, "
+                             "n = {}".format(tuple(F_hat.shape), tuple(evals.shape), pairs.n_shapes, n))
+        S, m, d = F_hat.shape
+        out = torch.empty(pairs.n_pairs, n, n, dtype=torch.float32, device=F_hat.device)
+        _lib.check(_lib.load().dn_fmap_solve_fwd_batched(
+            F_hat.data_ptr(), m * d, evals.data_ptr(), evals.shape[1], S, pairs.pair_x.data_ptr(),
+            pairs.pair_y.data_ptr(), pairs.n_pairs, n, d, float(lambda_param), out.data_ptr(), ops._stream()),
+            "dn_fmap_solve_fwd_batched")
+        ctx.pairs, ctx.n, ctx.lam = pairs, n, float(lambda_param)
+        ctx.save_for_backward(F_hat, evals)
+        return out
+
+    @staticmethod
+    @ops._device_guard
+    def backward(ctx, g):
+        F_hat, evals = ctx.saved_tensors
+        pairs, n = ctx.pairs, ctx.n
+        g = ops._f32c(g)
+        S, m, d = F_hat.shape
+        lib = _lib.load()
+        gF = torch.zeros_like(F_hat)
+        ws = torch.empty(int(lib.dn_fmap_solve_batched_workspace_bytes(pairs.n_pairs, n, d)), dtype=torch.uint8,
+                         device=F_hat.device)
+        _lib.check(lib.dn_fmap_solve_bwd_batched(
+            F_hat.data_ptr(), m * d, evals.data_ptr(), evals.shape[1], S, pairs.pair_x.data_ptr(),
+            pairs.pair_y.data_ptr(), pairs.n_pairs, pairs._role_begin.data_ptr(), pairs._role_list.data_ptr(), n, d,
+            ctx.lam, g.data_ptr(), gF.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()),
+            "dn_fmap_solve_bwd_batched")
+        return gF, None, None, None, None
+
+
+def fmap_solve_batched(F_hat, evals, pairs, n, lambda_param=1e-3):
+    """C (P, n, n) for every pair of ``pairs`` (a PairList) from the stacked spectral features ``F_hat`` (S, >= n, d; the
+    first n rows of each shape used) and eigenvalues ``evals`` (S, >= n).  Differentiable in F_hat."""
+    ops._require_cuda(F_hat, evals)
+    _check_n(int(n), "functional-map solve")
+    if torch.is_grad_enabled():
+        ops._no_operator_grads(("evals", evals))
+    return FmapSolveBatchedFn.apply(F_hat, evals, pairs, int(n), lambda_param)
+
+
+def pointwise_map_batch(C_pred, pair_batch, n_fmap=30):
+    """``pointwise_map`` for every pair of ``pair_batch``: a list of P int64 tensors (V_{y_p},), the p-th bitwise equal to
+    ``pointwise_map(C_pred[p], evecs_{x_p}, evecs_{y_p}, n_fmap)``.  C_pred is (P, >= n, >= n).  The products and the
+    searches of all pairs run in chunks of up to 64 pairs, 2 or 3 launches per chunk (dn_fmap_pointwise_map_batched)."""
+    ops._require_cuda(C_pred)
+    n = int(n_fmap)
+    pb = pair_batch
+    mb = pb.mesh_batch
+    P = pb.n_pairs
+    if C_pred.dim() != 3 or C_pred.shape[0] != P or C_pred.shape[1] < n or C_pred.shape[2] < n or mb.K < n:
+        raise ValueError("pointwise_map_batch: C_pred {} does not hold {} pairs of n_fmap = {} (K = {})".format(
+            tuple(C_pred.shape), P, n, mb.K))
+    _check_n(n, "pointwise_map_batch")
+    lib = _lib.load()
+    px, py = _lib.int_array(pb.pairs.pair_x_host), _lib.int_array(pb.pairs.pair_y_host)
+    rb, nr = _lib.int_array(pb.row_begin_host), _lib.int_array(pb.n_rows_host)
+    counts = [pb.n_rows_host[y] for y in pb.pairs.pair_y_host]
+    with torch.no_grad(), ops._on(C_pred):
+        Cm = ops._f32c(C_pred[:, :n, :n].contiguous())
+        out = torch.empty(sum(counts), dtype=torch.int64, device=C_pred.device)
+        wsb = int(lib.dn_fmap_pointwise_map_batched_workspace_bytes(n, P, px, py, rb, nr, pb.n_shapes))
+        if wsb < 0:
+            _lib.check(wsb, "dn_fmap_pointwise_map_batched_workspace_bytes")
+        ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=C_pred.device)
+        _lib.check(lib.dn_fmap_pointwise_map_batched(Cm.data_ptr(), n, mb.evecs.data_ptr(), mb.K, rb, nr, pb.n_shapes,
+                                                     px, py, P, out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                     ops._stream()), "dn_fmap_pointwise_map_batched")
+    return list(torch.split(out, counts))

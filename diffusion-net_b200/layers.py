@@ -282,19 +282,7 @@ class DiffusionNet(nn.Module):
             if elems is None:
                 raise ValueError("forward_batch with outputs_at='{0}' needs '{0}' in every MeshBatch item".format(
                     self.outputs_at))
-        x = xs if torch.is_tensor(xs) else batch.pack(xs)
-        if x.shape[-1] != self.C_in:
-            raise ValueError("DiffusionNet was constructed with C_in={}, but x_in has last dim={}".format(
-                self.C_in, x.shape[-1]))
-        needs_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))
-        dropout = any(blk.training and blk.dropout for blk in self.blocks)
-        if needs_grad or dropout:
-            x = ops.mlp_apply([x], [self.first_lin.weight], [self.first_lin.bias])
-            for blk in self.blocks:
-                x = blk._forward_batch(batch, x)
-            x = ops.mlp_apply([x], [self.last_lin.weight], [self.last_lin.bias])
-        else:
-            x = self._forward_batch_fused(batch, x)
+        x = self._forward_batch_layout(batch, xs)
         if elems is not None:
             # mean of the per-vertex outputs over each element's corners (as in forward), one gather for the batch
             y = x[elems.view(-1)].view(elems.shape + (x.shape[-1],)).mean(dim=1)
@@ -310,6 +298,22 @@ class DiffusionNet(nn.Module):
         if self.last_activation != None:
             outs = [self.last_activation(o) for o in outs]
         return outs
+
+    def _forward_batch_layout(self, batch, xs):
+        """forward_batch up to last_lin: the (V, C_out) per-vertex output in the batch layout (padding rows included),
+        before any remap to elements, global mean or last activation."""
+        x = xs if torch.is_tensor(xs) else batch.pack(xs)
+        if x.shape[-1] != self.C_in:
+            raise ValueError("DiffusionNet was constructed with C_in={}, but x_in has last dim={}".format(
+                self.C_in, x.shape[-1]))
+        needs_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))
+        dropout = any(blk.training and blk.dropout for blk in self.blocks)
+        if needs_grad or dropout:
+            x = ops.mlp_apply([x], [self.first_lin.weight], [self.first_lin.bias])
+            for blk in self.blocks:
+                x = blk._forward_batch(batch, x)
+            return ops.mlp_apply([x], [self.last_lin.weight], [self.last_lin.bias])
+        return self._forward_batch_fused(batch, x)
 
     def _forward_batch_fused(self, batch, x):
         """Inference route of forward_batch: one dn_block_fwd_batched per block, last_lin fused behind the last one when

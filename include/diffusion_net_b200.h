@@ -445,6 +445,66 @@ int dn_learned_time_diffusion_bwd_batched(const float* grad_out, const float* ma
                                           float* grad_time, void* workspace, int64_t ws_bytes, int engine,
                                           dn_stream_t stream);
 
+/* The spectral projection over a batch laid out as above (the functional-map head of many shapes at once):
+ *   dn_to_basis_batched:   out (n_meshes, K, C), out[b] = Phi_b^T M_b F_b: the grouped to_basis partials (tb_rows), then
+ *                          each mesh's CTA partials summed in CTA order.  mass may be NULL (no weighting).  2 launches
+ *                          (3 for C = 256).
+ *   dn_from_basis_batched: out (V, C), the rows of mesh b = row_scale (.) Phi_b G_b with G = values (n_meshes, K, C),
+ *                          exactly 0 on padding rows (the basis is 0 there).  Every G_b is packed in one launch and the
+ *                          from_basis chain picks G_b per 128-row tile.  row_scale may be NULL.  2 launches.
+ * The launch counts do not depend on n_meshes.  Envelope and workspace as dn_learned_time_diffusion_fwd_batched's
+ * (tensor-core engines only; the SIMT engine is DN_ERR_UNSUPPORTED before any work is enqueued). */
+int dn_to_basis_batched(const float* values, const float* basis, const float* mass, const dn_mesh_batch* batch,
+                        int64_t V, int K, int C, float* out, void* workspace, int64_t ws_bytes, int engine,
+                        dn_stream_t stream);
+int dn_from_basis_batched(const float* values, const float* basis, const float* row_scale, const dn_mesh_batch* batch,
+                          int64_t V, int K, int C, float* out, void* workspace, int64_t ws_bytes, int engine,
+                          dn_stream_t stream);
+
+/* ---- functional maps over a pair batch ------------------------------------------------------------------------------
+ * S shapes and P ordered pairs (x_p, y_p) of shape indices (self-pairs, repeats and unused shapes allowed).  The spectral
+ * features are one stack F: shape s at F + s * ld_shape, n x d with row stride d (ld_shape >= n d, so a padded (S, K, d)
+ * projection is read in place); evals (S, ld_evals), the first n of each row used.  pair_x, pair_y are device int32 [P]
+ * with every index in [0, S) (the caller checks).  C is (P, n, n).  Pair p computes exactly what dn_fmap_solve_fwd /
+ * _bwd compute for A = F_{x_p}, B = F_{y_p}, evals_x = evals[x_p], evals_y = evals[y_p]: bitwise the same C, NaN rows
+ * where S_i is singular.  1 <= n <= 128, P < 65536, S < 65536 (DN_ERR_UNSUPPORTED above); no host read, so both calls
+ * capture in a CUDA graph.
+ *   fwd: 1 launch, one CTA per (row, pair).
+ *   bwd: 3 launches whatever P is: the per-(row, pair) re-solve, the per-pair dA_p, dB_p (fp32, as dn_fmap_solve_bwd
+ *        writes them), then grad_F[s] = sum over the entries of shape s in the role list of dA_p (role x) or dB_p
+ *        (role y), summed in fp32 from 0 in list order, with no atomics.  role_begin (device int32 [S + 1]) and role_list
+ *        (device int32 [2 P], entry 2 p + role, role 0 = x, 1 = y) form a CSR from shape to entries; each shape's entries
+ *        are in increasing order (increasing p, the x role before the y role of a self-pair).  The n x d block of every
+ *        shape in grad_F (same layout as F) is OVERWRITTEN, exactly 0 for a shape in no pair; the rest of each ld_shape
+ *        stride is not written.  Workspace: dn_fmap_solve_batched_workspace_bytes(P, n, d), 16 n^2 P + 8 n d P bytes
+ *        (each part rounded up to 256). */
+int64_t dn_fmap_solve_batched_workspace_bytes(int n_pairs, int n, int d);
+int dn_fmap_solve_fwd_batched(const float* F, int64_t ld_shape, const float* evals, int64_t ld_evals, int n_shapes,
+                              const int32_t* pair_x, const int32_t* pair_y, int n_pairs, int n, int d, double lambda,
+                              float* C, dn_stream_t stream);
+int dn_fmap_solve_bwd_batched(const float* F, int64_t ld_shape, const float* evals, int64_t ld_evals, int n_shapes,
+                              const int32_t* pair_x, const int32_t* pair_y, int n_pairs, const int32_t* role_begin,
+                              const int32_t* role_list, int n, int d, double lambda, const float* grad_C,
+                              float* grad_F, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
+/* The pointwise maps of a pair batch: for every pair, out_index[o_p + v] (o_p = sum_{q<p} V_{y_q}) is the index of the
+ * nearest row of T_p = Phi_{x_p}[:, :n] C_p^T to row v of Phi_{y_p}[:, :n], bitwise what dn_from_basis on the SIMT engine
+ * followed by dn_nearest_neighbor give for that pair (ties to the lowest index).  Phi is `evecs` in a batch layout
+ * (shape s at rows row_begin_host[s] .. + n_rows_host[s], row stride ld_evecs >= n); C is (P, n, n) dense; the pair and
+ * row arrays are HOST int32 arrays (indices checked here).  T_p goes to the workspace, entries formed as one fmaf chain in
+ * increasing k from 0 (the SIMT kernel's order).  Pairs run in chunks of at most 64 pairs whose T rows total at most
+ * 2^24 floats (a chunk holds at least one pair); per chunk 2 launches, or 3 when the chunk's source rows are too few to
+ * fill the GPU and the targets are split into ranges.  Workspace (dn_fmap_pointwise_map_batched_workspace_bytes): the
+ * largest chunk's T (4 NP sum V_x bytes, NP = n rounded up to a power of two >= 4; at most 64 MiB unless one pair is
+ * larger) plus its split partials (8 splits sum V_y bytes, splits <= 16). */
+int64_t dn_fmap_pointwise_map_batched_workspace_bytes(int n, int n_pairs, const int32_t* pair_x_host,
+                                                      const int32_t* pair_y_host, const int32_t* row_begin_host,
+                                                      const int32_t* n_rows_host, int n_shapes);
+int dn_fmap_pointwise_map_batched(const float* C, int n, const float* evecs, int64_t ld_evecs,
+                                  const int32_t* row_begin_host, const int32_t* n_rows_host, int n_shapes,
+                                  const int32_t* pair_x_host, const int32_t* pair_y_host, int n_pairs,
+                                  int64_t* out_index, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
 /* Linear head fused behind a block (SURVEY.md 8f-1): `DiffusionNet.last_lin` (layers.py:366-370 -- the nn.Linear applied
  * to the last block's output) computed in the epilogue of that block's MiniMLP chain, in exact fp32, so that the
  * C_width-wide block output is never written: out_head[v][o] = bias[o] + sum_c weight[o][c] * block_out[v][c]. */

@@ -4,11 +4,14 @@ Each chain is called alone through its C-ABI entry point, tc3x, K = C = 128:
 
   from_basis   dn_from_basis,   evecs (V, 128) -> (V, 128)
   pq           dn_mini_mlp_fwd, one 128 -> 256 layer (the [P|Q] shape of the gradient features)
+  front        from_basis, P and Q as the one chain the block forward runs (dn_block_fwd_profile, its from_basis_pq
+               stage): evecs (V, 128) -> x_diffuse (V, 128), then P, Q (V, 128) each into one (V, 256) buffer
   mlp          dn_mini_mlp_fwd, cat(3 x (V, 128)) -> 128 -> 128 with ReLU, biases and the residual (the MiniMLP)
   to_basis     dn_to_basis,     evecs^T (mass * x): the split-V to_basis kernel and its partial reduction
 
 A call is the weight-pack launch (a few microseconds) plus the chain launch; it is timed with CUDA events over
---iters calls after --warmup calls.  Bytes and TF32 MMA operations come from the shapes (3 MMA passes in tc3x); the
+--iters calls after --warmup calls.  The front chain is timed inside a whole block forward (CUDA events around its
+launch alone, from the profiling entry point, averaged over --iters forwards after --warmup), so it has no pack launch.  Bytes and TF32 MMA operations come from the shapes (3 MMA passes in tc3x); the
 floors are bytes over the data-sheet HBM rate and MMA operations over a TF32 rate measured in the same run with a
 large torch matmul (TF32 on).  The weight bytes each 128-row tile streams from L2 are reported as an implied L2 rate.
 The same chains at V = 20k, whose inputs stay resident in the 50 MB L2, give the time per row without HBM latency.
@@ -46,6 +49,8 @@ def chain_model(name, V):
         layers, rows_in, rows_out = [(K, C)], K, C
     elif name == "pq":
         layers, rows_in, rows_out = [(C, 2 * C)], C, 2 * C
+    elif name == "front":  # evecs in; x_diffuse, P and Q out
+        layers, rows_in, rows_out = [(K, C), (C, C), (C, C)], K, 3 * C
     elif name == "to_basis":  # evecs, x and mass in; a K x C result (no weights)
         return 4 * V * (K + C + 1), 2 * V * K * C * PASSES, 0
     else:  # mlp: 3 sources + residual in, C out
@@ -137,8 +142,31 @@ def main():
             _lib.check(lib.dn_to_basis(x.data_ptr(), evecs.data_ptr(), mass.data_ptr(), V, K, C, out_kc.data_ptr(),
                                        ws.data_ptr(), ws.numel(), eng, st), "dn_to_basis")
 
-        for name, fn in (("from_basis", call_fb), ("pq", call_pq), ("mlp", call_mlp), ("to_basis", call_tb)):
-            ms = timed(fn, args.iters, args.warmup)
+        # the front chain as the block forward runs it, at the block's shapes (with rotations, MiniMLP 384 -> 128 -> 128)
+        n_side = 500 if V == 200_000 else 200
+        mass_b, _, evals_b, evecs_b, gX, gY = dn.synthetic.structural_operators(n_side, V // n_side, K, seed=0, device=dev)
+        blk = dn.DiffusionNetBlock(C_width=C, mlp_hidden_dims=[C, C], dropout=False)
+        blk.load_state_dict(dn.synthetic.block_weights(C, seed=0), strict=True)
+        blk = blk.to(dev).eval()
+        gops = dn.prepare_operators(gX, gY)
+        A_re, A_im = blk.gradient_features.weights()
+        lins = blk.mlp.linears()
+        front_stage = ops.PROFILE_STAGES.index("from_basis_pq")
+
+        def time_front(iters, warm):
+            tot = 0.0
+            with torch.no_grad():
+                for i in range(warm + iters):
+                    prof = []
+                    ops.block_forward_raw(x, mass_b, evals_b, evecs_b, gops, blk.diffusion.diffusion_time, A_re, A_im,
+                                          [l.weight for l in lins], [l.bias for l in lins], True, profile=prof)
+                    if i >= warm:
+                        tot += prof[front_stage]
+            return tot / iters
+
+        for name, fn in (("from_basis", call_fb), ("pq", call_pq), ("front", None), ("mlp", call_mlp),
+                         ("to_basis", call_tb)):
+            ms = time_front(args.iters, args.warmup) if fn is None else timed(fn, args.iters, args.warmup)
             hbm, flops, l2w = chain_model(name, V)
             rows.append({
                 "chain": name, "V": V, "ms": round(ms, 4), "ns_per_row": round(ms * 1e6 / V, 3),

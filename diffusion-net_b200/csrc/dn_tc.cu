@@ -32,22 +32,39 @@ constexpr int CHAIN_THREADS = 384;              // warpgroups 0, 1: consumers; w
 // first-layer activations: 16-column x 128-row fp32 stages, each two 8-column boxes of [128 rows][8 floats]
 constexpr int A_BOX_BYTES = 8 * TILE_M * 4;     // 4 KiB
 constexpr int A_STAGE_BYTES = 2 * A_BOX_BYTES;
-constexpr int A_NST = 8;                        // activation stages in flight (64 KiB per SM)
+constexpr int A_NST_MAX = 8;                  // activation stages in flight (64 KiB per SM)
+constexpr int SMEM_OPTIN = 232448;              // sm_90 opt-in dynamic shared memory per block
+constexpr int OUT_ROWS = 64;                    // rows of an output / residual box: one consumer warpgroup's rows
+constexpr int OUT_BOX_BYTES = 8 * OUT_ROWS * 4; // 8 columns x 64 rows, [64 rows][8 floats]
 
 enum { MODE_TF32 = 1, MODE_TF32X3 = 3, MODE_BF16 = DN_PASSES_BF16 };
 
-// Weight ring of rows_chain_kernel<MODE, NMAX>: a slot holds one K stage of an NMAX-wide layer as the producer streams
-// it (tf32x3: hi | lo images, 8 bytes per weight; tf32: hi, 4; bf16: 2).  At NMAX = 128 / 256: tc3x 8 slots of 16 KiB /
-// 4 of 32 KiB; tc1x 8 of 8 KiB / 8 of 16 KiB; bf16 8 of 4 KiB / 8 of 8 KiB.  (With 16 slots for the narrower stages,
-// repeated bf16 mesh-batch forwards once gave differing bits; the cause was not found, so the depth stays at 8.)
+// Shared memory of rows_chain_kernel<MODE, NMAX>.  Weight ring: a slot holds one K stage of an NMAX-wide layer as the
+// producer streams it (tf32x3: hi | lo images, 8 bytes per weight; tf32: hi, 4; bf16: 2), as many as fit in
+// W_RING_BYTES, at most 8.  (With 16 slots for the narrower stages, repeated bf16 mesh-batch forwards once gave
+// differing bits; the cause was not found, so the depth stays at 8.)  The TF32 chains at NMAX <= 128 also hold one output /
+// residual staging buffer per consumer warpgroup (64 rows x NMAX fp32, 32 KiB at NMAX = 128).  Where everything does
+// not fit the opt-in limit (tc3x at NMAX = 128 only), the weight ring gives up two slots and the activation ring one:
+// 6 weight and 7 activation slots measured slightly faster than 5 and 8 (DESIGN.md §5).  At NMAX = 128 / 256: tc3x 6 slots of
+// 16 KiB / 4 of 32 KiB; tc1x 8 of 8 KiB / 8 of 16 KiB; bf16 8 of 4 KiB / 8 of 8 KiB.  `set_chain_smem` and the launch
+// both read SMEM.
 template <int MODE, int NMAX>
 struct ChainRing {
   static constexpr int STAGE = KC * NMAX * (MODE == MODE_TF32X3 ? 8 : MODE == MODE_TF32 ? 4 : 2);
-  static constexpr int NST = W_RING_BYTES / STAGE < W_NST_MAX ? W_RING_BYTES / STAGE : W_NST_MAX;
-  static constexpr int BARS = 8 * (2 * NST + 2 * A_NST);   // full / empty of both rings
+  static constexpr int NST_FULL = W_RING_BYTES / STAGE < W_NST_MAX ? W_RING_BYTES / STAGE : W_NST_MAX;
+  // (bf16 stores from registers: with the staging buffer two identical bf16 calls at V = 200k + 37 gave different
+  // bits, and the cause was not found)
+  static constexpr int STG = NMAX <= 128 && MODE != MODE_BF16 ? 2 * OUT_ROWS * NMAX * 4 : 0;
   // every layer's bias, staged once per CTA (NMAX = 256 chains run a single layer)
   static constexpr int BIAS = (NMAX <= 128 ? DN_MAX_LAYERS : 1) * NMAX * 4;
-  static constexpr int SMEM = NST * STAGE + A_NST * A_STAGE_BYTES + BIAS + BARS;
+  static constexpr int bars(int nst, int anst) { return 8 * (2 * nst + 2 * anst + 2); }   // full / empty, residual
+  static constexpr int bytes(int nst, int anst) { return nst * STAGE + anst * A_STAGE_BYTES + STG + BIAS + bars(nst, anst); }
+  static constexpr bool kFull = bytes(NST_FULL, A_NST_MAX) <= SMEM_OPTIN;
+  static constexpr int NST = kFull ? NST_FULL : NST_FULL - 2;
+  static constexpr int A_NST = kFull ? A_NST_MAX : A_NST_MAX - 1;
+  static constexpr int BARS = bars(NST, A_NST);
+  static constexpr int SMEM = bytes(NST, A_NST);
+  static_assert(SMEM <= SMEM_OPTIN, "rows_chain_kernel: shared memory over the opt-in limit");
 };
 
 // bytes of one packed K stage of an N-wide layer: tf32 hi image (KC * N * 4) then lo image; bf16 uses the first quarter
@@ -172,6 +189,10 @@ struct HcLayer {
 
 struct HcParams {
   CUtensorMap amap[DN_MAX_SRC];   // layer 0's sources: fp32 [V rows][width], 8 x 128 boxes, rows >= V zero-filled
+  // TF32 engines, NMAX <= 128: each layer's `out` and `residual` as fp32 [V rows][N] (row stride ld_out / ld_res), 8 x 64 boxes;
+  // rows >= V are not written (out) or zero-filled (residual)
+  CUtensorMap omap[DN_MAX_LAYERS];
+  CUtensorMap rmap[DN_MAX_LAYERS];
   DnRowsSrc src;
   HcLayer layer[DN_MAX_LAYERS];
   int n_layers;
@@ -184,6 +205,7 @@ struct HcParams {
   int64_t ld_head_out;
   int head_n;
 };
+static_assert(sizeof(HcParams) <= 4096, "HcParams must fit the 4 KiB kernel parameter space");
 
 // Both consumer warpgroups own 64 rows of the tile each and share the weight stages; one lane of warpgroup 2 streams
 // the stages with bulk TMA (that warpgroup hands its registers to the consumers with setmaxnreg).  A second lane
@@ -202,21 +224,35 @@ struct HcParams {
 // WIDE: every layer is exactly NMAX wide (so every later layer's K is NMAX too).  Widths and trip counts are then
 // compile-time and each k8 slice of a pass is one m64nNMAXk8 MMA over the whole accumulator; otherwise the layer is
 // covered by N / 16 m64n16 MMAs per slice and pass.
+// Outputs (TF32, NMAX <= 128): each consumer warpgroup writes a layer's result into its own staging buffer, laid out like
+// the activation ring (box b = columns 8b .. 8b+7 as [64 rows][8 floats], so a warp's float2 writes cover 256
+// contiguous bytes), and one elected lane stores the boxes with 2-D TMA (rows >= V clipped by the tensor map) and goes
+// on.  A layer's residual comes into the same buffer by TMA, issued before the layer's MMAs; each lane reads its
+// residual from the slot it then overwrites with the result.  Ordering: every thread that touched the buffer fences
+// (generic -> async proxy) and passes the warpgroup's named barrier before the store is issued; before the buffer is
+// written again (an epilogue, or a residual load) the elected lane waits until the previous stores have read it; and in
+// the CTA's last tile it waits for its stores to complete before it goes on.  NMAX = 256 chains (their staging tile
+// would not fit next to the rings) and the bf16 engine (ChainRing::STG) store from registers.
 template <int MODE, int NMAX, bool WIDE>
 __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __grid_constant__ HcParams p) {
   constexpr bool kChain = NMAX <= 128;
+  constexpr bool kStage = ChainRing<MODE, NMAX>::STG > 0;   // outputs and residuals through shared memory
   constexpr int NB = NMAX / 16;
-  constexpr int NST = ChainRing<MODE, NMAX>::NST, STAGE_BYTES = ChainRing<MODE, NMAX>::STAGE;
+  using Ring = ChainRing<MODE, NMAX>;
+  constexpr int NST = Ring::NST, STAGE_BYTES = Ring::STAGE, A_NST = Ring::A_NST;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* aring = smem + NST * STAGE_BYTES;
-  float* sbias = reinterpret_cast<float*>(aring + A_NST * A_STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(aring + A_NST * A_STAGE_BYTES + ChainRing<MODE, NMAX>::BIAS);
+  uint8_t* stage_out = aring + A_NST * A_STAGE_BYTES;
+  float* sbias = reinterpret_cast<float*>(stage_out + Ring::STG);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stage_out + Ring::STG + Ring::BIAS);
   const uint32_t full = smem_u32(bars), empty = smem_u32(bars + NST);
   const uint32_t afull = smem_u32(bars + 2 * NST), aempty = smem_u32(bars + 2 * NST + A_NST);
+  const uint32_t rfull = smem_u32(bars + 2 * NST + 2 * A_NST);   // residual loaded, one per consumer warpgroup
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < NST; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 8); }
     for (int i = 0; i < A_NST; ++i) { mbar_init(afull + 8 * i, 1); mbar_init(aempty + 8 * i, 8); }
+    for (int i = 0; i < 2; ++i) mbar_init(rfull + 8 * i, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -278,23 +314,44 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
   named_bar_sync(1, 256);                     // the consumers' copies are done (the producers do not take part)
   const int g = lane >> 2, t = lane & 3;
   const int rloc = (warp >> 2) * 64 + (warp & 3) * 16 + g;
+  // output / residual staging (NMAX <= 128)
+  const int wg = warp >> 2;
+  const bool elected = (threadIdx.x & 127) == 0;   // issues the warpgroup's TMA loads and stores
+  // box b (columns 8b .. 8b+7, [64 rows][8 floats]) of this warpgroup's buffer
+  auto stg_box = [&](int b) { return reinterpret_cast<float*>(stage_out) + (wg * NMAX + 8 * b) * OUT_ROWS; };
   float acc[NB * 8];
   float act[kChain ? NB * 8 : 1];
-  uint32_t s = 0, ph = 0, as = 0, aph = 0;
+  uint32_t s = 0, ph = 0, as = 0, aph = 0, rph = 0;
 
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int64_t r0 = tile * TILE_M + rloc, r1 = r0 + 8;
     const bool ok0 = r0 < p.V, ok1 = r1 < p.V;
+    const int row0 = (int)(tile * TILE_M) + wg * OUT_ROWS;   // this warpgroup's first row (V < 2^31 - 256)
     for (int l = 0; l < L; ++l) {
       const HcLayer& Lr = p.layer[l];
       const int N = WIDE ? NMAX : Lr.N, nb = N / 16;
       const int K = (WIDE && l > 0) ? NMAX : Lr.K, nst = (K + KC - 1) / KC;
       const uint32_t lbo = (uint32_t)N * 16;
       int prev = -1;
-      // The epilogue reads the rows' residual, emul and relu-mask values from global memory one column block after the
-      // other (their loads cannot all be in flight at once: the registers do not fit), so each is a round trip.  Asking
-      // L2 for those rows now, while this layer's MMAs run, makes every one of those round trips an L2 hit.  The four
-      // lanes that share a row pair ask for one 128-byte line each of every 512 bytes; lane 0 also for the row's end.
+      if constexpr (kStage) {
+        // the residual rows come into the staging buffer while the layer's MMAs run, once the buffer's last stores
+        // have read it (issued a layer or more ago); a warpgroup wholly past V loads nothing (its rows are not stored)
+        if (Lr.residual && elected) {
+          bulk_wait_read<0>();
+          if (row0 < p.V) {
+            mbar_arrive_expect_tx(rfull + 8 * wg, (uint32_t)(Lr.N / 8 * OUT_BOX_BYTES));
+            for (int b = 0; b < Lr.N / 8; ++b)
+              tma_tile_2d_g2s(smem_u32(stg_box(b)), &p.rmap[l], 8 * b, row0, rfull + 8 * wg);
+          } else {
+            mbar_arrive(rfull + 8 * wg);
+          }
+        }
+      }
+      // The epilogue reads the rows' emul and relu-mask values (NMAX = 256: also the residual) from global memory one
+      // column block after the other (their loads cannot all be in flight at once: the registers do not fit), so each
+      // is a round trip.  Asking L2 for those rows now, while this layer's MMAs run, makes every one of those round
+      // trips an L2 hit.  The four lanes that share a row pair ask for one 128-byte line each of every 512 bytes; lane 0
+      // also for the row's end.
       auto prefetch_rows = [&](const float* base, int64_t ld) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -304,7 +361,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
           if (t == 0) prefetch_l2(row + N * 4 - 4);
         }
       };
-      if (Lr.residual) prefetch_rows(Lr.residual, Lr.ld_res);
+      if (!kStage && Lr.residual) prefetch_rows(Lr.residual, Lr.ld_res);
       if (Lr.emul) prefetch_rows(Lr.emul, N);
       if (Lr.relu_mask) prefetch_rows(Lr.relu_mask, N);
       // one K stage: q[0], q[1] = rows (r0, r1) x columns (2t, 2t+1); q[2], q[3] the same 8 columns further.  All A
@@ -435,6 +492,18 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
       float hp0[kChain ? 1 : 8], hp1[kChain ? 1 : 8];   // head partial sums of a single-layer (256-wide) chain
 #pragma unroll
       for (int o = 0; o < (kChain ? 1 : 8); ++o) hp0[o] = hp1[o] = 0.f;
+      if constexpr (kStage) {
+        if (Lr.residual) {
+          // the residual is in the staging buffer.  The elected lane waits and the barrier passes the news on: every
+          // lane of the warpgroup spinning here made ptxas spill and serialize the MMAs
+          if (elected) mbar_wait(rfull + 8 * wg, rph);
+          rph ^= 1;
+          named_bar_sync(2 + wg, 128);
+        } else if (Lr.out) {
+          if (elected) bulk_wait_read<0>();  // the buffer's last stores have read it
+          named_bar_sync(2 + wg, 128);
+        }
+      }
       // the bound is read from the layer even where it is known at compile time: the branch keeps the compiler from
       // hoisting the epilogue loads of every column block ahead of the first one, which would not fit in registers
       const int nb_epi = Lr.N / 16;
@@ -469,19 +538,32 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
             }
           }
           if (Lr.row_scale) { v0.x *= rs0; v0.y *= rs0; v1.x *= rs1; v1.y *= rs1; }
-          if (Lr.residual) {
-            if (ok0) {
-              const float2 r = __ldg(reinterpret_cast<const float2*>(Lr.residual + r0 * Lr.ld_res + col));
-              v0.x = fmaf(Lr.res_scale, r.x, v0.x); v0.y = fmaf(Lr.res_scale, r.y, v0.y);
+          if constexpr (kStage) {
+            float* so = stg_box(2 * j + h) + ((warp & 3) * 16 + g) * 8 + 2 * t;   // rows 16w+g, +8 at so + 64
+            if (Lr.residual) {
+              const float2 ra = *reinterpret_cast<const float2*>(so), rb = *reinterpret_cast<const float2*>(so + 64);
+              v0.x = fmaf(Lr.res_scale, ra.x, v0.x); v0.y = fmaf(Lr.res_scale, ra.y, v0.y);
+              v1.x = fmaf(Lr.res_scale, rb.x, v1.x); v1.y = fmaf(Lr.res_scale, rb.y, v1.y);
             }
-            if (ok1) {
-              const float2 r = __ldg(reinterpret_cast<const float2*>(Lr.residual + r1 * Lr.ld_res + col));
-              v1.x = fmaf(Lr.res_scale, r.x, v1.x); v1.y = fmaf(Lr.res_scale, r.y, v1.y);
+            if (Lr.out) {
+              *reinterpret_cast<float2*>(so) = v0;
+              *reinterpret_cast<float2*>(so + 64) = v1;
             }
-          }
-          if (Lr.out) {
-            if (ok0) *reinterpret_cast<float2*>(Lr.out + r0 * Lr.ld_out + col) = v0;
-            if (ok1) *reinterpret_cast<float2*>(Lr.out + r1 * Lr.ld_out + col) = v1;
+          } else {
+            if (Lr.residual) {
+              if (ok0) {
+                const float2 r = __ldg(reinterpret_cast<const float2*>(Lr.residual + r0 * Lr.ld_res + col));
+                v0.x = fmaf(Lr.res_scale, r.x, v0.x); v0.y = fmaf(Lr.res_scale, r.y, v0.y);
+              }
+              if (ok1) {
+                const float2 r = __ldg(reinterpret_cast<const float2*>(Lr.residual + r1 * Lr.ld_res + col));
+                v1.x = fmaf(Lr.res_scale, r.x, v1.x); v1.y = fmaf(Lr.res_scale, r.y, v1.y);
+              }
+            }
+            if (Lr.out) {
+              if (ok0) *reinterpret_cast<float2*>(Lr.out + r0 * Lr.ld_out + col) = v0;
+              if (ok1) *reinterpret_cast<float2*>(Lr.out + r1 * Lr.ld_out + col) = v1;
+            }
           }
           if constexpr (kChain) {
             if (!keep_act) {
@@ -497,6 +579,21 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
               hp0[o] = fmaf(w.y, v0.y, fmaf(w.x, v0.x, hp0[o]));
               hp1[o] = fmaf(w.y, v1.y, fmaf(w.x, v1.x, hp1[o]));
             }
+          }
+        }
+      }
+      if constexpr (kStage) {
+        if (Lr.out || Lr.residual) {
+          // this warpgroup's reads and writes of the buffer come before the async proxy's next access to it
+          fence_proxy_async();
+          named_bar_sync(2 + wg, 128);
+          if (Lr.out && elected && row0 < p.V) {
+            for (int b = 0; b < Lr.N / 8; ++b)
+              tma_tile_2d_s2g(&p.omap[l], 8 * b, row0, smem_u32(stg_box(b)));
+            bulk_commit();
+            // in the CTA's last tile, every store is complete before the lane goes on (and so before it exits).  The
+            // same wait after the tile loop made ptxas spill the bf16 full-width chain.
+            if (tile + gridDim.x >= ntiles) bulk_wait<0>();
           }
         }
       }
@@ -844,8 +941,8 @@ bool tc_supported_device() {
 static bool aligned8(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 7) == 0; }
 static bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
-// shapes rows_chain_kernel takes (bf16: 16-wide K steps; tf32: 8-wide).  Layer 0's sources are TMA tensor maps: base
-// 16-byte aligned, row stride a multiple of 16 bytes.
+// shapes rows_chain_kernel takes (bf16: 16-wide K steps; tf32: 8-wide).  Layer 0's sources and every layer's out and
+// residual are TMA tensor maps: base 16-byte aligned, row stride a multiple of 16 bytes.
 static int chain_supported(const DnRowsSrc& src, const DnLayer* layers, int n_layers, bool bf16) {
   const int ks = bf16 ? 16 : 8;
   if (n_layers < 1 || n_layers > DN_MAX_LAYERS) return DN_ERR_UNSUPPORTED;
@@ -865,8 +962,9 @@ static int chain_supported(const DnRowsSrc& src, const DnLayer* layers, int n_la
     if (l > 0 && (L.K != (L.sibling ? layers[l - 1].K : layers[l - 1].N) || L.tile_group)) return DN_ERR_UNSUPPORTED;
     if (L.emul && !aligned8(L.emul)) return DN_ERR_UNSUPPORTED;
     if (L.relu_mask_src && !aligned8(L.relu_mask_src)) return DN_ERR_UNSUPPORTED;
-    if (L.residual && (L.ld_res % 2 || !aligned8(L.residual))) return DN_ERR_UNSUPPORTED;
-    if (L.out && (L.ld_out % 2 || !aligned8(L.out))) return DN_ERR_UNSUPPORTED;
+    // out and residual are TMA tensor maps too (the same rule as layer 0's sources)
+    if (L.residual && (L.ld_res % 4 || !aligned16(L.residual))) return DN_ERR_UNSUPPORTED;
+    if (L.out && (L.ld_out % 4 || !aligned16(L.out))) return DN_ERR_UNSUPPORTED;
     if (!last && L.head_w) return DN_ERR_UNSUPPORTED;
     if (last && !L.out && !L.head_w) return DN_ERR_UNSUPPORTED;
     if (L.head_w && (!L.head_out || L.head_n < 1 || L.head_n > 8 || !aligned8(L.head_w))) return DN_ERR_UNSUPPORTED;
@@ -960,18 +1058,20 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
   p.V = V;
   p.tile_group = layers[0].tile_group;
   p.group_stride = layers[0].group_stride;
-  // one tensor map per source of layer 0 (encoded on the host; a captured graph keeps them with the launch)
+  // tensor maps (encoded on the host; a captured graph keeps them with the launch): fp32 [V rows][width], row stride ld
   const PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
   if (!encode) return DN_ERR_UNSUPPORTED;
-  for (int s = 0; s < src.nsrc; ++s) {
-    const cuuint64_t dims[2] = {(cuuint64_t)src.width[s], (cuuint64_t)V};
-    const cuuint64_t strides[1] = {(cuuint64_t)src.ld[s] * 4};
-    const cuuint32_t box[2] = {8, TILE_M}, estr[2] = {1, 1};
-    if (encode(&p.amap[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(src.ptr[s]), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return DN_ERR_UNSUPPORTED;
-  }
+  auto encode_rows = [&](CUtensorMap* m, const float* base, int width, int64_t ld, int box_rows) {
+    const cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)V};
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+    const cuuint32_t box[2] = {8, (cuuint32_t)box_rows}, estr[2] = {1, 1};
+    return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  };
+  // one per source of layer 0
+  for (int s = 0; s < src.nsrc; ++s)
+    if (!encode_rows(&p.amap[s], src.ptr[s], src.width[s], src.ld[s], TILE_M)) return DN_ERR_UNSUPPORTED;
   int nmax = 0, nmin = 1 << 30;
   for (int l = 0; l < n_layers; ++l) {
     const DnLayer& L = layers[l];
@@ -982,6 +1082,14 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
     if (L.N > nmax) nmax = L.N;
     if (L.N < nmin) nmin = L.N;
   }
+  // the TF32 chains at NMAX <= 128 store each layer's out and load its residual through shared memory: one map each, 8 x 64 boxes
+  // (a column slice such as P or Q of [P|Q] is its own map: base at the slice, width N, the buffer's row stride)
+  if (nmax <= 128 && !bf16)
+    for (int l = 0; l < n_layers; ++l) {
+      const DnLayer& L = layers[l];
+      if (L.out && !encode_rows(&p.omap[l], L.out, L.N, L.ld_out, OUT_ROWS)) return DN_ERR_UNSUPPORTED;
+      if (L.residual && !encode_rows(&p.rmap[l], L.residual, L.N, L.ld_res, OUT_ROWS)) return DN_ERR_UNSUPPORTED;
+    }
   const bool wide = nmin == nmax && (nmax == 128 || nmax == 256);
   const DnLayer& Ll = layers[n_layers - 1];
   p.head_w = Ll.head_w; p.head_b = Ll.head_b; p.head_out = Ll.head_out; p.ld_head_out = Ll.ld_head_out; p.head_n = Ll.head_n;

@@ -77,6 +77,23 @@ __device__ __forceinline__ void tma_tile_2d_g2s(uint32_t dst_smem, const void* t
       : "memory");
 }
 
+// ---- tiled TMA store shared -> global, bulk-group completion --------------------------------------
+// 2-D tiled store of the box at (column c0, row c1) of `tmap` from shared memory; elements outside the tensor are not
+// written.  The stores a thread issued since its last commit form one bulk group.
+__device__ __forceinline__ void tma_tile_2d_s2g(const void* tmap, int c0, int c1, uint32_t src_smem) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];" ::"l"(
+                   reinterpret_cast<uint64_t>(tmap)),
+               "r"(c0), "r"(c1), "r"(src_smem)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source (the source may be rewritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups are incomplete (their global writes are done)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
 // ---- wgmma ------------------------------------------------------------------------------------
 // shared-memory matrix descriptor, no swizzle, K-major: core matrices of 8 rows x 16 bytes;
 //   LBO = byte distance between core matrices adjacent in K, SBO = between 8-row groups

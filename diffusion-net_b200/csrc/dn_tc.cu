@@ -641,34 +641,41 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
 // ---------------------------------------------------------------------------------------------
 // to_basis, split over V:  partial[cta][k][c] = sum_{v in cta's range} Phi[v][k] * m[v] * x[v][c]
 //   D = Phi^T (M = K_eig rows: warpgroup 0 rows 0..63, warpgroup 1 rows 64..127) times (m x) (N = C columns); the
-//   reduction runs over v in 16-row chunks.  Warp 8 copies 16 consecutive rows of Phi and of x into a staging ring
-//   with bulk TMA; the A fragments are read from there, B = (m x)^T is written K-major (hi | lo) by all consumers.
-//   The MMA accumulator is folded into an fp32 sum in shared memory every TB_FOLD chunks: short accumulation chains keep the
-//   tensor core's accumulation below fp32 noise even for V = 200k.
+//   reduction runs over v in stages of TB_ROWS = 32 rows (4 k8 slices).  Warp 8 loads a stage of Phi and of x with
+//   2-D tiled TMA, 8 columns x 32 rows per box, each box laid out [row][8 floats] (columns >= K or C and rows >= V come
+//   back as zeros); the A fragments are read from there, B = (m x)^T is written K-major (hi | lo) by all consumers.
+//   Both reads and the B-image stores put a warp's 32 lanes on 32 banks: a warp builds one 8-channel x 4-row core
+//   matrix of B per step from one box row run, and a fragment read of Phi covers 4 rows x 8 columns of one box.
+//   One named barrier per stage: before it every consumer has built its part of stage c's B image and has waited for
+//   its own MMAs of stage c - 1, so after it stage c's MMAs may start and stage c + 1 may overwrite the B slot of c - 1.
+//   The MMA accumulator is folded into an fp32 sum in shared memory every 128 rows (TB_FOLD stages): short
+//   accumulation chains keep the tensor core's accumulation below fp32 noise even for V = 200k.
 //   The channel count C = 16 NBC is a compile-time parameter, so every MMA sits on a path ptxas can see is uniform.
 //   C == 128: each k8 slice of a pass is one m64n128k8 MMA; otherwise NBC m64n16 MMAs.  Both warpgroups always
 //   issue their MMAs (a warpgroup whose 64 eigen-rows all lie beyond K multiplies zero A fragments and stores nothing),
 //   so no MMA sits on a path that depends on the warp index.
 // ---------------------------------------------------------------------------------------------
-constexpr int TB_NST = 4;                    // raw staging ring depth
-constexpr int TB_RAW_HALF = KC * 128 * 4;    // 16 rows x up to 128 floats
-constexpr int TB_RAW = 2 * TB_RAW_HALF;      // raw Phi rows + raw x rows
-constexpr int TB_BIMG = KC * 128 * 4;        // one tf32 image of B: up to 128 channels x 16 v
+constexpr int TB_ROWS = 32;                  // rows per stage
+constexpr int TB_NST = 3;                    // raw staging ring depth
+constexpr int TB_BOX = TB_ROWS * 8 * 4;      // one TMA box: 32 rows x 8 floats
+constexpr int TB_RAW_HALF = 16 * TB_BOX;     // up to 128 columns
+constexpr int TB_RAW = 2 * TB_RAW_HALF;      // Phi boxes | x boxes
+constexpr int TB_BIMG = TB_ROWS * 128 * 4;   // one tf32 image of B: up to 128 channels x 32 v
 constexpr int TB_BSTAGE = 2 * TB_BIMG;       // hi | lo
 constexpr int TB_THREADS = 288;              // warps 0..7 consumers (two warpgroups), warp 8 TMA
 constexpr int TB_SUMS = 64 * 256 * 4;        // fp32 fold sums: 64 per consumer thread, [i][thread] (conflict-free)
 constexpr int TB_SMEM = TB_NST * TB_RAW + 2 * TB_BSTAGE + TB_SUMS + 256;
-constexpr int TB_FOLD = 8;
+constexpr int TB_FOLD = 128 / TB_ROWS;       // stages per accumulation chain
+static_assert(TB_SMEM <= 227 * 1024, "to_basis shared memory");
 
 struct TcToBasisParams {
-  const float* values;   // (V, C)
-  const float* basis;    // (V, K)
+  CUtensorMap phi_map;   // basis: fp32 [V rows][K], 8 x 32 boxes
+  CUtensorMap x_map;     // values: fp32 [V rows][C], row stride ld_values, 8 x 32 boxes
   const float* mass;     // (V) or null
   float* partial;        // (grid, K, C)
   int64_t V;
   int K, C;
-  int64_t chunks_per_cta;
-  int64_t ld_values;     // row stride of `values` (floats): == C for a contiguous matrix, > C for a column slice
+  int64_t chunks_per_cta;   // 16-row chunks per CTA
   int64_t ldp;           // row stride of a partial (floats): partial[cta][k][ldp]
   const int32_t* cta_rows;   // optional device [2 * grid]: the row range [begin, end) CTA i reduces (mesh batches: a CTA
 };                           //   never crosses a mesh boundary); null = uniform chunks_per_cta * 16 rows per CTA
@@ -697,27 +704,24 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
     re = rb + p.chunks_per_cta * KC;
     if (re > p.V) re = p.V;
   }
-  const int64_t nch = re > rb ? (re - rb + KC - 1) / KC : 0;
-  constexpr int C = 16 * NBC;
+  const int64_t nst = re > rb ? (re - rb + TB_ROWS - 1) / TB_ROWS : 0;
+  constexpr int C = 16 * NBC, XB = C / 8;   // x boxes per stage
   const int K = p.K;
 
   if (warp == 8) {
     if (lane == 0) {
-      for (int64_t c = 0; c < nch; ++c) {
+      const int kbn = (K + 7) / 8;            // Phi boxes per stage
+      const uint32_t bytes = (uint32_t)(kbn + XB) * TB_BOX;
+      for (int64_t c = 0; c < nst; ++c) {
         const uint32_t s = c % TB_NST, ph = (c / TB_NST) & 1;
         mbar_wait(st_empty + 8 * s, ph ^ 1);
-        const int64_t v0 = rb + c * KC;
-        const int nv = (int)((re - v0) < KC ? (re - v0) : KC);
-        const uint32_t ba = (uint32_t)nv * K * 4, bb = (uint32_t)nv * C * 4;
-        mbar_arrive_expect_tx(st_full + 8 * s, ba + bb);
-        tma_bulk_g2s(smem_u32(raw + s * TB_RAW), p.basis + v0 * K, ba, st_full + 8 * s);
-        if (p.ld_values == C) {
-          tma_bulk_g2s(smem_u32(raw + s * TB_RAW + TB_RAW_HALF), p.values + v0 * C, bb, st_full + 8 * s);
-        } else {   // a column slice of a wider matrix: one copy per row
-          for (int j = 0; j < nv; ++j)
-            tma_bulk_g2s(smem_u32(raw + s * TB_RAW + TB_RAW_HALF) + (uint32_t)j * C * 4, p.values + (v0 + j) * p.ld_values,
-                         (uint32_t)C * 4, st_full + 8 * s);
-        }
+        const int v0 = (int)(rb + c * TB_ROWS);
+        const uint32_t dst = smem_u32(raw + s * TB_RAW);
+        mbar_arrive_expect_tx(st_full + 8 * s, bytes);
+        for (int b = 0; b < kbn; ++b) tma_tile_2d_g2s(dst + b * TB_BOX, &p.phi_map, 8 * b, v0, st_full + 8 * s);
+#pragma unroll
+        for (int b = 0; b < XB; ++b)
+          tma_tile_2d_g2s(dst + TB_RAW_HALF + b * TB_BOX, &p.x_map, 8 * b, v0, st_full + 8 * s);
       }
     }
     return;
@@ -725,69 +729,61 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
 
   const int g = lane >> 2, t = lane & 3;
   const int m0 = (warp >> 2) * 64 + (warp & 3) * 16 + g;   // eigen-index rows m0, m0 + 8
+  const int abox = m0 >> 3;                                 // their Phi boxes abox, abox + 1 (column m0 & 7 == g)
   const uint32_t lbo = (uint32_t)C * 16;
-  // the fold sums live in shared memory: the 64 accumulators, two stages of A fragments and the addressing fit the
-  // kernel's 168 registers, a second register array of 64 would not
+  // B image: this thread writes row bv of every stage, channels 8 b + (lane & 7); the core matrix of rows
+  // 4 warp .. 4 warp + 3 and channels 8 b .. 8 b + 7 sits at boff + 128 b
+  const int bv = 4 * warp + (lane >> 3);
+  const uint32_t boff = (uint32_t)warp * C * 16 + (lane & 7) * 16 + (lane >> 3) * 4;
+  // the fold sums live in shared memory: the 64 accumulators, the A fragments of a stage and the addressing fit the
+  // register budget, a second register array of 64 would not
   float acc[64];
   float* sum = sums + threadIdx.x;
 #pragma unroll
   for (int i = 0; i < 64; ++i) sum[256 * i] = 0.f;
 
-  for (int64_t c = 0; c < nch; ++c) {
+  for (int64_t c = 0; c < nst; ++c) {
     const uint32_t s = c % TB_NST, ph = (c / TB_NST) & 1;
-    const int64_t v0 = rb + c * KC;
-    const int nv = (int)((re - v0) < KC ? (re - v0) : KC);
+    const int64_t v0 = rb + c * TB_ROWS;
+    const int nv = (int)((re - v0) < TB_ROWS ? (re - v0) : TB_ROWS);   // rows >= nv are another range's: zeroed
     const int fold = (int)(c % TB_FOLD);
+    // the mass value (global) is loaded before the wait, so its latency overlaps it; row bv >= nv reads a valid row
+    float mv = 1.f;
+    if (p.mass) mv = __ldg(p.mass + v0 + (bv < nv ? bv : nv - 1));
+    mbar_wait(st_full + 8 * s, ph);
+    const float* rphi = reinterpret_cast<const float*>(raw + s * TB_RAW);
+    const float* rx = reinterpret_cast<const float*>(raw + s * TB_RAW + TB_RAW_HALF);
+    uint8_t* bh = bimg + (c & 1) * TB_BSTAGE;   // stage c - 2's MMAs, its last readers, were waited for before the
+    float xv[XB];                               //   previous stage's barrier
+#pragma unroll
+    for (int b = 0; b < XB; ++b) xv[b] = rx[b * (TB_BOX / 4) + 32 * warp + lane];   // box b, row bv, column lane & 7
+#pragma unroll
+    for (int b = 0; b < XB; ++b) {
+      float x = 0.f;
+      if (bv < nv) x = p.mass ? xv[b] * mv : xv[b];     // (values * massvec), geometry.py:583
+      float hi, lo;
+      split_tf32_fast(x, hi, lo);
+      *reinterpret_cast<float*>(bh + boff + 128 * b) = hi;
+      if (MODE == MODE_TF32X3) *reinterpret_cast<float*>(bh + TB_BIMG + boff + 128 * b) = lo;
+    }
+    // the A fragment registers are the same in every stage: the MMAs of stage c - 1, which read them, must be done
+    // before they are rewritten (they ran while this stage's B image was built)
+    wgmma_wait<0>();
     if (fold == 0 && c > 0) {              // fold the finished accumulation chain into the sum
-      wgmma_wait<0>();
 #pragma unroll
       for (int j = 0; j < 8; ++j) fence_acc8(acc + 8 * j);
 #pragma unroll
       for (int i = 0; i < 64; ++i) sum[256 * i] += acc[i];
-    }                                      // (this warp's MMAs of chunk c - 2 are done: waited for in chunk c - 1)
-    // B image: element i of this thread is e = 256 i + thread (KC * C = 256 NBC elements).  Every load is issued
-    // before any is used: the mass values (global) before the two waits below, so their latency overlaps them, and the
-    // x values (staging ring) as one batch.  Loaded one element at a time behind a branch, each global round trip came
-    // in series with the next.  Rows >= nv read a valid row and are then replaced by zero.
-    float mv[NBC], xv[NBC];
-    if (p.mass) {
-#pragma unroll
-      for (int i = 0; i < NBC; ++i) {
-        const int vv = (256 * i + (int)threadIdx.x) / C;
-        mv[i] = __ldg(p.mass + v0 + (vv < nv ? vv : nv - 1));
-      }
     }
-    named_bar_sync(1, 256);                // every warp's MMAs of chunk c - 2 are done: its B slot is free
-    mbar_wait(st_full + 8 * s, ph);
-    const float* rphi = reinterpret_cast<const float*>(raw + s * TB_RAW);
-    const float* rx = reinterpret_cast<const float*>(raw + s * TB_RAW + TB_RAW_HALF);
-    uint8_t* bh = bimg + (c & 1) * TB_BSTAGE;
+    uint32_t ah[4][4], al[4][4];           // A fragments, all formed before wgmma_fence
 #pragma unroll
-    for (int i = 0; i < NBC; ++i) xv[i] = rx[256 * i + (int)threadIdx.x];   // row vv, channel cc: vv * C + cc = e
-#pragma unroll
-    for (int i = 0; i < NBC; ++i) {
-      const int e = 256 * i + (int)threadIdx.x;
-      const int vv = e / C, cc = e - vv * C;
-      float x = 0.f;
-      if (vv < nv) x = p.mass ? xv[i] * mv[i] : xv[i];     // (values * massvec), geometry.py:583
-      float hi, lo;
-      split_tf32_fast(x, hi, lo);
-      const uint32_t off = (vv >> 2) * C * 16 + (cc >> 3) * 128 + (cc & 7) * 16 + (vv & 3) * 4;
-      *reinterpret_cast<float*>(bh + off) = hi;
-      if (MODE == MODE_TF32X3) *reinterpret_cast<float*>(bh + TB_BIMG + off) = lo;
-    }
-    // the A fragment registers are the same in every chunk: the MMAs of chunk c - 1, which read them, must be done
-    // before they are rewritten (they ran while this chunk's B image was built)
-    wgmma_wait<0>();
-    uint32_t ah[2][4], al[2][4];           // A fragments, all formed before wgmma_fence
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks)
+    for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int vv = 8 * ks + t + 4 * (i >> 1), k = m0 + 8 * (i & 1);
-        // read unconditionally and select: vv * K + k < 16 * 128 stays inside the staging slot, and a load under a
-        // lane-dependent branch would put the MMA operands on a divergent path
-        const float v = rphi[vv * K + k];
+        // read unconditionally and select: the box stays inside the staging slot, and a load under a lane-dependent
+        // branch would put the MMA operands on a divergent path
+        const float v = rphi[(abox + (i & 1)) * (TB_BOX / 4) + vv * 8 + g];
         float h, lo;
         split_tf32_fast((vv < nv && k < K) ? v : 0.f, h, lo);
         ah[ks][i] = __float_as_uint(h);
@@ -796,16 +792,16 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
     fence_proxy_async();
     __syncwarp();
     if (lane == 0) mbar_arrive(st_empty + 8 * s);
-    named_bar_sync(2, 256);                // the B image is complete
+    named_bar_sync(1, 256);                // the B image is complete; every warp's MMAs of stage c - 1 are done
     const uint32_t sb = smem_u32(bh);
 #pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
+    for (int ks = 0; ks < 4; ++ks) {
       fence_frag4(ah[ks]);
       if (MODE == MODE_TF32X3) fence_frag4(al[ks]);
     }
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
+    for (int ks = 0; ks < 4; ++ks) {
       const uint32_t acc0 = (fold > 0 || ks > 0) ? 1u : 0u;
       if constexpr (NBC == 8) {
         const uint32_t base = sb + ks * 2 * lbo;
@@ -837,7 +833,7 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
   wgmma_wait<0>();
 #pragma unroll
   for (int j = 0; j < 8; ++j) fence_acc8(acc + 8 * j);
-  if (nch > 0)
+  if (nst > 0)
 #pragma unroll
     for (int i = 0; i < 64; ++i) sum[256 * i] += acc[i];
   float* out = p.partial + (int64_t)blockIdx.x * K * p.ldp;
@@ -1118,9 +1114,24 @@ int tc_to_basis_partial(const float* values, const float* basis, const float* ma
   if ((reinterpret_cast<uintptr_t>(values) & 15) || (reinterpret_cast<uintptr_t>(basis) & 15) || (ld_values % 4) ||
       (ldp % 2) || (reinterpret_cast<uintptr_t>(partial) & 7))
     return DN_ERR_UNSUPPORTED;
+  if (V >= (1ll << 31) - 256) return DN_ERR_UNSUPPORTED;   // TMA row coordinates are 32-bit
   TcToBasisParams p;
-  p.values = values; p.basis = basis; p.mass = massvec; p.partial = partial;
-  p.ld_values = ld_values; p.ldp = ldp; p.cta_rows = cta_rows;
+  memset(&p, 0, sizeof(p));
+  // tensor maps (encoded on the host; a captured graph keeps them with the launch): fp32 [V rows][width], row stride
+  // ld, 8 x TB_ROWS boxes; columns >= width and rows >= V are zero-filled
+  const PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
+  if (!encode) return DN_ERR_UNSUPPORTED;
+  auto encode_rows = [&](CUtensorMap* m, const float* base, int width, int64_t ld) {
+    const cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)(V > 0 ? V : 1)};
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+    const cuuint32_t box[2] = {8, (cuuint32_t)TB_ROWS}, estr[2] = {1, 1};
+    return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  };
+  if (!encode_rows(&p.phi_map, basis, K, K) || !encode_rows(&p.x_map, values, C, ld_values)) return DN_ERR_UNSUPPORTED;
+  p.mass = massvec; p.partial = partial;
+  p.ldp = ldp; p.cta_rows = cta_rows;
   p.V = V; p.K = K; p.C = C; p.chunks_per_cta = 0;
   int grid;
   if (cta_rows) {                       // batch of meshes: the caller planned the CTAs (dn_mesh_batch_plan)

@@ -159,7 +159,7 @@ class DiffusionNetBlock(nn.Module):
             self.MLP_C += self.C_width
         self.mlp = MiniMLP([self.MLP_C] + self.mlp_hidden_dims + [self.C_width], dropout=self.dropout)
 
-    def _forward_mesh(self, x_in, mass, evals, evecs, gops, fused, head=None, lap=None):
+    def _forward_mesh(self, x_in, mass, evals, evecs, gops, fused, head=None, lap=None, out=None):
         A_re = A_im = None
         if self.with_gradient_features:
             A_re, A_im = self.gradient_features.weights()
@@ -167,7 +167,7 @@ class DiffusionNetBlock(nn.Module):
             lins = self.mlp.linears()
             return ops.block_forward_raw(x_in, mass, evals, evecs, gops, self.diffusion.diffusion_time, A_re, A_im,
                                          [l.weight for l in lins], [l.bias for l in lins],
-                                         self.with_gradient_features, head=head)
+                                         self.with_gradient_features, head=head, out=out)
         if head is not None:
             raise ops.HeadNotFused()
         x_diffuse = self.diffusion(x_in, lap, mass, evals, evecs)
@@ -218,6 +218,13 @@ class DiffusionNetBlock(nn.Module):
         fused = (not implicit) and (not needs_grad) and self.mlp._fused_ok and not (self.training and self.dropout)
         if head is not None and not fused:
             raise ops.HeadNotFused()
+        if fused:   # every mesh writes its slice of one fresh result: no stacking copy
+            n_res = self.C_width if head is None else int(head[0].shape[0])
+            res = torch.empty(B, x_in.shape[1], n_res, dtype=torch.float32, device=x_in.device)
+            for b in range(B):
+                self._forward_mesh(x_in[b], mass[b], pick(evals, b), pick(evecs, b), gops[b], fused, head, laps[b],
+                                   out=res[b])
+            return res
         outs = [self._forward_mesh(x_in[b], mass[b], pick(evals, b), pick(evecs, b), gops[b], fused, head, laps[b])
                 for b in range(B)]
         return torch.stack(outs, dim=0)

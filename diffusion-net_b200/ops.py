@@ -555,18 +555,26 @@ def head_fusable(n_out):
 
 
 def block_forward_raw(x_in, mass, evals, evecs, ops, time, A_re, A_im, weights, biases, with_features,
-                      profile=None, head=None, batch_desc=None):
+                      profile=None, head=None, batch_desc=None, out=None):
     """Fused inference forward of one block on one mesh (dn_block_fwd).  ``profile``: a list that receives the
     per-stage device times in ms (``PROFILE_STAGES`` order; dn_block_fwd_profile, synchronises).
     ``head=(weight, bias)``: a linear head (``DiffusionNet.last_lin``) fused behind the block -- the return value is then
     the (V, n_out) head output and the block output is never written; raises ``HeadNotFused`` when the MiniMLP is not
     on the fused tensor-core chain (the caller applies the head separately).  ``batch_desc``: a ``_lib.dn_mesh_batch``
-    (see batch.MeshBatch) when ``x_in`` / the operators are a batch laid out as one vertex range."""
+    (see batch.MeshBatch) when ``x_in`` / the operators are a batch laid out as one vertex range.  ``out``: a
+    contiguous fp32 tensor on ``x_in``'s device that receives the result ((V, C), or (V, n_out) with ``head``) and is
+    returned; it must not overlap ``x_in``.  None allocates it."""
     lib = _lib.load()
     x_in, mass, evals, evecs = _f32c(x_in), _f32c(mass), _f32c(evals), _f32c(evecs)
     V, Cc = x_in.shape
     K = evecs.shape[1]
-    out = torch.empty_like(x_in)
+    n_res = Cc if head is None else int(head[0].shape[0])
+    if out is None:
+        out = torch.empty(V, n_res, dtype=torch.float32, device=x_in.device)
+    elif (out.dtype != torch.float32 or out.device != x_in.device or tuple(out.shape) != (V, n_res)
+          or not out.is_contiguous()):
+        raise ValueError("block_forward_raw: out must be a contiguous float32 ({}, {}) tensor on {}".format(
+            V, n_res, x_in.device))
     dims = [weights[0].shape[1]] + [w.shape[0] for w in weights]
     # contiguous copies (if any were needed) must outlive the launch: keep them in locals, not temporaries
     wc = [_f32c(w) for w in weights]
@@ -590,9 +598,8 @@ def block_forward_raw(x_in, mass, evals, evecs, ops, time, A_re, A_im, weights, 
             if head is not None:
                 hw = _f32c(head[0])
                 hb = _f32c(head[1]) if head[1] is not None else None
-                hout = torch.empty(V, hw.shape[0], dtype=torch.float32, device=x_in.device)
                 hd = _lib.dn_head(hw.data_ptr(), hb.data_ptr() if hb is not None else None, int(hw.shape[0]),
-                                  hout.data_ptr(), int(hw.shape[0]))
+                                  out.data_ptr(), int(hw.shape[0]))
             rc = lib.dn_block_fwd_ex(x_in.data_ptr(), mass.data_ptr(), evals.data_ptr(), evecs.data_ptr(), csr, C.byref(prm),
                                      C.byref(batch_desc) if batch_desc is not None else None,
                                      C.byref(hd) if hd is not None else None, V, K, Cc,
@@ -601,7 +608,7 @@ def block_forward_raw(x_in, mass, evals, evecs, ops, time, A_re, A_im, weights, 
             if rc == -2 and head is not None:      # DN_ERR_UNSUPPORTED: the chain that would carry the head is not available
                 raise HeadNotFused()
             _lib.check(rc, "dn_block_fwd_ex")
-            return hout if head is not None else out
+            return out
         if profile is not None:
             ms = (C.c_float * 6)()
             _lib.check(lib.dn_block_fwd_profile(x_in.data_ptr(), mass.data_ptr(), evals.data_ptr(), evecs.data_ptr(),

@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import math
 
+import numpy as np
 import torch
 
 from . import _lib, ops
@@ -27,8 +28,50 @@ MAX_ITERATIONS = 500
 
 
 def block_size(V, k):
-    """B = min(V, k + guard), guard = max(16, k / 4)."""
-    return min(V, k + max(16, k // 4))
+    """B = min(V, k + guard), guard = max(16, k / 4); for V = None the unclamped k + guard (a mesh batch's width)."""
+    B = k + max(16, k // 4)
+    return B if V is None else min(V, B)
+
+
+def chebyshev_coefficients(degree, lo, cut, hi):
+    """Yields (alpha, beta, gamma) for each of the ``degree`` steps of the scaled Chebyshev filter that damps [cut, hi]
+    (``lo`` estimates the bottom of the spectrum, for scaling only): step 0 is ``Y1 = alpha A Y0 + beta Y0``, step
+    d > 0 ``Y_{d+1} = alpha A Y_d + beta Y_d + gamma Y_{d-1}``.  (lo, cut, hi) are floats, or float64 arrays with one
+    entry per mesh; either way each entry goes through the same float64 operations, so a mesh's coefficients do not
+    depend on which form computed them.  A generator, so that a caller can launch each step as soon as it has its
+    coefficients."""
+    e, c = (hi - cut) / 2.0, (hi + cut) / 2.0
+    sigma = e / (lo - c)
+    sigma1 = sigma
+    yield sigma1 / e, -c * sigma1 / e, 0.0 * e             # gamma is unused without Y_prev; e > 0, so +0.0
+    for _ in range(1, degree):
+        sigma2 = 1.0 / (2.0 / sigma1 - sigma)
+        a = 2.0 * sigma2 / e
+        yield a, -c * a, -sigma * sigma2
+        sigma = sigma2
+
+
+def filter_degree(theta, res, tol, cut, hi):
+    """The degree of the next filter: what the slowest of the wanted pairs (Ritz values ``theta``, residual norms
+    ``res``) with ``res > tol`` needs to reach ``tol`` when [cut, hi] is damped, clamped to [MIN_DEGREE, MAX_DEGREE]."""
+    e, c = (hi - cut) / 2.0, (hi + cut) / 2.0
+    need = MIN_DEGREE
+    for th, r in zip(theta, res):
+        if r > tol:
+            t = abs((th - c) / e)
+            if t > 1.0 + 1e-12:
+                need = max(need, math.ceil(math.acosh(r / tol) / math.acosh(t)))
+            else:
+                need = MAX_DEGREE
+    return min(need, MAX_DEGREE)
+
+
+def _svqb(G):
+    """SVQB (Stathopoulos & Wu) of Gram matrices G (..., n, n): C with C^T G C = I on G's numerical range."""
+    d = G.diagonal(dim1=-2, dim2=-1).clamp_min(1e-300).rsqrt()
+    S, U = torch.linalg.eigh(d[..., :, None] * G * d[..., None, :])
+    S = torch.maximum(S, S.amax(dim=-1, keepdim=True) * 1e-15)
+    return d[..., :, None] * U * S.rsqrt()[..., None, :]
 
 
 class LaplaceOperator:
@@ -95,18 +138,14 @@ class _Solver:
     def chebyshev(self, c0, degree, lo, cut, hi):
         """Scaled Chebyshev filter of degree ``degree`` on columns [c0, B) of Q, damping [cut, hi]; ``lo`` estimates
         the bottom of the spectrum (scaling only).  Returns the buffer holding the result."""
-        e, c = (hi - cut) / 2.0, (hi + cut) / 2.0
-        sigma = e / (lo - c)
-        sigma1 = sigma
+        coef = chebyshev_coefficients(degree, lo, cut, hi)
         bufs = [self.Q, self.T[0], self.T[1]]
         prev, cur = 0, 1
-        self.filt(bufs[prev], None, bufs[cur], c0, sigma1 / e, -c * sigma1 / e, 0.0)
-        for _ in range(2, degree + 1):
+        self.filt(bufs[prev], None, bufs[cur], c0, *next(coef))
+        for step in coef:
             nxt = 3 - prev - cur
-            sigma2 = 1.0 / (2.0 / sigma1 - sigma)
-            a = 2.0 * sigma2 / e
-            self.filt(bufs[cur], bufs[prev], bufs[nxt], c0, a, -c * a, -sigma * sigma2)
-            prev, cur, sigma = cur, nxt, sigma2
+            self.filt(bufs[cur], bufs[prev], bufs[nxt], c0, *step)
+            prev, cur = cur, nxt
         self.steps += degree
         self.col_steps += degree * (self.B - c0)
         return bufs[cur]
@@ -124,11 +163,8 @@ class _Solver:
             R, info = torch.linalg.cholesky_ex(G, upper=True)
             if int(info) == 0:
                 Cm = torch.linalg.solve_triangular(R, torch.eye(n, dtype=G.dtype, device=G.device), upper=True)
-            else:                                        # SVQB (Stathopoulos & Wu)
-                d = G.diagonal().clamp_min(1e-300).rsqrt()
-                S, U = torch.linalg.eigh(d[:, None] * G * d[None, :])
-                S = S.clamp_min(S.max() * 1e-15)
-                Cm = d[:, None] * U * S.rsqrt()[None, :]
+            else:
+                Cm = _svqb(G)
             Z = next(b for b in (self.T[0], self.T[1], self.W2) if b is not Y)
             self.rotate(Y, c0, n, Cm, Z, c0, n)
             Y = Z
@@ -197,20 +233,7 @@ def lowest_eigenpairs(op, k, seed=0, stats=None):
         cut, lo = th_host[-1], th_host[0]
         if cut >= op.bound:
             raise ValueError("failed to compute eigendecomp: the block's Ritz values reach the spectral bound")
-        e, c = (op.bound - cut) / 2.0, (op.bound + cut) / 2.0
-        need = MIN_DEGREE
-        r_host = res_a.tolist()
-        for i, th in enumerate(th_host[lead:]):
-            if nl + i >= k:
-                break
-            r = r_host[i]
-            if r > tol:
-                t = abs((th - c) / e)
-                if t > 1.0 + 1e-12:
-                    need = max(need, math.ceil(math.acosh(r / tol) / math.acosh(t)))
-                else:
-                    need = MAX_DEGREE
-        degree = min(max(need, MIN_DEGREE), MAX_DEGREE)
+        degree = filter_degree(th_host[lead:lead + k - nl], res_a[:k - nl].tolist(), tol, cut, op.bound)
         f0 = _event()
         Y = s.chebyshev(nl, degree, lo, cut, op.bound)
         f1 = _event()
@@ -246,7 +269,6 @@ class BatchPlan:
     """``dn_eig_batch`` for meshes of ``Vs`` vertices laid out one after the other: the struct and its device arrays."""
 
     def __init__(self, Vs, device):
-        import numpy as np
         Vs = np.asarray(Vs, dtype=np.int64)
         n = len(Vs)
         begin = lambda c: np.concatenate(([0], np.cumsum(c)))
@@ -335,18 +357,7 @@ class _BatchSolver:
 
     def chebyshev(self, degree, lo, cut, hi):
         """_Solver.chebyshev with every mesh's own (lo, cut, hi): the coefficients of all steps go up in one copy."""
-        import numpy as np
-        e, c = (hi - cut) / 2.0, (hi + cut) / 2.0
-        sigma = e / (lo - c)
-        sigma1 = sigma
-        coef = np.zeros((degree, 3, self.n))
-        coef[0, 0], coef[0, 1] = sigma1 / e, -c * sigma1 / e
-        for d in range(1, degree):
-            sigma2 = 1.0 / (2.0 / sigma1 - sigma)
-            a = 2.0 * sigma2 / e
-            coef[d] = a, -c * a, -sigma * sigma2
-            sigma = sigma2
-        coef = torch.from_numpy(coef).to(self.dev)
+        coef = torch.from_numpy(np.array(list(chebyshev_coefficients(degree, lo, cut, hi)))).to(self.dev)
         bufs = [self.Q, self.T[0], self.T[1]]
         prev, cur = 0, 1
         self.filt(bufs[prev], None, bufs[cur], coef[0])
@@ -369,11 +380,7 @@ class _BatchSolver:
                 R[bad] = self.eye
                 Cm = torch.linalg.solve_triangular(R, self.eye.expand_as(R), upper=True)
                 if bad.numel():
-                    Gb = G[bad]
-                    d = Gb.diagonal(dim1=1, dim2=2).clamp_min(1e-300).rsqrt()
-                    S, U = torch.linalg.eigh(d[:, :, None] * Gb * d[:, None, :])
-                    S = torch.maximum(S, S.max(dim=1, keepdim=True).values * 1e-15)
-                    Cm[bad] = d[:, :, None] * U * S.rsqrt()[:, None, :]
+                    Cm[bad] = _svqb(G[bad])
                 self.Cm[self.act] = Cm
             self._dense(dense)
             Z = next(b for b in (self.T[0], self.T[1], self.W2) if b is not Y)
@@ -421,7 +428,6 @@ def lowest_eigenpairs_batch(ops_, k, seed=0, stats=None, first=0):
     ``ops_[0]`` in the caller's list).
     ``stats`` (dict, optional) receives iterations, filter_steps, block, n_stacked and filter / Rayleigh-Ritz / dense
     ``torch.linalg`` times in ms (the dense time is part of the Rayleigh-Ritz time)."""
-    import numpy as np
     n, k = len(ops_), int(k)
     for i, op in enumerate(ops_):
         if 0 < k and k >= op.V:
@@ -430,7 +436,7 @@ def lowest_eigenpairs_batch(ops_, k, seed=0, stats=None, first=0):
     out = [None] * n
     if k <= 0:
         return [lowest_eigenpairs(op, k, seed=seed) for op in ops_]
-    B = k + max(16, k // 4)
+    B = block_size(None, k)
     stack = [i for i, op in enumerate(ops_) if op.V >= B]
     for i, op in enumerate(ops_):
         if op.V < B:
@@ -468,18 +474,7 @@ def lowest_eigenpairs_batch(ops_, k, seed=0, stats=None, first=0):
                 raise ValueError("mesh {}: failed to compute eigendecomp: the block's Ritz values reach the spectral bound"
                                  .format(first + stack[b]))
             cut[~active], lo[~active] = 0.5 * bound[~active], 0.0       # placeholders: inactive rows are not touched
-            e, c = (bound - cut) / 2.0, (bound + cut) / 2.0
-            need = MIN_DEGREE
-            for b in np.nonzero(active)[0]:
-                for i in range(k):
-                    r = res[b, i]
-                    if r > tol[b]:
-                        t = abs((th[b, i] - c[b]) / e[b])
-                        if t > 1.0 + 1e-12:
-                            need = max(need, math.ceil(math.acosh(r / tol[b]) / math.acosh(t)))
-                        else:
-                            need = MAX_DEGREE
-            degree = min(max(need, MIN_DEGREE), MAX_DEGREE)
+            degree = max(filter_degree(th[b, :k], res[b, :k], tol[b], cut[b], bound[b]) for b in np.nonzero(active)[0])
             s.set_active(active)
             f0 = _event()
             Y = s.chebyshev(degree, lo, cut, bound)

@@ -237,47 +237,66 @@ def get_all_operators(verts_list, faces_list, k_eig, op_cache_dir=None, normals=
 EPS = 1e-8          # geometry.py:308: mass shift (times the mean) and eigenproblem shift
 
 
+def _vertex_normals(v64, f64, frames):
+    """dn_vertex_frames on a mesh or a disjoint union of meshes: (V,3) fp64 vertex normals (NaN where a vertex has
+    none) and whether any is NaN (one host read).  ``frames`` receives frames built from these unrounded normals, for
+    ``_frames_from_normals`` to overwrite."""
+    V, F = int(v64.shape[0]), int(f64.shape[0])
+    dev = v64.device
+    nrm = torch.empty(V, 3, dtype=torch.float64, device=dev)
+    nbad = torch.zeros(1, dtype=torch.int32, device=dev)
+    ws = torch.empty(12 * F + 8 * V + 1024, dtype=torch.uint8, device=dev)
+    _lib_check(_lib_load().dn_vertex_frames(v64.data_ptr(), f64.data_ptr(), F, V, None, nrm.data_ptr(), frames.data_ptr(),
+                                            nbad.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()), "dn_vertex_frames")
+    return nrm, int(nbad.item()) > 0
+
+
+def _frames_from_normals(normals, dtype, frames):
+    """dn_vertex_frames from given (V,3) normals into ``frames`` (V,3,3) fp64; the normals are rounded to ``dtype``
+    first, as the reference converts them (geometry.py:144)."""
+    nbad = torch.zeros(1, dtype=torch.int32, device=frames.device)
+    n_in = normals.to(device=frames.device, dtype=dtype).to(torch.float64).contiguous()
+    _lib_check(_lib_load().dn_vertex_frames(None, None, 0, int(frames.shape[0]), n_in.data_ptr(), None, frames.data_ptr(),
+                                            nbad.data_ptr(), None, 0, ops._stream()), "dn_vertex_frames")
+    return frames
+
+
 def _vertex_frames(v64, f64, normals, dtype, verts):
     """geometry.py:101-177 for meshes: (V,3,3) fp64 frames from dn_vertex_frames, with the reference's remedy for NaN
     normals (geometry.py:128-141: wiggle the bad vertices with RandomState(777) and recompute; if still NaN, random
     normals from the same seed).  Normals are rounded to ``dtype`` before the frames are built, as the reference
     converts them (geometry.py:144)."""
-    lib = _lib_load()
-    V, F = int(v64.shape[0]), int(f64.shape[0])
     dev = v64.device
-    frames = torch.empty(V, 3, 3, dtype=torch.float64, device=dev)
-    nbad = torch.zeros(1, dtype=torch.int32, device=dev)
+    frames = torch.empty(int(v64.shape[0]), 3, 3, dtype=torch.float64, device=dev)
     if normals is None:
-        nrm = torch.empty(V, 3, dtype=torch.float64, device=dev)
-        ws = torch.empty(12 * F + 8 * V + 1024, dtype=torch.uint8, device=dev)
-        call = lambda v: _lib_check(lib.dn_vertex_frames(v.data_ptr(), f64.data_ptr(), F, V, None, nrm.data_ptr(),
-                                                         frames.data_ptr(), nbad.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                         ops._stream()), "dn_vertex_frames")
-        call(v64)
-        if int(nbad.item()) > 0:
+        normals, any_bad = _vertex_normals(v64, f64, frames)
+        if any_bad:
             verts_np = _to_np(verts)
-            bad = torch.isnan(nrm).any(dim=1, keepdim=True).cpu().numpy()
+            bad = torch.isnan(normals).any(dim=1, keepdim=True).cpu().numpy()
             bbox = np.amax(verts_np, axis=0) - np.amin(verts_np, axis=0)
             wiggle = (np.random.RandomState(seed=777).rand(*verts_np.shape) - 0.5) * (np.linalg.norm(bbox) * 1e-4)
-            call(torch.from_numpy(np.ascontiguousarray(verts_np + bad * wiggle, dtype=np.float64)).to(dev))
-            if int(nbad.item()) > 0:
-                bad = torch.isnan(nrm).any(dim=1).cpu().numpy()
+            wiggled = torch.from_numpy(np.ascontiguousarray(verts_np + bad * wiggle, dtype=np.float64)).to(dev)
+            normals, any_bad = _vertex_normals(wiggled, f64, frames)
+            if any_bad:
+                bad = torch.isnan(normals).any(dim=1).cpu().numpy()
                 rnd = (np.random.RandomState(seed=777).rand(*verts_np.shape) - 0.5)[bad, :]
                 rnd = rnd / np.linalg.norm(rnd, axis=-1)[:, None]
-                nrm[torch.from_numpy(bad).to(dev)] = torch.from_numpy(rnd).to(dev)
-        normals = nrm
-    n_in = normals.to(device=dev, dtype=dtype).to(torch.float64).contiguous()
-    _lib_check(lib.dn_vertex_frames(None, None, F, V, n_in.data_ptr(), None, frames.data_ptr(), nbad.data_ptr(), None,
-                                    0, ops._stream()), "dn_vertex_frames")
-    return frames
+                normals[torch.from_numpy(bad).to(dev)] = torch.from_numpy(rnd).to(dev)
+    return _frames_from_normals(normals, dtype, frames)
 
 
-def mesh_laplacian(v64, f64, eps=EPS):
+def mesh_laplacian(v64, f64, eps=EPS, row_begin=None, first=0):
     """dn_mesh_laplacian: ``(rowptr, colidx, L_vals, mass, A_vals, A_diag, bound)`` on the device (fp64 values, int32
     indices), the reference's cotan Laplacian and lumped mass (geometry.py:322-329) and the operator the eigensolver
-    runs on.  Raises the reference's RuntimeError on a NaN Laplacian or mass (geometry.py:326-329)."""
+    runs on.  Raises the reference's RuntimeError on a NaN Laplacian or mass (geometry.py:326-329).
+
+    With ``row_begin`` (the n + 1 row offsets, an int32 device tensor, of the n meshes whose disjoint union v64 / f64
+    hold): dn_mesh_laplacian_batched, which gives each mesh its own mass shift and bound.  ``bound`` is then a numpy
+    array of n, an eighth value holds the offsets ``rowptr[row_begin]`` of the meshes' entries (numpy int64), and the
+    NaN errors name their mesh, counted from ``first``."""
     lib = _lib_load()
     V, F = int(v64.shape[0]), int(f64.shape[0])
+    n = 1 if row_begin is None else int(row_begin.numel()) - 1
     dev = v64.device
     cap = max(6 * F + V, 1)
     rowptr = torch.empty(V + 1, dtype=torch.int32, device=dev)
@@ -286,20 +305,30 @@ def mesh_laplacian(v64, f64, eps=EPS):
     avals = torch.empty(cap, dtype=torch.float64, device=dev)
     mass = torch.empty(V, dtype=torch.float64, device=dev)
     adiag = torch.empty(V, dtype=torch.float64, device=dev)
-    bound = torch.empty(1, dtype=torch.float64, device=dev)
-    nan = torch.empty(2, dtype=torch.int32, device=dev)
+    bound = torch.empty(n, dtype=torch.float64, device=dev)
+    nan = torch.empty(n, 2, dtype=torch.int32, device=dev)
     ws = torch.empty(120 * F + 12 * V + 2048, dtype=torch.uint8, device=dev)
-    _lib_check(lib.dn_mesh_laplacian(v64.data_ptr(), f64.data_ptr(), F, V, eps, rowptr.data_ptr(), colidx.data_ptr(),
-                                     lvals.data_ptr(), mass.data_ptr(), avals.data_ptr(), adiag.data_ptr(),
-                                     bound.data_ptr(), nan.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()),
-               "dn_mesh_laplacian")
-    nan_l, nan_m = nan.tolist()
-    if nan_l:
-        raise RuntimeError("NaN Laplace matrix")
-    if nan_m:
-        raise RuntimeError("NaN mass matrix")
-    nnz = int(rowptr[-1].item())
-    return rowptr, colidx[:nnz], lvals[:nnz], mass, avals[:nnz], adiag, float(bound.item())
+    out = (rowptr.data_ptr(), colidx.data_ptr(), lvals.data_ptr(), mass.data_ptr(), avals.data_ptr(), adiag.data_ptr(),
+           bound.data_ptr(), nan.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream())
+    if row_begin is None:
+        _lib_check(lib.dn_mesh_laplacian(v64.data_ptr(), f64.data_ptr(), F, V, eps, *out), "dn_mesh_laplacian")
+        ends = rowptr[-1:]
+    else:
+        _lib_check(lib.dn_mesh_laplacian_batched(v64.data_ptr(), f64.data_ptr(), F, V, n, row_begin.data_ptr(), eps, *out),
+                   "dn_mesh_laplacian_batched")
+        ends = rowptr[row_begin.long()]
+    del ws
+    host = torch.cat((bound, nan.flatten().double(), ends.double())).cpu().numpy()      # one read of all three
+    bound_h, nan_h, nzb = host[:n], host[n:3 * n].reshape(n, 2), host[3 * n:].astype(np.int64)
+    for b in range(n):
+        mesh = "" if row_begin is None else "mesh {}: ".format(first + b)
+        if nan_h[b, 0]:
+            raise RuntimeError(mesh + "NaN Laplace matrix")
+        if nan_h[b, 1]:
+            raise RuntimeError(mesh + "NaN mass matrix")
+    nnz = int(nzb[-1])
+    csr = (rowptr, colidx[:nnz], lvals[:nnz], mass, avals[:nnz], adiag)
+    return csr + (float(bound_h[0]),) if row_begin is None else csr + (bound_h, nzb)
 
 
 def _lib_load():
@@ -433,7 +462,8 @@ def _compute_operators_batch(verts_list, faces_list, k_eig, normals, device, max
     k_eig = int(k_eig)
     Vs = [int(v.shape[0]) for v in verts_list]
     if max_rows is None:
-        B = k_eig + max(16, k_eig // 4)
+        from . import eigen
+        B = eigen.block_size(None, k_eig)
         with torch.cuda.device(device):
             max_rows = max(torch.cuda.mem_get_info()[0] // 3 // (5 * 8 * B + 8 * k_eig + 2048), 1)
     out = []
@@ -449,7 +479,6 @@ def _compute_operators_batch(verts_list, faces_list, k_eig, normals, device, max
 
 def _compute_group(verts_list, faces_list, k_eig, normals, device, dtype, first, stats):
     from . import eigen
-    lib = _lib_load()
     n = len(verts_list)
     ev = []
     mark = lambda: ev.append(torch.cuda.Event(enable_timing=True)) or ev[-1].record()
@@ -465,51 +494,22 @@ def _compute_group(verts_list, faces_list, k_eig, normals, device, dtype, first,
             raise ValueError("mesh {}: faces index vertices outside [0, {})".format(first + b, Vs[b]))
     v64 = torch.cat(v64s)
     f64 = torch.cat([f + int(rb[b]) for b, f in enumerate(f64s)]).contiguous()
-    F = int(f64.shape[0])
     row_begin = torch.from_numpy(rb.astype(np.int32)).to(device)
     # Laplacian + mass of the union, (mass shift, bound, NaN flags) per mesh
-    cap = max(6 * F + V, 1)
-    rowptr = torch.empty(V + 1, dtype=torch.int32, device=device)
-    colidx = torch.empty(cap, dtype=torch.int32, device=device)
-    lvals = torch.empty(cap, dtype=torch.float64, device=device)
-    avals = torch.empty(cap, dtype=torch.float64, device=device)
-    mass = torch.empty(V, dtype=torch.float64, device=device)
-    adiag = torch.empty(V, dtype=torch.float64, device=device)
-    bound = torch.empty(n, dtype=torch.float64, device=device)
-    nan = torch.empty(n, 2, dtype=torch.int32, device=device)
-    ws = torch.empty(120 * F + 12 * V + 2048, dtype=torch.uint8, device=device)
-    _lib_check(lib.dn_mesh_laplacian_batched(v64.data_ptr(), f64.data_ptr(), F, V, n, row_begin.data_ptr(), EPS,
-                                             rowptr.data_ptr(), colidx.data_ptr(), lvals.data_ptr(), mass.data_ptr(),
-                                             avals.data_ptr(), adiag.data_ptr(), bound.data_ptr(), nan.data_ptr(),
-                                             ws.data_ptr(), ws.numel(), ops._stream()), "dn_mesh_laplacian_batched")
-    del ws
-    host = torch.cat((bound, nan.flatten().double(), rowptr[row_begin.long()].double())).cpu().numpy()
-    bound_h, nan_h, nzb = host[:n], host[n:3 * n].reshape(n, 2), host[3 * n:].astype(np.int64)
-    for b in range(n):
-        if nan_h[b, 0]:
-            raise RuntimeError("mesh {}: NaN Laplace matrix".format(first + b))
-        if nan_h[b, 1]:
-            raise RuntimeError("mesh {}: NaN mass matrix".format(first + b))
+    rowptr, colidx, lvals, mass, avals, adiag, bound_h, nzb = mesh_laplacian(v64, f64, row_begin=row_begin, first=first)
     nnz = int(nzb[-1])
-    colidx, lvals, avals = colidx[:nnz], lvals[:nnz], avals[:nnz]
     mark()
     # frames of the union; a mesh with a NaN normal takes compute_operators' own route (its remedy is a host step)
     frames = torch.empty(V, 3, 3, dtype=torch.float64, device=device)
-    nbad = torch.zeros(1, dtype=torch.int32, device=device)
-    nrm = torch.empty(V, 3, dtype=torch.float64, device=device)
-    ws = torch.empty(12 * F + 8 * V + 1024, dtype=torch.uint8, device=device)
-    _lib_check(lib.dn_vertex_frames(v64.data_ptr(), f64.data_ptr(), F, V, None, nrm.data_ptr(), frames.data_ptr(),
-                                    nbad.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()), "dn_vertex_frames")
+    nrm, any_bad = _vertex_normals(v64, f64, frames)
     redo = []
-    if int(nbad.item()) > 0:
+    if any_bad:
         bad_rows = torch.isnan(nrm).any(dim=1).cpu().numpy()
         redo = [b for b in range(n) if normals[b] is None and bad_rows[rb[b]:rb[b + 1]].any()]
     for b, nb in enumerate(normals):
         if nb is not None:
             nrm[rb[b]:rb[b + 1]] = nb.to(device=device, dtype=torch.float64)
-    n_in = nrm.to(dtype).to(torch.float64).contiguous()
-    _lib_check(lib.dn_vertex_frames(None, None, F, V, n_in.data_ptr(), None, frames.data_ptr(), nbad.data_ptr(), None, 0,
-                                    ops._stream()), "dn_vertex_frames")
+    _frames_from_normals(nrm, dtype, frames)
     for b in redo:
         frames[rb[b]:rb[b + 1]] = _vertex_frames(v64s[b], f64s[b].contiguous(), None, dtype, verts_list[b])
     mark()

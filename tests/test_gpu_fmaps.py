@@ -379,8 +379,8 @@ def _nn_fp64(source, target, rows=None, chunk=64):
     return torch.cat(idx), torch.cat(d1), torch.cat(d2)
 
 
-def _check_nn(idx, source, target, rows, n):
-    gi, d1, d2 = _nn_fp64(source, target, rows)
+def _check_nn(idx, source, target, rows, n, chunk=64):
+    gi, d1, d2 = _nn_fp64(source, target, rows, chunk=chunk)
     tau = (n + 2) * U32 / (1 - (n + 2) * U32)
     lim = d1 * (1 + tau) / (1 - tau)
     q = source.to(torch.float64) if rows is None else source[rows].to(torch.float64)

@@ -11,6 +11,11 @@
 // reduction over V is a per-CTA partial (warps added in a fixed order) followed by a sum over the CTAs in index order,
 // with no atomics: two calls on the same device give bitwise-equal results.
 //
+// A column whose b_c is not finite (a NaN or inf in x or grad_out, a NaN mass entry), or whose p.q, alpha, r.r or r.z
+// turns non-finite during the iteration (an inf in the data, a NaN in L), is frozen at once with a NaN result, as the
+// reference's dense solve returns NaN: active[c] = -1, where 1 is iterating and 0 converged.  It does not count as
+// unconverged, so the other columns are still written.
+//
 // Data written by other CTAs inside the kernel is read with ld.global.cg (L2), never through the non-coherent L1 or
 // read-only paths.
 #include <cooperative_groups.h>
@@ -43,7 +48,7 @@ struct ImplicitArgs {
   double* ldiag;            // V
   double* part;             // 2 x kMaxCtas x C
   double* col;              // 6 x C: rz, |b|, alpha, beta, r.r, and the iteration count
-  int* active;              // C
+  int* active;              // C: 1 iterating, 0 converged, -1 non-finite (NaN result)
   int* n_active;            // 1
 };
 
@@ -145,8 +150,8 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
       rr[c] = bb;
       iters[c] = 0.0;
       const int live = bb > 0.0;        // b_c = 0: x_c = 0 is exact
-      a.active[c] = live;
-      act += live;
+      a.active[c] = isfinite(bb) ? live : -1;
+      act += live && isfinite(bb);
     }
     for (int o = 16; o > 0; o >>= 1) act += __shfl_xor_sync(0xffffffffu, act, o);
     if (lane == 0) s_act[threadIdx.x >> 5] = act;
@@ -162,7 +167,7 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
   for (int it = 0; it < a.max_iter && ldg_cg(a.n_active) > 0; ++it) {
     bool on[NC];
 #pragma unroll
-    for (int q = 0; q < NC; ++q) on[q] = cok[q] && ldg_cg(a.active + lane + 32 * q) != 0;
+    for (int q = 0; q < NC; ++q) on[q] = cok[q] && ldg_cg(a.active + lane + 32 * q) > 0;
 
     // ---- q = M p + t (L p), partial p.q
 #pragma unroll
@@ -194,7 +199,7 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
     grid.sync();
     if (first_cta)
       for (int c = threadIdx.x; c < C; c += kThreads)
-        if (a.active[c]) alpha[c] = rz[c] / cta_sum(part0, G, C, c);
+        if (a.active[c] > 0) alpha[c] = rz[c] / cta_sum(part0, G, C, c);
     grid.sync();
 
     // ---- x += alpha p, r -= alpha q; partials r.r and r.z
@@ -223,11 +228,13 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
     if (first_cta) {
       int act = 0;
       for (int c = threadIdx.x; c < C; c += kThreads) {
-        if (!a.active[c]) continue;
+        if (a.active[c] <= 0) continue;
         const double r2 = cta_sum(part0, G, C, c), rzn = cta_sum(part1, G, C, c);
         rr[c] = r2;
         iters[c] += 1.0;
-        if (sqrt(r2) <= a.rtol * bnorm[c]) {
+        if (!(isfinite(alpha[c]) && isfinite(r2) && isfinite(rzn))) {   // p.q or the data went non-finite
+          a.active[c] = -1;
+        } else if (sqrt(r2) <= a.rtol * bnorm[c]) {
           a.active[c] = 0;              // frozen: x_c is final
         } else {
           beta[c] = rzn / rz[c];
@@ -251,7 +258,7 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
     double be[NC];
 #pragma unroll
     for (int q = 0; q < NC; ++q) {
-      on[q] = cok[q] && ldg_cg(a.active + lane + 32 * q) != 0;
+      on[q] = cok[q] && ldg_cg(a.active + lane + 32 * q) > 0;
       be[q] = on[q] ? ldg_cg(beta + lane + 32 * q) : 0.0;
     }
     for (int64_t v = warp0; v < V; v += n_warps) {
@@ -274,7 +281,9 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
       const double itc = ldg_cg(iters + c);
       a.status[2 + c] = itc;
       const double bn = ldg_cg(bnorm + c);
-      a.status[2 + C + c] = bn > 0.0 ? sqrt(ldg_cg(rr + c)) / bn : 0.0;
+      a.status[2 + C + c] = ldg_cg(a.active + c) < 0 ? __longlong_as_double(0x7ff8000000000000ll)
+                            : bn > 0.0              ? sqrt(ldg_cg(rr + c)) / bn
+                                                    : 0.0;
       worst_it = fmax(worst_it, itc);
     }
     for (int o = 16; o > 0; o >>= 1) worst_it = fmax(worst_it, __shfl_xor_sync(0xffffffffu, worst_it, o));
@@ -292,11 +301,16 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
   }
   if (unconverged) return;
 
+  // on[q]: this lane's column q is written from x; a non-finite column is written as NaN
+  const float fnan = __int_as_float(0x7fc00000);
+  bool on[NC];
+#pragma unroll
+  for (int q = 0; q < NC; ++q) on[q] = cok[q] && ldg_cg(a.active + lane + 32 * q) == 0;
   if (!a.backward) {
     for (int64_t v = warp0; v < V; v += n_warps)
 #pragma unroll
       for (int q = 0; q < NC; ++q)
-        if (cok[q]) a.out[v * C + lane + 32 * q] = (float)a.X[v * C + lane + 32 * q];
+        if (cok[q]) a.out[v * C + lane + 32 * q] = on[q] ? (float)a.X[v * C + lane + 32 * q] : fnan;
     return;
   }
   // backward: grad_x = M w; grad_time[c] += -sum_v w[v][c] (L y)[v][c]
@@ -320,14 +334,15 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
       if (!cok[q]) continue;
       const int64_t i = v * C + lane + 32 * q;
       const double w = a.X[i];
-      a.out[i] = (float)(m * w);
+      a.out[i] = on[q] ? (float)(m * w) : fnan;
       acc0[q] = fma(w, ly[q], acc0[q]);
     }
   }
   cta_partial<NC>(red[0], acc0, C, part0);
   grid.sync();
   if (first_cta)
-    for (int c = threadIdx.x; c < C; c += kThreads) a.grad_time[c] += (float)(-cta_sum(part0, G, C, c));
+    for (int c = threadIdx.x; c < C; c += kThreads)
+      a.grad_time[c] += ldg_cg(a.active + c) == 0 ? (float)(-cta_sum(part0, G, C, c)) : fnan;
 }
 
 template <int NC>

@@ -348,6 +348,9 @@ int dn_eig_finalize_batched(const double* Y, int64_t ldy, const int32_t* cols, i
  * [0] the number of columns that did not converge within max_iter iterations, [1] the largest iteration count,
  * [2 + c] the iterations of column c, [2 + C + c] its final ||r_c|| / ||b_c|| (0 when b_c = 0).  When [0] > 0 the
  * outputs are not written (grad_time is not accumulated); the caller reads `status` to find out.
+ * Non-finite data gives NaN, at once: a column whose b_c is not finite, or whose p.q, alpha, r.r or r.z turns
+ * non-finite (an inf in the data, a NaN in L), stops with a NaN result: that column of x_diffuse (grad_x) is NaN and
+ * grad_time[c] becomes NaN; [2 + c] holds its iterations and [2 + C + c] is NaN.  It does not count in [0].
  *   fwd: time (C) is clamped in place (layers.py:48-49) whether or not the solve converges, as the reference clamps
  *        before solving.
  *   bwd: with A_c = M + t_c L and w_c = A_c^-1 grad_out[:, c]: grad_x = M w, grad_time[c] += -sum_v w[v][c] (L x_diffuse)[v][c]

@@ -24,17 +24,23 @@ def from_basis(values, basis):
 
 
 def block_forward(x_in, mass, evals, evecs, gradX, gradY, params, with_gradient_features=True, relu_masks=None,
-                  pre_acts=None):
+                  pre_acts=None, diffuse=None):
     """layers.py:200-241 for a batched input (B,V,C); gradX/gradY sparse COO (B,V,V) or lists of (V,V).
 
     Test hooks (not reference behaviour): ``pre_acts`` (a list) receives every hidden layer's pre-activation;
     ``relu_masks`` (one bool tensor per hidden layer) replaces ``relu(h)`` by ``h * mask`` so that a gradient can be
     checked under a GIVEN activation pattern -- the gradient of ReLU is discontinuous at 0, and an fp32 forward may
-    land on the other side of a kink than the fp64 one for pre-activations of order 1e-7."""
+    land on the other side of a kink than the fp64 one for pre-activations of order 1e-7.  ``diffuse`` (a callable
+    ``(x_in, t) -> x_diffuse`` with t already clamped) replaces the spectral diffusion, so that a test can compose the
+    block around another solve of the heat equation (the implicit method, layers.py:69-84); ``evals`` / ``evecs`` are
+    then not read."""
     t = torch.clamp(params["diffusion.diffusion_time"], min=1e-8)                  # layers.py:48-49
-    x_spec = to_basis(x_in, evecs, mass)                                           # :59
-    coefs = torch.exp(-evals.unsqueeze(-1) * t.unsqueeze(0))                       # :62-63
-    x_diffuse = from_basis(coefs * x_spec, evecs)                                  # :64-67
+    if diffuse is not None:
+        x_diffuse = diffuse(x_in, t)
+    else:
+        x_spec = to_basis(x_in, evecs, mass)                                       # :59
+        coefs = torch.exp(-evals.unsqueeze(-1) * t.unsqueeze(0))                   # :62-63
+        x_diffuse = from_basis(coefs * x_spec, evecs)                              # :64-67
     feats = [x_in, x_diffuse]
     if with_gradient_features:
         grads = []

@@ -63,15 +63,6 @@ struct DnLayer {
   int head_n;
 };
 
-#ifdef __CUDACC__
-// tanh of the gradient features (layers.py:130): 1 - 2 / (exp(2x) + 1) with the fast exp / divide; absolute error
-// <= ~1.5e-7 over the whole range, saturates to +-1, NaN propagates.  Every kernel that forms features uses this one.
-__device__ __forceinline__ float dn_feat_tanh(float x) {
-  const float e = __expf(2.f * x);
-  return 1.f - __fdividef(2.f, e + 1.f);
-}
-#endif
-
 struct DnRowsSrc {
   const float* ptr[DN_MAX_SRC];
   int width[DN_MAX_SRC];

@@ -8,6 +8,7 @@
 #include "dn_internal.h"
 #include "dn_tc_ptx.cuh"
 #include <math.h>
+#include <type_traits>
 
 namespace {
 
@@ -388,131 +389,114 @@ __global__ void grad_spmm_pair_kernel(const int32_t* __restrict__ rowptr, const 
   }
 }
 
-struct Acc4 {
-  float4 gX, gY, bre, bim;
-};
+// ---------------------------------------------------------------------------------------------
+// gradient features (layers.py:121-130):  feat = tanh(gX*Bre + gY*Bim),  gX = GX x, gY = GY x,
+// Bre = GX P - GY Q, Bim = GY P + GX Q, with P = xd A_re^T, Q = xd A_im^T ([P|Q], row stride ld_pq)
+//
+// Every kernel below that forms or differentiates the features accumulates a CSR row with feat_entry, in CSR order,
+// and the forward kernels finish with feat_value, so they are bit-identical to each other.  Lane type T is float (one
+// channel) or float4 (four consecutive channels, one 16-byte access per row and stream).
+// ---------------------------------------------------------------------------------------------
 
 // tanh(x) = 1 - 2 / (exp(2x) + 1) with the hardware exp2 and fast division: ~6 instructions instead of tanhf's ~30
 // (the gather kernel issues instructions on 53 % of its cycles, profiles/r01: the four tanhf per lane were a fifth of
-// them).  Absolute error <= ~1.5e-7 over the whole range (saturates to +-1, NaN propagates); every gather variant
-// uses this one function so that they stay bit-identical to each other.
-__device__ __forceinline__ float feat_tanh(float x) { return dn_feat_tanh(x); }
+// them).  Absolute error <= ~1.5e-7 over the whole range, saturates to +-1, NaN propagates.
+__device__ __forceinline__ float dn_feat_tanh(float x) {
+  const float e = __expf(2.f * x);
+  return 1.f - __fdividef(2.f, e + 1.f);
+}
 
-template <bool ROT>
-__device__ __forceinline__ Acc4 gather_row(const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
-                                           const float* __restrict__ xd, const float* __restrict__ pq, int ld_pq,
-                                           int C, int s, int e, int c4) {
-  Acc4 a;
-  a.gX = a.gY = a.bre = a.bim = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 4
+// f applied channel by channel to lanes of type float or float4
+template <class F, class... A>
+__device__ __forceinline__ float per_ch(F f, float a, A... b) { return f(a, b...); }
+template <class F, class... A>
+__device__ __forceinline__ float4 per_ch(F f, float4 a, A... b) {
+  return make_float4(f(a.x, b.x...), f(a.y, b.y...), f(a.z, b.z...), f(a.w, b.w...));
+}
+
+template <class T>
+__device__ __forceinline__ T vfma(float w, T v, T acc) {
+  return per_ch([w](float vi, float ai) { return fmaf(w, vi, ai); }, v, acc);
+}
+
+template <class T>
+__device__ __forceinline__ T ldg_lane(const float* p) {
+  if constexpr (sizeof(T) == sizeof(float4)) return ldg4(p);
+  else return __ldg(p);
+}
+
+template <class T>
+struct FeatAcc {
+  T gX, gY, bre, bim;
+};
+
+// one CSR entry (col, g = (gx, gy)) of a row: x, P, Q are the lanes of row col of xd, P and Q.  The one place the
+// per-channel FMA sequence is written.
+template <bool ROT, class T>
+__device__ __forceinline__ void feat_entry(FeatAcc<T>& a, float2 g, T x, T P, T Q) {
+  a.gX = vfma(g.x, x, a.gX);
+  a.gY = vfma(g.y, x, a.gY);
+  a.bre = vfma(g.x, P, a.bre);
+  a.bim = vfma(g.y, P, a.bim);
+  if (ROT) {
+    a.bre = vfma(-g.y, Q, a.bre);
+    a.bim = vfma(g.x, Q, a.bim);
+  }
+}
+
+template <class T>
+__device__ __forceinline__ T feat_value(const FeatAcc<T>& a) {
+  return per_ch([](float gX, float gY, float bre, float bim) { return dn_feat_tanh(fmaf(gX, bre, gY * bim)); },
+                a.gX, a.gY, a.bre, a.bim);
+}
+
+// the accumulators of channels [c, c + |T|) over a row's CSR entries [s, e)
+template <bool ROT, class T>
+__device__ __forceinline__ FeatAcc<T> gather_row(const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
+                                                 const float* __restrict__ xd, const float* __restrict__ pq, int ld_pq,
+                                                 int C, int s, int e, int c) {
+  FeatAcc<T> a = {};
   for (int p = s; p < e; ++p) {
     const int64_t col = __ldg(colidx + p);
     const float2 g = __ldg(vals + p);
-    const float4 x = ldg4(xd + col * C + c4 * 4);
-    const float4 P = ldg4(pq + col * ld_pq + c4 * 4);
-    a.gX.x = fmaf(g.x, x.x, a.gX.x); a.gX.y = fmaf(g.x, x.y, a.gX.y);
-    a.gX.z = fmaf(g.x, x.z, a.gX.z); a.gX.w = fmaf(g.x, x.w, a.gX.w);
-    a.gY.x = fmaf(g.y, x.x, a.gY.x); a.gY.y = fmaf(g.y, x.y, a.gY.y);
-    a.gY.z = fmaf(g.y, x.z, a.gY.z); a.gY.w = fmaf(g.y, x.w, a.gY.w);
-    a.bre.x = fmaf(g.x, P.x, a.bre.x); a.bre.y = fmaf(g.x, P.y, a.bre.y);
-    a.bre.z = fmaf(g.x, P.z, a.bre.z); a.bre.w = fmaf(g.x, P.w, a.bre.w);
-    a.bim.x = fmaf(g.y, P.x, a.bim.x); a.bim.y = fmaf(g.y, P.y, a.bim.y);
-    a.bim.z = fmaf(g.y, P.z, a.bim.z); a.bim.w = fmaf(g.y, P.w, a.bim.w);
-    if (ROT) {
-      const float4 Q = ldg4(pq + col * ld_pq + C + c4 * 4);
-      a.bre.x = fmaf(-g.y, Q.x, a.bre.x); a.bre.y = fmaf(-g.y, Q.y, a.bre.y);
-      a.bre.z = fmaf(-g.y, Q.z, a.bre.z); a.bre.w = fmaf(-g.y, Q.w, a.bre.w);
-      a.bim.x = fmaf(g.x, Q.x, a.bim.x); a.bim.y = fmaf(g.x, Q.y, a.bim.y);
-      a.bim.z = fmaf(g.x, Q.z, a.bim.z); a.bim.w = fmaf(g.x, Q.w, a.bim.w);
-    }
+    const T x = ldg_lane<T>(xd + col * C + c);
+    const T P = ldg_lane<T>(pq + col * ld_pq + c);
+    feat_entry<ROT>(a, g, x, P, ROT ? ldg_lane<T>(pq + col * ld_pq + C + c) : T{});
   }
   return a;
 }
 
-// feat = tanh(gX*Bre + gY*Bim), Bre/Bim gathered from P = xd A_re^T, Q = xd A_im^T (layers.py:121-130)
-template <bool ROT>
+// Runs body(row, s, e, c) for each lane of channels [c, c + |T|) the thread owns in a row-gather kernel, [s, e) being
+// the row's CSR entries.  float4 lanes: G threads per row (a power of two, whole warps of 32 / G rows), each stepping
+// over the row by 4 G channels.  float lanes (C % 4 != 0): one thread per (row, channel).
+template <class T, class F>
+__device__ __forceinline__ void feat_lanes(const int32_t* __restrict__ rowptr, int64_t V, int C, int G, F body) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if constexpr (sizeof(T) == sizeof(float4)) {
+    const int lane = threadIdx.x & 31;
+    const int64_t row = (t >> 5) * (32 / G) + lane / G;
+    if (row >= V) return;
+    const int s = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
+    for (int c = 4 * (lane % G); c < C; c += 4 * G) body(row, s, e, c);
+  } else {
+    if (t >= V * C) return;
+    const int64_t row = t / C;
+    const int c = (int)(t - row * C);
+    body(row, __ldg(rowptr + row), __ldg(rowptr + row + 1), c);
+  }
+}
+
+// feat = tanh(gX*Bre + gY*Bim) row by row, threads mapped by feat_lanes
+template <bool ROT, class T>
 __global__ void __launch_bounds__(256) spmm_features_kernel(const int32_t* __restrict__ rowptr,
                                                             const int32_t* __restrict__ colidx,
                                                             const float2* __restrict__ vals,
                                                             const float* __restrict__ xd, const float* __restrict__ pq,
                                                             int ld_pq, int64_t V, int C, int G,
                                                             float* __restrict__ feat) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t row = warp * (32 / G) + lane / G;
-  const int gl = lane % G;
-  if (row >= V) return;
-  const int s = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
-  for (int c4 = gl; c4 < (C >> 2); c4 += G) {
-    const Acc4 a = gather_row<ROT>(colidx, vals, xd, pq, ld_pq, C, s, e, c4);
-    float4 o;
-    o.x = feat_tanh(fmaf(a.gX.x, a.bre.x, a.gY.x * a.bim.x));
-    o.y = feat_tanh(fmaf(a.gX.y, a.bre.y, a.gY.y * a.bim.y));
-    o.z = feat_tanh(fmaf(a.gX.z, a.bre.z, a.gY.z * a.bim.z));
-    o.w = feat_tanh(fmaf(a.gX.w, a.bre.w, a.gY.w * a.bim.w));
-    *reinterpret_cast<float4*>(feat + row * C + c4 * 4) = o;
-  }
-}
-
-// Scalar-lane forms of the features kernels for C % 4 != 0 (no float4 row access): one thread per (row, channel), the
-// same per-element operation order as gather_row and the float4 kernels.
-struct Acc1 {
-  float gX, gY, bre, bim;
-};
-
-template <bool ROT>
-__device__ __forceinline__ Acc1 gather_row_scalar(const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
-                                                  const float* __restrict__ xd, const float* __restrict__ pq,
-                                                  int ld_pq, int C, int s, int e, int c) {
-  Acc1 a = {0.f, 0.f, 0.f, 0.f};
-  for (int p = s; p < e; ++p) {
-    const int64_t col = __ldg(colidx + p);
-    const float2 g = __ldg(vals + p);
-    const float x = __ldg(xd + col * C + c);
-    const float P = __ldg(pq + col * ld_pq + c);
-    a.gX = fmaf(g.x, x, a.gX);
-    a.gY = fmaf(g.y, x, a.gY);
-    a.bre = fmaf(g.x, P, a.bre);
-    a.bim = fmaf(g.y, P, a.bim);
-    if (ROT) {
-      const float Q = __ldg(pq + col * ld_pq + C + c);
-      a.bre = fmaf(-g.y, Q, a.bre);
-      a.bim = fmaf(g.x, Q, a.bim);
-    }
-  }
-  return a;
-}
-
-template <bool ROT>
-__global__ void __launch_bounds__(256) spmm_features_scalar_kernel(const int32_t* __restrict__ rowptr,
-                                                                   const int32_t* __restrict__ colidx,
-                                                                   const float2* __restrict__ vals,
-                                                                   const float* __restrict__ xd,
-                                                                   const float* __restrict__ pq, int ld_pq, int64_t V,
-                                                                   int C, float* __restrict__ feat) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= V * C) return;
-  const int64_t row = idx / C;
-  const int c = (int)(idx - row * C);
-  const Acc1 a = gather_row_scalar<ROT>(colidx, vals, xd, pq, ld_pq, C, __ldg(rowptr + row), __ldg(rowptr + row + 1), c);
-  feat[row * C + c] = feat_tanh(fmaf(a.gX, a.bre, a.gY * a.bim));
-}
-
-__device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(unsigned long long v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-// d = a * b + d on both fp32 halves (two IEEE fp32 FMAs)
-__device__ __forceinline__ void fma2(unsigned long long& d, unsigned long long a, unsigned long long b) {
-  float d0, d1, a0, a1, b0, b1;
-  unpack2(d, d0, d1);
-  unpack2(a, a0, a1);
-  unpack2(b, b0, b1);
-  d = pack2(fmaf(a0, b0, d0), fmaf(a1, b1, d1));
+  feat_lanes<T>(rowptr, V, C, G, [&](int64_t row, int s, int e, int c) {
+    *reinterpret_cast<T*>(feat + row * C + c) = feat_value(gather_row<ROT, T>(colidx, vals, xd, pq, ld_pq, C, s, e, c));
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -522,41 +506,31 @@ __device__ __forceinline__ void fma2(unsigned long long& d, unsigned long long a
 //     kernel) becomes one latency per 64 rows plus the gathers themselves;
 //   * a warp issues every neighbour-row load of a batch of NB entries (3 x NB independent 16-byte loads per lane)
 //     before the first FMA; 8 warps walk 8 consecutive rows at a time, so the band structure of a locally ordered
-//     mesh hits L1;
-//   * fp32 FMAs on pairs of channels (fma2), bit-identical to fmaf per element.
-// Entry order = CSR order and the arithmetic per element is the same fmaf sequence as gather_row: bit-identical output.
+//     mesh hits L1.
 // ---------------------------------------------------------------------------------------------
 constexpr int GB_ROWS = 64;      // rows per CTA
 constexpr int GB_NNZ = 1024;     // staged entries per CTA (entries past it are read from global memory)
 
 struct __align__(16) GxyEnt { int col; int pad; float gx, gy; };   // (gx, gy) 8-byte aligned: one LDS.64
 
-// one CSR entry of the (x, P, Q) gather: three 16-byte slices of the neighbour's rows, then 12 paired FMAs (fma2)
-#define DN_FEAT_LOAD(J, ENT)                                                                         \
-  const char* pr##J;                                                                                 \
-  ulonglong2 x##J, P##J, Q##J = make_ulonglong2(0ull, 0ull);                                         \
-  {                                                                                                  \
-    const int64_t col = (ENT).col;                                                                   \
-    x##J = __ldg(reinterpret_cast<const ulonglong2*>(xb + col * x_row_bytes));                       \
-    pr##J = pb + col * pq_row_bytes;                                                                 \
-    P##J = __ldg(reinterpret_cast<const ulonglong2*>(pr##J));                                        \
-    if (ROT) Q##J = __ldg(reinterpret_cast<const ulonglong2*>(pr##J + x_row_bytes));                 \
+// NB entries: every 16-byte slice of the batch's neighbour rows is loaded before the first FMA.  The weights are read
+// again from the entry at FMA time: a broadcast LDS.64 is cheaper than 2 x NB live registers.  The row strides are
+// 32-bit: with 64-bit ones the C = 128 rotation instance spills at its 128-register cap.
+template <bool ROT, int NB>
+__device__ __forceinline__ void blk_entries(FeatAcc<float4>& a, const GxyEnt* en, const char* xb, const char* pb,
+                                            int x_row_bytes, int pq_row_bytes) {
+  float4 x[NB], P[NB], Q[NB];
+#pragma unroll
+  for (int j = 0; j < NB; ++j) {
+    const int64_t col = en[j].col;
+    const char* pr = pb + col * pq_row_bytes;
+    x[j] = __ldg(reinterpret_cast<const float4*>(xb + col * x_row_bytes));
+    P[j] = __ldg(reinterpret_cast<const float4*>(pr));
+    Q[j] = ROT ? __ldg(reinterpret_cast<const float4*>(pr + x_row_bytes)) : float4{};
   }
-// (the weights are re-read from the staged entry at FMA time: a broadcast LDS.64 is cheaper than 14 live registers)
-#define DN_FEAT_FMA(J, ENT)                                                                          \
-  {                                                                                                  \
-    const float2 w = *reinterpret_cast<const float2*>(&(ENT).gx);                                    \
-    const unsigned long long gx2 = pack2(w.x, w.x), gy2 = pack2(w.y, w.y);                           \
-    fma2(gX0, gx2, x##J.x); fma2(gX1, gx2, x##J.y);                                                  \
-    fma2(gY0, gy2, x##J.x); fma2(gY1, gy2, x##J.y);                                                  \
-    fma2(re0, gx2, P##J.x); fma2(re1, gx2, P##J.y);                                                  \
-    fma2(im0, gy2, P##J.x); fma2(im1, gy2, P##J.y);                                                  \
-    if (ROT) {                                                                                       \
-      const unsigned long long ngy2 = pack2(-w.y, -w.y);                                             \
-      fma2(re0, ngy2, Q##J.x); fma2(re1, ngy2, Q##J.y);                                              \
-      fma2(im0, gx2, Q##J.x); fma2(im1, gx2, Q##J.y);                                                \
-    }                                                                                                \
-  }
+#pragma unroll
+  for (int j = 0; j < NB; ++j) feat_entry<ROT>(a, *reinterpret_cast<const float2*>(&en[j].gx), x[j], P[j], Q[j]);
+}
 
 // (16-byte entry records, unpredicated full batches -- the first version,
 // with per-entry predicates and separate col / value arrays, spent half of its issue slots on bookkeeping.)
@@ -566,7 +540,7 @@ spmm_features_blk_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
                          const float2* __restrict__ vals, const float* __restrict__ xd,
                          const float* __restrict__ pq, int ld_pq, int64_t V, float* __restrict__ feat) {
   constexpr int C = 128 * NH;          // a warp covers 128 channels per pass (one float4 per lane), NH passes per row
-  constexpr int64_t x_row_bytes = (int64_t)C * 4;
+  constexpr int x_row_bytes = C * 4;
   __shared__ int s_rp[GB_ROWS + 1];
   __shared__ GxyEnt s_e[GB_NNZ];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -586,64 +560,42 @@ spmm_features_blk_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
     }
   }
   __syncthreads();
-  const int64_t pq_row_bytes = (int64_t)ld_pq * 4;
+  const int pq_row_bytes = ld_pq * 4;
 #pragma unroll 1
   for (int rh = warp; rh < nrows * NH; rh += 8) {
     const int r = rh / NH, h = rh % NH;
     const char* xb = reinterpret_cast<const char*>(xd) + h * 512 + lane * 16;
     const char* pb = reinterpret_cast<const char*>(pq) + h * 512 + lane * 16;
     const int s = s_rp[r] - e0, e = s_rp[r + 1] - e0;
-    unsigned long long gX0 = 0ull, gX1 = 0ull, gY0 = 0ull, gY1 = 0ull, re0 = 0ull, re1 = 0ull, im0 = 0ull, im1 = 0ull;
+    FeatAcc<float4> a = {};
     if (staged) {
       int p = s;
 #pragma unroll 1
-      for (; p + 7 <= e; p += 7) {                                // full batches: 21 independent loads, no predicates
-        DN_FEAT_LOAD(0, s_e[p]) DN_FEAT_LOAD(1, s_e[p + 1]) DN_FEAT_LOAD(2, s_e[p + 2]) DN_FEAT_LOAD(3, s_e[p + 3])
-        DN_FEAT_LOAD(4, s_e[p + 4]) DN_FEAT_LOAD(5, s_e[p + 5]) DN_FEAT_LOAD(6, s_e[p + 6])
-        DN_FEAT_FMA(0, s_e[p]) DN_FEAT_FMA(1, s_e[p + 1]) DN_FEAT_FMA(2, s_e[p + 2]) DN_FEAT_FMA(3, s_e[p + 3])
-        DN_FEAT_FMA(4, s_e[p + 4]) DN_FEAT_FMA(5, s_e[p + 5]) DN_FEAT_FMA(6, s_e[p + 6])
-      }
+      for (; p + 7 <= e; p += 7)                                  // full batches: 21 independent loads, no predicates
+        blk_entries<ROT, 7>(a, s_e + p, xb, pb, x_row_bytes, pq_row_bytes);
 #pragma unroll 1
-      for (; p + 2 <= e; p += 2) {                                // remainder: pairs, then a single entry
-        DN_FEAT_LOAD(0, s_e[p]) DN_FEAT_LOAD(1, s_e[p + 1])
-        DN_FEAT_FMA(0, s_e[p]) DN_FEAT_FMA(1, s_e[p + 1])
-      }
-      if (p < e) {
-        DN_FEAT_LOAD(0, s_e[p])
-        DN_FEAT_FMA(0, s_e[p])
-      }
+      for (; p + 2 <= e; p += 2)                                  // remainder: pairs, then a single entry
+        blk_entries<ROT, 2>(a, s_e + p, xb, pb, x_row_bytes, pq_row_bytes);
+      if (p < e) blk_entries<ROT, 1>(a, s_e + p, xb, pb, x_row_bytes, pq_row_bytes);
     } else {
 #pragma unroll 1
       for (int p = s; p < e; ++p) {                               // (a block with more than GB_NNZ entries)
         GxyEnt en;
         const float2 g = __ldg(vals + e0 + p);
         en.col = __ldg(colidx + e0 + p); en.gx = g.x; en.gy = g.y; en.pad = 0;
-        DN_FEAT_LOAD(0, en)
-        DN_FEAT_FMA(0, en)
+        blk_entries<ROT, 1>(a, &en, xb, pb, x_row_bytes, pq_row_bytes);
       }
     }
-    float gXv[4], gYv[4], rev[4], imv[4];
-    unpack2(gX0, gXv[0], gXv[1]); unpack2(gX1, gXv[2], gXv[3]);
-    unpack2(gY0, gYv[0], gYv[1]); unpack2(gY1, gYv[2], gYv[3]);
-    unpack2(re0, rev[0], rev[1]); unpack2(re1, rev[2], rev[3]);
-    unpack2(im0, imv[0], imv[1]); unpack2(im1, imv[2], imv[3]);
-    float4 o;
-    o.x = feat_tanh(fmaf(gXv[0], rev[0], gYv[0] * imv[0]));
-    o.y = feat_tanh(fmaf(gXv[1], rev[1], gYv[1] * imv[1]));
-    o.z = feat_tanh(fmaf(gXv[2], rev[2], gYv[2] * imv[2]));
-    o.w = feat_tanh(fmaf(gXv[3], rev[3], gYv[3] * imv[3]));
-    *reinterpret_cast<float4*>(feat + (base + r) * C + h * 128 + lane * 4) = o;
+    *reinterpret_cast<float4*>(feat + (base + r) * C + h * 128 + lane * 4) = feat_value(a);
   }
 }
-#undef DN_FEAT_LOAD
-#undef DN_FEAT_FMA
 
 // Patch variant (dn_patches, built once for resident operators): one CTA per patch of graph-adjacent rows.
 // Phase 1 copies the patch's distinct neighbour rows of x_diffuse and [P|Q] into shared memory, coalesced, each row
 // exactly once; phase 2 is the same gather as above but out of shared memory.  At V = 200k the plain kernel moves
 // ~1.1 GB from L2 into the SMs (every neighbour row is re-fetched by ~half of the vertices that touch it: 47 % L1
-// hits); here it is (distinct rows / rows) x 1.5 KB per vertex.  Entries keep their CSR order and the arithmetic is
-// gather_row's, so the result is bit-identical.
+// hits); here it is (distinct rows / rows) x 1.5 KB per vertex.  Entries keep their CSR order, so the result is
+// bit-identical.
 template <bool ROT>
 __global__ void __launch_bounds__(512) spmm_features_patch_kernel(const dn_patches P, const float* __restrict__ xd,
                                                                   const float* __restrict__ pq, int ld_pq, int C,
@@ -700,12 +652,11 @@ __global__ void __launch_bounds__(512) spmm_features_patch_kernel(const dn_patch
   }
   __syncthreads();
 
-  // phase 2: the gather, out of shared memory; entries in CSR order, gather_row's arithmetic
+  // phase 2: the gather, out of shared memory, entries in CSR order
   for (int i = warp; i < nt; i += nwarps) {
     const Meta nxt = load_meta(i + nwarps);
     for (int c4 = lane; c4 < xq; c4 += 32) {
-      Acc4 a;
-      a.gX = a.gY = a.bre = a.bim = make_float4(0.f, 0.f, 0.f, 0.f);
+      FeatAcc<float4> a = {};
       for (int base = 0; base < cur.n; base += 32) {
         int lc_l = cur.lc;
         float2 g_l = cur.g;
@@ -720,141 +671,56 @@ __global__ void __launch_bounds__(512) spmm_features_patch_kernel(const dn_patch
           g.x = __shfl_sync(0xffffffffu, g_l.x, e);
           g.y = __shfl_sync(0xffffffffu, g_l.y, e);
           const float4* src = sm4 + (size_t)lc * rowf4;
-          const float4 x = src[c4];
-          const float4 Pv = src[xq + c4];
-          a.gX.x = fmaf(g.x, x.x, a.gX.x); a.gX.y = fmaf(g.x, x.y, a.gX.y);
-          a.gX.z = fmaf(g.x, x.z, a.gX.z); a.gX.w = fmaf(g.x, x.w, a.gX.w);
-          a.gY.x = fmaf(g.y, x.x, a.gY.x); a.gY.y = fmaf(g.y, x.y, a.gY.y);
-          a.gY.z = fmaf(g.y, x.z, a.gY.z); a.gY.w = fmaf(g.y, x.w, a.gY.w);
-          a.bre.x = fmaf(g.x, Pv.x, a.bre.x); a.bre.y = fmaf(g.x, Pv.y, a.bre.y);
-          a.bre.z = fmaf(g.x, Pv.z, a.bre.z); a.bre.w = fmaf(g.x, Pv.w, a.bre.w);
-          a.bim.x = fmaf(g.y, Pv.x, a.bim.x); a.bim.y = fmaf(g.y, Pv.y, a.bim.y);
-          a.bim.z = fmaf(g.y, Pv.z, a.bim.z); a.bim.w = fmaf(g.y, Pv.w, a.bim.w);
-          if (ROT) {
-            const float4 Q = src[2 * xq + c4];
-            a.bre.x = fmaf(-g.y, Q.x, a.bre.x); a.bre.y = fmaf(-g.y, Q.y, a.bre.y);
-            a.bre.z = fmaf(-g.y, Q.z, a.bre.z); a.bre.w = fmaf(-g.y, Q.w, a.bre.w);
-            a.bim.x = fmaf(g.x, Q.x, a.bim.x); a.bim.y = fmaf(g.x, Q.y, a.bim.y);
-            a.bim.z = fmaf(g.x, Q.z, a.bim.z); a.bim.w = fmaf(g.x, Q.w, a.bim.w);
-          }
+          feat_entry<ROT>(a, g, src[c4], src[xq + c4], ROT ? src[2 * xq + c4] : float4{});
         }
       }
-      float4 o;
-      o.x = feat_tanh(fmaf(a.gX.x, a.bre.x, a.gY.x * a.bim.x));
-      o.y = feat_tanh(fmaf(a.gX.y, a.bre.y, a.gY.y * a.bim.y));
-      o.z = feat_tanh(fmaf(a.gX.z, a.bre.z, a.gY.z * a.bim.z));
-      o.w = feat_tanh(fmaf(a.gX.w, a.bre.w, a.gY.w * a.bim.w));
-      *reinterpret_cast<float4*>(feat + cur.row * C + c4 * 4) = o;
+      *reinterpret_cast<float4*>(feat + cur.row * C + c4 * 4) = feat_value(a);
     }
     cur = nxt;
   }
 }
 
 // U[v] = [dd*Bre | dd*Bim | dd*gX | dd*gY],  dd = dfeat * (1 - feat^2)
-template <bool ROT>
+template <bool ROT, class T>
 __global__ void __launch_bounds__(256) features_bwd_local_kernel(
     const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
     const float* __restrict__ xd, const float* __restrict__ pq, int ld_pq, const float* __restrict__ feat,
     const float* __restrict__ dfeat, int64_t V, int C, int G, float* __restrict__ U) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t row = warp * (32 / G) + lane / G;
-  const int gl = lane % G;
-  if (row >= V) return;
-  const int s = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
-  for (int c4 = gl; c4 < (C >> 2); c4 += G) {
-    const Acc4 a = gather_row<ROT>(colidx, vals, xd, pq, ld_pq, C, s, e, c4);
-    const float4 f = ldg4(feat + row * C + c4 * 4);
-    const float4 d = ldg4(dfeat + row * C + c4 * 4);
-    float4 dd;
-    dd.x = d.x * (1.f - f.x * f.x); dd.y = d.y * (1.f - f.y * f.y);
-    dd.z = d.z * (1.f - f.z * f.z); dd.w = d.w * (1.f - f.w * f.w);
-    float* u = U + row * 4 * C + c4 * 4;
-    *reinterpret_cast<float4*>(u) = make_float4(dd.x * a.bre.x, dd.y * a.bre.y, dd.z * a.bre.z, dd.w * a.bre.w);
-    *reinterpret_cast<float4*>(u + C) = make_float4(dd.x * a.bim.x, dd.y * a.bim.y, dd.z * a.bim.z, dd.w * a.bim.w);
-    *reinterpret_cast<float4*>(u + 2 * C) = make_float4(dd.x * a.gX.x, dd.y * a.gX.y, dd.z * a.gX.z, dd.w * a.gX.w);
-    *reinterpret_cast<float4*>(u + 3 * C) = make_float4(dd.x * a.gY.x, dd.y * a.gY.y, dd.z * a.gY.z, dd.w * a.gY.w);
-  }
+  const auto mul = [](float d, float v) { return d * v; };
+  feat_lanes<T>(rowptr, V, C, G, [&](int64_t row, int s, int e, int c) {
+    const FeatAcc<T> a = gather_row<ROT, T>(colidx, vals, xd, pq, ld_pq, C, s, e, c);
+    const T dd = per_ch([](float d, float f) { return d * (1.f - f * f); }, ldg_lane<T>(dfeat + row * C + c),
+                        ldg_lane<T>(feat + row * C + c));
+    float* u = U + row * 4 * C + c;
+    *reinterpret_cast<T*>(u) = per_ch(mul, dd, a.bre);
+    *reinterpret_cast<T*>(u + C) = per_ch(mul, dd, a.bim);
+    *reinterpret_cast<T*>(u + 2 * C) = per_ch(mul, dd, a.gX);
+    *reinterpret_cast<T*>(u + 3 * C) = per_ch(mul, dd, a.gY);
+  });
 }
 
 // transpose gather over the CSR of G^T:  dxd = GX^T U1 + GY^T U2;  dP = GX^T U3 + GY^T U4;
 // dQ = -GY^T U3 + GX^T U4
-template <bool ROT>
+template <bool ROT, class T>
 __global__ void __launch_bounds__(256) features_bwd_transpose_kernel(
     const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
     const float* __restrict__ U, int64_t V, int C, int G, float* __restrict__ dxd, float* __restrict__ dP,
     float* __restrict__ dQ, int64_t ld_pq) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t row = warp * (32 / G) + lane / G;
-  const int gl = lane % G;
-  if (row >= V) return;
-  const int s = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
-  for (int c4 = gl; c4 < (C >> 2); c4 += G) {
-    float4 ax = make_float4(0.f, 0.f, 0.f, 0.f), ap = ax, aq = ax;
+  feat_lanes<T>(rowptr, V, C, G, [&](int64_t row, int s, int e, int c) {
+    T ax = {}, ap = {}, aq = {};
     for (int p = s; p < e; ++p) {
       const int64_t i = __ldg(colidx + p);
       const float2 g = __ldg(vals + p);
-      const float* u = U + i * 4 * C + c4 * 4;
-      const float4 u1 = ldg4(u), u2 = ldg4(u + C), u3 = ldg4(u + 2 * C), u4 = ldg4(u + 3 * C);
-      ax.x += g.x * u1.x + g.y * u2.x; ax.y += g.x * u1.y + g.y * u2.y;
-      ax.z += g.x * u1.z + g.y * u2.z; ax.w += g.x * u1.w + g.y * u2.w;
-      ap.x += g.x * u3.x + g.y * u4.x; ap.y += g.x * u3.y + g.y * u4.y;
-      ap.z += g.x * u3.z + g.y * u4.z; ap.w += g.x * u3.w + g.y * u4.w;
-      if (ROT) {
-        aq.x += g.x * u4.x - g.y * u3.x; aq.y += g.x * u4.y - g.y * u3.y;
-        aq.z += g.x * u4.z - g.y * u3.z; aq.w += g.x * u4.w - g.y * u3.w;
-      }
+      const float* u = U + i * 4 * C + c;
+      const T u1 = ldg_lane<T>(u), u2 = ldg_lane<T>(u + C), u3 = ldg_lane<T>(u + 2 * C), u4 = ldg_lane<T>(u + 3 * C);
+      ax = per_ch([g](float ax, float u1, float u2) { return ax += g.x * u1 + g.y * u2; }, ax, u1, u2);
+      ap = per_ch([g](float ap, float u3, float u4) { return ap += g.x * u3 + g.y * u4; }, ap, u3, u4);
+      if (ROT) aq = per_ch([g](float aq, float u3, float u4) { return aq += g.x * u4 - g.y * u3; }, aq, u3, u4);
     }
-    *reinterpret_cast<float4*>(dxd + row * C + c4 * 4) = ax;
-    *reinterpret_cast<float4*>(dP + row * ld_pq + c4 * 4) = ap;
-    if (ROT) *reinterpret_cast<float4*>(dQ + row * ld_pq + c4 * 4) = aq;
-  }
-}
-
-// scalar-lane forms of the two kernels above (C % 4 != 0)
-template <bool ROT>
-__global__ void __launch_bounds__(256) features_bwd_local_scalar_kernel(
-    const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
-    const float* __restrict__ xd, const float* __restrict__ pq, int ld_pq, const float* __restrict__ feat,
-    const float* __restrict__ dfeat, int64_t V, int C, float* __restrict__ U) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= V * C) return;
-  const int64_t row = idx / C;
-  const int c = (int)(idx - row * C);
-  const Acc1 a = gather_row_scalar<ROT>(colidx, vals, xd, pq, ld_pq, C, __ldg(rowptr + row), __ldg(rowptr + row + 1), c);
-  const float f = __ldg(feat + row * C + c);
-  const float dd = __ldg(dfeat + row * C + c) * (1.f - f * f);
-  float* u = U + row * 4 * C + c;
-  u[0] = dd * a.bre;
-  u[C] = dd * a.bim;
-  u[2 * C] = dd * a.gX;
-  u[3 * C] = dd * a.gY;
-}
-
-template <bool ROT>
-__global__ void __launch_bounds__(256) features_bwd_transpose_scalar_kernel(
-    const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const float2* __restrict__ vals,
-    const float* __restrict__ U, int64_t V, int C, float* __restrict__ dxd, float* __restrict__ dP,
-    float* __restrict__ dQ, int64_t ld_pq) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= V * C) return;
-  const int64_t row = idx / C;
-  const int c = (int)(idx - row * C);
-  const int s = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
-  float ax = 0.f, ap = 0.f, aq = 0.f;
-  for (int p = s; p < e; ++p) {
-    const int64_t i = __ldg(colidx + p);
-    const float2 g = __ldg(vals + p);
-    const float* u = U + i * 4 * C + c;
-    const float u1 = __ldg(u), u2 = __ldg(u + C), u3 = __ldg(u + 2 * C), u4 = __ldg(u + 3 * C);
-    ax += g.x * u1 + g.y * u2;
-    ap += g.x * u3 + g.y * u4;
-    if (ROT) aq += g.x * u4 - g.y * u3;
-  }
-  dxd[row * C + c] = ax;
-  dP[row * ld_pq + c] = ap;
-  if (ROT) dQ[row * ld_pq + c] = aq;
+    *reinterpret_cast<T*>(dxd + row * C + c) = ax;
+    *reinterpret_cast<T*>(dP + row * ld_pq + c) = ap;
+    if (ROT) *reinterpret_cast<T*>(dQ + row * ld_pq + c) = aq;
+  });
 }
 
 __global__ void deinterleave_vc2_kernel(const float2* __restrict__ vc2, int64_t V, int C, float* __restrict__ g01) {
@@ -877,10 +743,25 @@ __global__ void complex_dots_tanh_kernel(const float* __restrict__ g01, const fl
   out[idx] = tanhf(d);
 }
 
-inline int pick_group(int C) {
-  int g = 1;
-  while (g * 2 <= 32 && g * 2 <= (C >> 2)) g *= 2;
-  return g;
+// Launches a row-gather features kernel (threads mapped by feat_lanes) for C's lane width and for `rotations`:
+// launch(rot, lane, blocks, G), rot a std::bool_constant, lane a float or float4 value.
+template <class F>
+int launch_feat_rows(int64_t V, int C, int rotations, F launch) {
+  if (V <= 0) return DN_OK;
+  if (C % 4) {                                   // float lanes: one thread per (row, channel)
+    const unsigned blocks = (unsigned)((V * C + 255) / 256);
+    if (rotations) launch(std::true_type{}, float{}, blocks, C);
+    else launch(std::false_type{}, float{}, blocks, C);
+  } else {                                       // float4 lanes: G = min(32, C / 4) rounded down to a power of two
+    int G = 1;
+    while (G * 2 <= 32 && G * 2 <= (C >> 2)) G *= 2;
+    const int64_t warps = (V + (32 / G) - 1) / (32 / G);
+    const unsigned blocks = (unsigned)((warps * 32 + 255) / 256);
+    if (rotations) launch(std::true_type{}, float4{}, blocks, G);
+    else launch(std::false_type{}, float4{}, blocks, G);
+  }
+  DN_LAUNCH_CHECK();
+  return DN_OK;
 }
 
 }  // namespace
@@ -1031,13 +912,6 @@ int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int 
                          float* feat, cudaStream_t st) {
   if (V <= 0) return DN_OK;
   const float2* vals = reinterpret_cast<const float2*>(g->vals);
-  if (C % 4) {   // no float4 row access: one thread per (row, channel)
-    const unsigned blocks = (unsigned)((V * C + 255) / 256);
-    if (rotations) spmm_features_scalar_kernel<true><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, 2 * C, V, C, feat);
-    else spmm_features_scalar_kernel<false><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, C, V, C, feat);
-    DN_LAUNCH_CHECK();
-    return DN_OK;
-  }
   // the patched kernel when the host built patches for this operator (bit-identical to the plain kernel, both ROT
   // variants).  C == 128 only: that is the shape validated on the GPU; the phase-2 shuffles also assume every lane owns
   // a float4 of the row (C/4 a multiple of 32)
@@ -1071,65 +945,28 @@ int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int 
     DN_LAUNCH_CHECK();
     return DN_OK;
   }
-  const int G = pick_group(C);
-  const int64_t warps = (V + (32 / G) - 1) / (32 / G);
-  const unsigned blocks = (unsigned)((warps * 32 + 255) / 256);
-  if (rotations)
-    spmm_features_kernel<true><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, 2 * C, V, C, G, feat);
-  else
-    spmm_features_kernel<false><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, C, V, C, G, feat);
-  DN_LAUNCH_CHECK();
-  return DN_OK;
+  return launch_feat_rows(V, C, rotations, [&](auto rot, auto lane, unsigned blocks, int G) {
+    spmm_features_kernel<decltype(rot)::value, decltype(lane)><<<blocks, 256, 0, st>>>(
+        g->rowptr, g->colidx, vals, xd, pq, rot ? 2 * C : C, V, C, G, feat);
+  });
 }
 
 int launch_features_bwd_local(const dn_csr* g, const float* xd, const float* pq, const float* feat,
                               const float* dfeat, int rotations, int64_t V, int C, float* U, cudaStream_t st) {
-  if (V <= 0) return DN_OK;
   const float2* vals = reinterpret_cast<const float2*>(g->vals);
-  if (C % 4) {
-    const unsigned sb = (unsigned)((V * C + 255) / 256);
-    if (rotations)
-      features_bwd_local_scalar_kernel<true><<<sb, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, 2 * C, feat, dfeat, V, C, U);
-    else
-      features_bwd_local_scalar_kernel<false><<<sb, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, C, feat, dfeat, V, C, U);
-    DN_LAUNCH_CHECK();
-    return DN_OK;
-  }
-  const int G = pick_group(C);
-  const int64_t warps = (V + (32 / G) - 1) / (32 / G);
-  const unsigned blocks = (unsigned)((warps * 32 + 255) / 256);
-  if (rotations)
-    features_bwd_local_kernel<true><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, 2 * C, feat, dfeat,
-                                                             V, C, G, U);
-  else
-    features_bwd_local_kernel<false><<<blocks, 256, 0, st>>>(g->rowptr, g->colidx, vals, xd, pq, C, feat, dfeat, V,
-                                                              C, G, U);
-  DN_LAUNCH_CHECK();
-  return DN_OK;
+  return launch_feat_rows(V, C, rotations, [&](auto rot, auto lane, unsigned blocks, int G) {
+    features_bwd_local_kernel<decltype(rot)::value, decltype(lane)><<<blocks, 256, 0, st>>>(
+        g->rowptr, g->colidx, vals, xd, pq, rot ? 2 * C : C, feat, dfeat, V, C, G, U);
+  });
 }
 
 int launch_features_bwd_transpose(const dn_csr* gt, const float* U, int rotations, int64_t V, int C, float* dxd,
                                   float* dP, float* dQ, int64_t ld_pq, cudaStream_t st) {
-  if (V <= 0) return DN_OK;
   const float2* vals = reinterpret_cast<const float2*>(gt->vals);
-  if (C % 4) {
-    const unsigned sb = (unsigned)((V * C + 255) / 256);
-    if (rotations)
-      features_bwd_transpose_scalar_kernel<true><<<sb, 256, 0, st>>>(gt->rowptr, gt->colidx, vals, U, V, C, dxd, dP, dQ, ld_pq);
-    else
-      features_bwd_transpose_scalar_kernel<false><<<sb, 256, 0, st>>>(gt->rowptr, gt->colidx, vals, U, V, C, dxd, dP, dQ, ld_pq);
-    DN_LAUNCH_CHECK();
-    return DN_OK;
-  }
-  const int G = pick_group(C);
-  const int64_t warps = (V + (32 / G) - 1) / (32 / G);
-  const unsigned blocks = (unsigned)((warps * 32 + 255) / 256);
-  if (rotations)
-    features_bwd_transpose_kernel<true><<<blocks, 256, 0, st>>>(gt->rowptr, gt->colidx, vals, U, V, C, G, dxd, dP, dQ, ld_pq);
-  else
-    features_bwd_transpose_kernel<false><<<blocks, 256, 0, st>>>(gt->rowptr, gt->colidx, vals, U, V, C, G, dxd, dP, dQ, ld_pq);
-  DN_LAUNCH_CHECK();
-  return DN_OK;
+  return launch_feat_rows(V, C, rotations, [&](auto rot, auto lane, unsigned blocks, int G) {
+    features_bwd_transpose_kernel<decltype(rot)::value, decltype(lane)><<<blocks, 256, 0, st>>>(
+        gt->rowptr, gt->colidx, vals, U, V, C, G, dxd, dP, dQ, ld_pq);
+  });
 }
 
 int launch_deinterleave_vc2(const float* vc2, int64_t V, int C, float* g01, cudaStream_t st) {

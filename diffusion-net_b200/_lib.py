@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libdiffusion_net_b200.so")
 SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_eig.cu", "dn_implicit.cu", "dn_fmap.cu", "dn_fmap_batch.cu", "dn_tc.cu",
-           "dn_capi.cu"]
+           "dn_head.cu", "dn_capi.cu"]
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "diffusion_net_b200.h")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -146,6 +146,11 @@ SIGNATURES = {
     "dn_fmap_solve_bwd_batched": (_I, [_P, _L, _P, _L, _I, _P, _P, _I, _P, _P, _I, _I, _D, _P, _P, _P, _L, _P]),
     "dn_fmap_pointwise_map_batched_workspace_bytes": (_L, [_I, _I, _P, _P, _P, _P, _I]),
     "dn_fmap_pointwise_map_batched": (_I, [_P, _I, _P, _L, _P, _P, _I, _P, _P, _I, _P, _P, _L, _P]),
+    "dn_linear_nll_workspace_bytes": (_L, [_L, _I, _I]),
+    "dn_linear_nll_fwd": (_I, [_P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _I, _P]),
+    "dn_linear_nll_bwd": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _P, _L, _I, _P]),
+    "dn_element_mean_fwd": (_I, [_P, _L, _I, _P, _L, _I, _P, _P]),
+    "dn_element_mean_bwd": (_I, [_P, _L, _I, _P, _P, _L, _I, _P, _P]),
 }
 
 _lib = None

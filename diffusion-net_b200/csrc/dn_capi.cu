@@ -1099,3 +1099,64 @@ int dn_block_fwd_profile(const float* x_in, const float* mass, const float* eval
 }
 
 }  // extern "C"
+
+// ---- fused classification head ----
+namespace {
+int linear_nll_check(const float* x, const float* weight, const int64_t* labels, int64_t R, int C, int n_class,
+                     int engine, Engine* e) {
+  if (!x || !weight || !labels || R < 1 || n_class < 1 || C < 1) return DN_ERR_INVALID_ARGUMENT;
+  if (C % 16 != 0 || C > 256 || R >= (1ll << 31) || (int64_t)n_class * C >= (1ll << 31)) return DN_ERR_UNSUPPORTED;
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(weight)) & 15) return DN_ERR_UNSUPPORTED;
+  const int rc = resolve(engine, e);
+  if (rc != DN_OK) return rc;
+  return e->tc ? DN_OK : DN_ERR_UNSUPPORTED;   // tensor cores only: the SIMT engine composes mlp + log_softmax instead
+}
+}  // namespace
+
+extern "C" {
+
+int64_t dn_linear_nll_workspace_bytes(int64_t R, int C, int n_class) {
+  if (R < 1 || C < 1 || n_class < 1) return 0;
+  return head_ws_bytes(R, C, n_class);
+}
+
+int dn_linear_nll_fwd(const float* x, const float* weight, const float* bias, const int64_t* labels, int64_t R, int C,
+                      int n_class, int64_t ignore_index, float* nll, int64_t* argmax, float* lse, int engine,
+                      dn_stream_t stream) {
+  Engine e;
+  int rc = linear_nll_check(x, weight, labels, R, C, n_class, engine, &e);
+  if (rc != DN_OK) return rc;
+  if (!nll || !argmax || !lse) return DN_ERR_INVALID_ARGUMENT;
+  return launch_linear_nll_fwd(x, weight, bias, labels, R, C, n_class, ignore_index, nll, argmax, lse, e.passes,
+                               (cudaStream_t)stream);
+}
+
+int dn_linear_nll_bwd(const float* x, const float* weight, const float* bias, const int64_t* labels, const float* lse,
+                      const float* grad_nll, int64_t R, int C, int n_class, int64_t ignore_index, float* grad_x,
+                      float* grad_weight, float* grad_bias, void* workspace, int64_t ws_bytes, int engine,
+                      dn_stream_t stream) {
+  Engine e;
+  int rc = linear_nll_check(x, weight, labels, R, C, n_class, engine, &e);
+  if (rc != DN_OK) return rc;
+  if (!lse || !grad_nll || !grad_x || !grad_weight || (bias && !grad_bias)) return DN_ERR_INVALID_ARGUMENT;
+  if (!workspace || ws_bytes < head_ws_bytes(R, C, n_class)) return DN_ERR_WORKSPACE;
+  return launch_linear_nll_bwd(x, weight, bias, labels, lse, grad_nll, R, C, n_class, ignore_index, grad_x, grad_weight,
+                               bias ? grad_bias : nullptr, workspace, e.passes, (cudaStream_t)stream);
+}
+
+int dn_element_mean_fwd(const float* x, int64_t V, int C, const int64_t* elems, int64_t E, int k, float* out,
+                        dn_stream_t stream) {
+  if (V < 1 || C < 1 || E < 0 || k < 1 || (E > 0 && (!x || !elems || !out))) return DN_ERR_INVALID_ARGUMENT;
+  if (E == 0) return DN_OK;
+  return launch_element_mean_fwd(x, C, elems, E, k, out, (cudaStream_t)stream);
+}
+
+int dn_element_mean_bwd(const float* grad_out, int64_t E, int C, const int32_t* rowptr, const int32_t* entries,
+                        int64_t V, int k, float* grad_x, dn_stream_t stream) {
+  if (V < 1 || C < 1 || E < 0 || k < 1 || !rowptr || !grad_x || (E > 0 && (!grad_out || !entries)))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (E * k >= (1ll << 31)) return DN_ERR_UNSUPPORTED;
+  return launch_element_mean_bwd(grad_out, C, rowptr, entries, V, k, grad_x, (cudaStream_t)stream);
+}
+
+}  // extern "C"

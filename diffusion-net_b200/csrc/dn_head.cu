@@ -1,0 +1,710 @@
+// Fused classification head: z = X W^T + b, log_softmax and the NLL loss per row, forward and backward, on wgmma.
+// The (R x n_class) logits, probabilities and logit gradients live only in registers and shared memory.
+//
+// Every kernel runs 256 threads: two warpgroups of 64 rows each own the 128 rows of a CTA tile (rows of X, or classes
+// of W in the weight-gradient kernel).  A 128-wide tile of the other operand streams through a B image in shared memory
+// in 32-deep K stages, in the canonical K-major layout of the chain kernels (dn_tc.cu): 8-row core matrices of 16 bytes,
+// 8-column groups 128 B apart, K groups lbo = 128 * 16 B apart; 3xTF32 keeps a hi image and a lo image.
+#include <math.h>
+#include <cuda.h>
+#include <cudaTypedefs.h>
+#include "dn_internal.h"
+#include "dn_tc_ptx.cuh"
+
+using namespace tc;
+
+namespace {
+
+constexpr int HT = 128;                   // CTA rows, class-tile width and MMA N
+constexpr int KS = 32;                    // K per B stage
+constexpr int NTHR = 256;
+constexpr uint32_t LBO = HT * 16;
+constexpr int B_IMG = KS * HT * 4;        // one tf32 image of a stage
+enum { M_TF32X3 = 0, M_TF32 = 1, M_BF16 = 2 };
+
+__host__ __device__ constexpr int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// byte offset of element (k, n) of a stage's B image
+template <int MODE>
+__device__ __forceinline__ uint32_t b_off(int k, int n) {
+  if constexpr (MODE == M_BF16) return (k >> 3) * LBO + (n >> 3) * 128 + (n & 7) * 16 + (k & 7) * 2;
+  else return (k >> 2) * LBO + (n >> 3) * 128 + (n & 7) * 16 + (k & 3) * 4;
+}
+
+template <int MODE>
+__device__ __forceinline__ void b_put(uint8_t* img, int k, int n, float v) {
+  if constexpr (MODE == M_BF16) {
+    *reinterpret_cast<uint16_t*>(img + b_off<MODE>(k, n)) = (uint16_t)(pack_bf16x2(v, 0.f) & 0xFFFFu);
+  } else {
+    float hi, lo;
+    split_tf32(v, hi, lo);
+    *reinterpret_cast<float*>(img + b_off<MODE>(k, n)) = hi;
+    if (MODE == M_TF32X3) *reinterpret_cast<float*>(img + B_IMG + b_off<MODE>(k, n)) = lo;
+  }
+}
+
+// Every B stage reaches shared memory by TMA as a raw fp32 box with the 128-byte swizzle, through a two-slot ring
+// (one mbarrier per slot, stage q + 2 in flight while stage q is consumed); all threads then convert it into the MMA
+// image.  The swizzle makes both sides of the conversion free of bank conflicts: a warp writes 128 consecutive bytes of
+// the image and reads 8 rows x 4 floats of the raw box whose 16-byte chunks the swizzle spreads over all banks.
+constexpr int RAW_BYTES = KS * HT * 4;    // one raw stage (16 KB)
+
+// raw (row, col) of a box with 128-byte rows (32 floats) and the 128-byte swizzle
+__device__ __forceinline__ float raw_at(const uint8_t* raw, int row, int col) {
+  return *reinterpret_cast<const float*>(raw + row * 128 + ((((col >> 2) ^ row) & 7) << 4) + (col & 3) * 4);
+}
+
+// image coordinates of the w-th word a thread converts: consecutive w are consecutive image words (TF32 layout)
+__device__ __forceinline__ void img_coords(int w, int& kl, int& n) {
+  kl = (w >> 9) * 4 + (w & 3);
+  n = ((w >> 5) & 15) * 8 + ((w >> 2) & 7);
+}
+
+// rows stage: B(k, n) = src row n, column k: one {32, 128} box (TMA zero-fills rows and columns outside the source)
+template <int MODE>
+__device__ void convert_rows(uint8_t* img, const uint8_t* raw) {
+  for (int w = threadIdx.x; w < KS * HT; w += NTHR) {
+    int k, n;
+    img_coords(w, k, n);
+    b_put<MODE>(img, k, n, raw_at(raw, n, k));
+  }
+}
+
+// columns stage: B(k, n) = src row k, column n, from four {32, 32} boxes (box j holds n in [32 j, 32 j + 32)); zero
+// outside k < nk, n < nn (boxes wholly outside the source are not loaded).  For the TF32 engines the K order inside every
+// 8-group is permuted to match A fragments taken from an accumulator (mma_reg_a).
+template <int MODE>
+__device__ void convert_cols(uint8_t* img, const uint8_t* raw, int nk, int nn) {
+  for (int w = threadIdx.x; w < KS * HT; w += NTHR) {
+    int kl, n;
+    img_coords(w, kl, n);
+    const int j = kl & 7;
+    const int k = MODE == M_BF16 ? kl : ((kl & ~7) | (j < 4 ? 2 * j : 2 * (j - 4) + 1));
+    const float v = (k < nk && n < nn) ? raw_at(raw + (n >> 5) * (RAW_BYTES / 4), k, n & 31) : 0.f;
+    b_put<MODE>(img, kl, n, v);
+  }
+}
+
+// The stage sequence of a CTA: `ntiles` tiles, tile t = nst rows stages of map a (rows a0 + 128 t, columns KS i) then
+// ncol columns stages of map b (rows b0 + 128 t + KS j, columns c0 .. c0 + 127).
+struct Seq {
+  int64_t a0, b0, ntiles;
+  int nst, ncol, c0;
+  int64_t b_rows;    // rows of map b's source
+  int b_cols;        // columns of map b's source
+};
+
+struct Ring {
+  uint8_t* raw;      // 2 slots of RAW_BYTES, 1024-byte aligned
+  uint32_t bar;      // 2 mbarriers
+  int64_t q;         // next stage to consume
+};
+
+__device__ __forceinline__ void ring_issue(const Ring& rg, const Seq& sq, const CUtensorMap* amap, const CUtensorMap* bmap,
+                                           int64_t q) {
+  const int per = sq.nst + sq.ncol;
+  const int64_t t = q / per;
+  if (t >= sq.ntiles) return;
+  const int i = (int)(q % per);
+  const uint32_t bar = rg.bar + 8 * (uint32_t)(q & 1), dst = smem_u32(rg.raw + (q & 1) * RAW_BYTES);
+  if (i < sq.nst) {
+    mbar_arrive_expect_tx(bar, RAW_BYTES);
+    tma_tile_2d_g2s(dst, amap, KS * i, (int)(sq.a0 + HT * t), bar);
+    return;
+  }
+  const int64_t row = sq.b0 + HT * t + KS * (i - sq.nst);
+  int nbox = 0;
+  for (int j = 0; j < 4; ++j) nbox += (row < sq.b_rows && sq.c0 + 32 * j < sq.b_cols) ? 1 : 0;
+  if (nbox == 0) { mbar_arrive(bar); return; }
+  mbar_arrive_expect_tx(bar, nbox * (RAW_BYTES / 4));
+  for (int j = 0; j < 4; ++j)
+    if (row < sq.b_rows && sq.c0 + 32 * j < sq.b_cols)
+      tma_tile_2d_g2s(dst + j * (RAW_BYTES / 4), bmap, sq.c0 + 32 * j, (int)row, bar);
+}
+
+// one stage: wait for its box, convert it into the image once every warpgroup's MMAs on the image are done, then hand
+// the raw slot to stage q + 2
+template <typename Convert>
+__device__ __forceinline__ void ring_next(Ring& rg, const Seq& sq, const CUtensorMap* amap, const CUtensorMap* bmap,
+                                          uint8_t* img, Convert convert) {
+  mbar_wait(rg.bar + 8 * (uint32_t)(rg.q & 1), (uint32_t)((rg.q >> 1) & 1));
+  __syncthreads();
+  convert(img, rg.raw + (rg.q & 1) * RAW_BYTES);
+  fence_proxy_async();
+  __syncthreads();
+  if (threadIdx.x == 0) ring_issue(rg, sq, amap, bmap, rg.q + 2);
+  ++rg.q;
+}
+
+// acc (+)= A[rows of this warp][k0, k0 + nk) * B image; A is a fp32 row-major tile in shared memory (row stride lda)
+template <int MODE>
+__device__ __forceinline__ void mma_smem_a(float* acc, const float* As, int lda, int r, int k0, int nk, uint32_t sb,
+                                           bool first) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const float* a0 = As + (r + g) * lda + k0;
+  const float* a1 = a0 + 8 * lda;
+  constexpr int STEPS = MODE == M_BF16 ? KS / 16 : KS / 8;
+  uint32_t ah[STEPS][4], al[STEPS][4];
+#pragma unroll
+  for (int s = 0; s < STEPS; ++s) {
+    if constexpr (MODE == M_BF16) {
+      const int c = 16 * s + 2 * t;
+      ah[s][0] = pack_bf16x2(a0[c], a0[c + 1]);
+      ah[s][1] = pack_bf16x2(a1[c], a1[c + 1]);
+      ah[s][2] = pack_bf16x2(a0[c + 8], a0[c + 9]);
+      ah[s][3] = pack_bf16x2(a1[c + 8], a1[c + 9]);
+    } else {
+      const int c = 8 * s + t;
+      const float x[4] = {a0[c], a1[c], a0[c + 4], a1[c + 4]};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        float h, l;
+        split_tf32_fast(x[i], h, l);
+        ah[s][i] = __float_as_uint(h);
+        al[s][i] = __float_as_uint(l);
+      }
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < STEPS; ++s) {
+    fence_frag4(ah[s]);
+    if (MODE == M_TF32X3) fence_frag4(al[s]);
+  }
+  wgmma_fence();
+  const int steps = MODE == M_BF16 ? nk / 16 : nk / 8;
+#pragma unroll
+  for (int s = 0; s < STEPS; ++s) {
+    if (s >= steps) break;
+    const uint32_t accumulate = (!first || s > 0) ? 1u : 0u;
+    const uint32_t base = sb + s * 2 * LBO;
+    const uint64_t dh = make_desc(base, LBO, 128);
+    if constexpr (MODE == M_BF16) {
+      wgmma_bf16_n128(acc, ah[s], dh, accumulate);
+    } else if constexpr (MODE == M_TF32X3) {
+      wgmma_tf32_n128(acc, al[s], dh, accumulate);
+      wgmma_tf32_n128(acc, ah[s], make_desc(base + B_IMG, LBO, 128), 1u);
+      wgmma_tf32_n128(acc, ah[s], dh, 1u);
+    } else {
+      wgmma_tf32_n128(acc, ah[s], dh, accumulate);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int j = 0; j < 8; ++j) fence_acc8(acc + 8 * j);
+}
+
+// acc (+)= Z[:, 32 c, 32 c + 32) * B image, where Z is the 64 x 128 accumulator z of this warpgroup taken as the A
+// operand (columns of z = K).  TF32: the fragment of k8 slice b is z[4b], z[4b+2], z[4b+1], z[4b+3], i.e. logical
+// columns t, t + 4 hold actual columns 2t, 2t + 1 (stage_cols permutes B alike); bf16: the accumulator layout is the
+// fragment layout.
+template <int MODE, int CH>
+__device__ __forceinline__ void mma_reg_a(float* acc, const float* z, uint32_t sb, bool first) {
+  constexpr int STEPS = MODE == M_BF16 ? KS / 16 : KS / 8;
+  uint32_t ah[STEPS][4], al[STEPS][4];
+#pragma unroll
+  for (int s = 0; s < STEPS; ++s) {
+    if constexpr (MODE == M_BF16) {
+      const int b = 4 * CH + 2 * s;
+      ah[s][0] = pack_bf16x2(z[4 * b], z[4 * b + 1]);
+      ah[s][1] = pack_bf16x2(z[4 * b + 2], z[4 * b + 3]);
+      ah[s][2] = pack_bf16x2(z[4 * b + 4], z[4 * b + 5]);
+      ah[s][3] = pack_bf16x2(z[4 * b + 6], z[4 * b + 7]);
+    } else {
+      const int b = 4 * CH + s;
+      const float x[4] = {z[4 * b], z[4 * b + 2], z[4 * b + 1], z[4 * b + 3]};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        float h, l;
+        split_tf32_fast(x[i], h, l);
+        ah[s][i] = __float_as_uint(h);
+        al[s][i] = __float_as_uint(l);
+      }
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < STEPS; ++s) {
+    fence_frag4(ah[s]);
+    if (MODE == M_TF32X3) fence_frag4(al[s]);
+  }
+  wgmma_fence();
+#pragma unroll
+  for (int s = 0; s < STEPS; ++s) {
+    const uint32_t accumulate = (!first || s > 0) ? 1u : 0u;
+    const uint32_t base = sb + s * 2 * LBO;
+    const uint64_t dh = make_desc(base, LBO, 128);
+    if constexpr (MODE == M_BF16) {
+      wgmma_bf16_n128(acc, ah[s], dh, accumulate);
+    } else if constexpr (MODE == M_TF32X3) {
+      wgmma_tf32_n128(acc, al[s], dh, accumulate);
+      wgmma_tf32_n128(acc, ah[s], make_desc(base + B_IMG, LBO, 128), 1u);
+      wgmma_tf32_n128(acc, ah[s], dh, 1u);
+    } else {
+      wgmma_tf32_n128(acc, ah[s], dh, accumulate);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int j = 0; j < 8; ++j) fence_acc8(acc + 8 * j);
+}
+
+// rows [r0, r0 + nr) of src (R x C, row stride C) into the shared tile As (128 x (C + 4)), zero rows past nr
+__device__ void load_tile(float* As, const float* __restrict__ src, int64_t r0, int nr, int C) {
+  const int lda = C + 4, q = C / 4;
+  for (int i = threadIdx.x; i < HT * q; i += NTHR) {
+    const int r = i / q, c = 4 * (i % q);
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (r < nr) v = __ldg(reinterpret_cast<const float4*>(src + (r0 + r) * C + c));
+    *reinterpret_cast<float4*>(As + r * lda + c) = v;
+  }
+}
+
+// acc = As (this warp's rows) x src[n0 .. n0 + nn)^T over the full C: the 128-wide logit tile, bias not added
+template <int MODE>
+__device__ __forceinline__ void logit_tile(float* acc, const float* As, int C, int r, Ring& rg, const Seq& sq,
+                                           const CUtensorMap* amap, const CUtensorMap* bmap, uint8_t* img) {
+  const uint32_t sb = smem_u32(img);
+  for (int k0 = 0; k0 < C; k0 += KS) {
+    const int nk = C - k0 < KS ? C - k0 : KS;
+    ring_next(rg, sq, amap, bmap, img, [](uint8_t* im, const uint8_t* raw) { convert_rows<MODE>(im, raw); });
+    mma_smem_a<MODE>(acc, As, C + 4, r, k0, nk, sb, k0 == 0);
+  }
+}
+
+// shared memory: the raw ring (1024-byte aligned for the swizzle), the A tile, the B image, per-row factors, mbarriers
+struct HeadSmem {
+  Ring rg;
+  float* As;
+  uint8_t* img;
+  float* rows;
+};
+
+__device__ __forceinline__ HeadSmem head_smem_carve(uint8_t* smem, int C, const Seq& sq, const CUtensorMap* amap,
+                                                    const CUtensorMap* bmap) {
+  HeadSmem h;
+  uint8_t* base = smem + ((1024 - (smem_u32(smem) & 1023)) & 1023);
+  h.rg.raw = base;
+  h.As = reinterpret_cast<float*>(base + 2 * RAW_BYTES);
+  h.img = base + 2 * RAW_BYTES + (size_t)HT * (C + 4) * 4;
+  h.rows = reinterpret_cast<float*>(h.img + 2 * B_IMG);
+  h.rg.bar = smem_u32(h.rows + 3 * HT);
+  h.rg.q = 0;
+  if (threadIdx.x == 0) {
+    mbar_init(h.rg.bar, 1);
+    mbar_init(h.rg.bar + 8, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    ring_issue(h.rg, sq, amap, bmap, 0);
+    ring_issue(h.rg, sq, amap, bmap, 1);
+  }
+  return h;
+}
+
+// per-row factor of the logit gradient: dZ = coef * (softmax - onehot); 0 for padding and ignored rows, NaN for a label
+// outside [0, n_class)
+__device__ __forceinline__ float row_coef(int64_t lab, float g, int n_class, int64_t ignore_index, bool valid) {
+  if (!valid || lab == ignore_index) return 0.f;
+  if (lab < 0 || lab >= n_class) return __int_as_float(0x7fc00000);
+  return g;
+}
+
+struct HeadArgs {
+  const float* X;
+  const float* W;
+  const float* b;
+  const int64_t* labels;
+  const float* lse;       // bwd: saved by the forward
+  const float* g;         // bwd: upstream per-row weight
+  int64_t R;
+  int C, n_class;
+  int64_t ignore_index;
+  float* nll;             // fwd
+  int64_t* argmax;        // fwd
+  float* lse_out;         // fwd
+  float* dX;              // bwd
+  float* dWp;             // bwd: [S][n_class][C] partials
+  float* dbp;             // bwd: [S][n_class]
+  int S;                  // row splits of the weight-gradient kernel
+  CUtensorMap amap;       // logits' B source (W: forward and dX; X: dW), {32, 128} boxes
+  CUtensorMap bmap;       // dX / dW's B source (W / X), {32, 32} boxes
+};
+
+template <int MODE>
+__global__ void __launch_bounds__(NTHR, 1) linear_nll_fwd_kernel(const __grid_constant__ HeadArgs p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const Seq sq{0, 0, cdiv(p.n_class, HT), (int)cdiv(p.C, KS), 0, 0, 0, 0};
+  HeadSmem hs = head_smem_carve(smem, p.C, sq, &p.amap, &p.bmap);
+  float* As = hs.As;
+  uint8_t* img = hs.img;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = lane & 3;
+  const int r = (warp >> 2) * 64 + (warp & 3) * 16;        // rows r + g, r + g + 8 of the tile
+  const int64_t row0 = (int64_t)blockIdx.x * HT;
+  const int nr = p.R - row0 < HT ? (int)(p.R - row0) : HT;
+  load_tile(As, p.X, row0, nr, p.C);
+  const int64_t rows[2] = {row0 + r + (lane >> 2), row0 + r + (lane >> 2) + 8};
+  int64_t lab[2];
+  float m[2], s[2], zl[2], best[2];
+  int bi[2];
+  bool bad[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    lab[h] = rows[h] < p.R ? p.labels[rows[h]] : p.ignore_index;
+    m[h] = -INFINITY; s[h] = 0.f; zl[h] = 0.f; best[h] = -INFINITY; bi[h] = 0; bad[h] = false;
+  }
+  float acc[64];
+  for (int64_t n0 = 0; n0 < p.n_class; n0 += HT) {
+    const int nn = p.n_class - n0 < HT ? (int)(p.n_class - n0) : HT;
+    logit_tile<MODE>(acc, As, p.C, r, hs.rg, sq, &p.amap, &p.bmap, img);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      // online log-sum-exp over the valid columns (padding columns are skipped, not set to -inf)
+      float tmax = -INFINITY;
+#pragma unroll
+      for (int b = 0; b < 16; ++b)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * b + 2 * t + e;
+          if (c < nn) {
+            const float z = acc[4 * b + 2 * h + e] + (p.b ? __ldg(p.b + n0 + c) : 0.f);
+            acc[4 * b + 2 * h + e] = z;
+            if (!isfinite(z)) bad[h] = true;
+            tmax = fmaxf(tmax, z);
+            if (z > best[h]) { best[h] = z; bi[h] = (int)(n0 + c); }
+            if (n0 + c == lab[h]) zl[h] = z;
+          }
+        }
+      tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 1));
+      tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
+      const float mn = fmaxf(m[h], tmax);
+      float sum = s[h] * expf(m[h] - mn);
+#pragma unroll
+      for (int b = 0; b < 16; ++b)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * b + 2 * t + e < nn) sum += expf(acc[4 * b + 2 * h + e] - mn);
+      m[h] = mn;
+      s[h] = sum;
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      s[h] += __shfl_xor_sync(0xffffffffu, s[h], o);
+      zl[h] += __shfl_xor_sync(0xffffffffu, zl[h], o);
+      bad[h] = __shfl_xor_sync(0xffffffffu, (int)bad[h], o) != 0;
+      const float ob = __shfl_xor_sync(0xffffffffu, best[h], o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi[h], o);
+      if (ob > best[h] || (ob == best[h] && oi < bi[h])) { best[h] = ob; bi[h] = oi; }
+    }
+    if (t == 0 && rows[h] < p.R) {
+      const float nan = __int_as_float(0x7fc00000);
+      const float lse = bad[h] ? nan : m[h] + logf(s[h]);
+      float nll = lse - zl[h];
+      if (lab[h] == p.ignore_index) nll = 0.f;
+      else if (lab[h] < 0 || lab[h] >= p.n_class) nll = nan;
+      p.nll[rows[h]] = nll;
+      p.lse_out[rows[h]] = lse;
+      p.argmax[rows[h]] = bi[h];
+    }
+  }
+}
+
+// dX[:, c0 .. c0 + 128) = sum over class tiles of dZ_tile W_tile[:, c0 ..]; grid (row tiles, column halves)
+template <int MODE>
+__global__ void __launch_bounds__(NTHR, 1) linear_nll_dx_kernel(const __grid_constant__ HeadArgs p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int c0 = blockIdx.y * HT, nc = p.C - c0 < HT ? p.C - c0 : HT;
+  const Seq sq{0, 0, cdiv(p.n_class, HT), (int)cdiv(p.C, KS), HT / KS, c0, p.n_class, p.C};
+  HeadSmem hs = head_smem_carve(smem, p.C, sq, &p.amap, &p.bmap);
+  float* As = hs.As;
+  uint8_t* img = hs.img;
+  const uint32_t sb = smem_u32(img);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = lane & 3;
+  const int r = (warp >> 2) * 64 + (warp & 3) * 16;
+  const int64_t row0 = (int64_t)blockIdx.x * HT;
+  const int nr = p.R - row0 < HT ? (int)(p.R - row0) : HT;
+  load_tile(As, p.X, row0, nr, p.C);
+  const int64_t rows[2] = {row0 + r + (lane >> 2), row0 + r + (lane >> 2) + 8};
+  int64_t lab[2];
+  float coef[2], lse[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const bool v = rows[h] < p.R;
+    lab[h] = v ? p.labels[rows[h]] : p.ignore_index;
+    coef[h] = row_coef(lab[h], v ? p.g[rows[h]] : 0.f, p.n_class, p.ignore_index, v);
+    lse[h] = v ? p.lse[rows[h]] : 0.f;
+  }
+  float z[64], acc[64];
+  for (int64_t n0 = 0; n0 < p.n_class; n0 += HT) {
+    const int nn = p.n_class - n0 < HT ? (int)(p.n_class - n0) : HT;
+    logit_tile<MODE>(z, As, p.C, r, hs.rg, sq, &p.amap, &p.bmap, img);
+#pragma unroll
+    for (int b = 0; b < 16; ++b)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int c = 8 * b + 2 * t + (e & 1), h = e >> 1;
+        float d = 0.f;
+        if (c < nn && coef[h] != 0.f) {
+          const float zz = z[4 * b + e] + (p.b ? __ldg(p.b + n0 + c) : 0.f);
+          d = coef[h] * (expf(zz - lse[h]) - (n0 + c == lab[h] ? 1.f : 0.f));
+        }
+        z[4 * b + e] = d;
+      }
+#define DN_HEAD_DX_CHUNK(CH)                                                                                      \
+    {                                                                                                             \
+      const int64_t k0 = n0 + KS * (CH);                                                                          \
+      const int nk = (int)(p.n_class - k0 < KS ? p.n_class - k0 : KS);                                            \
+      ring_next(hs.rg, sq, &p.amap, &p.bmap, img,                                                                 \
+                [=](uint8_t* im, const uint8_t* raw) { convert_cols<MODE>(im, raw, nk, nc); });                   \
+      mma_reg_a<MODE, CH>(acc, z, sb, n0 == 0 && (CH) == 0);                                                       \
+    }
+    DN_HEAD_DX_CHUNK(0) DN_HEAD_DX_CHUNK(1) DN_HEAD_DX_CHUNK(2) DN_HEAD_DX_CHUNK(3)
+#undef DN_HEAD_DX_CHUNK
+  }
+#pragma unroll
+  for (int b = 0; b < 16; ++b)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int c = 8 * b + 2 * t + (e & 1), h = e >> 1;
+      if (c < nc && rows[h] < p.R) p.dX[rows[h] * p.C + c0 + c] = acc[4 * b + e];
+    }
+}
+
+// Weight and bias gradient partials: CTA (class tile, column half, row split s) sums dZ^T X over the row tiles of split
+// s, recomputing the transposed logit tile W_tile X_rows^T.  dbp is written by the column-half-0 CTAs.
+template <int MODE>
+__global__ void __launch_bounds__(NTHR, 1) linear_nll_dw_kernel(const __grid_constant__ HeadArgs p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = lane & 3;
+  const int r = (warp >> 2) * 64 + (warp & 3) * 16;
+  const int64_t n0 = (int64_t)blockIdx.x * HT;
+  const int nn = p.n_class - n0 < HT ? (int)(p.n_class - n0) : HT;
+  const int c0 = blockIdx.y * HT, nc = p.C - c0 < HT ? p.C - c0 : HT;
+  const int split = blockIdx.z;
+  const int64_t RT = cdiv(p.R, HT);
+  const int64_t t_begin = RT * split / p.S, t_end = RT * (split + 1) / p.S;
+  const Seq sq{HT * t_begin, HT * t_begin, t_end - t_begin, (int)cdiv(p.C, KS), HT / KS, c0, p.R, p.C};
+  HeadSmem hs = head_smem_carve(smem, p.C, sq, &p.amap, &p.bmap);
+  float* As = hs.As;
+  uint8_t* img = hs.img;
+  const uint32_t sb = smem_u32(img);
+  float* rcoef = hs.rows;
+  float* rlse = rcoef + HT;
+  int* rlab = reinterpret_cast<int*>(rlse + HT);
+  load_tile(As, p.W, n0, nn, p.C);
+  const int cls[2] = {r + (lane >> 2), r + (lane >> 2) + 8};
+  float bias[2], dbs[2] = {0.f, 0.f};
+#pragma unroll
+  for (int h = 0; h < 2; ++h) bias[h] = (p.b && cls[h] < nn) ? p.b[n0 + cls[h]] : 0.f;
+  float z[64], acc[64];
+  for (int64_t rt = t_begin; rt < t_end; ++rt) {
+    const int64_t row0 = rt * HT;
+    const int nr = p.R - row0 < HT ? (int)(p.R - row0) : HT;
+    // the tile's per-row factors go to shared memory (read after logit_tile's barriers); kept in registers for all 32
+    // columns of a thread they would spill
+    if (threadIdx.x < HT) {
+      const int c = threadIdx.x;
+      const bool v = c < nr;
+      const int64_t lab = v ? __ldg(p.labels + row0 + c) : p.ignore_index;
+      rcoef[c] = row_coef(lab, v ? __ldg(p.g + row0 + c) : 0.f, p.n_class, p.ignore_index, v);
+      rlse[c] = v ? __ldg(p.lse + row0 + c) : 0.f;
+      rlab[c] = (lab >= n0 && lab < n0 + nn) ? (int)(lab - n0) : -1;
+    }
+    logit_tile<MODE>(z, As, p.C, r, hs.rg, sq, &p.amap, &p.bmap, img);
+#pragma unroll
+    for (int b = 0; b < 16; ++b)
+#pragma unroll
+      for (int e2 = 0; e2 < 2; ++e2) {
+        const int c = 8 * b + 2 * t + e2;
+        const float coef = rcoef[c], lse = rlse[c];
+        const int lab = rlab[c];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float d = 0.f;
+          if (cls[h] < nn && coef != 0.f)
+            d = coef * (expf(z[4 * b + 2 * h + e2] + bias[h] - lse) - (cls[h] == lab ? 1.f : 0.f));
+          z[4 * b + 2 * h + e2] = d;
+          dbs[h] += d;
+        }
+      }
+#define DN_HEAD_DW_CHUNK(CH)                                                                                      \
+    {                                                                                                             \
+      const int64_t k0 = row0 + KS * (CH);                                                                        \
+      const int nk = (int)(p.R - k0 < KS ? (p.R - k0 < 0 ? 0 : p.R - k0) : KS);                                   \
+      ring_next(hs.rg, sq, &p.amap, &p.bmap, img,                                                                 \
+                [=](uint8_t* im, const uint8_t* raw) { convert_cols<MODE>(im, raw, nk, nc); });                   \
+      mma_reg_a<MODE, CH>(acc, z, sb, rt == t_begin && (CH) == 0);                                                 \
+    }
+    DN_HEAD_DW_CHUNK(0) DN_HEAD_DW_CHUNK(1) DN_HEAD_DW_CHUNK(2) DN_HEAD_DW_CHUNK(3)
+#undef DN_HEAD_DW_CHUNK
+  }
+  float* dw = p.dWp + (int64_t)split * p.n_class * p.C;
+#pragma unroll
+  for (int b = 0; b < 16; ++b)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int c = 8 * b + 2 * t + (e & 1), h = e >> 1;
+      if (c < nc && cls[h] < nn) dw[(n0 + cls[h]) * p.C + c0 + c] = acc[4 * b + e];
+    }
+  if (blockIdx.y == 0) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      dbs[h] += __shfl_xor_sync(0xffffffffu, dbs[h], 1);
+      dbs[h] += __shfl_xor_sync(0xffffffffu, dbs[h], 2);
+      if (t == 0 && cls[h] < nn) p.dbp[(int64_t)split * p.n_class + n0 + cls[h]] = dbs[h];
+    }
+  }
+}
+
+// dW = sum_s dWp[s], db = sum_s dbp[s], in split order (OVERWRITTEN)
+__global__ void linear_nll_reduce_kernel(const float* __restrict__ dWp, const float* __restrict__ dbp, int S,
+                                         int64_t nw, int64_t nb, float* dW, float* db) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nw + nb; i += (int64_t)gridDim.x * blockDim.x) {
+    const bool w = i < nw;
+    const float* src = w ? dWp + i : dbp + (i - nw);
+    const int64_t stride = w ? nw : nb;
+    float s = 0.f;
+    for (int k = 0; k < S; ++k) s += src[k * stride];
+    if (w) dW[i] = s;
+    else if (db) db[i - nw] = s;
+  }
+}
+
+// out[e][c] = (sum_j x[elems[e][j]][c]) / k, corners summed in order j = 0 .. k-1
+__global__ void element_mean_fwd_kernel(const float* __restrict__ x, int C, const int64_t* __restrict__ elems, int64_t E,
+                                        int k, float* out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < E * C; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t e = i / C;
+    const int c = (int)(i % C);
+    float s = 0.f;
+    for (int j = 0; j < k; ++j) s += __ldg(x + __ldg(elems + e * k + j) * C + c);
+    out[i] = s / (float)k;
+  }
+}
+
+// grad_x[v][c] = sum over the CSR entries of v (element ids, in list order) of grad_out[e][c] / k
+__global__ void element_mean_bwd_kernel(const float* __restrict__ g, int C, const int32_t* __restrict__ rowptr,
+                                        const int32_t* __restrict__ ent, int64_t V, int k, float* gx) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < V * C; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t v = i / C;
+    const int c = (int)(i % C);
+    float s = 0.f;
+    for (int j = rowptr[v]; j < rowptr[v + 1]; ++j) s += __ldg(g + (int64_t)ent[j] * C + c) / (float)k;
+    gx[i] = s;
+  }
+}
+
+size_t head_smem(int C) { return 1024 + 2 * RAW_BYTES + (size_t)HT * (C + 4) * 4 + 2 * B_IMG + 3 * HT * 4 + 16; }
+
+template <typename K>
+int launch(K kernel, dim3 grid, int C, const HeadArgs& a, cudaStream_t st) {
+  const size_t sm = head_smem(C);
+  DN_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  kernel<<<grid, NTHR, sm, st>>>(a);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
+// fp32 [rows][C] (row stride C) as 2-D boxes of {32 columns, box_rows rows} with the 128-byte swizzle
+bool encode_map(CUtensorMap* m, const float* base, int64_t rows, int C, int box_rows) {
+  const auto encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(dn_tensor_map_encoder());
+  if (!encode) return false;
+  const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)C * 4};
+  const cuuint32_t box[2] = {32, (cuuint32_t)box_rows}, estr[2] = {1, 1};
+  return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
+                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+int mode_of(int passes) { return passes == DN_PASSES_BF16 ? M_BF16 : (passes == 1 ? M_TF32 : M_TF32X3); }
+
+}  // namespace
+
+int head_splits(int64_t R, int C, int n_class) {
+  const int64_t tiles = cdiv(n_class, HT) * cdiv(C, HT);
+  int64_t s = cdiv(2ll * dn_sm_count(), tiles);
+  const int64_t rt = cdiv(R, HT);
+  if (s > rt) s = rt;
+  if (s > 1024) s = 1024;
+  return (int)(s < 1 ? 1 : s);
+}
+
+int64_t head_ws_bytes(int64_t R, int C, int n_class) {
+  return 4ll * head_splits(R, C, n_class) * n_class * (C + 1);
+}
+
+int launch_linear_nll_fwd(const float* X, const float* W, const float* b, const int64_t* labels, int64_t R, int C,
+                          int n_class, int64_t ignore_index, float* nll, int64_t* argmax, float* lse, int passes,
+                          cudaStream_t st) {
+  HeadArgs a{};
+  a.X = X; a.W = W; a.b = b; a.labels = labels; a.R = R; a.C = C; a.n_class = n_class; a.ignore_index = ignore_index;
+  a.nll = nll; a.argmax = argmax; a.lse_out = lse;
+  if (!encode_map(&a.amap, W, n_class, C, HT)) return DN_ERR_UNSUPPORTED;
+  a.bmap = a.amap;
+  const dim3 grid((unsigned)cdiv(R, HT));
+  switch (mode_of(passes)) {
+    case M_TF32X3: return launch(linear_nll_fwd_kernel<M_TF32X3>, grid, C, a, st);
+    case M_TF32: return launch(linear_nll_fwd_kernel<M_TF32>, grid, C, a, st);
+    default: return launch(linear_nll_fwd_kernel<M_BF16>, grid, C, a, st);
+  }
+}
+
+int launch_linear_nll_bwd(const float* X, const float* W, const float* b, const int64_t* labels, const float* lse,
+                          const float* g, int64_t R, int C, int n_class, int64_t ignore_index, float* dX, float* dW,
+                          float* db, void* ws, int passes, cudaStream_t st) {
+  HeadArgs a{};
+  a.X = X; a.W = W; a.b = b; a.labels = labels; a.lse = lse; a.g = g; a.R = R; a.C = C; a.n_class = n_class;
+  a.ignore_index = ignore_index; a.dX = dX;
+  a.S = head_splits(R, C, n_class);
+  a.dWp = static_cast<float*>(ws);
+  a.dbp = a.dWp + (int64_t)a.S * n_class * C;
+  HeadArgs aw = a;       // the weight-gradient kernel streams X, the dX kernel W
+  if (!encode_map(&a.amap, W, n_class, C, HT) || !encode_map(&a.bmap, W, n_class, C, KS) ||
+      !encode_map(&aw.amap, X, R, C, HT) || !encode_map(&aw.bmap, X, R, C, KS))
+    return DN_ERR_UNSUPPORTED;
+  const dim3 gx((unsigned)cdiv(R, HT), (unsigned)cdiv(C, HT));
+  const dim3 gw((unsigned)cdiv(n_class, HT), (unsigned)cdiv(C, HT), (unsigned)a.S);
+  int rc;
+  switch (mode_of(passes)) {
+    case M_TF32X3:
+      if ((rc = launch(linear_nll_dx_kernel<M_TF32X3>, gx, C, a, st))) return rc;
+      if ((rc = launch(linear_nll_dw_kernel<M_TF32X3>, gw, C, aw, st))) return rc;
+      break;
+    case M_TF32:
+      if ((rc = launch(linear_nll_dx_kernel<M_TF32>, gx, C, a, st))) return rc;
+      if ((rc = launch(linear_nll_dw_kernel<M_TF32>, gw, C, aw, st))) return rc;
+      break;
+    default:
+      if ((rc = launch(linear_nll_dx_kernel<M_BF16>, gx, C, a, st))) return rc;
+      if ((rc = launch(linear_nll_dw_kernel<M_BF16>, gw, C, aw, st))) return rc;
+  }
+  const int64_t nw = (int64_t)n_class * C;
+  const int64_t blocks = cdiv(nw + n_class, 256);
+  linear_nll_reduce_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(a.dWp, a.dbp, a.S, nw, n_class,
+                                                                                      dW, db);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
+int launch_element_mean_fwd(const float* x, int C, const int64_t* elems, int64_t E, int k, float* out,
+                            cudaStream_t st) {
+  const int64_t blocks = cdiv(E * C, 256);
+  element_mean_fwd_kernel<<<(unsigned)(blocks < 8192 ? (blocks > 0 ? blocks : 1) : 8192), 256, 0, st>>>(x, C, elems, E,
+                                                                                                      k, out);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
+int launch_element_mean_bwd(const float* g, int C, const int32_t* rowptr, const int32_t* ent, int64_t V, int k,
+                            float* gx, cudaStream_t st) {
+  const int64_t blocks = cdiv(V * C, 256);
+  element_mean_bwd_kernel<<<(unsigned)(blocks < 8192 ? (blocks > 0 ? blocks : 1) : 8192), 256, 0, st>>>(g, C, rowptr,
+                                                                                                      ent, V, k, gx);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}

@@ -215,3 +215,19 @@ int64_t tc_chain_ws_bytes(const DnLayer* layers, int n_layers, int n_meshes = 1)
 // one launch: pack the weights of n layers (layer 0 the spectral multiplier when sp is given) into ws and set
 // layers[i].prepacked
 int tc_pack_layers(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, const TcSpectral* sp, cudaStream_t st);
+
+// ---- fused classification head (dn_head.cu) ----
+// cuTensorMapEncodeTiled (a PFN_cuTensorMapEncodeTiled_v12000) from the loaded driver, null if absent (dn_tc.cu)
+void* dn_tensor_map_encoder();
+// row splits of the weight-gradient kernel and the workspace its partials need
+int head_splits(int64_t R, int C, int n_class);
+int64_t head_ws_bytes(int64_t R, int C, int n_class);
+int launch_linear_nll_fwd(const float* X, const float* W, const float* b, const int64_t* labels, int64_t R, int C,
+                          int n_class, int64_t ignore_index, float* nll, int64_t* argmax, float* lse, int passes,
+                          cudaStream_t st);
+int launch_linear_nll_bwd(const float* X, const float* W, const float* b, const int64_t* labels, const float* lse,
+                          const float* g, int64_t R, int C, int n_class, int64_t ignore_index, float* dX, float* dW,
+                          float* db, void* ws, int passes, cudaStream_t st);
+int launch_element_mean_fwd(const float* x, int C, const int64_t* elems, int64_t E, int k, float* out, cudaStream_t st);
+int launch_element_mean_bwd(const float* g, int C, const int32_t* rowptr, const int32_t* ent, int64_t V, int k,
+                            float* gx, cudaStream_t st);

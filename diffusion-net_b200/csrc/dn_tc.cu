@@ -895,6 +895,8 @@ PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
 
 }  // namespace
 
+void* dn_tensor_map_encoder() { return reinterpret_cast<void*>(tensor_map_encoder()); }
+
 static DevState* cur_dev_state() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDev) {

@@ -316,11 +316,15 @@ class DiffusionNet(nn.Module):
         needs_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))
         dropout = any(blk.training and blk.dropout for blk in self.blocks)
         if needs_grad or dropout:
-            x = ops.mlp_apply([x], [self.first_lin.weight], [self.first_lin.bias])
-            for blk in self.blocks:
-                x = blk._forward_batch(batch, x)
-            return ops.mlp_apply([x], [self.last_lin.weight], [self.last_lin.bias])
+            return ops.mlp_apply([self._forward_batch_blocks(batch, x)], [self.last_lin.weight], [self.last_lin.bias])
         return self._forward_batch_fused(batch, x)
+
+    def _forward_batch_blocks(self, batch, x):
+        """The differentiable route of forward_batch from the packed input to the last block's (V, C_width) output."""
+        x = ops.mlp_apply([x], [self.first_lin.weight], [self.first_lin.bias])
+        for blk in self.blocks:
+            x = blk._forward_batch(batch, x)
+        return x
 
     def _forward_batch_fused(self, batch, x):
         """Inference route of forward_batch: one dn_block_fwd_batched per block, last_lin fused behind the last one when
@@ -347,6 +351,97 @@ class DiffusionNet(nn.Module):
         if not head_done:
             x = ops.mlp_apply([x], [self.last_lin.weight], [self.last_lin.bias])
         return x
+
+    def _head_nll(self, x, labels, elems, csr, ignore_index):
+        """(per-row nll, pred) of last_lin + log_softmax + nll_loss on the (V, C_width) block output ``x``, on element
+        rows (the mean of the corner features) when ``elems`` is given."""
+        if elems is not None:
+            x = ops.element_mean(x, elems, csr)
+        return ops.linear_nll(x, self.last_lin.weight, self.last_lin.bias, labels, ignore_index)
+
+    def _check_nll_head(self):
+        if self.outputs_at == 'global_mean':
+            raise ValueError("forward_nll / forward_batch_nll: outputs_at='global_mean' is not supported (use forward "
+                             "and torch's nll_loss)")
+
+    def forward_nll(self, x_in, mass, L=None, evals=None, evecs=None, gradX=None, gradY=None, labels=None, edges=None,
+                    faces=None, ignore_index=-100):
+        """Training step of a segmentation / per-vertex classification net on one mesh: ``(loss, pred_labels)`` with
+        ``loss = F.nll_loss(F.log_softmax(last_lin(...)), labels, ignore_index=ignore_index)`` (mean over the rows whose
+        label is not ignore_index, as torch defines it) and ``pred_labels`` the argmax of the logits.  For nets whose
+        ``last_activation`` is log_softmax: it is not applied here, the fused head (ops.linear_nll) replaces last_lin,
+        log_softmax and nll_loss, so the (rows, C_out) logits are never formed.  The blocks run as in ``forward``.
+        x_in is [N, C] (one mesh); labels int64 per vertex, or per face / edge for outputs_at 'faces' / 'edges' (the
+        head then runs on the mean of each element's corner features, equal to the mean of its corner logits).
+        A label outside [0, C_out) that is not ignore_index makes the loss NaN instead of a device assert."""
+        self._check_nll_head()
+        if labels is None:
+            raise ValueError("forward_nll needs labels")
+        if x_in.dim() != 2 or x_in.shape[-1] != self.C_in:
+            raise ValueError("forward_nll takes one mesh: x_in [N, {}], got {}".format(self.C_in, tuple(x_in.shape)))
+        ops._require_cuda(x_in, mass, labels)
+        elems = None
+        if self.outputs_at in ('edges', 'faces'):
+            elems = edges if self.outputs_at == 'edges' else faces
+            if elems is None:
+                raise ValueError("forward_nll with outputs_at='{0}' needs {0}".format(self.outputs_at))
+        mass_b = mass.unsqueeze(0)
+        evals_b = evals.unsqueeze(0) if evals is not None else None
+        evecs_b = evecs.unsqueeze(0) if evecs is not None else None
+        Lb = [L] if L is not None else None
+        gX = [gradX] if gradX is not None else None
+        gY = [gradY] if gradY is not None else None
+        x = self._linear(self.first_lin, x_in.unsqueeze(0))
+        for b in self.blocks:
+            x = b(x, mass_b, Lb, evals_b, evecs_b, gX, gY)
+        nll, pred = self._head_nll(x[0], labels, elems, None, ignore_index)
+        n_valid = (labels != ignore_index).sum().to(nll.dtype)
+        return nll.sum() / n_valid, pred
+
+    def forward_batch_nll(self, batch, xs, labels, ignore_index=-100):
+        """forward_nll over a ``batch.MeshBatch``: ``labels`` is the list of per-mesh label tensors (per vertex, or per
+        face / edge).  Returns ``(losses, preds)``: the (n_meshes,) per-mesh mean losses and the list of per-mesh
+        predictions; ``losses.sum().backward()`` accumulates the gradients of the per-mesh loop.  The blocks run on
+        forward_batch's differentiable route; padding rows of the batch layout carry ignore_index."""
+        self._check_nll_head()
+        if self.diffusion_method != 'spectral':
+            raise NotImplementedError("forward_batch_nll: spectral diffusion only")
+        if len(labels) != batch.n_meshes:
+            raise ValueError("forward_batch_nll: {} label tensors for {} meshes".format(len(labels), batch.n_meshes))
+        x = xs if torch.is_tensor(xs) else batch.pack(xs)
+        if x.shape[-1] != self.C_in:
+            raise ValueError("DiffusionNet was constructed with C_in={}, but x_in has last dim={}".format(
+                self.C_in, x.shape[-1]))
+        x = self._forward_batch_blocks(batch, x)
+        elems = None
+        if self.outputs_at in ('edges', 'faces'):
+            elems = batch.faces if self.outputs_at == 'faces' else batch.edges
+            if elems is None:
+                raise ValueError("forward_batch_nll with outputs_at='{0}' needs '{0}' in every MeshBatch item".format(
+                    self.outputs_at))
+            counts = batch.elem_counts(self.outputs_at)
+            for b, (l, n) in enumerate(zip(labels, counts)):
+                if l.shape != (n,):
+                    raise ValueError("forward_batch_nll: mesh {} has {} {}, got labels of shape {}".format(
+                        b, n, self.outputs_at, tuple(l.shape)))
+            lab = torch.cat(list(labels))
+        else:
+            counts = batch.n_rows
+            lab = torch.full((batch.V,), ignore_index, dtype=torch.int64, device=x.device)
+            for b, l in enumerate(labels):
+                if l.shape != (batch.n_rows[b],):
+                    raise ValueError("forward_batch_nll: mesh {} has {} vertices, got labels of shape {}".format(
+                        b, batch.n_rows[b], tuple(l.shape)))
+                lab[batch.row_begin[b]:batch.row_begin[b] + batch.n_rows[b]] = l
+        nll, pred = self._head_nll(x, lab, elems, None, ignore_index)
+        if elems is not None:
+            nlls, preds, labs = torch.split(nll, counts), list(torch.split(pred, counts)), labels
+        else:
+            nlls = [nll[r0:r0 + n] for r0, n in zip(batch.row_begin, batch.n_rows)]
+            preds = [pred[r0:r0 + n] for r0, n in zip(batch.row_begin, batch.n_rows)]
+            labs = labels
+        losses = torch.stack([v.sum() / (l != ignore_index).sum().to(v.dtype) for v, l in zip(nlls, labs)])
+        return losses, preds
 
     def forward(self, x_in, mass, L=None, evals=None, evecs=None, gradX=None, gradY=None, edges=None, faces=None):
         """[N,C] or [B,N,C] in, [N,C_out] or [B,N,C_out] out (reference layers.py:314-407)."""

@@ -894,3 +894,135 @@ class MLPFn(torch.autograd.Function):
 def mlp_apply(srcs, weights, biases, residual=None, drop_p=0.0):
     args = list(srcs) + list(weights) + list(biases) + ([residual] if residual is not None else [])
     return MLPFn.apply(len(srcs), len(weights), residual is not None, float(drop_p), *args)
+
+
+# ---- fused classification head: last_lin -> log_softmax -> nll_loss ----------------------------------------------------
+class LinearNLLFn(torch.autograd.Function):
+    """Per-row ``nll_loss(log_softmax(x @ weight.T + bias), labels, reduction='none')`` and the row argmax in one
+    tensor-core launch (dn_linear_nll_fwd); the (R, n_class) logits are never formed.  Backward: 3 launches
+    (dn_linear_nll_bwd), gradients to x, weight and bias, reproducible bit for bit."""
+
+    @staticmethod
+    @_device_guard
+    def forward(ctx, x, weight, bias, labels, ignore_index):
+        x, weight = _f32c(x), _f32c(weight)
+        bias = _f32c(bias) if bias is not None else None
+        labels = labels.contiguous()
+        R, Cc = x.shape
+        n_class = weight.shape[0]
+        nll = torch.empty(R, dtype=torch.float32, device=x.device)
+        lse = torch.empty(R, dtype=torch.float32, device=x.device)
+        pred = torch.empty(R, dtype=torch.int64, device=x.device)
+        _lib.check(_lib.load().dn_linear_nll_fwd(x.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None
+                                                 else None, labels.data_ptr(), R, Cc, n_class, int(ignore_index),
+                                                 nll.data_ptr(), pred.data_ptr(), lse.data_ptr(), _engine, _stream()),
+                   "dn_linear_nll_fwd")
+        ctx.save_for_backward(x, weight, bias, labels, lse)
+        ctx.ignore_index = int(ignore_index)
+        ctx.mark_non_differentiable(pred)
+        return nll, pred
+
+    @staticmethod
+    @_device_guard
+    def backward(ctx, g, _g_pred):
+        x, weight, bias, labels, lse = ctx.saved_tensors
+        R, Cc = x.shape
+        n_class = weight.shape[0]
+        g = _f32c(g)
+        gx = torch.empty_like(x)
+        gw = torch.empty_like(weight)
+        gb = torch.empty_like(bias) if bias is not None else None
+        lib = _lib.load()
+        ws_bytes = lib.dn_linear_nll_workspace_bytes(R, Cc, n_class)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        _lib.check(lib.dn_linear_nll_bwd(x.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None else None,
+                                         labels.data_ptr(), lse.data_ptr(), g.data_ptr(), R, Cc, n_class,
+                                         ctx.ignore_index, gx.data_ptr(), gw.data_ptr(),
+                                         gb.data_ptr() if gb is not None else None, ws.data_ptr(), ws_bytes, _engine,
+                                         _stream()), "dn_linear_nll_bwd")
+        return gx, gw, gb, None, None
+
+
+def linear_nll(x, weight, bias, labels, ignore_index=-100):
+    """``(nll_per_row, argmax)`` of the classification head ``log_softmax(x @ weight.T + bias)`` for int64 ``labels``:
+    nll_per_row[r] = -log_softmax(z)[r, labels[r]], 0 where labels[r] == ignore_index.  Reductions stay with the caller.
+    Gradients reach x, weight and bias.  On the tensor-core engines one fused op; a label outside [0, n_class) that is
+    not ignore_index gives a NaN row (and NaN gradients) instead of torch's device assert.  On the 'simt' engine the
+    composed path (exact SIMT linear layer, then torch's log_softmax and nll_loss) with torch's semantics."""
+    _require_cuda(x, weight, bias, labels)
+    if x.dim() != 2 or weight.dim() != 2 or x.shape[1] != weight.shape[1]:
+        raise ValueError("linear_nll: x (R, C) and weight (n_class, C) expected; got {} and {}".format(
+            tuple(x.shape), tuple(weight.shape)))
+    if labels.dtype != torch.int64 or labels.shape != (x.shape[0],):
+        raise ValueError("linear_nll: labels must be int64 of shape ({},)".format(x.shape[0]))
+    if _engine == _lib.ENGINE_SIMT:
+        z = mlp_apply([x], [weight], [bias])
+        nll = torch.nn.functional.nll_loss(torch.log_softmax(z, dim=-1), labels, reduction='none',
+                                           ignore_index=ignore_index)
+        return nll, z.detach().argmax(dim=-1)
+    return LinearNLLFn.apply(x, weight, bias, labels, int(ignore_index))
+
+
+def element_csr(elems, V):
+    """Vertex -> element CSR of an (E, k) corner array, for ElementMeanFn's backward: rowptr int32 (V + 1) and the
+    element of every corner slot, each vertex's elements in increasing order (a stable sort of the corner list)."""
+    flat = elems.reshape(-1)
+    order = torch.sort(flat, stable=True).indices
+    ent = (order // elems.shape[1]).to(torch.int32)
+    counts = torch.zeros(V, dtype=torch.int64, device=elems.device).scatter_add_(0, flat, torch.ones_like(flat))
+    rowptr = torch.zeros(V + 1, dtype=torch.int32, device=elems.device)
+    rowptr[1:] = torch.cumsum(counts, 0).to(torch.int32)
+    return rowptr, ent
+
+
+class ElementMeanFn(torch.autograd.Function):
+    """out[e] = mean of x over the corners of element e (layers.py:394-398 applied to features), one launch each way."""
+
+    @staticmethod
+    @_device_guard
+    def forward(ctx, x, elems, csr):
+        x = _f32c(x)
+        elems = elems.contiguous()
+        V, Cc = x.shape
+        E, k = elems.shape
+        out = torch.empty(E, Cc, dtype=torch.float32, device=x.device)
+        _lib.check(_lib.load().dn_element_mean_fwd(x.data_ptr(), V, Cc, elems.data_ptr(), E, k, out.data_ptr(),
+                                                   _stream()), "dn_element_mean_fwd")
+        ctx.save_for_backward(*csr)
+        ctx.shape = (V, Cc, E, k)
+        return out
+
+    @staticmethod
+    @_device_guard
+    def backward(ctx, g):
+        rowptr, ent = ctx.saved_tensors
+        V, Cc, E, k = ctx.shape
+        g = _f32c(g)
+        gx = torch.empty(V, Cc, dtype=torch.float32, device=g.device)
+        _lib.check(_lib.load().dn_element_mean_bwd(g.data_ptr(), E, Cc, rowptr.data_ptr(), ent.data_ptr(), V, k,
+                                                   gx.data_ptr(), _stream()), "dn_element_mean_bwd")
+        return gx, None, None
+
+
+_elem_csr_cache = {}
+
+
+def cached_element_csr(elems, V):
+    """element_csr(elems, V), built once per element array: memoised on the tensor's identity, version and V, and
+    dropped when the tensor dies (a replayed CUDA graph and every later step reuse it)."""
+    key = (id(elems), elems.data_ptr(), elems._version, tuple(elems.shape), int(V))
+    hit = _elem_csr_cache.get(key)
+    if hit is None:
+        hit = element_csr(elems, V)
+        _elem_csr_cache[key] = hit
+        weakref.finalize(elems, _elem_csr_cache.pop, key, None)
+    return hit
+
+
+def element_mean(x, elems, csr=None):
+    """Mean of the (V, C) rows of x over the corners of each row of the int64 (E, k) ``elems``; ``csr`` is
+    element_csr(elems, V), taken from cached_element_csr when not given."""
+    _require_cuda(x, elems)
+    if csr is None:
+        csr = cached_element_csr(elems, x.shape[0])
+    return ElementMeanFn.apply(x, elems, csr)

@@ -526,6 +526,48 @@ int dn_block_fwd_ex(const float* x_in, const float* mass, const float* evals, co
                     const dn_block_params* params, const dn_mesh_batch* batch, const dn_head* head, int64_t V, int K,
                     int C, float* out, void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream);
 
+/* ---- fused classification head: last_lin -> log_softmax -> nll_loss (SURVEY.md 8f-1, training) -------------------
+ * The head of the segmentation and per-vertex classification experiments (last_lin, last_activation = log_softmax,
+ * F.nll_loss) as one op on R rows: z = x weight^T + bias (x (R, C), weight (n_class, C) nn.Linear layout, bias (n_class)
+ * or NULL, labels int64 (R)), and per row
+ *   nll[r] = lse[r] - z[r][labels[r]],  lse[r] = log sum_n exp z[r][n],  argmax[r] = argmax_n z[r][n]
+ * with ties to the lowest class.  The (R, n_class) logits and log-probabilities are never written to memory: every CTA
+ * owns 128 rows and streams the weights in 128-class tiles through wgmma, keeping a running (max, sum-exp), the label's
+ * logit and the running argmax per row.  Any n_class >= 1; C a multiple of 16 up to 256; x and weight 16-byte aligned
+ * (DN_ERR_UNSUPPORTED otherwise).  Tensor-core engines only (the arithmetic of the logits is the engine's: 3xTF32,
+ * TF32 or bf16; the softmax is fp32): DN_ENGINE_SIMT is DN_ERR_UNSUPPORTED, and so is every refusal, before any work is
+ * enqueued.  Rows with labels[r] == ignore_index get nll = 0 and no gradient.  A label outside [0, n_class) that is not
+ * ignore_index gives nll = NaN on that row and a NaN gradient, and the call goes on (torch's nll_loss asserts on the
+ * device instead); a row with a non-finite logit gets lse = nll = NaN.  Nothing is read back on the host, so both
+ * calls capture in a CUDA graph.
+ *   fwd: 1 launch.  nll, lse (R floats) and argmax (R int64) are OVERWRITTEN; lse is what the backward needs.
+ *   bwd: 3 launches whatever R and n_class are.  With dZ = grad_nll[r] (softmax(z[r]) - onehot(labels[r])), the logits
+ *        recomputed from the saved lse: grad_x = dZ weight (R, C), grad_weight = dZ^T x (n_class, C) and
+ *        grad_bias = sum_r dZ (n_class; may be NULL when bias is NULL), all OVERWRITTEN.  The weight and bias gradients
+ *        are per-row-range partials in the workspace (dn_linear_nll_workspace_bytes(R, C, n_class)), summed in a fixed
+ *        order without atomics: two calls give bitwise-equal results. */
+int64_t dn_linear_nll_workspace_bytes(int64_t R, int C, int n_class);
+int dn_linear_nll_fwd(const float* x, const float* weight, const float* bias, const int64_t* labels, int64_t R, int C,
+                      int n_class, int64_t ignore_index, float* nll, int64_t* argmax, float* lse, int engine,
+                      dn_stream_t stream);
+int dn_linear_nll_bwd(const float* x, const float* weight, const float* bias, const int64_t* labels, const float* lse,
+                      const float* grad_nll, int64_t R, int C, int n_class, int64_t ignore_index, float* grad_x,
+                      float* grad_weight, float* grad_bias, void* workspace, int64_t ws_bytes, int engine,
+                      dn_stream_t stream);
+
+/* Element rows of the head for outputs_at = 'faces' / 'edges' (layers.py:394-398 takes the mean of the corner logits;
+ * the mean commutes with last_lin, so the head runs on the mean of the corner features instead).
+ *   fwd: out[e][c] = (sum_j x[elems[e][j]][c]) / k over the k corners in order, x (V, C), elems int64 (E, k) with every
+ *        index in [0, V) (the caller checks); out (E, C) OVERWRITTEN.  1 launch (none when E = 0).
+ *   bwd: grad_x[v][c] = sum over the entries of vertex v of grad_out[e][c] / k, through a vertex -> element CSR
+ *        (rowptr int32 (V + 1), entries int32: the element of each corner slot, each vertex's entries in increasing
+ *        element order) built once per element array; grad_x (V, C) OVERWRITTEN, in a fixed order without atomics.
+ *        1 launch. */
+int dn_element_mean_fwd(const float* x, int64_t V, int C, const int64_t* elems, int64_t E, int k, float* out,
+                        dn_stream_t stream);
+int dn_element_mean_bwd(const float* grad_out, int64_t E, int C, const int32_t* rowptr, const int32_t* entries,
+                        int64_t V, int k, float* grad_x, dn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -3,11 +3,9 @@
 //
 // Every kernel runs 256 threads: two warpgroups of 64 rows each own the 128 rows of a CTA tile (rows of X, or classes
 // of W in the weight-gradient kernel).  A 128-wide tile of the other operand streams through a B image in shared memory
-// in 32-deep K stages, in the canonical K-major layout of the chain kernels (dn_tc.cu): 8-row core matrices of 16 bytes,
-// 8-column groups 128 B apart, K groups lbo = 128 * 16 B apart; 3xTF32 keeps a hi image and a lo image.
+// in 32-deep K stages, in the K-major layout of the chain kernels (kmajor_off, dn_tc_ptx.cuh) with N = 128; 3xTF32 keeps
+// a hi image and a lo image.
 #include <math.h>
-#include <cuda.h>
-#include <cudaTypedefs.h>
 #include "dn_internal.h"
 #include "dn_tc_ptx.cuh"
 
@@ -20,26 +18,20 @@ constexpr int KS = 32;                    // K per B stage
 constexpr int NTHR = 256;
 constexpr uint32_t LBO = HT * 16;
 constexpr int B_IMG = KS * HT * 4;        // one tf32 image of a stage
-enum { M_TF32X3 = 0, M_TF32 = 1, M_BF16 = 2 };
 
 __host__ __device__ constexpr int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// byte offset of element (k, n) of a stage's B image
-template <int MODE>
-__device__ __forceinline__ uint32_t b_off(int k, int n) {
-  if constexpr (MODE == M_BF16) return (k >> 3) * LBO + (n >> 3) * 128 + (n & 7) * 16 + (k & 7) * 2;
-  else return (k >> 2) * LBO + (n >> 3) * 128 + (n & 7) * 16 + (k & 3) * 4;
-}
-
+// element (k, n) of a stage's B image
 template <int MODE>
 __device__ __forceinline__ void b_put(uint8_t* img, int k, int n, float v) {
-  if constexpr (MODE == M_BF16) {
-    *reinterpret_cast<uint16_t*>(img + b_off<MODE>(k, n)) = (uint16_t)(pack_bf16x2(v, 0.f) & 0xFFFFu);
+  const uint32_t off = kmajor_off<MODE>(k, n, HT);
+  if constexpr (MODE == MODE_BF16) {
+    *reinterpret_cast<uint16_t*>(img + off) = (uint16_t)(pack_bf16x2(v, 0.f) & 0xFFFFu);
   } else {
     float hi, lo;
     split_tf32(v, hi, lo);
-    *reinterpret_cast<float*>(img + b_off<MODE>(k, n)) = hi;
-    if (MODE == M_TF32X3) *reinterpret_cast<float*>(img + B_IMG + b_off<MODE>(k, n)) = lo;
+    *reinterpret_cast<float*>(img + off) = hi;
+    if (MODE == MODE_TF32X3) *reinterpret_cast<float*>(img + B_IMG + off) = lo;
   }
 }
 
@@ -72,14 +64,13 @@ __device__ void convert_rows(uint8_t* img, const uint8_t* raw) {
 
 // columns stage: B(k, n) = src row k, column n, from four {32, 32} boxes (box j holds n in [32 j, 32 j + 32)); zero
 // outside k < nk, n < nn (boxes wholly outside the source are not loaded).  For the TF32 engines the K order inside every
-// 8-group is permuted to match A fragments taken from an accumulator (mma_reg_a).
+// 8-group is permuted to match A fragments taken from an accumulator (tf32_k_slot, mma_dz).
 template <int MODE>
 __device__ void convert_cols(uint8_t* img, const uint8_t* raw, int nk, int nn) {
   for (int w = threadIdx.x; w < KS * HT; w += NTHR) {
     int kl, n;
     img_coords(w, kl, n);
-    const int j = kl & 7;
-    const int k = MODE == M_BF16 ? kl : ((kl & ~7) | (j < 4 ? 2 * j : 2 * (j - 4) + 1));
+    const int k = MODE == MODE_BF16 ? kl : tf32_slot_k(kl);
     const float v = (k < nk && n < nn) ? raw_at(raw + (n >> 5) * (RAW_BYTES / 4), k, n & 31) : 0.f;
     b_put<MODE>(img, kl, n, v);
   }
@@ -136,112 +127,24 @@ __device__ __forceinline__ void ring_next(Ring& rg, const Seq& sq, const CUtenso
   ++rg.q;
 }
 
-// acc (+)= A[rows of this warp][k0, k0 + nk) * B image; A is a fp32 row-major tile in shared memory (row stride lda)
-template <int MODE>
-__device__ __forceinline__ void mma_smem_a(float* acc, const float* As, int lda, int r, int k0, int nk, uint32_t sb,
-                                           bool first) {
-  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const float* a0 = As + (r + g) * lda + k0;
-  const float* a1 = a0 + 8 * lda;
-  constexpr int STEPS = MODE == M_BF16 ? KS / 16 : KS / 8;
+// acc (+)= A * B image over the first `steps` K slices of a stage (k8 TF32, k16 bf16); frag(s, ah, al) forms the A
+// fragment of slice s.  Every fragment is formed before wgmma_fence.
+template <int MODE, typename Frag>
+__device__ __forceinline__ void mma_stage(float* acc, uint32_t sb, bool first, int steps, Frag frag) {
+  constexpr int STEPS = MODE == MODE_BF16 ? KS / 16 : KS / 8;
   uint32_t ah[STEPS][4], al[STEPS][4];
 #pragma unroll
-  for (int s = 0; s < STEPS; ++s) {
-    if constexpr (MODE == M_BF16) {
-      const int c = 16 * s + 2 * t;
-      ah[s][0] = pack_bf16x2(a0[c], a0[c + 1]);
-      ah[s][1] = pack_bf16x2(a1[c], a1[c + 1]);
-      ah[s][2] = pack_bf16x2(a0[c + 8], a0[c + 9]);
-      ah[s][3] = pack_bf16x2(a1[c + 8], a1[c + 9]);
-    } else {
-      const int c = 8 * s + t;
-      const float x[4] = {a0[c], a1[c], a0[c + 4], a1[c + 4]};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        float h, l;
-        split_tf32_fast(x[i], h, l);
-        ah[s][i] = __float_as_uint(h);
-        al[s][i] = __float_as_uint(l);
-      }
-    }
-  }
+  for (int s = 0; s < STEPS; ++s) frag(s, ah[s], al[s]);
 #pragma unroll
   for (int s = 0; s < STEPS; ++s) {
     fence_frag4(ah[s]);
-    if (MODE == M_TF32X3) fence_frag4(al[s]);
+    if (MODE == MODE_TF32X3) fence_frag4(al[s]);
   }
   wgmma_fence();
-  const int steps = MODE == M_BF16 ? nk / 16 : nk / 8;
 #pragma unroll
   for (int s = 0; s < STEPS; ++s) {
     if (s >= steps) break;
-    const uint32_t accumulate = (!first || s > 0) ? 1u : 0u;
-    const uint32_t base = sb + s * 2 * LBO;
-    const uint64_t dh = make_desc(base, LBO, 128);
-    if constexpr (MODE == M_BF16) {
-      wgmma_bf16_n128(acc, ah[s], dh, accumulate);
-    } else if constexpr (MODE == M_TF32X3) {
-      wgmma_tf32_n128(acc, al[s], dh, accumulate);
-      wgmma_tf32_n128(acc, ah[s], make_desc(base + B_IMG, LBO, 128), 1u);
-      wgmma_tf32_n128(acc, ah[s], dh, 1u);
-    } else {
-      wgmma_tf32_n128(acc, ah[s], dh, accumulate);
-    }
-  }
-  wgmma_commit();
-  wgmma_wait<0>();
-#pragma unroll
-  for (int j = 0; j < 8; ++j) fence_acc8(acc + 8 * j);
-}
-
-// acc (+)= Z[:, 32 c, 32 c + 32) * B image, where Z is the 64 x 128 accumulator z of this warpgroup taken as the A
-// operand (columns of z = K).  TF32: the fragment of k8 slice b is z[4b], z[4b+2], z[4b+1], z[4b+3], i.e. logical
-// columns t, t + 4 hold actual columns 2t, 2t + 1 (stage_cols permutes B alike); bf16: the accumulator layout is the
-// fragment layout.
-template <int MODE, int CH>
-__device__ __forceinline__ void mma_reg_a(float* acc, const float* z, uint32_t sb, bool first) {
-  constexpr int STEPS = MODE == M_BF16 ? KS / 16 : KS / 8;
-  uint32_t ah[STEPS][4], al[STEPS][4];
-#pragma unroll
-  for (int s = 0; s < STEPS; ++s) {
-    if constexpr (MODE == M_BF16) {
-      const int b = 4 * CH + 2 * s;
-      ah[s][0] = pack_bf16x2(z[4 * b], z[4 * b + 1]);
-      ah[s][1] = pack_bf16x2(z[4 * b + 2], z[4 * b + 3]);
-      ah[s][2] = pack_bf16x2(z[4 * b + 4], z[4 * b + 5]);
-      ah[s][3] = pack_bf16x2(z[4 * b + 6], z[4 * b + 7]);
-    } else {
-      const int b = 4 * CH + s;
-      const float x[4] = {z[4 * b], z[4 * b + 2], z[4 * b + 1], z[4 * b + 3]};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        float h, l;
-        split_tf32_fast(x[i], h, l);
-        ah[s][i] = __float_as_uint(h);
-        al[s][i] = __float_as_uint(l);
-      }
-    }
-  }
-#pragma unroll
-  for (int s = 0; s < STEPS; ++s) {
-    fence_frag4(ah[s]);
-    if (MODE == M_TF32X3) fence_frag4(al[s]);
-  }
-  wgmma_fence();
-#pragma unroll
-  for (int s = 0; s < STEPS; ++s) {
-    const uint32_t accumulate = (!first || s > 0) ? 1u : 0u;
-    const uint32_t base = sb + s * 2 * LBO;
-    const uint64_t dh = make_desc(base, LBO, 128);
-    if constexpr (MODE == M_BF16) {
-      wgmma_bf16_n128(acc, ah[s], dh, accumulate);
-    } else if constexpr (MODE == M_TF32X3) {
-      wgmma_tf32_n128(acc, al[s], dh, accumulate);
-      wgmma_tf32_n128(acc, ah[s], make_desc(base + B_IMG, LBO, 128), 1u);
-      wgmma_tf32_n128(acc, ah[s], dh, 1u);
-    } else {
-      wgmma_tf32_n128(acc, ah[s], dh, accumulate);
-    }
+    mma_step<MODE, HT>(acc, ah[s], al[s], sb + s * 2 * LBO, B_IMG, LBO, (!first || s > 0) ? 1u : 0u);
   }
   wgmma_commit();
   wgmma_wait<0>();
@@ -265,11 +168,48 @@ template <int MODE>
 __device__ __forceinline__ void logit_tile(float* acc, const float* As, int C, int r, Ring& rg, const Seq& sq,
                                            const CUtensorMap* amap, const CUtensorMap* bmap, uint8_t* img) {
   const uint32_t sb = smem_u32(img);
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, lda = C + 4;
   for (int k0 = 0; k0 < C; k0 += KS) {
     const int nk = C - k0 < KS ? C - k0 : KS;
     ring_next(rg, sq, amap, bmap, img, [](uint8_t* im, const uint8_t* raw) { convert_rows<MODE>(im, raw); });
-    mma_smem_a<MODE>(acc, As, C + 4, r, k0, nk, sb, k0 == 0);
+    // A = rows r + g, r + g + 8 of the shared tile, columns k0 ..
+    const float* a0 = As + (r + g) * lda + k0;
+    const float* a1 = a0 + 8 * lda;
+    mma_stage<MODE>(acc, sb, k0 == 0, MODE == MODE_BF16 ? nk / 16 : nk / 8, [&](int s, uint32_t* ah, uint32_t* al) {
+      if constexpr (MODE == MODE_BF16) {
+        const int c = 16 * s + 2 * t;
+        const float x[8] = {a0[c], a0[c + 1], a1[c], a1[c + 1], a0[c + 8], a0[c + 9], a1[c + 8], a1[c + 9]};
+        frag_bf16(x, ah);
+      } else {
+        const int c = 8 * s + t;
+        const float x[4] = {a0[c], a1[c], a0[c + 4], a1[c + 4]};
+        frag_tf32(x, ah, al);
+      }
+    });
   }
+}
+
+// acc (+)= Z[:, 32 ch, 32 ch + 32) * B_ch for ch = CH .. 3: Z is this warpgroup's 64 x 128 accumulator z as the A operand
+// (columns of z = K), B_ch the next columns stage (source rows k0 + 32 ch .. of `extent` rows, columns c0 .. c0 + nc).
+// `first`: chunk 0 starts the sum.
+template <int MODE, int CH = 0>
+__device__ __forceinline__ void mma_dz(float* acc, const float* z, int64_t k0, int64_t extent, int nc, bool first,
+                                       Ring& rg, const Seq& sq, const CUtensorMap* amap, const CUtensorMap* bmap,
+                                       uint8_t* img) {
+  const int64_t rem = extent - (k0 + KS * CH);
+  const int nk = (int)(rem < KS ? rem : KS);   // <= 0: no row of the stage is in the source
+  ring_next(rg, sq, amap, bmap, img, [=](uint8_t* im, const uint8_t* raw) { convert_cols<MODE>(im, raw, nk, nc); });
+  constexpr int STEPS = MODE == MODE_BF16 ? KS / 16 : KS / 8;
+  mma_stage<MODE>(acc, smem_u32(img), first && CH == 0, STEPS, [&](int s, uint32_t* ah, uint32_t* al) {
+    if constexpr (MODE == MODE_BF16) {
+      frag_bf16(z + 4 * (4 * CH + 2 * s), ah);
+    } else {
+      const float* zb = z + 4 * (4 * CH + s);
+      const float x[4] = {zb[0], zb[2], zb[1], zb[3]};
+      frag_tf32(x, ah, al);
+    }
+  });
+  if constexpr (CH + 1 < HT / KS) mma_dz<MODE, CH + 1>(acc, z, k0, extent, nc, first, rg, sq, amap, bmap, img);
 }
 
 // shared memory: the raw ring (1024-byte aligned for the swizzle), the A tile, the B image, per-row factors, mbarriers
@@ -422,7 +362,6 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_dx_kernel(const __grid_con
   HeadSmem hs = head_smem_carve(smem, p.C, sq, &p.amap, &p.bmap);
   float* As = hs.As;
   uint8_t* img = hs.img;
-  const uint32_t sb = smem_u32(img);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t = lane & 3;
   const int r = (warp >> 2) * 64 + (warp & 3) * 16;
   const int64_t row0 = (int64_t)blockIdx.x * HT;
@@ -454,16 +393,7 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_dx_kernel(const __grid_con
         }
         z[4 * b + e] = d;
       }
-#define DN_HEAD_DX_CHUNK(CH)                                                                                      \
-    {                                                                                                             \
-      const int64_t k0 = n0 + KS * (CH);                                                                          \
-      const int nk = (int)(p.n_class - k0 < KS ? p.n_class - k0 : KS);                                            \
-      ring_next(hs.rg, sq, &p.amap, &p.bmap, img,                                                                 \
-                [=](uint8_t* im, const uint8_t* raw) { convert_cols<MODE>(im, raw, nk, nc); });                   \
-      mma_reg_a<MODE, CH>(acc, z, sb, n0 == 0 && (CH) == 0);                                                       \
-    }
-    DN_HEAD_DX_CHUNK(0) DN_HEAD_DX_CHUNK(1) DN_HEAD_DX_CHUNK(2) DN_HEAD_DX_CHUNK(3)
-#undef DN_HEAD_DX_CHUNK
+    mma_dz<MODE>(acc, z, n0, p.n_class, nc, n0 == 0, hs.rg, sq, &p.amap, &p.bmap, img);
   }
 #pragma unroll
   for (int b = 0; b < 16; ++b)
@@ -491,7 +421,6 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_dw_kernel(const __grid_con
   HeadSmem hs = head_smem_carve(smem, p.C, sq, &p.amap, &p.bmap);
   float* As = hs.As;
   uint8_t* img = hs.img;
-  const uint32_t sb = smem_u32(img);
   float* rcoef = hs.rows;
   float* rlse = rcoef + HT;
   int* rlab = reinterpret_cast<int*>(rlse + HT);
@@ -531,16 +460,7 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_dw_kernel(const __grid_con
           dbs[h] += d;
         }
       }
-#define DN_HEAD_DW_CHUNK(CH)                                                                                      \
-    {                                                                                                             \
-      const int64_t k0 = row0 + KS * (CH);                                                                        \
-      const int nk = (int)(p.R - k0 < KS ? (p.R - k0 < 0 ? 0 : p.R - k0) : KS);                                   \
-      ring_next(hs.rg, sq, &p.amap, &p.bmap, img,                                                                 \
-                [=](uint8_t* im, const uint8_t* raw) { convert_cols<MODE>(im, raw, nk, nc); });                   \
-      mma_reg_a<MODE, CH>(acc, z, sb, rt == t_begin && (CH) == 0);                                                 \
-    }
-    DN_HEAD_DW_CHUNK(0) DN_HEAD_DW_CHUNK(1) DN_HEAD_DW_CHUNK(2) DN_HEAD_DW_CHUNK(3)
-#undef DN_HEAD_DW_CHUNK
+    mma_dz<MODE>(acc, z, row0, p.R, nc, rt == t_begin, hs.rg, sq, &p.amap, &p.bmap, img);
   }
   float* dw = p.dWp + (int64_t)split * p.n_class * p.C;
 #pragma unroll
@@ -609,19 +529,11 @@ int launch(K kernel, dim3 grid, int C, const HeadArgs& a, cudaStream_t st) {
   return DN_OK;
 }
 
-// fp32 [rows][C] (row stride C) as 2-D boxes of {32 columns, box_rows rows} with the 128-byte swizzle
-bool encode_map(CUtensorMap* m, const float* base, int64_t rows, int C, int box_rows) {
-  const auto encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(dn_tensor_map_encoder());
-  if (!encode) return false;
-  const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)C * 4};
-  const cuuint32_t box[2] = {32, (cuuint32_t)box_rows}, estr[2] = {1, 1};
-  return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+template <int MODE>
+int launch_bwd(dim3 gx, dim3 gw, int C, const HeadArgs& a, const HeadArgs& aw, cudaStream_t st) {
+  const int rc = launch(linear_nll_dx_kernel<MODE>, gx, C, a, st);
+  return rc ? rc : launch(linear_nll_dw_kernel<MODE>, gw, C, aw, st);
 }
-
-int mode_of(int passes) { return passes == DN_PASSES_BF16 ? M_BF16 : (passes == 1 ? M_TF32 : M_TF32X3); }
 
 }  // namespace
 
@@ -644,14 +556,12 @@ int launch_linear_nll_fwd(const float* X, const float* W, const float* b, const 
   HeadArgs a{};
   a.X = X; a.W = W; a.b = b; a.labels = labels; a.R = R; a.C = C; a.n_class = n_class; a.ignore_index = ignore_index;
   a.nll = nll; a.argmax = argmax; a.lse_out = lse;
-  if (!encode_map(&a.amap, W, n_class, C, HT)) return DN_ERR_UNSUPPORTED;
+  if (!encode_tensor_map_f32(&a.amap, W, n_class, C, C, 32, HT, true)) return DN_ERR_UNSUPPORTED;
   a.bmap = a.amap;
   const dim3 grid((unsigned)cdiv(R, HT));
-  switch (mode_of(passes)) {
-    case M_TF32X3: return launch(linear_nll_fwd_kernel<M_TF32X3>, grid, C, a, st);
-    case M_TF32: return launch(linear_nll_fwd_kernel<M_TF32>, grid, C, a, st);
-    default: return launch(linear_nll_fwd_kernel<M_BF16>, grid, C, a, st);
-  }
+  if (passes == DN_PASSES_BF16) return launch(linear_nll_fwd_kernel<MODE_BF16>, grid, C, a, st);
+  if (passes == 1) return launch(linear_nll_fwd_kernel<MODE_TF32>, grid, C, a, st);
+  return launch(linear_nll_fwd_kernel<MODE_TF32X3>, grid, C, a, st);
 }
 
 int launch_linear_nll_bwd(const float* X, const float* W, const float* b, const int64_t* labels, const float* lse,
@@ -664,25 +574,18 @@ int launch_linear_nll_bwd(const float* X, const float* W, const float* b, const 
   a.dWp = static_cast<float*>(ws);
   a.dbp = a.dWp + (int64_t)a.S * n_class * C;
   HeadArgs aw = a;       // the weight-gradient kernel streams X, the dX kernel W
-  if (!encode_map(&a.amap, W, n_class, C, HT) || !encode_map(&a.bmap, W, n_class, C, KS) ||
-      !encode_map(&aw.amap, X, R, C, HT) || !encode_map(&aw.bmap, X, R, C, KS))
+  // fp32 [rows][C] in boxes of 32 columns with the 128-byte swizzle
+  if (!encode_tensor_map_f32(&a.amap, W, n_class, C, C, 32, HT, true) ||
+      !encode_tensor_map_f32(&a.bmap, W, n_class, C, C, 32, KS, true) ||
+      !encode_tensor_map_f32(&aw.amap, X, R, C, C, 32, HT, true) ||
+      !encode_tensor_map_f32(&aw.bmap, X, R, C, C, 32, KS, true))
     return DN_ERR_UNSUPPORTED;
   const dim3 gx((unsigned)cdiv(R, HT), (unsigned)cdiv(C, HT));
   const dim3 gw((unsigned)cdiv(n_class, HT), (unsigned)cdiv(C, HT), (unsigned)a.S);
-  int rc;
-  switch (mode_of(passes)) {
-    case M_TF32X3:
-      if ((rc = launch(linear_nll_dx_kernel<M_TF32X3>, gx, C, a, st))) return rc;
-      if ((rc = launch(linear_nll_dw_kernel<M_TF32X3>, gw, C, aw, st))) return rc;
-      break;
-    case M_TF32:
-      if ((rc = launch(linear_nll_dx_kernel<M_TF32>, gx, C, a, st))) return rc;
-      if ((rc = launch(linear_nll_dw_kernel<M_TF32>, gw, C, aw, st))) return rc;
-      break;
-    default:
-      if ((rc = launch(linear_nll_dx_kernel<M_BF16>, gx, C, a, st))) return rc;
-      if ((rc = launch(linear_nll_dw_kernel<M_BF16>, gw, C, aw, st))) return rc;
-  }
+  const int rc = passes == DN_PASSES_BF16 ? launch_bwd<MODE_BF16>(gx, gw, C, a, aw, st)
+                 : passes == 1             ? launch_bwd<MODE_TF32>(gx, gw, C, a, aw, st)
+                                           : launch_bwd<MODE_TF32X3>(gx, gw, C, a, aw, st);
+  if (rc) return rc;
   const int64_t nw = (int64_t)n_class * C;
   const int64_t blocks = cdiv(nw + n_class, 256);
   linear_nll_reduce_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(a.dWp, a.dbp, a.S, nw, n_class,

@@ -1,6 +1,7 @@
 // Internal (non-ABI) declarations shared by the SIMT kernels, the wgmma kernels and the
 // C-ABI glue.  Everything here is device-pointer based; no torch types anywhere in csrc/.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
@@ -216,9 +217,13 @@ int64_t tc_chain_ws_bytes(const DnLayer* layers, int n_layers, int n_meshes = 1)
 // layers[i].prepacked
 int tc_pack_layers(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, const TcSpectral* sp, cudaStream_t st);
 
+// 2-D tensor map of fp32 [rows][width] with a row stride of ld floats, boxes of box_cols x box_rows and the 128-byte
+// swizzle or none; false where the driver has no encoder or rejects the map.  Elements outside the tensor are
+// zero-filled on loads and not written by stores.
+bool encode_tensor_map_f32(CUtensorMap* m, const float* base, int64_t rows, int width, int64_t ld, int box_cols,
+                           int box_rows, bool swizzle128);
+
 // ---- fused classification head (dn_head.cu) ----
-// cuTensorMapEncodeTiled (a PFN_cuTensorMapEncodeTiled_v12000) from the loaded driver, null if absent (dn_tc.cu)
-void* dn_tensor_map_encoder();
 // row splits of the weight-gradient kernel and the workspace its partials need
 int head_splits(int64_t R, int C, int n_class);
 int64_t head_ws_bytes(int64_t R, int C, int n_class);

@@ -37,8 +37,6 @@ constexpr int SMEM_OPTIN = 232448;              // sm_90 opt-in dynamic shared m
 constexpr int OUT_ROWS = 64;                    // rows of an output / residual box: one consumer warpgroup's rows
 constexpr int OUT_BOX_BYTES = 8 * OUT_ROWS * 4; // 8 columns x 64 rows, [64 rows][8 floats]
 
-enum { MODE_TF32 = 1, MODE_TF32X3 = 3, MODE_BF16 = DN_PASSES_BF16 };
-
 // Shared memory of rows_chain_kernel<MODE, NMAX>.  Weight ring: a slot holds one K stage of an NMAX-wide layer as the
 // producer streams it (tf32x3: hi | lo images, 8 bytes per weight; tf32: hi, 4; bf16: 2), as many as fit in
 // W_RING_BYTES, at most 8.  (With 16 slots for the narrower stages, repeated bf16 mesh-batch forwards once gave
@@ -101,16 +99,13 @@ struct PackJobs {
 __device__ __forceinline__ void pack_store(float* dst, int fmt, int N, int k, int n, float w) {
   char* base = reinterpret_cast<char*>(dst) + (int64_t)(k / KC) * stage_stride(N);
   const int kk = k % KC;
-  const int64_t rowoff = (int64_t)(n >> 3) * 128 + (n & 7) * 16;
   if (fmt == 2) {
-    *reinterpret_cast<__nv_bfloat16*>(base + (int64_t)(kk >> 3) * N * 16 + rowoff + (kk & 7) * 2) = __float2bfloat16_rn(w);
+    *reinterpret_cast<__nv_bfloat16*>(base + kmajor_off<MODE_BF16>(kk, n, N)) = __float2bfloat16_rn(w);
     return;
   }
-  const int j = kk & 7;
-  const int slot = (kk & 8) | ((j & 1) ? 4 + (j >> 1) : (j >> 1));
   float hi, lo;
   split_tf32(w, hi, lo);
-  char* q = base + (int64_t)(slot >> 2) * N * 16 + rowoff + (slot & 3) * 4;
+  char* q = base + kmajor_off<MODE_TF32>(tf32_k_slot(kk), n, N);
   *reinterpret_cast<float*>(q) = hi;
   *reinterpret_cast<float*>(q + (int64_t)KC * N * 4) = lo;
 }
@@ -375,62 +370,34 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
       // the previous stage's slot is handed back once that stage's MMAs are done.
       auto stage = [&](int c, const float2* q, bool two) {
         mbar_wait(full + 8 * s, ph);
+        // a stage is one k16 slice (bf16) or two k8 slices (TF32)
+        constexpr int SLICES = MODE == MODE_BF16 ? 1 : 2;
         uint32_t ah[2][4], al[2][4];
-        if (MODE == MODE_BF16) {
-          ah[0][0] = pack_bf16x2(q[0].x, q[0].y); ah[0][1] = pack_bf16x2(q[1].x, q[1].y);
-          ah[0][2] = pack_bf16x2(q[2].x, q[2].y); ah[0][3] = pack_bf16x2(q[3].x, q[3].y);
+        if constexpr (MODE == MODE_BF16) {
+          const float x[8] = {q[0].x, q[0].y, q[1].x, q[1].y, q[2].x, q[2].y, q[3].x, q[3].y};
+          frag_bf16(x, ah[0]);
         } else {
 #pragma unroll
           for (int ks = 0; ks < 2; ++ks) {
             const float2 u = q[2 * ks], v = q[2 * ks + 1];
             const float x[4] = {u.x, v.x, u.y, v.y};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              float h, lo;
-              split_tf32_fast(x[i], h, lo);
-              ah[ks][i] = __float_as_uint(h);
-              al[ks][i] = __float_as_uint(lo);
-            }
+            frag_tf32(x, ah[ks], al[ks]);
           }
         }
         const uint32_t sb = smem_u32(smem + s * STAGE_BYTES);
         wgmma_fence();
-        if (MODE == MODE_BF16) {
+#pragma unroll
+        for (int ks = 0; ks < SLICES; ++ks) {
+          if (ks == 1 && !two) break;
+          const uint32_t acc0 = (c > 0 || ks > 0) ? 1u : 0u;
+          const uint32_t base = sb + ks * 2 * lbo;
           if constexpr (WIDE) {
-            wgmma_bf16<NMAX>(acc, ah[0], make_desc(sb, lbo, 128), c > 0 ? 1u : 0u);
+            mma_step<MODE, NMAX>(acc, ah[ks], al[ks], base, KC * N * 4, lbo, acc0);
           } else {
 #pragma unroll
-            for (int j = 0; j < NB; ++j)
-              if (j < nb) wgmma_bf16_n16(acc + 8 * j, ah[0], make_desc(sb + j * 256, lbo, 128), c > 0 ? 1u : 0u);
-          }
-        } else {
-#pragma unroll
-          for (int ks = 0; ks < 2; ++ks) {
-            if (ks == 1 && !two) break;
-            const uint32_t acc0 = (c > 0 || ks > 0) ? 1u : 0u;
-            const uint32_t base = sb + ks * 2 * lbo;
-            if constexpr (WIDE) {
-              const uint64_t dh = make_desc(base, lbo, 128);
-              const uint32_t* a0 = MODE == MODE_TF32X3 ? al[ks] : ah[ks];
-              wgmma_tf32<NMAX>(acc, a0, dh, acc0);
-              if (MODE == MODE_TF32X3) {
-                wgmma_tf32<NMAX>(acc, ah[ks], make_desc(base + KC * N * 4, lbo, 128), 1u);
-                wgmma_tf32<NMAX>(acc, ah[ks], dh, 1u);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < NB; ++j) {
-                if (j >= nb) break;
-                const uint64_t dh = make_desc(base + j * 256, lbo, 128);
-                if (MODE == MODE_TF32X3) {
-                  const uint64_t dl = make_desc(base + KC * N * 4 + j * 256, lbo, 128);
-                  wgmma_tf32_n16(acc + 8 * j, al[ks], dh, acc0);
-                  wgmma_tf32_n16(acc + 8 * j, ah[ks], dl, 1u);
-                  wgmma_tf32_n16(acc + 8 * j, ah[ks], dh, 1u);
-                } else {
-                  wgmma_tf32_n16(acc + 8 * j, ah[ks], dh, acc0);
-                }
-              }
+            for (int j = 0; j < NB; ++j) {
+              if (j >= nb) break;
+              mma_step<MODE, 16>(acc + 8 * j, ah[ks], al[ks], base + j * 256, KC * N * 4, lbo, acc0);
             }
           }
         }
@@ -731,8 +698,8 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
   const int m0 = (warp >> 2) * 64 + (warp & 3) * 16 + g;   // eigen-index rows m0, m0 + 8
   const int abox = m0 >> 3;                                 // their Phi boxes abox, abox + 1 (column m0 & 7 == g)
   const uint32_t lbo = (uint32_t)C * 16;
-  // B image: this thread writes row bv of every stage, channels 8 b + (lane & 7); the core matrix of rows
-  // 4 warp .. 4 warp + 3 and channels 8 b .. 8 b + 7 sits at boff + 128 b
+  // B image: this thread writes row bv of every stage, channels 8 b + (lane & 7), at boff + 128 b = kmajor_off(bv,
+  // 8 b + (lane & 7), C).  (boff written with kmajor_off costs ptxas up to 4 more registers in some instances.)
   const int bv = 4 * warp + (lane >> 3);
   const uint32_t boff = (uint32_t)warp * C * 16 + (lane & 7) * 16 + (lane >> 3) * 4;
   // the fold sums live in shared memory: the 64 accumulators, the A fragments of a stage and the addressing fit the
@@ -777,18 +744,18 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
     }
     uint32_t ah[4][4], al[4][4];           // A fragments, all formed before wgmma_fence
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
+    for (int ks = 0; ks < 4; ++ks) {
+      float x[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int vv = 8 * ks + t + 4 * (i >> 1), k = m0 + 8 * (i & 1);
         // read unconditionally and select: the box stays inside the staging slot, and a load under a lane-dependent
         // branch would put the MMA operands on a divergent path
         const float v = rphi[(abox + (i & 1)) * (TB_BOX / 4) + vv * 8 + g];
-        float h, lo;
-        split_tf32_fast((vv < nv && k < K) ? v : 0.f, h, lo);
-        ah[ks][i] = __float_as_uint(h);
-        al[ks][i] = __float_as_uint(lo);
+        x[i] = (vv < nv && k < K) ? v : 0.f;
       }
+      frag_tf32(x, ah[ks], al[ks]);
+    }
     fence_proxy_async();
     __syncwarp();
     if (lane == 0) mbar_arrive(st_empty + 8 * s);
@@ -803,29 +770,12 @@ __global__ void __launch_bounds__(TB_THREADS, 1) to_basis_kernel(const __grid_co
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) {
       const uint32_t acc0 = (fold > 0 || ks > 0) ? 1u : 0u;
+      const uint32_t base = sb + ks * 2 * lbo;
       if constexpr (NBC == 8) {
-        const uint32_t base = sb + ks * 2 * lbo;
-        const uint64_t dh = make_desc(base, lbo, 128);
-        if (MODE == MODE_TF32X3) {
-          wgmma_tf32_n128(acc, al[ks], dh, acc0);
-          wgmma_tf32_n128(acc, ah[ks], make_desc(base + TB_BIMG, lbo, 128), 1u);
-          wgmma_tf32_n128(acc, ah[ks], dh, 1u);
-        } else {
-          wgmma_tf32_n128(acc, ah[ks], dh, acc0);
-        }
+        mma_step<MODE, 128>(acc, ah[ks], al[ks], base, TB_BIMG, lbo, acc0);
       } else {
 #pragma unroll
-        for (int j = 0; j < NBC; ++j) {
-          const uint32_t base = sb + ks * 2 * lbo + j * 256;
-          const uint64_t dh = make_desc(base, lbo, 128);
-          if (MODE == MODE_TF32X3) {
-            wgmma_tf32_n16(acc + 8 * j, al[ks], dh, acc0);
-            wgmma_tf32_n16(acc + 8 * j, ah[ks], make_desc(base + TB_BIMG, lbo, 128), 1u);
-            wgmma_tf32_n16(acc + 8 * j, ah[ks], dh, 1u);
-          } else {
-            wgmma_tf32_n16(acc + 8 * j, ah[ks], dh, acc0);
-          }
-        }
+        for (int j = 0; j < NBC; ++j) mma_step<MODE, 16>(acc + 8 * j, ah[ks], al[ks], base + j * 256, TB_BIMG, lbo, acc0);
       }
     }
     wgmma_commit();
@@ -895,7 +845,17 @@ PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
 
 }  // namespace
 
-void* dn_tensor_map_encoder() { return reinterpret_cast<void*>(tensor_map_encoder()); }
+bool encode_tensor_map_f32(CUtensorMap* m, const float* base, int64_t rows, int width, int64_t ld, int box_cols,
+                           int box_rows, bool swizzle128) {
+  const PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
+  if (!encode) return false;
+  const cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows}, estr[2] = {1, 1};
+  return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
+                CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
 
 static DevState* cur_dev_state() {
   int dev = 0;
@@ -1056,20 +1016,11 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
   p.V = V;
   p.tile_group = layers[0].tile_group;
   p.group_stride = layers[0].group_stride;
-  // tensor maps (encoded on the host; a captured graph keeps them with the launch): fp32 [V rows][width], row stride ld
-  const PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
-  if (!encode) return DN_ERR_UNSUPPORTED;
-  auto encode_rows = [&](CUtensorMap* m, const float* base, int width, int64_t ld, int box_rows) {
-    const cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)V};
-    const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-    const cuuint32_t box[2] = {8, (cuuint32_t)box_rows}, estr[2] = {1, 1};
-    return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-  };
-  // one per source of layer 0
+  // tensor maps (encoded on the host; a captured graph keeps them with the launch): fp32 [V rows][width], row stride
+  // ld, 8-column boxes; one per source of layer 0
   for (int s = 0; s < src.nsrc; ++s)
-    if (!encode_rows(&p.amap[s], src.ptr[s], src.width[s], src.ld[s], TILE_M)) return DN_ERR_UNSUPPORTED;
+    if (!encode_tensor_map_f32(&p.amap[s], src.ptr[s], V, src.width[s], src.ld[s], 8, TILE_M, false))
+      return DN_ERR_UNSUPPORTED;
   int nmax = 0, nmin = 1 << 30;
   for (int l = 0; l < n_layers; ++l) {
     const DnLayer& L = layers[l];
@@ -1085,8 +1036,10 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
   if (nmax <= 128 && !bf16)
     for (int l = 0; l < n_layers; ++l) {
       const DnLayer& L = layers[l];
-      if (L.out && !encode_rows(&p.omap[l], L.out, L.N, L.ld_out, OUT_ROWS)) return DN_ERR_UNSUPPORTED;
-      if (L.residual && !encode_rows(&p.rmap[l], L.residual, L.N, L.ld_res, OUT_ROWS)) return DN_ERR_UNSUPPORTED;
+      if (L.out && !encode_tensor_map_f32(&p.omap[l], L.out, V, L.N, L.ld_out, 8, OUT_ROWS, false))
+        return DN_ERR_UNSUPPORTED;
+      if (L.residual && !encode_tensor_map_f32(&p.rmap[l], L.residual, V, L.N, L.ld_res, 8, OUT_ROWS, false))
+        return DN_ERR_UNSUPPORTED;
     }
   const bool wide = nmin == nmax && (nmax == 128 || nmax == 256);
   const DnLayer& Ll = layers[n_layers - 1];
@@ -1121,17 +1074,10 @@ int tc_to_basis_partial(const float* values, const float* basis, const float* ma
   memset(&p, 0, sizeof(p));
   // tensor maps (encoded on the host; a captured graph keeps them with the launch): fp32 [V rows][width], row stride
   // ld, 8 x TB_ROWS boxes; columns >= width and rows >= V are zero-filled
-  const PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
-  if (!encode) return DN_ERR_UNSUPPORTED;
-  auto encode_rows = [&](CUtensorMap* m, const float* base, int width, int64_t ld) {
-    const cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)(V > 0 ? V : 1)};
-    const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-    const cuuint32_t box[2] = {8, (cuuint32_t)TB_ROWS}, estr[2] = {1, 1};
-    return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-  };
-  if (!encode_rows(&p.phi_map, basis, K, K) || !encode_rows(&p.x_map, values, C, ld_values)) return DN_ERR_UNSUPPORTED;
+  const int64_t rows = V > 0 ? V : 1;
+  if (!encode_tensor_map_f32(&p.phi_map, basis, rows, K, K, 8, TB_ROWS, false) ||
+      !encode_tensor_map_f32(&p.x_map, values, rows, C, ld_values, 8, TB_ROWS, false))
+    return DN_ERR_UNSUPPORTED;
   p.mass = massvec; p.partial = partial;
   p.ldp = ldp; p.cta_rows = cta_rows;
   p.V = V; p.K = K; p.C = C; p.chunks_per_cta = 0;

@@ -1,10 +1,17 @@
 // Inline-PTX wrappers for the Hopper (sm_90a) features the tensor-core engine uses:
-// mbarrier, bulk and tiled TMA copies, proxy fences and warpgroup MMA (wgmma) with the A operand in registers.
+// mbarrier, bulk and tiled TMA copies, proxy fences and warpgroup MMA (wgmma) with the A operand in registers; and the
+// MMA step every tensor-core kernel (dn_tc.cu, dn_head.cu) shares: engine mode, A fragments, the MMAs of one K slice and
+// the B-image layout.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "dn_internal.h"
 
 namespace tc {
+
+// The engine a tensor-core kernel instance runs, keyed on the pass count of the engine (`passes`, dn_internal.h):
+// 1xTF32, 3xTF32 (lo*hi + hi*lo + hi*hi) or bf16.
+enum { MODE_TF32 = 1, MODE_TF32X3 = 3, MODE_BF16 = DN_PASSES_BF16 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -184,17 +191,19 @@ DN_WGMMA_WIDE(wgmma_bf16_n256, "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16
 #undef DN_ACC64
 #undef DN_ACC8
 
-// one MMA over the whole N-wide accumulator (N = 128 or 256); `accumulate` = 0 starts a new sum (D = A B)
+// one MMA over the whole N-wide accumulator (N = 16, 128 or 256); `accumulate` = 0 starts a new sum (D = A B)
 template <int N>
 __device__ __forceinline__ void wgmma_tf32(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
-  static_assert(N == 128 || N == 256, "wgmma_tf32: unsupported width");
-  if constexpr (N == 128) wgmma_tf32_n128(d, a, b_desc, accumulate);
+  static_assert(N == 16 || N == 128 || N == 256, "wgmma_tf32: unsupported width");
+  if constexpr (N == 16) wgmma_tf32_n16(d, a, b_desc, accumulate);
+  else if constexpr (N == 128) wgmma_tf32_n128(d, a, b_desc, accumulate);
   else wgmma_tf32_n256(d, a, b_desc, accumulate);
 }
 template <int N>
 __device__ __forceinline__ void wgmma_bf16(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
-  static_assert(N == 128 || N == 256, "wgmma_bf16: unsupported width");
-  if constexpr (N == 128) wgmma_bf16_n128(d, a, b_desc, accumulate);
+  static_assert(N == 16 || N == 128 || N == 256, "wgmma_bf16: unsupported width");
+  if constexpr (N == 16) wgmma_bf16_n16(d, a, b_desc, accumulate);
+  else if constexpr (N == 128) wgmma_bf16_n128(d, a, b_desc, accumulate);
   else wgmma_bf16_n256(d, a, b_desc, accumulate);
 }
 
@@ -220,6 +229,61 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
 __device__ __forceinline__ void split_tf32_fast(float x, float& hi, float& lo) {
   hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
   lo = x - hi;
+}
+
+// ---- one MMA step of the tensor-core kernels -------------------------------------------------------------------
+// A operand of one k8 TF32 slice from its four values in fragment order (a0 .. a3 of wgmma_tf32_n16): the hi and lo
+// registers of the split x = hi + lo (the 1xTF32 engine issues hi only)
+__device__ __forceinline__ void frag_tf32(const float* x, uint32_t* ah, uint32_t* al) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float h, l;
+    split_tf32_fast(x[i], h, l);
+    ah[i] = __float_as_uint(h);
+    al[i] = __float_as_uint(l);
+  }
+}
+// A operand of one k16 bf16 slice from its eight values in fragment order: a_i = (x[2i], x[2i + 1]) (wgmma_bf16_n16)
+__device__ __forceinline__ void frag_bf16(const float* x, uint32_t* a) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) a[i] = pack_bf16x2(x[2 * i], x[2 * i + 1]);
+}
+
+// acc[64 x N] (+)= A * B over one K slice (k8 TF32, k16 bf16): one MMA, or for 3xTF32 lo*B_hi, hi*B_lo, hi*B_hi.  B is
+// a K-major image at b_addr (kmajor_off, K groups lbo bytes apart), its 3xTF32 lo image lo_offset bytes further.
+// `accumulate` = 0 starts a new sum.  The caller forms the fragments and fences, commits and waits.
+template <int MODE, int N>
+__device__ __forceinline__ void mma_step(float* acc, const uint32_t* ah, const uint32_t* al, uint32_t b_addr,
+                                         uint32_t lo_offset, uint32_t lbo, uint32_t accumulate) {
+  const uint64_t dh = make_desc(b_addr, lbo, 128);
+  if constexpr (MODE == MODE_BF16) {
+    wgmma_bf16<N>(acc, ah, dh, accumulate);
+  } else if constexpr (MODE == MODE_TF32X3) {
+    wgmma_tf32<N>(acc, al, dh, accumulate);
+    wgmma_tf32<N>(acc, ah, make_desc(b_addr + lo_offset, lbo, 128), 1u);
+    wgmma_tf32<N>(acc, ah, dh, 1u);
+  } else {
+    wgmma_tf32<N>(acc, ah, dh, accumulate);
+  }
+}
+
+// Byte offset of element (k, n) in an N-column B image in the K-major canonical layout (no swizzle): core matrices of
+// 8 columns x 16 bytes of K, 8-column groups 128 B apart, K groups (4 tf32 / 8 bf16) N * 16 B apart.
+template <int MODE>
+__host__ __device__ __forceinline__ uint32_t kmajor_off(int k, int n, int N) {
+  if constexpr (MODE == MODE_BF16) return (k >> 3) * N * 16 + (n >> 3) * 128 + (n & 7) * 16 + (k & 7) * 2;
+  else return (k >> 2) * N * 16 + (n >> 3) * 128 + (n & 7) * 16 + (k & 3) * 4;
+}
+// TF32 B images whose A operand is an accumulator fragment (columns 2t, 2t + 1 of a lane in every 8-column block) store
+// K permuted inside every group of 8: slot s < 4 holds k = 2s, slot 4 + s holds k = 2s + 1.  The fragment of k8 slice
+// b is then z[4b], z[4b + 2], z[4b + 1], z[4b + 3].  (bf16 fragments already match the accumulator layout.)
+__host__ __device__ __forceinline__ int tf32_k_slot(int k) {
+  const int j = k & 7;
+  return (k & ~7) | ((j & 1) ? 4 + (j >> 1) : (j >> 1));
+}
+__host__ __device__ __forceinline__ int tf32_slot_k(int s) {
+  const int j = s & 7;
+  return (s & ~7) | (j < 4 ? 2 * j : 2 * (j - 4) + 1);
 }
 
 }  // namespace tc

@@ -4,7 +4,7 @@ ptxas serializes warpgroup MMAs (every wgmma waits for the previous one) when th
 after the wgmma fence, when too many registers are live across the asynchronous window, or when an MMA depends on a
 compiler-inserted warpgroup arrive in a divergent path.  The kernels still compute the right result, only several
 times slower, so nothing but the compiler's report shows it.  These tests read that report, and check that the
-gradient-features kernels of dn_simt.cu do not spill."""
+gradient-features kernels of dn_simt.cu and the classification-head kernels of dn_head.cu do not spill."""
 import os
 import re
 import shutil
@@ -78,4 +78,14 @@ def test_features_kernels_no_spills(tmp_path_factory):
     registers of its two CTAs per SM (with 64-bit row strides its C = 128 rotation instance spilled)."""
     per = _ptxas(tmp_path_factory, "dn_simt.cu", ("spmm_features", "features_bwd"))
     assert sum("spmm_features_blk_kernel" in k for k in per) == 4 and len(per) == 18, sorted(per)
+    _assert_no_spills(per)
+
+
+def test_head_kernels_no_spills(tmp_path_factory):
+    """Every kernel of dn_head.cu keeps its state in registers: the forward, dX and dW kernels of the fused
+    classification head on each engine (dX and dW hold two 64-float accumulators and run within a few registers of
+    the cap), its partial reduction, and the element-mean forward and backward."""
+    per = _ptxas(tmp_path_factory, "dn_head.cu", ("linear_nll", "element_mean"))
+    assert len(per) == 12, sorted(per)
+    assert sum(any(k in n for k in ("linear_nll_fwd", "linear_nll_dx", "linear_nll_dw")) for n in per) == 9, sorted(per)
     _assert_no_spills(per)

@@ -163,7 +163,7 @@ int atb(const float* A, int64_t lda, int I, const float* B, int64_t ldb, int J, 
       (int64_t)dn_sm_count() * I * J <= part_floats) {
     int P = 0;
     int rc = tc_to_basis_partial(B, A, nullptr, V, I, J, part, &P, e.passes, st);
-    if (rc == DN_OK) return launch_reduce_partials_ld(part, P, I, J, out, ld_out, accumulate, st);
+    if (rc == DN_OK) return launch_reduce_partials(part, P, nullptr, 1, I, J, out, ld_out, accumulate, st);
     if (rc != DN_ERR_UNSUPPORTED) return rc;
   }
   if (e.tc) { const int rc = note_simt_fallback("a weight gradient", I, J); if (rc) return rc; }
@@ -539,7 +539,7 @@ int dn_to_basis(const float* values, const float* basis, const float* massvec, i
   if (!partial) return DN_ERR_WORKSPACE;
   int P = 0;
   if ((rc = to_basis_partials(values, basis, massvec, V, K, C, partial, pf, &P, e, st))) return rc;
-  return launch_reduce_partials(partial, P, (int64_t)K * C, out, st);
+  return launch_reduce_partials(partial, P, nullptr, 1, K, C, out, C, 0, st);
 }
 
 int dn_from_basis(const float* values, const float* basis, const float* row_scale, int64_t V, int K, int C,
@@ -599,7 +599,7 @@ int dn_learned_time_diffusion_bwd(const float* grad_out, const float* mass, cons
     // took 4.5 ms (V = 7k); sum them first (coalesced, parallel) and hand it one
     float* red = ws.take((int64_t)K * C);
     if (!red) return DN_ERR_WORKSPACE;
-    if ((rc = launch_reduce_partials(partial, P, (int64_t)K * C, red, st))) return rc;
+    if ((rc = launch_reduce_partials(partial, P, nullptr, 1, K, C, red, C, 0, st))) return rc;
     rc = launch_spectral_bwd(red, 1, evals, time, x_spec, K, C, dS, grad_time, st);
   } else {
     rc = launch_spectral_bwd(partial, P, evals, time, x_spec, K, C, dS, grad_time, st);
@@ -668,7 +668,7 @@ int dn_to_basis_batched(const float* values, const float* basis, const float* ma
   cudaStream_t st = (cudaStream_t)stream;
   int P = 0;
   if ((rc = to_basis_partials(values, basis, mass, V, K, C, b.partial, b.pf, &P, b.e, st, batch))) return rc;
-  return launch_reduce_mesh_partials(b.partial, batch->mesh_cta_begin, batch->n_meshes, (int64_t)K * C, out, st);
+  return launch_reduce_partials(b.partial, P, batch->mesh_cta_begin, batch->n_meshes, K, C, out, C, 0, st);
 }
 
 int dn_from_basis_batched(const float* values, const float* basis, const float* row_scale, const dn_mesh_batch* batch,

@@ -26,7 +26,7 @@ __global__ void __launch_bounds__(256) hks_warp_kernel(const float* __restrict__
   for (int j = 0; j < KPL; ++j) {
     const float ev = evals[lane + 32 * j];
 #pragma unroll
-    for (int s = 0; s < 16; ++s) coef[j][s] = (s < S) ? expf(-(ev * scales[s < S ? s : 0])) : 0.f;
+    for (int s = 0; s < 16; ++s) coef[j][s] = (s < S) ? dn_heat(ev, scales[s < S ? s : 0]) : 0.f;
   }
   const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4, b1 = lane & 2;
   const int s_mine = (b4 ? 8 : 0) + (b3 ? 4 : 0) + (b2 ? 2 : 0) + (b1 ? 1 : 0);
@@ -82,7 +82,7 @@ __global__ void hks_generic_kernel(const float* __restrict__ evals, const float*
     float acc = 0.f;
     for (int k = lane; k < K; k += 32) {
       const float f = __ldg(evecs + row * K + k);
-      acc = fmaf(expf(-(evals[k] * t)), f * f, acc);
+      acc = fmaf(dn_heat(evals[k], t), f * f, acc);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);

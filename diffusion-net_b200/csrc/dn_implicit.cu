@@ -109,7 +109,7 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
   for (int q = 0; q < NC; ++q) {
     const int c = lane + 32 * q;
     cok[q] = c < C;
-    t[q] = cok[q] ? (double)fmaxf(a.time[c], 1e-8f) : 0.0;
+    t[q] = cok[q] ? (double)dn_clamp_time(a.time[c]) : 0.0;
   }
 
   // ---- init: L_vv, b, x = 0, r = b, p = z = r / d; partials of b.b and r.z
@@ -297,7 +297,7 @@ __global__ void __launch_bounds__(kThreads) implicit_cg_kernel(ImplicitArgs a) {
       a.status[1] = w;
     }
     if (!a.backward)   // the clamp write-back (reference layers.py:48-49), every CTA has read `time` by now
-      for (int c = threadIdx.x; c < C; c += kThreads) a.time[c] = fmaxf(a.time[c], 1e-8f);
+      for (int c = threadIdx.x; c < C; c += kThreads) a.time[c] = dn_clamp_time(a.time[c]);
   }
   if (unconverged) return;
 

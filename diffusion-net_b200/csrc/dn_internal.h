@@ -64,6 +64,21 @@ struct DnLayer {
   int head_n;
 };
 
+// ---- the spectral multiplier exp(-lambda max(t, 1e-8)) (layers.py:48-49, 62-64) ----
+// torch.clamp(t, min=1e-8): the diffusion time every spectral, implicit and write-back path uses
+__device__ __forceinline__ float dn_clamp_time(float t) { return fmaxf(t, 1e-8f); }
+// exp(-lambda t), the heat factor of eigenvalue lambda (also the HKS kernels' factor at scale t)
+__device__ __forceinline__ float dn_heat(float lam, float t) { return expf(-(lam * t)); }
+// one eigenpair's term of dL/dt: g * (-lambda) * e * x_spec with e = dn_heat(lambda, t), multiplied left to right
+__device__ __forceinline__ float dn_time_grad_term(float g, float lam, float e, float x_spec) {
+  return g * (-lam) * e * x_spec;
+}
+// x[0] + ... + x[(N - 1) * stride] as a pairwise tree: ((x0 + x1) + (x2 + x3)) + ... for N a power of two
+template <int N> __device__ __forceinline__ float pairwise_sum(const float* x, int stride) {
+  if constexpr (N == 1) return x[0];
+  else return pairwise_sum<N / 2>(x, stride) + pairwise_sum<N / 2>(x + (N / 2) * stride, stride);
+}
+
 struct DnRowsSrc {
   const float* ptr[DN_MAX_SRC];
   int width[DN_MAX_SRC];
@@ -89,12 +104,12 @@ int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int a
 // (x_spec) and the clamped time back.  s_trans: write S as [c][k].
 int launch_spectral_scale(const float* partial, int P, const float* evals, float* time, int K, int C,
                           float* x_spec_out, float* S_out, int clamp_writeback, cudaStream_t st);
-int launch_reduce_partials(const float* partial, int P, int64_t n, float* out, cudaStream_t st);
-// out[b] = sum over the to_basis CTAs of mesh b of a mesh batch's partials (n floats each), in CTA order
-int launch_reduce_mesh_partials(const float* partial, const int32_t* mesh_cta_begin, int n_meshes, int64_t n, float* out,
-                                cudaStream_t st);
-int launch_reduce_partials_ld(const float* partial, int P, int rows, int cols, float* out, int64_t ld_out,
-                              int accumulate, cudaStream_t st);
+// Sums split-V partials, each a [rows][cols] matrix, in partial order from 0 into out (row stride ld_out; accumulate:
+// added to what out holds).  Without mesh_cta_begin the sum runs over partials [0, P); with it (a mesh batch, n_meshes
+// meshes, P unused) mesh b sums its to_basis CTAs [mesh_cta_begin[b], mesh_cta_begin[b + 1]) into rows
+// [b * rows, (b + 1) * rows) of out.
+int launch_reduce_partials(const float* partial, int P, const int32_t* mesh_cta_begin, int n_meshes, int64_t rows,
+                           int cols, float* out, int64_t ld_out, int accumulate, cudaStream_t st);
 int launch_csr_from_coo(const int64_t* rows, const int64_t* cols, const float* vx, const float* vy,
                         int64_t nnz, int64_t V, int32_t* rowptr, int32_t* colidx, float* vals, cudaStream_t st);
 int launch_compute_hks(const float* evals, const float* evecs, const float* scales, int64_t V, int K, int S,

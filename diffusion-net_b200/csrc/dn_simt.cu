@@ -223,34 +223,19 @@ __global__ void __launch_bounds__(256) atb_partial_kernel(const float* __restric
   }
 }
 
-__global__ void reduce_partials_ld_kernel(const float* __restrict__ partial, int P, int I, int J,
-                                          float* __restrict__ out, int64_t ld_out, int accumulate) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)I * J) return;
-  float s = 0.f;
-  for (int p = 0; p < P; ++p) s += partial[(int64_t)p * I * J + idx];
-  const int i = (int)(idx / J), j = (int)(idx % J);
-  float* o = out + (int64_t)i * ld_out + j;
-  *o = accumulate ? (*o + s) : s;
-}
-
-__global__ void reduce_partials_kernel(const float* __restrict__ partial, int P, int64_t n, float* __restrict__ out) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n) return;
-  float s = 0.f;
-  for (int p = 0; p < P; ++p) s += partial[(int64_t)p * n + idx];
-  out[idx] = s;
-}
-
-// out[b][i] = sum over the CTAs p of mesh b (mesh_cta_begin) of partial[p][i], in CTA order from 0
-__global__ void reduce_mesh_partials_kernel(const float* __restrict__ partial, const int32_t* __restrict__ mesh_cta_begin,
-                                            int64_t n, float* __restrict__ out) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+// out[b * rows + i][j] (+)= sum over the partials p of mesh b of partial[p][i][j], in partial order from 0: p in
+// [mesh_cta_begin[b], mesh_cta_begin[b + 1]) with a per-mesh CTA table (grid y = meshes), [0, P) without one
+__global__ void reduce_partials_kernel(const float* __restrict__ partial, int P, const int32_t* __restrict__ mesh_cta_begin,
+                                       int64_t rows, int cols, float* __restrict__ out, int64_t ld_out, int accumulate) {
+  const int64_t n = rows * cols, idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (idx >= n) return;
+  const int p0 = mesh_cta_begin ? mesh_cta_begin[b] : 0, p1 = mesh_cta_begin ? mesh_cta_begin[b + 1] : P;
+  const float* src = partial + (int64_t)p0 * n + idx;
   float s = 0.f;
-  for (int p = mesh_cta_begin[b]; p < mesh_cta_begin[b + 1]; ++p) s += partial[(int64_t)p * n + idx];
-  out[(int64_t)b * n + idx] = s;
+  for (int q = 0; q < p1 - p0; ++q) s += src[(int64_t)q * n];
+  float* o = out + ((int64_t)b * rows + idx / cols) * ld_out + idx % cols;
+  *o = accumulate ? (*o + s) : s;
 }
 
 // partial[p][n] = sum over the rows of slice p of A[v][n].  Block (32, 8): 32 columns x 8 row lanes, combined in a
@@ -291,11 +276,10 @@ __global__ void spectral_scale_kernel(const float* __restrict__ partial, int P, 
   __syncthreads();
   if (sl != 0 || idx >= K * C) return;
   const int k = idx / C, c = idx % C;
-  const float s = (red[0][e] + red[1][e]) + (red[2][e] + red[3][e]);
-  const float t = fmaxf(time[c], 1e-8f);              // torch.clamp(t, min=1e-8)
-  const float coef = expf(-(evals[k] * t));           // torch.exp(-evals.unsqueeze(-1) * time.unsqueeze(0))
+  const float s = pairwise_sum<4>(&red[0][e], 64);
+  const float t = dn_clamp_time(time[c]);
   if (x_spec_out) x_spec_out[idx] = s;
-  S_out[idx] = coef * s;
+  S_out[idx] = dn_heat(evals[k], t) * s;
   // every thread of row k == 0 re-writes the clamped time (same value from all writers is benign)
   if (clamp_writeback && k == K - 1) {
     // last row, after all reads of time[c] by this thread; other threads read the same c only
@@ -310,16 +294,16 @@ __global__ void spectral_bwd_kernel(const float* __restrict__ partial, int P, co
                                     float* __restrict__ dS, float* __restrict__ grad_time) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float t = fmaxf(time[c], 1e-8f);
+  const float t = dn_clamp_time(time[c]);
   float dt = 0.f;
   for (int k = 0; k < K; ++k) {
     const int idx = k * C + c;
     float g = 0.f;
     for (int p = 0; p < P; ++p) g += partial[(int64_t)p * K * C + idx];
     const float lam = evals[k];
-    const float e = expf(-(lam * t));
+    const float e = dn_heat(lam, t);
     dS[idx] = e * g;
-    dt += g * (-lam) * e * x_spec[idx];
+    dt += dn_time_grad_term(g, lam, e, x_spec[idx]);
   }
   grad_time[c] += dt;
 }
@@ -333,12 +317,11 @@ __global__ void spectral_time_grad_batched_kernel(const float* __restrict__ G, c
   const int c = blockIdx.x * 32 + threadIdx.x;
   float dt = 0.f;
   if (c < C) {
-    const float t = fmaxf(time[c], 1e-8f);
+    const float t = dn_clamp_time(time[c]);
     for (int r = threadIdx.y; r < rows; r += 16) {   // r = b * K + k
       const int64_t idx = (int64_t)r * C + c;
       const float lam = evals[r];
-      const float e = expf(-(lam * t));
-      dt += G[idx] * (-lam) * e * x_spec[idx];
+      dt += dn_time_grad_term(G[idx], lam, dn_heat(lam, t), x_spec[idx]);
     }
   }
   red[threadIdx.y][threadIdx.x] = dt;
@@ -791,20 +774,32 @@ int simt_rows_gemm(const DnRowsSrc& src, const DnLayer& L, int64_t V, cudaStream
   return DN_OK;
 }
 
-int simt_atb_partial_st(const float* A, int64_t lda, int I, const float* B, int64_t ldb, int J, const float* scale,
-                        int64_t V, float* ws, int64_t ws_floats, int* P_out, cudaStream_t st) {
-  const int tiles = ((I + 63) / 64) * ((J + 63) / 64);
+// Row slices of a split-V reduction over V rows and `tiles` column tiles, each slice's partial `slice_floats` floats:
+// slices of >= 2048 rows, at most 4 CTAs per SM over the column tiles and never more than ws holds, with the rows of a
+// slice rounded up to a multiple of `round`.  Sets *P and *rps (rows per slice); DN_ERR_WORKSPACE if one slice does not fit.
+static int plan_row_slices(int64_t V, int tiles, int64_t slice_floats, int64_t ws_floats, int round, int* P_out,
+                           int64_t* rps_out) {
   int P = (int)((V + 2047) / 2048);
   const int maxP = (4 * dn_sm_count()) / tiles > 1 ? (4 * dn_sm_count()) / tiles : 1;
   if (P > maxP) P = maxP;
   if (P < 1) P = 1;
-  while ((int64_t)P * I * J > ws_floats && P > 1) --P;
-  if ((int64_t)P * I * J > ws_floats) return DN_ERR_WORKSPACE;
+  while (P * slice_floats > ws_floats && P > 1) --P;
+  if (P * slice_floats > ws_floats) return DN_ERR_WORKSPACE;
   int64_t rps = (V + P - 1) / P;
-  rps = (rps + 15) / 16 * 16;
-  if (rps < 16) rps = 16;
+  rps = (rps + round - 1) / round * round;
+  if (rps < round) rps = round;
   P = (int)((V + rps - 1) / rps);
-  if (P < 1) P = 1;
+  *P_out = P < 1 ? 1 : P;
+  *rps_out = rps;
+  return DN_OK;
+}
+
+int simt_atb_partial_st(const float* A, int64_t lda, int I, const float* B, int64_t ldb, int J, const float* scale,
+                        int64_t V, float* ws, int64_t ws_floats, int* P_out, cudaStream_t st) {
+  const int tiles = ((I + 63) / 64) * ((J + 63) / 64);
+  int P;
+  int64_t rps;
+  if (plan_row_slices(V, tiles, (int64_t)I * J, ws_floats, 16, &P, &rps)) return DN_ERR_WORKSPACE;
   atb_partial_kernel<<<dim3(tiles, P), 256, 0, st>>>(A, lda, I, B, ldb, J, scale, V, rps, ws);
   DN_LAUNCH_CHECK();
   *P_out = P;
@@ -816,10 +811,7 @@ int simt_atb(const float* A, int64_t lda, int I, const float* B, int64_t ldb, in
   int P = 0;
   int rc = simt_atb_partial_st(A, lda, I, B, ldb, J, scale, V, ws, ws_floats, &P, st);
   if (rc) return rc;
-  const int64_t n = (int64_t)I * J;
-  reduce_partials_ld_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws, P, I, J, out, ld_out, accumulate);
-  DN_LAUNCH_CHECK();
-  return DN_OK;
+  return launch_reduce_partials(ws, P, nullptr, 1, I, J, out, ld_out, accumulate, st);
 }
 
 int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int accumulate, float* ws,
@@ -828,18 +820,13 @@ int simt_colsum(const float* A, int64_t lda, int N, int64_t V, float* out, int a
     if (!accumulate) DN_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * N, st));
     return DN_OK;
   }
-  // slices of >= 2048 rows, at most 4 CTAs per SM over the column tiles and never more than ws holds
   const int tiles = (N + 31) / 32;
-  int P = (int)((V + 2047) / 2048);
-  const int maxP = (4 * dn_sm_count()) / tiles > 1 ? (4 * dn_sm_count()) / tiles : 1;
-  if (P > maxP) P = maxP;
-  while ((int64_t)P * N > ws_floats && P > 1) --P;
-  if ((int64_t)P * N > ws_floats) return DN_ERR_WORKSPACE;
-  const int64_t rps = (V + P - 1) / P;
-  P = (int)((V + rps - 1) / rps);
+  int P;
+  int64_t rps;
+  if (plan_row_slices(V, tiles, N, ws_floats, 1, &P, &rps)) return DN_ERR_WORKSPACE;
   colsum_partial_kernel<<<dim3(P, tiles), dim3(32, 8), 0, st>>>(A, lda, N, V, rps, ws);
   DN_LAUNCH_CHECK();
-  return launch_reduce_partials_ld(ws, P, 1, N, out, N, accumulate, st);
+  return launch_reduce_partials(ws, P, nullptr, 1, 1, N, out, N, accumulate, st);
 }
 
 int launch_spectral_scale(const float* partial, int P, const float* evals, float* time, int K, int C,
@@ -850,25 +837,11 @@ int launch_spectral_scale(const float* partial, int P, const float* evals, float
   return DN_OK;
 }
 
-int launch_reduce_partials(const float* partial, int P, int64_t n, float* out, cudaStream_t st) {
-  reduce_partials_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(partial, P, n, out);
-  DN_LAUNCH_CHECK();
-  return DN_OK;
-}
-
-int launch_reduce_mesh_partials(const float* partial, const int32_t* mesh_cta_begin, int n_meshes, int64_t n, float* out,
-                                cudaStream_t st) {
-  reduce_mesh_partials_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)n_meshes), 256, 0, st>>>(partial,
-                                                                                                    mesh_cta_begin, n,
-                                                                                                    out);
-  DN_LAUNCH_CHECK();
-  return DN_OK;
-}
-
-int launch_reduce_partials_ld(const float* partial, int P, int rows, int cols, float* out, int64_t ld_out,
-                              int accumulate, cudaStream_t st) {
-  reduce_partials_ld_kernel<<<(unsigned)((rows * cols + 255) / 256), 256, 0, st>>>(partial, P, rows, cols, out, ld_out,
-                                                                                   accumulate);
+int launch_reduce_partials(const float* partial, int P, const int32_t* mesh_cta_begin, int n_meshes, int64_t rows,
+                           int cols, float* out, int64_t ld_out, int accumulate, cudaStream_t st) {
+  const int64_t n = rows * cols;
+  reduce_partials_kernel<<<dim3((unsigned)((n + 255) / 256), mesh_cta_begin ? (unsigned)n_meshes : 1u), 256, 0, st>>>(
+      partial, P, mesh_cta_begin, rows, cols, out, ld_out, accumulate);
   DN_LAUNCH_CHECK();
   return DN_OK;
 }

@@ -140,9 +140,9 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackJobs jobs) {
     __syncthreads();
     if (sl != 0 || idx >= K * N) return;
     k = idx / N; n = idx % N;
-    const float sum = ((red[0][e] + red[1][e]) + (red[2][e] + red[3][e])) + ((red[4][e] + red[5][e]) + (red[6][e] + red[7][e]));
-    const float t = fmaxf(jobs.sp.time[n], 1e-8f);         // torch.clamp(t, min=1e-8)
-    w = expf(-(jobs.sp.evals[(int64_t)b * K + k] * t)) * sum;
+    const float sum = pairwise_sum<8>(&red[0][e], 33);
+    const float t = dn_clamp_time(jobs.sp.time[n]);
+    w = dn_heat(jobs.sp.evals[(int64_t)b * K + k], t) * sum;
     pack_store(J.dst + b * jobs.sp_stride, J.fmt, N, k, n, w);
     if (jobs.sp.sum_out) jobs.sp.sum_out[(int64_t)b * K * N + idx] = sum;
     // the in-place clamp of the reference, written back by mesh 0 only: every other reader of t[n] in this launch reads

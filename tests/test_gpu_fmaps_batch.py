@@ -133,8 +133,9 @@ def test_model_torch_pairs_matches_per_pair_loop():
 
 
 @pytest.mark.skipif(shutil.which(NVCC) is None and not os.path.exists(NVCC), reason="nvcc not found")
-def test_fmap_batch_kernels_do_not_spill(tmp_path):
-    """The pair-batch kernels, the single-pair kernels whose bodies they share, and the per-mesh partial reduction."""
+def test_fmap_batch_kernels_and_partial_reduction_do_not_spill(tmp_path):
+    """The pair-batch kernels, the single-pair kernels whose bodies they share, and the split-V partial reduction that
+    sums each mesh's to_basis partials (one kernel for single meshes and mesh batches)."""
     flags = [f for f in dn._lib.NVCC_FLAGS if f != "-shared"]
     expect = {"dn_fmap_batch.cu": 16, "dn_fmap.cu": 9, "dn_simt.cu": None}
     for src, count in expect.items():
@@ -149,7 +150,7 @@ def test_fmap_batch_kernels_do_not_spill(tmp_path):
                 assert nxt, (src, l)
                 pairs.append((l, nxt[0]))
         if count is None:
-            pairs = [p for p in pairs if "reduce_mesh_partials" in p[0]]
+            pairs = [p for p in pairs if "reduce_partials_kernel" in p[0]]
             assert len(pairs) == 1, src
         else:
             assert len(pairs) == count, (src, len(pairs))

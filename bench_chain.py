@@ -13,7 +13,8 @@ A call is the weight-pack launch (a few microseconds) plus the chain launch; it 
 --iters calls after --warmup calls.  The front chain is timed inside a whole block forward (CUDA events around its
 launch alone, from the profiling entry point, averaged over --iters forwards after --warmup), so it has no pack launch.  Bytes and TF32 MMA operations come from the shapes (3 MMA passes in tc3x); the
 floors are bytes over the data-sheet HBM rate and MMA operations over a TF32 rate measured in the same run with a
-large torch matmul (TF32 on).  The weight bytes each 128-row tile streams from L2 are reported as an implied L2 rate.
+large torch matmul (TF32 on).  The weight bytes each row tile streams from L2 (192-row tiles for mlp, 128-row
+tiles for the single-layer chains and the front chain with its sibling) are reported as an implied L2 rate.
 The same chains at V = 20k, whose inputs stay resident in the 50 MB L2, give the time per row without HBM latency.
 
     python bench_chain.py [--root DIR] [--iters 100] [--warmup 10] [--json FILE]
@@ -57,7 +58,9 @@ def chain_model(name, V):
         layers, rows_in, rows_out = [(3 * C, C), (C, C), (C, C)], 4 * C, C
     hbm = 4 * V * (rows_in + rows_out)
     flops = 2 * V * sum(k * n for k, n in layers) * PASSES
-    tiles = (V + 127) // 128
+    # several layers, every one 128 wide, no sibling: three consumer warpgroups share each weight stage over 192-row tiles
+    tile = 192 if name == "mlp" else 128
+    tiles = (V + tile - 1) // tile
     l2w = tiles * sum(((k + KC - 1) // KC) * KC * n * 8 for k, n in layers)
     return hbm, flops, l2w
 

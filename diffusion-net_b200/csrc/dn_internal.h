@@ -196,7 +196,7 @@ int dn_sm_count();
 // layers[i].pack_fmt), or DN_ERR_UNSUPPORTED.  Layer 0's sources are copied with 2-D TMA: each must be 16-byte
 // aligned with a row stride that is a multiple of 4 floats.
 int tc_chain_plan(const DnRowsSrc& src, DnLayer* layers, int n_layers, int passes);
-// Fused chain of up to DN_MAX_LAYERS layers over 128-row tiles; layer 0 reads `src`.  The chain was planned
+// Fused chain of up to DN_MAX_LAYERS layers over 128- or 192-row tiles; layer 0 reads `src`.  The chain was planned
 // (tc_chain_plan) on a device that runs the tensor-core kernels; layers that are not prepacked are packed into ws.
 int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers, int n_layers, int64_t V, int passes, void* ws,
                   int64_t ws_bytes, cudaStream_t st);

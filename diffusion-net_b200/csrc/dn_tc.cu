@@ -1,6 +1,6 @@
 // Hopper tensor-core engine (sm_90a): the dense contractions of the DiffusionNetBlock path.
 //
-//   tc_rows_chain       fused chain of affine layers over 128-vertex row tiles
+//   tc_rows_chain       fused chain of affine layers over 128- or 192-vertex row tiles
 //                       (from_basis [+ complex-linear P|Q], MiniMLP + skip)      layers.py:56-67,229-239
 //   tc_to_basis_partial split-V  Phi^T (M x)                                      geometry.py:572-583
 //
@@ -11,8 +11,9 @@
 // Data movement: weights are pre-split and pre-laid-out in the wgmma canonical (no-swizzle, K-major) layout by a
 // small pack kernel and streamed per 16-wide K stage with bulk TMA copies (cp.async.bulk + mbarrier complete_tx).
 // The A operand of every MMA is in registers.  For the first layer of a chain it is read from a shared-memory ring
-// that a second producer lane fills from HBM with 2-D tiled TMA copies (8 columns x 128 rows per copy), running ahead
-// of the consumers across layers and tiles; every later layer's A is the previous layer's accumulator fragment.
+// that a second producer lane fills from HBM with 2-D tiled TMA copies (8 columns x a tile's rows per copy), running
+// ahead of the consumers across layers and tiles; every later layer's A is the previous layer's accumulator fragment
+// (three-warpgroup chains: read back from the shared-memory staging buffer the epilogue wrote it to).
 #include "dn_internal.h"
 #include "dn_tc_ptx.cuh"
 #include <cuda.h>
@@ -25,44 +26,52 @@ namespace {
 using namespace tc;
 
 constexpr int KC = 16;                          // k-elements per weight stage
-constexpr int TILE_M = 128;                     // vertex rows per tile: two consumer warpgroups of 64 rows
 constexpr int W_RING_BYTES = 128 * 1024;        // weight ring: as many stages of the instantiation's width as fit
 constexpr int W_NST_MAX = 8;                    // ... but no deeper than this
-constexpr int CHAIN_THREADS = 384;              // warpgroups 0, 1: consumers; warpgroup 2: producers (two lanes)
-// first-layer activations: 16-column x 128-row fp32 stages, each two 8-column boxes of [128 rows][8 floats]
-constexpr int A_BOX_BYTES = 8 * TILE_M * 4;     // 4 KiB
-constexpr int A_STAGE_BYTES = 2 * A_BOX_BYTES;
 constexpr int A_NST_MAX = 8;                  // activation stages in flight (64 KiB per SM)
 constexpr int SMEM_OPTIN = 232448;              // sm_90 opt-in dynamic shared memory per block
 constexpr int OUT_ROWS = 64;                    // rows of an output / residual box: one consumer warpgroup's rows
 constexpr int OUT_BOX_BYTES = 8 * OUT_ROWS * 4; // 8 columns x 64 rows, [64 rows][8 floats]
+constexpr int RES_ROWS = 16;                    // three-warpgroup chains: a residual box is one consumer warp's rows
 
-// Shared memory of rows_chain_kernel<MODE, NMAX>.  Weight ring: a slot holds one K stage of an NMAX-wide layer as the
-// producer streams it (tf32x3: hi | lo images, 8 bytes per weight; tf32: hi, 4; bf16: 2), as many as fit in
-// W_RING_BYTES, at most 8.  (With 16 slots for the narrower stages, repeated bf16 mesh-batch forwards once gave
-// differing bits; the cause was not found, so the depth stays at 8.)  The TF32 chains at NMAX <= 128 also hold one output /
-// residual staging buffer per consumer warpgroup (64 rows x NMAX fp32, 32 KiB at NMAX = 128).  Where everything does
-// not fit the opt-in limit (tc3x at NMAX = 128 only), the weight ring gives up two slots and the activation ring one:
-// 6 weight and 7 activation slots measured slightly faster than 5 and 8 (DESIGN.md §5).  At NMAX = 128 / 256: tc3x 6 slots of
-// 16 KiB / 4 of 32 KiB; tc1x 8 of 8 KiB / 8 of 16 KiB; bf16 8 of 4 KiB / 8 of 8 KiB.  `set_chain_smem` and the launch
-// both read SMEM.
-template <int MODE, int NMAX>
+// Shared memory of rows_chain_kernel<MODE, NMAX, WIDE, CWG> (CWG consumer warpgroups of 64 rows: a tile is 64 CWG
+// rows).  Weight ring: a slot holds one K stage of an NMAX-wide layer as the producer streams it (tf32x3: hi | lo
+// images, 8 bytes per weight; tf32: hi, 4; bf16: 2), as many as fit in W_RING_BYTES, at most 8.  (With 16 slots for
+// the narrower stages, repeated bf16 mesh-batch forwards once gave differing bits; the cause was not found, so the
+// depth stays at 8.)  The first layer's activations: 16-column x (64 CWG)-row fp32 stages, each two 8-column boxes of
+// [64 CWG rows][8 floats].  The TF32 chains at NMAX <= 128 also hold one output / residual staging buffer per consumer
+// warpgroup (64 rows x NMAX fp32, 32 KiB at NMAX = 128).  Two consumer warpgroups: where everything does not fit the
+// opt-in limit (tc3x at NMAX = 128 only), the weight ring gives up two slots and the activation ring one: 6 weight and
+// 7 activation slots measured slightly faster than 5 and 8 (DESIGN.md §5).  At NMAX = 128 / 256: tc3x 6 slots of
+// 16 KiB / 4 of 32 KiB; tc1x 8 of 8 KiB / 8 of 16 KiB; bf16 8 of 4 KiB / 8 of 8 KiB.  Three consumer warpgroups (full-
+// width TF32 at NMAX = 128): 64 KiB of weight slots (tc3x 4 of 16 KiB, tc1x 8 of 8 KiB), 5 activation slots of
+// 12 KiB and 96 KiB of staging.  `set_chain_smem` and the launch both read SMEM.
+template <int MODE, int NMAX, int CWG = 2>
 struct ChainRing {
+  static_assert(CWG == 2 || (CWG == 3 && NMAX == 128 && MODE != MODE_BF16), "rows_chain_kernel: unsupported variant");
+  static constexpr int TILE = 64 * CWG;                  // vertex rows per tile
+  static constexpr int THREADS = 128 * CWG + 128;        // consumer warpgroups, then the producer warpgroup
+  static constexpr int A_BOX = 8 * TILE * 4;
+  static constexpr int A_STAGE = 2 * A_BOX;
   static constexpr int STAGE = KC * NMAX * (MODE == MODE_TF32X3 ? 8 : MODE == MODE_TF32 ? 4 : 2);
-  static constexpr int NST_FULL = W_RING_BYTES / STAGE < W_NST_MAX ? W_RING_BYTES / STAGE : W_NST_MAX;
+  static constexpr int W_BYTES = CWG == 2 ? W_RING_BYTES : W_RING_BYTES / 2;
+  static constexpr int NST_FULL = W_BYTES / STAGE < W_NST_MAX ? W_BYTES / STAGE : W_NST_MAX;
+  static constexpr int A_NST_FULL = CWG == 2 ? A_NST_MAX : 5;
   // (bf16 stores from registers: with the staging buffer two identical bf16 calls at V = 200k + 37 gave different
   // bits, and the cause was not found)
-  static constexpr int STG = NMAX <= 128 && MODE != MODE_BF16 ? 2 * OUT_ROWS * NMAX * 4 : 0;
+  static constexpr int STG = NMAX <= 128 && MODE != MODE_BF16 ? CWG * OUT_ROWS * NMAX * 4 : 0;
   // every layer's bias, staged once per CTA (NMAX = 256 chains run a single layer)
   static constexpr int BIAS = (NMAX <= 128 ? DN_MAX_LAYERS : 1) * NMAX * 4;
-  static constexpr int bars(int nst, int anst) { return 8 * (2 * nst + 2 * anst + 2); }   // full / empty, residual
-  static constexpr int bytes(int nst, int anst) { return nst * STAGE + anst * A_STAGE_BYTES + STG + BIAS + bars(nst, anst); }
-  static constexpr bool kFull = bytes(NST_FULL, A_NST_MAX) <= SMEM_OPTIN;
+  static constexpr int RBARS = CWG;   // residual barriers: one per consumer warpgroup
+  static constexpr int bars(int nst, int anst) { return 8 * (2 * nst + 2 * anst + RBARS); }   // full / empty, residual
+  static constexpr int bytes(int nst, int anst) { return nst * STAGE + anst * A_STAGE + STG + BIAS + bars(nst, anst); }
+  static constexpr bool kFull = bytes(NST_FULL, A_NST_FULL) <= SMEM_OPTIN;
   static constexpr int NST = kFull ? NST_FULL : NST_FULL - 2;
-  static constexpr int A_NST = kFull ? A_NST_MAX : A_NST_MAX - 1;
+  static constexpr int A_NST = kFull ? A_NST_FULL : A_NST_FULL - 1;
   static constexpr int BARS = bars(NST, A_NST);
   static constexpr int SMEM = bytes(NST, A_NST);
   static_assert(SMEM <= SMEM_OPTIN, "rows_chain_kernel: shared memory over the opt-in limit");
+  static_assert(CWG == 2 || kFull, "rows_chain_kernel: the three-warpgroup rings are sized to fit");
 };
 
 // bytes of one packed K stage of an N-wide layer: tf32 hi image (KC * N * 4) then lo image; bf16 uses the first quarter
@@ -228,13 +237,26 @@ static_assert(sizeof(HcParams) <= 4096, "HcParams must fit the 4 KiB kernel para
 // written again (an epilogue, or a residual load) the elected lane waits until the previous stores have read it; and in
 // the CTA's last tile it waits for its stores to complete before it goes on.  NMAX = 256 chains (their staging tile
 // would not fit next to the rings) and the bf16 engine (ChainRing::STG) store from registers.
-template <int MODE, int NMAX, bool WIDE>
-__global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __grid_constant__ HcParams p) {
+// CWG = 3 (full-width TF32 chains at NMAX = 128 without a sibling layer or tile groups): three consumer warpgroups
+// share each weight stage, so a tile is 192 rows, a stage feeds 18 MMAs instead of 12 and the weights cross L2 a third
+// less often; warpgroup 3 holds the producers.  The registers (160 per consumer) do not hold the activations as well:
+// every layer's result goes to the staging buffer, and the next layer forms its A fragments there with the reads
+// layer 0 uses on the activation ring.  A lane reads and writes only its own (row, column) pairs there (the accumulator
+// layout is the A-fragment layout), so no barrier separates an epilogue from the next layer's reads.  A layer's
+// residual can then no longer come into the buffer before its MMAs: each warp, once it has formed stage c's fragments,
+// loads its own 16 rows of residual columns 16c .. 16c + 15 by TMA into the two boxes it has just read, on its
+// warpgroup's residual mbarrier.  The head reads the finished rows from the buffer.
+template <int MODE, int NMAX, bool WIDE, int CWG = 2>
+__global__ void __launch_bounds__(ChainRing<MODE, NMAX, CWG>::THREADS, 1) rows_chain_kernel(const __grid_constant__ HcParams p) {
   constexpr bool kChain = NMAX <= 128;
-  constexpr bool kStage = ChainRing<MODE, NMAX>::STG > 0;   // outputs and residuals through shared memory
+  constexpr bool kStage = ChainRing<MODE, NMAX, CWG>::STG > 0;   // outputs and residuals through shared memory
+  constexpr bool kSmemAct = CWG == 3;   // later layers' activations and the residual in the staging buffer
+  static_assert(!kSmemAct || (WIDE && kStage), "rows_chain_kernel: three consumer warpgroups need full-width staging");
   constexpr int NB = NMAX / 16;
-  using Ring = ChainRing<MODE, NMAX>;
+  using Ring = ChainRing<MODE, NMAX, CWG>;
   constexpr int NST = Ring::NST, STAGE_BYTES = Ring::STAGE, A_NST = Ring::A_NST;
+  constexpr int TILE = Ring::TILE, A_BOX_BYTES = Ring::A_BOX, A_STAGE_BYTES = Ring::A_STAGE;
+  constexpr int NCW = 4 * CWG;   // consumer warps: arrivals per ring slot
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* aring = smem + NST * STAGE_BYTES;
   uint8_t* stage_out = aring + A_NST * A_STAGE_BYTES;
@@ -245,18 +267,18 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
   const uint32_t rfull = smem_u32(bars + 2 * NST + 2 * A_NST);   // residual loaded, one per consumer warpgroup
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NST; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 8); }
-    for (int i = 0; i < A_NST; ++i) { mbar_init(afull + 8 * i, 1); mbar_init(aempty + 8 * i, 8); }
-    for (int i = 0; i < 2; ++i) mbar_init(rfull + 8 * i, 1);
+    for (int i = 0; i < NST; ++i) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, NCW); }
+    for (int i = 0; i < A_NST; ++i) { mbar_init(afull + 8 * i, 1); mbar_init(aempty + 8 * i, NCW); }
+    for (int i = 0; i < Ring::RBARS; ++i) mbar_init(rfull + 8 * i, CWG == 2 ? 1 : 4);
     fence_barrier_init();
   }
   __syncthreads();
   const int L = p.n_layers;
-  const int64_t ntiles = (p.V + TILE_M - 1) / TILE_M;
+  const int64_t ntiles = (p.V + TILE - 1) / TILE;
 
-  if (warp >= 8) {
-    setmaxnreg_dec<40>();
-    if (warp == 9 && lane == 0) {
+  if (warp >= NCW) {
+    setmaxnreg_dec<CWG == 2 ? 40 : 24>();
+    if (warp == NCW + 1 && lane == 0) {
       // ===================== layer-0 activation producer =====================
       const int K0 = p.layer[0].K, nst0 = (K0 + KC - 1) / KC;
       uint32_t s = 0, ph = 0;
@@ -269,13 +291,13 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
             int kc = c * KC + 8 * h, sidx = 0;
             while (sidx + 1 < p.src.nsrc && kc >= p.src.width[sidx]) { kc -= p.src.width[sidx]; ++sidx; }
             tma_tile_2d_g2s(smem_u32(aring + s * A_STAGE_BYTES + h * A_BOX_BYTES), &p.amap[sidx], kc,
-                            (int)(tile * TILE_M), afull + 8 * s);
+                            (int)(tile * TILE), afull + 8 * s);
           }
           if (++s == A_NST) { s = 0; ph ^= 1; }
         }
     }
     // ===================== weight producer =====================
-    if (warp == 8 && lane == 0) {
+    if (warp == NCW && lane == 0) {
       uint32_t s = 0, ph = 0;
       for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
         for (int l = 0; l < L; ++l) {
@@ -297,16 +319,16 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
   }
 
   // ===================== consumers =====================
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<CWG == 2 ? 232 : 160>();
   // The biases go to shared memory once per CTA.  Read from global memory in the epilogue they were one round trip per
   // column block (the epilogue's loads are kept in series, see below), and the residual and output traffic of the
   // tiles evicts them from L1: the two hidden-layer epilogues of the MiniMLP took about 10,000 cycles each that way.
   for (int l = 0; l < L; ++l) {
     const HcLayer& Lr = p.layer[l];
     if (!Lr.bias) continue;
-    for (int n = threadIdx.x; n < Lr.N; n += 256) sbias[l * NMAX + n] = __ldg(Lr.bias + n);
+    for (int n = threadIdx.x; n < Lr.N; n += 128 * CWG) sbias[l * NMAX + n] = __ldg(Lr.bias + n);
   }
-  named_bar_sync(1, 256);                     // the consumers' copies are done (the producers do not take part)
+  named_bar_sync(1, 128 * CWG);               // the consumers' copies are done (the producers do not take part)
   const int g = lane >> 2, t = lane & 3;
   const int rloc = (warp >> 2) * 64 + (warp & 3) * 16 + g;
   // output / residual staging (NMAX <= 128)
@@ -315,20 +337,47 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
   // box b (columns 8b .. 8b+7, [64 rows][8 floats]) of this warpgroup's buffer
   auto stg_box = [&](int b) { return reinterpret_cast<float*>(stage_out) + (wg * NMAX + 8 * b) * OUT_ROWS; };
   float acc[NB * 8];
-  float act[kChain ? NB * 8 : 1];
+  float act[kChain && !kSmemAct ? NB * 8 : 1];
   uint32_t s = 0, ph = 0, as = 0, aph = 0, rph = 0;
 
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int64_t r0 = tile * TILE_M + rloc, r1 = r0 + 8;
+    const int64_t r0 = tile * TILE + rloc, r1 = r0 + 8;
     const bool ok0 = r0 < p.V, ok1 = r1 < p.V;
-    const int row0 = (int)(tile * TILE_M) + wg * OUT_ROWS;   // this warpgroup's first row (V < 2^31 - 256)
+    const int row0 = (int)(tile * TILE) + wg * OUT_ROWS;   // this warpgroup's first row (V < 2^31 - 256)
     for (int l = 0; l < L; ++l) {
       const HcLayer& Lr = p.layer[l];
       const int N = WIDE ? NMAX : Lr.N, nb = N / 16;
       const int K = (WIDE && l > 0) ? NMAX : Lr.K, nst = (K + KC - 1) / KC;
       const uint32_t lbo = (uint32_t)N * 16;
       int prev = -1;
-      if constexpr (kStage) {
+      // kSmemAct: the stores of the layer before (in the previous tile, for layer 0) read the buffer this layer's
+      // residual loads and epilogue write
+      const bool pred_stored = kSmemAct && p.layer[l > 0 ? l - 1 : L - 1].out != nullptr;
+      // kSmemAct: this warp's residual columns 16c .. 16c + 15 come into boxes 2c, 2c + 1 of its 16 rows, once every
+      // lane's reads of them (generic proxy) are ordered before the async-proxy write; a warp wholly past V loads
+      // nothing (its rows are not stored).  The warpgroup's residual barrier takes one arrival per warp, each with
+      // its own bytes.
+      auto residual_load = [&](int c) {
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0) {
+          const int wrow0 = row0 + (warp & 3) * RES_ROWS;
+          if (c == 0) {
+            if (wrow0 < p.V) mbar_arrive_expect_tx(rfull + 8 * wg, (uint32_t)(N / 8 * RES_ROWS * 32));
+            else mbar_arrive(rfull + 8 * wg);
+          }
+          if (wrow0 < p.V)
+            for (int h = 0; h < 2; ++h)
+              tma_tile_2d_g2s(smem_u32(stg_box(2 * c + h) + (warp & 3) * RES_ROWS * 8), &p.rmap[l], 16 * c + 8 * h,
+                              wrow0, rfull + 8 * wg);
+        }
+      };
+      if constexpr (kSmemAct) {
+        if (pred_stored && Lr.residual) {
+          if (elected) bulk_wait_read<0>();
+          named_bar_sync(2 + wg, 128);
+        }
+      } else if constexpr (kStage) {
         // the residual rows come into the staging buffer while the layer's MMAs run, once the buffer's last stores
         // have read it (issued a layer or more ago); a warpgroup wholly past V loads nothing (its rows are not stored)
         if (Lr.residual && elected) {
@@ -435,6 +484,23 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
           __syncwarp();
           if (lane == 0) mbar_arrive(aempty + 8 * as);
           if (++as == A_NST) { as = 0; aph ^= 1; }
+          if constexpr (kSmemAct) {
+            if (Lr.residual && c < nb) residual_load(c);
+          }
+        }
+        if constexpr (kSmemAct) {
+          if (Lr.residual)
+            for (int c = nst; c < nb; ++c) residual_load(c);   // layer 0 narrower than its output
+        }
+      } else if constexpr (kSmemAct) {
+#pragma unroll
+        for (int c = 0; c < NB; ++c) {
+          const float* a = stg_box(2 * c) + ((warp & 3) * 16 + g) * 8 + 2 * t;
+          const float2 q[4] = {*reinterpret_cast<const float2*>(a), *reinterpret_cast<const float2*>(a + 64),
+                               *reinterpret_cast<const float2*>(a + 8 * OUT_ROWS),
+                               *reinterpret_cast<const float2*>(a + 8 * OUT_ROWS + 64)};
+          stage(c, q, true);
+          if (Lr.residual) residual_load(c);
         }
       } else if constexpr (kChain) {
 #pragma unroll
@@ -462,11 +528,12 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
       if constexpr (kStage) {
         if (Lr.residual) {
           // the residual is in the staging buffer.  The elected lane waits and the barrier passes the news on: every
-          // lane of the warpgroup spinning here made ptxas spill and serialize the MMAs
+          // lane of the warpgroup spinning here made ptxas spill and serialize the MMAs (kSmemAct: so did a per-warp
+          // barrier, with lane 0 or every lane of the warp waiting on it)
           if (elected) mbar_wait(rfull + 8 * wg, rph);
           rph ^= 1;
           named_bar_sync(2 + wg, 128);
-        } else if (Lr.out) {
+        } else if (kSmemAct ? pred_stored : Lr.out != nullptr) {
           if (elected) bulk_wait_read<0>();  // the buffer's last stores have read it
           named_bar_sync(2 + wg, 128);
         }
@@ -512,7 +579,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
               v0.x = fmaf(Lr.res_scale, ra.x, v0.x); v0.y = fmaf(Lr.res_scale, ra.y, v0.y);
               v1.x = fmaf(Lr.res_scale, rb.x, v1.x); v1.y = fmaf(Lr.res_scale, rb.y, v1.y);
             }
-            if (Lr.out) {
+            if (kSmemAct || Lr.out) {
               *reinterpret_cast<float2*>(so) = v0;
               *reinterpret_cast<float2*>(so + 64) = v1;
             }
@@ -532,7 +599,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
               if (ok1) *reinterpret_cast<float2*>(Lr.out + r1 * Lr.ld_out + col) = v1;
             }
           }
-          if constexpr (kChain) {
+          if constexpr (kChain && !kSmemAct) {
             if (!keep_act) {
               act[8 * j + 4 * h] = v0.x; act[8 * j + 4 * h + 1] = v0.y;
               act[8 * j + 4 * h + 2] = v1.x; act[8 * j + 4 * h + 3] = v1.y;
@@ -550,7 +617,8 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
         }
       }
       if constexpr (kStage) {
-        if (Lr.out || Lr.residual) {
+        // (kSmemAct: the next residual loads are ordered per warp behind the next layer's reads)
+        if (Lr.out || (!kSmemAct && Lr.residual)) {
           // this warpgroup's reads and writes of the buffer come before the async proxy's next access to it
           fence_proxy_async();
           named_bar_sync(2 + wg, 128);
@@ -585,10 +653,17 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) rows_chain_kernel(const __gr
               if (j >= nb) break;
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
-                const float* v = act + 8 * j + 4 * h;
                 const float2 w = __ldg(reinterpret_cast<const float2*>(p.head_w + (int64_t)o * N + 16 * j + 8 * h + 2 * t));
-                a0 = fmaf(w.y, v[1], fmaf(w.x, v[0], a0));
-                a1 = fmaf(w.y, v[3], fmaf(w.x, v[2], a1));
+                if constexpr (kSmemAct) {
+                  const float* so = stg_box(2 * j + h) + ((warp & 3) * 16 + g) * 8 + 2 * t;
+                  const float2 u0 = *reinterpret_cast<const float2*>(so), u1 = *reinterpret_cast<const float2*>(so + 64);
+                  a0 = fmaf(w.y, u0.y, fmaf(w.x, u0.x, a0));
+                  a1 = fmaf(w.y, u1.y, fmaf(w.x, u1.x, a1));
+                } else {
+                  const float* v = act + 8 * j + 4 * h;
+                  a0 = fmaf(w.y, v[1], fmaf(w.x, v[0], a0));
+                  a1 = fmaf(w.y, v[3], fmaf(w.x, v[2], a1));
+                }
               }
             }
             head_store(o, a0, a1);
@@ -824,8 +899,11 @@ void launch_to_basis(int nbc, int grid, const TcToBasisParams& p, cudaStream_t s
 template <int MODE>
 bool set_chain_smem() {
   constexpr int s128 = ChainRing<MODE, 128>::SMEM, s256 = ChainRing<MODE, 256>::SMEM;
-  return set_smem(rows_chain_kernel<MODE, 128, false>, s128) && set_smem(rows_chain_kernel<MODE, 128, true>, s128) &&
-         set_smem(rows_chain_kernel<MODE, 256, false>, s256) && set_smem(rows_chain_kernel<MODE, 256, true>, s256);
+  bool ok = set_smem(rows_chain_kernel<MODE, 128, false>, s128) && set_smem(rows_chain_kernel<MODE, 128, true>, s128) &&
+            set_smem(rows_chain_kernel<MODE, 256, false>, s256) && set_smem(rows_chain_kernel<MODE, 256, true>, s256);
+  if constexpr (MODE != MODE_BF16)
+    ok = ok && set_smem(rows_chain_kernel<MODE, 128, true, 3>, ChainRing<MODE, 128, 3>::SMEM);
+  return ok;
 }
 
 // cuTensorMapEncodeTiled from the driver the runtime already loaded (no link dependency on libcuda); null if absent
@@ -978,16 +1056,24 @@ int tc_pack_layers(DnLayer* layers, int n_layers, void* ws, int64_t ws_bytes, co
   return DN_OK;
 }
 
-// wide: every layer is exactly 128 wide, or the single layer is 256 wide (full-width MMAs)
+// wide: every layer is exactly 128 wide, or the single layer is 256 wide (full-width MMAs); cwg: consumer warpgroups
 template <int MODE>
-static void launch_chain(const HcParams& p, int nmax, bool wide, int grid, cudaStream_t st) {
-  constexpr int s128 = ChainRing<MODE, 128>::SMEM, s256 = ChainRing<MODE, 256>::SMEM;
+static void launch_chain(const HcParams& p, int nmax, bool wide, int cwg, int grid, cudaStream_t st) {
+  using R128 = ChainRing<MODE, 128>;
+  using R256 = ChainRing<MODE, 256>;
+  if constexpr (MODE != MODE_BF16) {
+    if (cwg == 3) {
+      using R3 = ChainRing<MODE, 128, 3>;
+      rows_chain_kernel<MODE, 128, true, 3><<<grid, R3::THREADS, R3::SMEM, st>>>(p);
+      return;
+    }
+  }
   if (nmax <= 128) {
-    if (wide) rows_chain_kernel<MODE, 128, true><<<grid, CHAIN_THREADS, s128, st>>>(p);
-    else rows_chain_kernel<MODE, 128, false><<<grid, CHAIN_THREADS, s128, st>>>(p);
+    if (wide) rows_chain_kernel<MODE, 128, true><<<grid, R128::THREADS, R128::SMEM, st>>>(p);
+    else rows_chain_kernel<MODE, 128, false><<<grid, R128::THREADS, R128::SMEM, st>>>(p);
   } else {
-    if (wide) rows_chain_kernel<MODE, 256, true><<<grid, CHAIN_THREADS, s256, st>>>(p);
-    else rows_chain_kernel<MODE, 256, false><<<grid, CHAIN_THREADS, s256, st>>>(p);
+    if (wide) rows_chain_kernel<MODE, 256, true><<<grid, R256::THREADS, R256::SMEM, st>>>(p);
+    else rows_chain_kernel<MODE, 256, false><<<grid, R256::THREADS, R256::SMEM, st>>>(p);
   }
 }
 
@@ -1016,12 +1102,8 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
   p.V = V;
   p.tile_group = layers[0].tile_group;
   p.group_stride = layers[0].group_stride;
-  // tensor maps (encoded on the host; a captured graph keeps them with the launch): fp32 [V rows][width], row stride
-  // ld, 8-column boxes; one per source of layer 0
-  for (int s = 0; s < src.nsrc; ++s)
-    if (!encode_tensor_map_f32(&p.amap[s], src.ptr[s], V, src.width[s], src.ld[s], 8, TILE_M, false))
-      return DN_ERR_UNSUPPORTED;
   int nmax = 0, nmin = 1 << 30;
+  bool sibling = false;
   for (int l = 0; l < n_layers; ++l) {
     const DnLayer& L = layers[l];
     HcLayer& T = p.layer[l];
@@ -1030,26 +1112,43 @@ int tc_rows_chain(const DnRowsSrc& src, const DnLayer* layers_in, int n_layers, 
     T.K = L.K; T.N = L.N; T.relu = L.relu; T.sibling = L.sibling;
     if (L.N > nmax) nmax = L.N;
     if (L.N < nmin) nmin = L.N;
+    sibling = sibling || L.sibling;
   }
-  // the TF32 chains at NMAX <= 128 store each layer's out and load its residual through shared memory: one map each, 8 x 64 boxes
+  const bool wide = nmin == nmax && (nmax == 128 || nmax == 256);
+  // Full-width TF32 chains of several layers at 128 without a sibling (which reads a layer's input after its epilogue)
+  // or per-tile weight groups run on three consumer warpgroups over 192-row tiles when the 128-row tiles would not fit
+  // in one wave on the SMs; everything else on two over 128-row tiles.  In one wave every CTA runs one tile either way,
+  // and the 192-row tiles only put each tile's MMAs on fewer SMs: the training forward's MiniMLP at V = 7056 (56 tiles
+  // of 128 rows, 37 of 192) made fwd_bwd slower on three.  (A build that also sent single-layer chains to three, before
+  // this rule, was slower on fwd_bwd too; single-layer chains were not measured under the rule.)
+  const int sms = dn_sm_count();
+  const int cwg = !bf16 && wide && nmax == 128 && n_layers > 1 && !sibling && !p.tile_group && (V + 127) / 128 > sms
+                      ? 3 : 2;
+  const int tile_rows = 64 * cwg;
+  // tensor maps (encoded on the host; a captured graph keeps them with the launch): fp32 [V rows][width], row stride
+  // ld, 8-column boxes of a tile's rows; one per source of layer 0
+  for (int s = 0; s < src.nsrc; ++s)
+    if (!encode_tensor_map_f32(&p.amap[s], src.ptr[s], V, src.width[s], src.ld[s], 8, tile_rows, false))
+      return DN_ERR_UNSUPPORTED;
+  // the TF32 chains at NMAX <= 128 store each layer's out and load its residual through shared memory: one map each,
+  // 8 x 64 boxes (residuals of the three-warpgroup chains: 8 x 16, one warp's rows)
   // (a column slice such as P or Q of [P|Q] is its own map: base at the slice, width N, the buffer's row stride)
   if (nmax <= 128 && !bf16)
     for (int l = 0; l < n_layers; ++l) {
       const DnLayer& L = layers[l];
       if (L.out && !encode_tensor_map_f32(&p.omap[l], L.out, V, L.N, L.ld_out, 8, OUT_ROWS, false))
         return DN_ERR_UNSUPPORTED;
-      if (L.residual && !encode_tensor_map_f32(&p.rmap[l], L.residual, V, L.N, L.ld_res, 8, OUT_ROWS, false))
+      if (L.residual &&
+          !encode_tensor_map_f32(&p.rmap[l], L.residual, V, L.N, L.ld_res, 8, cwg == 3 ? RES_ROWS : OUT_ROWS, false))
         return DN_ERR_UNSUPPORTED;
     }
-  const bool wide = nmin == nmax && (nmax == 128 || nmax == 256);
   const DnLayer& Ll = layers[n_layers - 1];
   p.head_w = Ll.head_w; p.head_b = Ll.head_b; p.head_out = Ll.head_out; p.ld_head_out = Ll.ld_head_out; p.head_n = Ll.head_n;
-  const int64_t ntiles = (V + TILE_M - 1) / TILE_M;
-  const int sms = dn_sm_count();
+  const int64_t ntiles = (V + tile_rows - 1) / tile_rows;
   const int grid = (int)(ntiles < sms ? ntiles : sms);
-  if (bf16) launch_chain<MODE_BF16>(p, nmax, wide, grid, st);
-  else if (passes == 3) launch_chain<MODE_TF32X3>(p, nmax, wide, grid, st);
-  else launch_chain<MODE_TF32>(p, nmax, wide, grid, st);
+  if (bf16) launch_chain<MODE_BF16>(p, nmax, wide, cwg, grid, st);
+  else if (passes == 3) launch_chain<MODE_TF32X3>(p, nmax, wide, cwg, grid, st);
+  else launch_chain<MODE_TF32>(p, nmax, wide, cwg, grid, st);
   DN_LAUNCH_CHECK();
   return DN_OK;
 }

@@ -151,6 +151,11 @@ SIGNATURES = {
     "dn_linear_nll_bwd": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _P, _L, _I, _P]),
     "dn_element_mean_fwd": (_I, [_P, _L, _I, _P, _L, _I, _P, _P]),
     "dn_element_mean_bwd": (_I, [_P, _L, _I, _P, _P, _L, _I, _P, _P]),
+    "dn_linear_nll_ls_fwd": (_I, [_P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _I, _P, C.c_float]),
+    "dn_linear_nll_ls_bwd": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _P, _L, _I, _P, C.c_float]),
+    "dn_global_mean_workspace_bytes": (_L, [_L, _I]),
+    "dn_global_mean_fwd": (_I, [_P, _P, _L, _I, _P, _P, _P, _I, _P, _P, _P, _L, _P]),
+    "dn_global_mean_bwd": (_I, [_P, _P, _P, _L, _I, _P, _P, _P, _I, _P, _P]),
 }
 
 _lib = None

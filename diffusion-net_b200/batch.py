@@ -86,6 +86,8 @@ class MeshBatch:
         self._cta_begin = torch.from_numpy(cta_begin).to(dev)
         self.desc = _lib.dn_mesh_batch(B, n_ctas, self._tile_mesh.data_ptr(), self._tb_rows.data_ptr(),
                                        self._cta_begin.data_ptr())
+        # one row segment per mesh, for the mass-weighted mean of outputs_at 'global_mean' (ops.global_mean_pool)
+        self.segments = ops.Segments(self.row_begin[:-1], self.n_rows, V, dev)
         # elements for outputs_at 'faces' / 'edges', vertex ids offset to batch rows (None unless every item has them)
         self.faces, self.edges, self._elem_counts = None, None, {}
         for name in ("faces", "edges"):

@@ -1111,6 +1111,18 @@ int linear_nll_check(const float* x, const float* weight, const int64_t* labels,
   if (rc != DN_OK) return rc;
   return e->tc ? DN_OK : DN_ERR_UNSUPPORTED;   // tensor cores only: the SIMT engine composes mlp + log_softmax instead
 }
+
+int smoothing_check(float s, int n_class) {
+  if (!(s >= 0.f && s <= 1.f) || (s > 0.f && n_class < 2)) return DN_ERR_INVALID_ARGUMENT;
+  return DN_OK;
+}
+
+int global_mean_check(const float* x, const float* mass, int64_t V, int C, const int32_t* begin, const int32_t* rows,
+                      const int32_t* tile_seg, int n_seg) {
+  if (!x || !mass || !begin || !rows || !tile_seg || V < 1 || n_seg < 1 || C < 1) return DN_ERR_INVALID_ARGUMENT;
+  if (C % 4 != 0 || C > 256 || V >= (1ll << 31) || (reinterpret_cast<uintptr_t>(x) & 15)) return DN_ERR_UNSUPPORTED;
+  return DN_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1127,8 +1139,20 @@ int dn_linear_nll_fwd(const float* x, const float* weight, const float* bias, co
   int rc = linear_nll_check(x, weight, labels, R, C, n_class, engine, &e);
   if (rc != DN_OK) return rc;
   if (!nll || !argmax || !lse) return DN_ERR_INVALID_ARGUMENT;
-  return launch_linear_nll_fwd(x, weight, bias, labels, R, C, n_class, ignore_index, nll, argmax, lse, e.passes,
+  return launch_linear_nll_fwd(x, weight, bias, labels, R, C, n_class, ignore_index, 0.f, nll, argmax, lse, e.passes,
                                (cudaStream_t)stream);
+}
+
+int dn_linear_nll_ls_fwd(const float* x, const float* weight, const float* bias, const int64_t* labels, int64_t R,
+                         int C, int n_class, int64_t ignore_index, float* nll, int64_t* argmax, float* lse, int engine,
+                         dn_stream_t stream, float label_smoothing) {
+  Engine e;
+  int rc = linear_nll_check(x, weight, labels, R, C, n_class, engine, &e);
+  if (rc == DN_OK) rc = smoothing_check(label_smoothing, n_class);
+  if (rc != DN_OK) return rc;
+  if (!nll || !argmax || !lse) return DN_ERR_INVALID_ARGUMENT;
+  return launch_linear_nll_fwd(x, weight, bias, labels, R, C, n_class, ignore_index, label_smoothing, nll, argmax, lse,
+                               e.passes, (cudaStream_t)stream);
 }
 
 int dn_linear_nll_bwd(const float* x, const float* weight, const float* bias, const int64_t* labels, const float* lse,
@@ -1140,8 +1164,23 @@ int dn_linear_nll_bwd(const float* x, const float* weight, const float* bias, co
   if (rc != DN_OK) return rc;
   if (!lse || !grad_nll || !grad_x || !grad_weight || (bias && !grad_bias)) return DN_ERR_INVALID_ARGUMENT;
   if (!workspace || ws_bytes < head_ws_bytes(R, C, n_class)) return DN_ERR_WORKSPACE;
-  return launch_linear_nll_bwd(x, weight, bias, labels, lse, grad_nll, R, C, n_class, ignore_index, grad_x, grad_weight,
-                               bias ? grad_bias : nullptr, workspace, e.passes, (cudaStream_t)stream);
+  return launch_linear_nll_bwd(x, weight, bias, labels, lse, grad_nll, R, C, n_class, ignore_index, 0.f, grad_x,
+                               grad_weight, bias ? grad_bias : nullptr, workspace, e.passes, (cudaStream_t)stream);
+}
+
+int dn_linear_nll_ls_bwd(const float* x, const float* weight, const float* bias, const int64_t* labels,
+                         const float* lse, const float* grad_nll, int64_t R, int C, int n_class, int64_t ignore_index,
+                         float* grad_x, float* grad_weight, float* grad_bias, void* workspace, int64_t ws_bytes,
+                         int engine, dn_stream_t stream, float label_smoothing) {
+  Engine e;
+  int rc = linear_nll_check(x, weight, labels, R, C, n_class, engine, &e);
+  if (rc == DN_OK) rc = smoothing_check(label_smoothing, n_class);
+  if (rc != DN_OK) return rc;
+  if (!lse || !grad_nll || !grad_x || !grad_weight || (bias && !grad_bias)) return DN_ERR_INVALID_ARGUMENT;
+  if (!workspace || ws_bytes < head_ws_bytes(R, C, n_class)) return DN_ERR_WORKSPACE;
+  return launch_linear_nll_bwd(x, weight, bias, labels, lse, grad_nll, R, C, n_class, ignore_index, label_smoothing,
+                               grad_x, grad_weight, bias ? grad_bias : nullptr, workspace, e.passes,
+                               (cudaStream_t)stream);
 }
 
 int dn_element_mean_fwd(const float* x, int64_t V, int C, const int64_t* elems, int64_t E, int k, float* out,
@@ -1157,6 +1196,35 @@ int dn_element_mean_bwd(const float* grad_out, int64_t E, int C, const int32_t* 
     return DN_ERR_INVALID_ARGUMENT;
   if (E * k >= (1ll << 31)) return DN_ERR_UNSUPPORTED;
   return launch_element_mean_bwd(grad_out, C, rowptr, entries, V, k, grad_x, (cudaStream_t)stream);
+}
+
+int64_t dn_global_mean_workspace_bytes(int64_t V, int C) {
+  if (V < 1 || C < 1) return 0;
+  return pool_ws_bytes(V, C);
+}
+
+int dn_global_mean_fwd(const float* x, const float* mass, int64_t V, int C, const int32_t* seg_begin,
+                       const int32_t* seg_rows, const int32_t* tile_seg, int n_seg, float* pooled, float* mass_sum,
+                       void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  const int rc = global_mean_check(x, mass, V, C, seg_begin, seg_rows, tile_seg, n_seg);
+  if (rc != DN_OK) return rc;
+  if (!pooled || !mass_sum) return DN_ERR_INVALID_ARGUMENT;
+  if (reinterpret_cast<uintptr_t>(pooled) & 15) return DN_ERR_UNSUPPORTED;
+  if (!workspace || ws_bytes < pool_ws_bytes(V, C)) return DN_ERR_WORKSPACE;
+  if (reinterpret_cast<uintptr_t>(workspace) & 15) return DN_ERR_UNSUPPORTED;
+  return launch_global_mean_fwd(x, mass, V, C, seg_begin, seg_rows, tile_seg, n_seg, pooled, mass_sum, workspace,
+                                (cudaStream_t)stream);
+}
+
+int dn_global_mean_bwd(const float* grad_pooled, const float* mass, const float* mass_sum, int64_t V, int C,
+                       const int32_t* seg_begin, const int32_t* seg_rows, const int32_t* tile_seg, int n_seg,
+                       float* grad_x, dn_stream_t stream) {
+  const int rc = global_mean_check(grad_pooled, mass, V, C, seg_begin, seg_rows, tile_seg, n_seg);
+  if (rc != DN_OK) return rc;
+  if (!mass_sum || !grad_x) return DN_ERR_INVALID_ARGUMENT;
+  if (reinterpret_cast<uintptr_t>(grad_x) & 15) return DN_ERR_UNSUPPORTED;
+  return launch_global_mean_bwd(grad_pooled, mass, mass_sum, V, C, seg_begin, seg_rows, tile_seg, n_seg, grad_x,
+                                (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1,5 +1,7 @@
-// Fused classification head: z = X W^T + b, log_softmax and the NLL loss per row, forward and backward, on wgmma.
-// The (R x n_class) logits, probabilities and logit gradients live only in registers and shared memory.
+// Fused classification head: z = X W^T + b, log_softmax and the NLL loss per row (optionally with a label-smoothed
+// target), forward and backward, on wgmma.  The (R x n_class) logits, probabilities and logit gradients live only in
+// registers and shared memory.  Also the rows the head runs on for face / edge outputs (element mean) and for
+// whole-shape outputs (mass-weighted mean per mesh).
 //
 // Every kernel runs 256 threads: two warpgroups of 64 rows each own the 128 rows of a CTA tile (rows of X, or classes
 // of W in the weight-gradient kernel).  A 128-wide tile of the other operand streams through a B image in shared memory
@@ -268,12 +270,18 @@ struct HeadArgs {
   float* dWp;             // bwd: [S][n_class][C] partials
   float* dbp;             // bwd: [S][n_class]
   int S;                  // row splits of the weight-gradient kernel
+  // label smoothing (set_smoothing): the target is ls_on for the label and ls_off = s / (n_class - 1) for every other
+  // class; ls_label = ls_on - ls_off.  Without smoothing ls_on = 1 and ls_off = 0 exactly, so the logit gradient
+  // g (softmax - target) is the one-hot expression bit for bit.
+  int smooth;
+  float ls_on, ls_off, ls_label;
   CUtensorMap amap;       // logits' B source (W: forward and dX; X: dW), {32, 128} boxes
   CUtensorMap bmap;       // dX / dW's B source (W / X), {32, 32} boxes
 };
 
+// at most 128 registers: two CTAs share an SM wherever their shared memory fits (C up to about 96)
 template <int MODE>
-__global__ void __launch_bounds__(NTHR, 1) linear_nll_fwd_kernel(const __grid_constant__ HeadArgs p) {
+__global__ void __launch_bounds__(NTHR, 2) linear_nll_fwd_kernel(const __grid_constant__ HeadArgs p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const Seq sq{0, 0, cdiv(p.n_class, HT), (int)cdiv(p.C, KS), 0, 0, 0, 0};
   HeadSmem hs = head_smem_carve(smem, p.C, sq, &p.amap, &p.bmap);
@@ -286,13 +294,14 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_fwd_kernel(const __grid_co
   load_tile(As, p.X, row0, nr, p.C);
   const int64_t rows[2] = {row0 + r + (lane >> 2), row0 + r + (lane >> 2) + 8};
   int64_t lab[2];
-  float m[2], s[2], zl[2], best[2];
+  float m[2], s[2], zl[2], best[2], dm[2];
   int bi[2];
   bool bad[2];
+  float cnt = 0.f;     // smoothing: this thread's valid columns so far
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     lab[h] = rows[h] < p.R ? p.labels[rows[h]] : p.ignore_index;
-    m[h] = -INFINITY; s[h] = 0.f; zl[h] = 0.f; best[h] = -INFINITY; bi[h] = 0; bad[h] = false;
+    m[h] = -INFINITY; s[h] = 0.f; zl[h] = 0.f; best[h] = -INFINITY; bi[h] = 0; bad[h] = false; dm[h] = 0.f;
   }
   float acc[64];
   for (int64_t n0 = 0; n0 < p.n_class; n0 += HT) {
@@ -320,14 +329,22 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_fwd_kernel(const __grid_co
       tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
       const float mn = fmaxf(m[h], tmax);
       float sum = s[h] * expf(m[h] - mn);
+      // smoothing: the running sum_j (m - z_j) over this thread's columns, moved to the new max; every term is >= 0,
+      // so the smoothed loss needs no difference of large sums
+      if (p.smooth && cnt > 0.f) dm[h] += cnt * (mn - m[h]);
 #pragma unroll
       for (int b = 0; b < 16; ++b)
 #pragma unroll
         for (int e = 0; e < 2; ++e)
-          if (8 * b + 2 * t + e < nn) sum += expf(acc[4 * b + 2 * h + e] - mn);
+          if (8 * b + 2 * t + e < nn) {
+            sum += expf(acc[4 * b + 2 * h + e] - mn);
+            if (p.smooth) dm[h] += mn - acc[4 * b + 2 * h + e];
+          }
       m[h] = mn;
       s[h] = sum;
     }
+    // this thread's columns of the tile are 8 b + 2 t + e < nn
+    if (p.smooth) cnt += (float)(cdiv(max(nn - 2 * t, 0), 8) + cdiv(max(nn - 2 * t - 1, 0), 8));
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -336,6 +353,7 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_fwd_kernel(const __grid_co
       s[h] += __shfl_xor_sync(0xffffffffu, s[h], o);
       zl[h] += __shfl_xor_sync(0xffffffffu, zl[h], o);
       bad[h] = __shfl_xor_sync(0xffffffffu, (int)bad[h], o) != 0;
+      if (p.smooth) dm[h] += __shfl_xor_sync(0xffffffffu, dm[h], o);
       const float ob = __shfl_xor_sync(0xffffffffu, best[h], o);
       const int oi = __shfl_xor_sync(0xffffffffu, bi[h], o);
       if (ob > best[h] || (ob == best[h] && oi < bi[h])) { best[h] = ob; bi[h] = oi; }
@@ -344,6 +362,9 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_fwd_kernel(const __grid_co
       const float nan = __int_as_float(0x7fc00000);
       const float lse = bad[h] ? nan : m[h] + logf(s[h]);
       float nll = lse - zl[h];
+      // smoothed: sum_j t_j (lse - z_j) = ls_label (lse - z_label) + ls_off sum_j (lse - z_j), and
+      // sum_j (lse - z_j) = sum_j (m - z_j) + n_class log(sum-exp)
+      if (p.smooth) nll = p.ls_label * nll + p.ls_off * (dm[h] + (float)p.n_class * logf(s[h]));
       if (lab[h] == p.ignore_index) nll = 0.f;
       else if (lab[h] < 0 || lab[h] >= p.n_class) nll = nan;
       p.nll[rows[h]] = nll;
@@ -389,7 +410,7 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_dx_kernel(const __grid_con
         float d = 0.f;
         if (c < nn && coef[h] != 0.f) {
           const float zz = z[4 * b + e] + (p.b ? __ldg(p.b + n0 + c) : 0.f);
-          d = coef[h] * (expf(zz - lse[h]) - (n0 + c == lab[h] ? 1.f : 0.f));
+          d = coef[h] * (expf(zz - lse[h]) - (n0 + c == lab[h] ? p.ls_on : p.ls_off));
         }
         z[4 * b + e] = d;
       }
@@ -455,7 +476,7 @@ __global__ void __launch_bounds__(NTHR, 1) linear_nll_dw_kernel(const __grid_con
         for (int h = 0; h < 2; ++h) {
           float d = 0.f;
           if (cls[h] < nn && coef != 0.f)
-            d = coef * (expf(z[4 * b + 2 * h + e2] + bias[h] - lse) - (cls[h] == lab ? 1.f : 0.f));
+            d = coef * (expf(z[4 * b + 2 * h + e2] + bias[h] - lse) - (cls[h] == lab ? p.ls_on : p.ls_off));
           z[4 * b + 2 * h + e2] = d;
           dbs[h] += d;
         }
@@ -518,7 +539,164 @@ __global__ void element_mean_bwd_kernel(const float* __restrict__ g, int C, cons
   }
 }
 
+// ---- mass-weighted mean over segments of rows (outputs_at = 'global_mean') ----
+// Segment b is rows [begin[b], begin[b] + rows[b]); it begins on a 128-row tile, and tile_seg[t] names the segment of
+// tile t (-1: none).  Rows outside every segment are never read.  The partial pass gives every CTA POOL_TILES
+// consecutive tiles; a run of them in one segment is summed into the slots of the run's last tile t:
+// wx[t][c] = sum mass[v] x[v][c], wm[t] = sum mass[v].  The reduction pass sums a segment's runs in tile order.
+constexpr int POOL_TILES = 2;     // small runs: a single 200k-row mesh gives ~6 CTAs per SM, evenly spread
+constexpr int POOL_THR = 256;
+constexpr int POOL_RTHR = 1024;   // reduction CTA: up to 1024 / (C / 4) slices of a segment's runs
+
+__device__ __forceinline__ int pool_seg(const int32_t* __restrict__ tile_seg, int n_seg, int64_t t) {
+  const int s = __ldg(tile_seg + t);
+  return s < n_seg ? s : -1;
+}
+
+// thread layout over C / 4 float4 columns: lane j of row group r (rows r, r + rg, ..); threads past q * rg idle
+struct PoolLanes {
+  int q, rg, j, r;
+  __device__ PoolLanes(int C, int nthr) {
+    q = C >> 2;
+    rg = nthr / q < HT ? nthr / q : HT;
+    j = threadIdx.x % q;
+    r = threadIdx.x / q;
+  }
+};
+
+__global__ void __launch_bounds__(POOL_THR) global_mean_pool_partial_kernel(
+    const float* __restrict__ x, int C, const float* __restrict__ mass, int64_t V, const int32_t* __restrict__ begin,
+    const int32_t* __restrict__ rows, const int32_t* __restrict__ tile_seg, int n_seg, float* wx, float* wm) {
+  __shared__ float4 red[POOL_THR];
+  __shared__ float redm[POOL_THR];
+  const PoolLanes l(C, POOL_THR);
+  const bool lead = l.r < l.rg;
+  const int64_t n_tiles = cdiv(V, HT);
+  const int64_t t0 = (int64_t)blockIdx.x * POOL_TILES;
+  const int64_t t1 = t0 + POOL_TILES < n_tiles ? t0 + POOL_TILES : n_tiles;
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  float am = 0.f;
+  int s = pool_seg(tile_seg, n_seg, t0);
+  for (int64_t t = t0; t < t1; ++t) {
+    const int s_next = t + 1 < t1 ? pool_seg(tile_seg, n_seg, t + 1) : -2;
+    if (s >= 0 && lead) {
+      const int64_t b = __ldg(begin + s);
+      int64_t e = b + __ldg(rows + s);
+      e = e < V ? e : V;
+      const int64_t v1 = HT * t + HT < e ? HT * t + HT : e;
+#pragma unroll 8
+      for (int64_t v = HT * t + l.r; v < v1; v += l.rg) {
+        if (v < b) continue;
+        const float m = __ldg(mass + v);
+        const float4 xv = __ldg(reinterpret_cast<const float4*>(x + v * C) + l.j);
+        acc.x += m * xv.x; acc.y += m * xv.y; acc.z += m * xv.z; acc.w += m * xv.w;
+        am += m;
+      }
+    }
+    if (s >= 0 && s_next != s) {   // the run ends at tile t: fold the row groups in order
+      red[threadIdx.x] = acc;
+      redm[threadIdx.x] = am;
+      __syncthreads();
+      if (threadIdx.x < l.q) {
+        float4 f = red[l.j];
+        for (int k = 1; k < l.rg; ++k) {
+          const float4 o = red[k * l.q + l.j];
+          f.x += o.x; f.y += o.y; f.z += o.z; f.w += o.w;
+        }
+        reinterpret_cast<float4*>(wx + t * C)[l.j] = f;
+        if (l.j == 0) {
+          float fm = redm[0];
+          for (int k = 1; k < l.rg; ++k) fm += redm[k * l.q];
+          wm[t] = fm;
+        }
+      }
+      __syncthreads();
+      acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      am = 0.f;
+    }
+    s = s_next;
+  }
+}
+
+// pooled[b] = (sum of segment b's runs) / (its mass sum), the runs split over rg slices in a fixed order; one CTA per
+// segment.  msum[b] (the mass sum) is what the backward needs.
+__global__ void __launch_bounds__(POOL_RTHR) global_mean_pool_reduce_kernel(
+    const float* __restrict__ wx, const float* __restrict__ wm, int64_t V, int C, const int32_t* __restrict__ begin,
+    const int32_t* __restrict__ rows, float* pooled, float* msum) {
+  __shared__ float4 red[POOL_RTHR];
+  __shared__ float redm[POOL_RTHR];
+  const PoolLanes l(C, POOL_RTHR);
+  const int sg = blockIdx.x;
+  const int64_t b = __ldg(begin + sg), e = b + __ldg(rows + sg);
+  const int64_t tb = b / HT, te = cdiv(e < V ? e : V, HT);
+  // run k of the segment ends at tile min(POOL_TILES k + POOL_TILES - 1, te - 1), k = tb / POOL_TILES ..
+  const int64_t k0 = tb / POOL_TILES, k1 = te > tb ? (te - 1) / POOL_TILES + 1 : k0;
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  float am = 0.f;
+  if (l.r < l.rg) {
+#pragma unroll 4
+    for (int64_t k = k0 + l.r; k < k1; k += l.rg) {
+      const int64_t t = POOL_TILES * k + POOL_TILES - 1 < te - 1 ? POOL_TILES * k + POOL_TILES - 1 : te - 1;
+      const float4 o = __ldg(reinterpret_cast<const float4*>(wx + t * C) + l.j);
+      acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
+      am += __ldg(wm + t);
+    }
+  }
+  red[threadIdx.x] = acc;
+  redm[threadIdx.x] = am;
+  __syncthreads();
+  if (threadIdx.x < l.q) {
+    float4 f = red[l.j];
+    float fm = redm[l.j];
+    for (int k = 1; k < l.rg; ++k) {
+      const float4 o = red[k * l.q + l.j];
+      f.x += o.x; f.y += o.y; f.z += o.z; f.w += o.w;
+      fm += redm[k * l.q + l.j];
+    }
+    reinterpret_cast<float4*>(pooled + (int64_t)sg * C)[l.j] = make_float4(f.x / fm, f.y / fm, f.z / fm, f.w / fm);
+    if (l.j == 0) msum[sg] = fm;
+  }
+}
+
+// grad_x[v] = mass[v] / msum[b] grad_pooled[b] on the rows of segment b, 0 on every other row
+__global__ void global_mean_pool_bwd_kernel(const float* __restrict__ g, const float* __restrict__ mass,
+                                            const float* __restrict__ msum, int64_t V, int C,
+                                            const int32_t* __restrict__ begin, const int32_t* __restrict__ rows,
+                                            const int32_t* __restrict__ tile_seg, int n_seg, float* gx) {
+  const int q = C >> 2;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < V * q; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t v = i / q;
+    const int j = (int)(i % q);
+    const int s = pool_seg(tile_seg, n_seg, v / HT);
+    float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (s >= 0) {
+      const int64_t b = __ldg(begin + s);
+      if (v >= b && v < b + __ldg(rows + s)) {
+        const float w = __ldg(mass + v) / __ldg(msum + s);
+        const float4 gv = __ldg(reinterpret_cast<const float4*>(g + (int64_t)s * C) + j);
+        o = make_float4(w * gv.x, w * gv.y, w * gv.z, w * gv.w);
+      }
+    }
+    reinterpret_cast<float4*>(gx)[i] = o;
+  }
+}
+
 size_t head_smem(int C) { return 1024 + 2 * RAW_BYTES + (size_t)HT * (C + 4) * 4 + 2 * B_IMG + 3 * HT * 4 + 16; }
+
+// target of the reference's label_smoothing_log_loss: 1 - s on the label, s / (n_class - 1) elsewhere (s in [0, 1], and
+// n_class >= 2 when s > 0: the caller checks)
+void set_smoothing(HeadArgs& a, float s) {
+  a.smooth = s > 0.f;
+  a.ls_on = 1.f;
+  a.ls_off = 0.f;
+  a.ls_label = 1.f;
+  if (a.smooth) {
+    const double off = (double)s / (a.n_class - 1);
+    a.ls_on = (float)(1.0 - s);
+    a.ls_off = (float)off;
+    a.ls_label = (float)(1.0 - s - off);
+  }
+}
 
 template <typename K>
 int launch(K kernel, dim3 grid, int C, const HeadArgs& a, cudaStream_t st) {
@@ -550,12 +728,38 @@ int64_t head_ws_bytes(int64_t R, int C, int n_class) {
   return 4ll * head_splits(R, C, n_class) * n_class * (C + 1);
 }
 
+int64_t pool_ws_bytes(int64_t V, int C) { return 4ll * cdiv(V, HT) * (C + 1); }
+
+int launch_global_mean_fwd(const float* x, const float* mass, int64_t V, int C, const int32_t* begin,
+                           const int32_t* rows, const int32_t* tile_seg, int n_seg, float* pooled, float* msum,
+                           void* ws, cudaStream_t st) {
+  float* wx = static_cast<float*>(ws);
+  float* wm = wx + cdiv(V, HT) * C;
+  global_mean_pool_partial_kernel<<<(unsigned)cdiv(cdiv(V, HT), POOL_TILES), POOL_THR, 0, st>>>(
+      x, C, mass, V, begin, rows, tile_seg, n_seg, wx, wm);
+  DN_LAUNCH_CHECK();
+  global_mean_pool_reduce_kernel<<<(unsigned)n_seg, POOL_RTHR, 0, st>>>(wx, wm, V, C, begin, rows, pooled, msum);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
+int launch_global_mean_bwd(const float* g, const float* mass, const float* msum, int64_t V, int C,
+                           const int32_t* begin, const int32_t* rows, const int32_t* tile_seg, int n_seg, float* gx,
+                           cudaStream_t st) {
+  const int64_t blocks = cdiv(V * (C / 4), 256);
+  global_mean_pool_bwd_kernel<<<(unsigned)(blocks < 8192 ? blocks : 8192), 256, 0, st>>>(g, mass, msum, V, C, begin,
+                                                                                       rows, tile_seg, n_seg, gx);
+  DN_LAUNCH_CHECK();
+  return DN_OK;
+}
+
 int launch_linear_nll_fwd(const float* X, const float* W, const float* b, const int64_t* labels, int64_t R, int C,
-                          int n_class, int64_t ignore_index, float* nll, int64_t* argmax, float* lse, int passes,
-                          cudaStream_t st) {
+                          int n_class, int64_t ignore_index, float label_smoothing, float* nll, int64_t* argmax,
+                          float* lse, int passes, cudaStream_t st) {
   HeadArgs a{};
   a.X = X; a.W = W; a.b = b; a.labels = labels; a.R = R; a.C = C; a.n_class = n_class; a.ignore_index = ignore_index;
   a.nll = nll; a.argmax = argmax; a.lse_out = lse;
+  set_smoothing(a, label_smoothing);
   if (!encode_tensor_map_f32(&a.amap, W, n_class, C, C, 32, HT, true)) return DN_ERR_UNSUPPORTED;
   a.bmap = a.amap;
   const dim3 grid((unsigned)cdiv(R, HT));
@@ -565,11 +769,12 @@ int launch_linear_nll_fwd(const float* X, const float* W, const float* b, const 
 }
 
 int launch_linear_nll_bwd(const float* X, const float* W, const float* b, const int64_t* labels, const float* lse,
-                          const float* g, int64_t R, int C, int n_class, int64_t ignore_index, float* dX, float* dW,
-                          float* db, void* ws, int passes, cudaStream_t st) {
+                          const float* g, int64_t R, int C, int n_class, int64_t ignore_index, float label_smoothing,
+                          float* dX, float* dW, float* db, void* ws, int passes, cudaStream_t st) {
   HeadArgs a{};
   a.X = X; a.W = W; a.b = b; a.labels = labels; a.lse = lse; a.g = g; a.R = R; a.C = C; a.n_class = n_class;
   a.ignore_index = ignore_index; a.dX = dX;
+  set_smoothing(a, label_smoothing);
   a.S = head_splits(R, C, n_class);
   a.dWp = static_cast<float*>(ws);
   a.dbp = a.dWp + (int64_t)a.S * n_class * C;

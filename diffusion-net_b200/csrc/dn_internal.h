@@ -242,12 +242,21 @@ bool encode_tensor_map_f32(CUtensorMap* m, const float* base, int64_t rows, int 
 // row splits of the weight-gradient kernel and the workspace its partials need
 int head_splits(int64_t R, int C, int n_class);
 int64_t head_ws_bytes(int64_t R, int C, int n_class);
+// label_smoothing: the reference's target (label 1 - s, every other class s / (n_class - 1)); 0 = plain NLL
 int launch_linear_nll_fwd(const float* X, const float* W, const float* b, const int64_t* labels, int64_t R, int C,
-                          int n_class, int64_t ignore_index, float* nll, int64_t* argmax, float* lse, int passes,
-                          cudaStream_t st);
+                          int n_class, int64_t ignore_index, float label_smoothing, float* nll, int64_t* argmax,
+                          float* lse, int passes, cudaStream_t st);
 int launch_linear_nll_bwd(const float* X, const float* W, const float* b, const int64_t* labels, const float* lse,
-                          const float* g, int64_t R, int C, int n_class, int64_t ignore_index, float* dX, float* dW,
-                          float* db, void* ws, int passes, cudaStream_t st);
+                          const float* g, int64_t R, int C, int n_class, int64_t ignore_index, float label_smoothing,
+                          float* dX, float* dW, float* db, void* ws, int passes, cudaStream_t st);
 int launch_element_mean_fwd(const float* x, int C, const int64_t* elems, int64_t E, int k, float* out, cudaStream_t st);
 int launch_element_mean_bwd(const float* g, int C, const int32_t* rowptr, const int32_t* ent, int64_t V, int k,
                             float* gx, cudaStream_t st);
+// mass-weighted mean over segments of 128-row tiles (dn_global_mean_fwd / _bwd)
+int64_t pool_ws_bytes(int64_t V, int C);
+int launch_global_mean_fwd(const float* x, const float* mass, int64_t V, int C, const int32_t* begin,
+                           const int32_t* rows, const int32_t* tile_seg, int n_seg, float* pooled, float* msum,
+                           void* ws, cudaStream_t st);
+int launch_global_mean_bwd(const float* g, const float* mass, const float* msum, int64_t V, int C,
+                           const int32_t* begin, const int32_t* rows, const int32_t* tile_seg, int n_seg, float* gx,
+                           cudaStream_t st);

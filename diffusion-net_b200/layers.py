@@ -352,20 +352,33 @@ class DiffusionNet(nn.Module):
             x = ops.mlp_apply([x], [self.last_lin.weight], [self.last_lin.bias])
         return x
 
-    def _head_nll(self, x, labels, elems, csr, ignore_index):
+    def _head_nll(self, x, labels, elems, csr, ignore_index, label_smoothing=0.0):
         """(per-row nll, pred) of last_lin + log_softmax + nll_loss on the (V, C_width) block output ``x``, on element
         rows (the mean of the corner features) when ``elems`` is given."""
         if elems is not None:
             x = ops.element_mean(x, elems, csr)
-        return ops.linear_nll(x, self.last_lin.weight, self.last_lin.bias, labels, ignore_index)
+        return ops.linear_nll(x, self.last_lin.weight, self.last_lin.bias, labels, ignore_index, label_smoothing)
 
     def _check_nll_head(self):
         if self.outputs_at == 'global_mean':
-            raise ValueError("forward_nll / forward_batch_nll: outputs_at='global_mean' is not supported (use forward "
-                             "and torch's nll_loss)")
+            raise ValueError("forward_nll / forward_batch_nll: outputs_at='global_mean' has one output per mesh: use "
+                             "forward_global_nll / forward_batch_global_nll")
+
+    def _forward_blocks(self, x_in, mass, L, evals, evecs, gradX, gradY):
+        """forward's route on one mesh from x_in [N, C_in] to the last block's [N, C_width] output, differentiable."""
+        mass_b = mass.unsqueeze(0)
+        evals_b = evals.unsqueeze(0) if evals is not None else None
+        evecs_b = evecs.unsqueeze(0) if evecs is not None else None
+        Lb = [L] if L is not None else None
+        gX = [gradX] if gradX is not None else None
+        gY = [gradY] if gradY is not None else None
+        x = self._linear(self.first_lin, x_in.unsqueeze(0))
+        for b in self.blocks:
+            x = b(x, mass_b, Lb, evals_b, evecs_b, gX, gY)
+        return x[0]
 
     def forward_nll(self, x_in, mass, L=None, evals=None, evecs=None, gradX=None, gradY=None, labels=None, edges=None,
-                    faces=None, ignore_index=-100):
+                    faces=None, ignore_index=-100, label_smoothing=0.0):
         """Training step of a segmentation / per-vertex classification net on one mesh: ``(loss, pred_labels)`` with
         ``loss = F.nll_loss(F.log_softmax(last_lin(...)), labels, ignore_index=ignore_index)`` (mean over the rows whose
         label is not ignore_index, as torch defines it) and ``pred_labels`` the argmax of the logits.  For nets whose
@@ -373,7 +386,8 @@ class DiffusionNet(nn.Module):
         log_softmax and nll_loss, so the (rows, C_out) logits are never formed.  The blocks run as in ``forward``.
         x_in is [N, C] (one mesh); labels int64 per vertex, or per face / edge for outputs_at 'faces' / 'edges' (the
         head then runs on the mean of each element's corner features, equal to the mean of its corner logits).
-        A label outside [0, C_out) that is not ignore_index makes the loss NaN instead of a device assert."""
+        A label outside [0, C_out) that is not ignore_index makes the loss NaN instead of a device assert.
+        ``label_smoothing``: the smoothed target of ops.linear_nll (the reference's label_smoothing_log_loss)."""
         self._check_nll_head()
         if labels is None:
             raise ValueError("forward_nll needs labels")
@@ -385,20 +399,12 @@ class DiffusionNet(nn.Module):
             elems = edges if self.outputs_at == 'edges' else faces
             if elems is None:
                 raise ValueError("forward_nll with outputs_at='{0}' needs {0}".format(self.outputs_at))
-        mass_b = mass.unsqueeze(0)
-        evals_b = evals.unsqueeze(0) if evals is not None else None
-        evecs_b = evecs.unsqueeze(0) if evecs is not None else None
-        Lb = [L] if L is not None else None
-        gX = [gradX] if gradX is not None else None
-        gY = [gradY] if gradY is not None else None
-        x = self._linear(self.first_lin, x_in.unsqueeze(0))
-        for b in self.blocks:
-            x = b(x, mass_b, Lb, evals_b, evecs_b, gX, gY)
-        nll, pred = self._head_nll(x[0], labels, elems, None, ignore_index)
+        x = self._forward_blocks(x_in, mass, L, evals, evecs, gradX, gradY)
+        nll, pred = self._head_nll(x, labels, elems, None, ignore_index, label_smoothing)
         n_valid = (labels != ignore_index).sum().to(nll.dtype)
         return nll.sum() / n_valid, pred
 
-    def forward_batch_nll(self, batch, xs, labels, ignore_index=-100):
+    def forward_batch_nll(self, batch, xs, labels, ignore_index=-100, label_smoothing=0.0):
         """forward_nll over a ``batch.MeshBatch``: ``labels`` is the list of per-mesh label tensors (per vertex, or per
         face / edge).  Returns ``(losses, preds)``: the (n_meshes,) per-mesh mean losses and the list of per-mesh
         predictions; ``losses.sum().backward()`` accumulates the gradients of the per-mesh loop.  The blocks run on
@@ -433,7 +439,7 @@ class DiffusionNet(nn.Module):
                     raise ValueError("forward_batch_nll: mesh {} has {} vertices, got labels of shape {}".format(
                         b, batch.n_rows[b], tuple(l.shape)))
                 lab[batch.row_begin[b]:batch.row_begin[b] + batch.n_rows[b]] = l
-        nll, pred = self._head_nll(x, lab, elems, None, ignore_index)
+        nll, pred = self._head_nll(x, lab, elems, None, ignore_index, label_smoothing)
         if elems is not None:
             nlls, preds, labs = torch.split(nll, counts), list(torch.split(pred, counts)), labels
         else:
@@ -442,6 +448,61 @@ class DiffusionNet(nn.Module):
             labs = labels
         losses = torch.stack([v.sum() / (l != ignore_index).sum().to(v.dtype) for v, l in zip(nlls, labs)])
         return losses, preds
+
+    def _check_global_head(self, what):
+        if self.outputs_at != 'global_mean':
+            raise ValueError("{}: needs outputs_at='global_mean', the net has outputs_at='{}' (use forward_nll / "
+                             "forward_batch_nll)".format(what, self.outputs_at))
+
+    def forward_global_nll(self, x_in, mass, L=None, evals=None, evecs=None, gradX=None, gradY=None, labels=None,
+                           label_smoothing=0.0, ignore_index=-100):
+        """Training step of a whole-shape classifier (outputs_at='global_mean') on one mesh: ``(loss, pred)`` with
+        ``loss = -sum_j t_j log_softmax(mean_mass(last_lin(...)))_j``, the reference's
+        ``utils.label_smoothing_log_loss(net(...), labels, label_smoothing)`` (t: 1 - s on the label, s / (C_out - 1)
+        elsewhere; s = 0 is nll_loss), and ``pred`` the 0-d argmax class.  For nets whose ``last_activation`` is
+        log_softmax: it is not applied here.  The blocks run as in ``forward``; the mass-weighted mean
+        (ops.global_mean_pool) then runs on the block output before the fused head (ops.linear_nll): the mean's weights
+        sum to 1, so pooling before last_lin equals the reference's last_lin, mean, log_softmax.  ``labels``: an int64
+        tensor of one element.  A label equal to ignore_index gives loss 0 and no gradient."""
+        self._check_global_head("forward_global_nll")
+        if labels is None or not torch.is_tensor(labels) or labels.dtype != torch.int64 or labels.numel() != 1:
+            raise ValueError("forward_global_nll needs labels: an int64 tensor of one element")
+        if x_in.dim() != 2 or x_in.shape[-1] != self.C_in:
+            raise ValueError("forward_global_nll takes one mesh: x_in [N, {}], got {}".format(self.C_in,
+                                                                                            tuple(x_in.shape)))
+        ops._require_cuda(x_in, mass, labels)
+        x = self._forward_blocks(x_in, mass, L, evals, evecs, gradX, gradY)
+        pooled = ops.global_mean_pool(x, mass)
+        nll, pred = ops.linear_nll(pooled, self.last_lin.weight, self.last_lin.bias, labels.reshape(1), ignore_index,
+                                   label_smoothing)
+        return nll[0], pred[0]
+
+    def forward_batch_global_nll(self, batch, xs, labels, label_smoothing=0.0, ignore_index=-100):
+        """forward_global_nll over a ``batch.MeshBatch``: ``labels`` an (n_meshes,) int64 tensor or a list of
+        one-element int64 tensors.  Returns ``(losses, preds)``, both (n_meshes,); ``losses.sum().backward()``
+        accumulates the gradients of the per-mesh loop.  The blocks run on forward_batch's differentiable route, then
+        one pool over every mesh (padding rows never read) and one fused head over the n_meshes pooled rows.  Spectral
+        diffusion only."""
+        self._check_global_head("forward_batch_global_nll")
+        if self.diffusion_method != 'spectral':
+            raise NotImplementedError("forward_batch_global_nll: spectral diffusion only")
+        if torch.is_tensor(labels):
+            lab = labels
+        else:
+            if any(not torch.is_tensor(l) or l.numel() != 1 for l in labels):
+                raise ValueError("forward_batch_global_nll: labels must be one-element tensors, one per mesh")
+            lab = torch.cat([l.reshape(1) for l in labels]) if len(labels) else None
+        if lab is None or lab.dtype != torch.int64 or lab.shape != (batch.n_meshes,):
+            raise ValueError("forward_batch_global_nll: {} meshes need {} int64 labels, got {}".format(
+                batch.n_meshes, batch.n_meshes, tuple(lab.shape) if lab is not None else 0))
+        x = xs if torch.is_tensor(xs) else batch.pack(xs)
+        if x.shape[-1] != self.C_in:
+            raise ValueError("DiffusionNet was constructed with C_in={}, but x_in has last dim={}".format(
+                self.C_in, x.shape[-1]))
+        ops._require_cuda(x, lab)
+        x = self._forward_batch_blocks(batch, x)
+        pooled = ops.global_mean_pool(x, batch.mass, batch.segments)
+        return ops.linear_nll(pooled, self.last_lin.weight, self.last_lin.bias, lab, ignore_index, label_smoothing)
 
     def forward(self, x_in, mass, L=None, evals=None, evecs=None, gradX=None, gradY=None, edges=None, faces=None):
         """[N,C] or [B,N,C] in, [N,C_out] or [B,N,C_out] out (reference layers.py:314-407)."""

@@ -900,11 +900,12 @@ def mlp_apply(srcs, weights, biases, residual=None, drop_p=0.0):
 class LinearNLLFn(torch.autograd.Function):
     """Per-row ``nll_loss(log_softmax(x @ weight.T + bias), labels, reduction='none')`` and the row argmax in one
     tensor-core launch (dn_linear_nll_fwd); the (R, n_class) logits are never formed.  Backward: 3 launches
-    (dn_linear_nll_bwd), gradients to x, weight and bias, reproducible bit for bit."""
+    (dn_linear_nll_bwd), gradients to x, weight and bias, reproducible bit for bit.  ``label_smoothing`` > 0 takes the
+    smoothed target through dn_linear_nll_ls_fwd / _bwd; 0 calls the plain entries."""
 
     @staticmethod
     @_device_guard
-    def forward(ctx, x, weight, bias, labels, ignore_index):
+    def forward(ctx, x, weight, bias, labels, ignore_index, label_smoothing=0.0):
         x, weight = _f32c(x), _f32c(weight)
         bias = _f32c(bias) if bias is not None else None
         labels = labels.contiguous()
@@ -913,12 +914,16 @@ class LinearNLLFn(torch.autograd.Function):
         nll = torch.empty(R, dtype=torch.float32, device=x.device)
         lse = torch.empty(R, dtype=torch.float32, device=x.device)
         pred = torch.empty(R, dtype=torch.int64, device=x.device)
-        _lib.check(_lib.load().dn_linear_nll_fwd(x.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None
-                                                 else None, labels.data_ptr(), R, Cc, n_class, int(ignore_index),
-                                                 nll.data_ptr(), pred.data_ptr(), lse.data_ptr(), _engine, _stream()),
-                   "dn_linear_nll_fwd")
+        lib = _lib.load()
+        args = (x.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None else None, labels.data_ptr(), R,
+                Cc, n_class, int(ignore_index), nll.data_ptr(), pred.data_ptr(), lse.data_ptr(), _engine, _stream())
+        if label_smoothing:
+            _lib.check(lib.dn_linear_nll_ls_fwd(*args, float(label_smoothing)), "dn_linear_nll_ls_fwd")
+        else:
+            _lib.check(lib.dn_linear_nll_fwd(*args), "dn_linear_nll_fwd")
         ctx.save_for_backward(x, weight, bias, labels, lse)
         ctx.ignore_index = int(ignore_index)
+        ctx.label_smoothing = float(label_smoothing)
         ctx.mark_non_differentiable(pred)
         return nll, pred
 
@@ -935,31 +940,59 @@ class LinearNLLFn(torch.autograd.Function):
         lib = _lib.load()
         ws_bytes = lib.dn_linear_nll_workspace_bytes(R, Cc, n_class)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        _lib.check(lib.dn_linear_nll_bwd(x.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None else None,
-                                         labels.data_ptr(), lse.data_ptr(), g.data_ptr(), R, Cc, n_class,
-                                         ctx.ignore_index, gx.data_ptr(), gw.data_ptr(),
-                                         gb.data_ptr() if gb is not None else None, ws.data_ptr(), ws_bytes, _engine,
-                                         _stream()), "dn_linear_nll_bwd")
-        return gx, gw, gb, None, None
+        args = (x.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None else None, labels.data_ptr(),
+                lse.data_ptr(), g.data_ptr(), R, Cc, n_class, ctx.ignore_index, gx.data_ptr(), gw.data_ptr(),
+                gb.data_ptr() if gb is not None else None, ws.data_ptr(), ws_bytes, _engine, _stream())
+        if ctx.label_smoothing:
+            _lib.check(lib.dn_linear_nll_ls_bwd(*args, ctx.label_smoothing), "dn_linear_nll_ls_bwd")
+        else:
+            _lib.check(lib.dn_linear_nll_bwd(*args), "dn_linear_nll_bwd")
+        return gx, gw, gb, None, None, None
 
 
-def linear_nll(x, weight, bias, labels, ignore_index=-100):
+def _smoothed_nll(logp, labels, ignore_index, s):
+    """-sum_j t_j logp[r, j] with the reference's smoothed target (1 - s on the label, s / (n_class - 1) elsewhere): 0
+    on ignore_index rows, NaN on a label outside [0, n_class)."""
+    n_class = logp.shape[-1]
+    off = s / (n_class - 1)
+    keep = labels != ignore_index
+    ok = (labels >= 0) & (labels < n_class)
+    z_lab = -logp.gather(1, labels.clamp(0, n_class - 1)[:, None])[:, 0]
+    nll = (1.0 - s - off) * z_lab + off * -logp.sum(dim=-1)
+    nll = torch.where(keep, nll, torch.zeros_like(nll))
+    return torch.where(keep & ~ok, torch.full_like(nll, float("nan")), nll)
+
+
+def linear_nll(x, weight, bias, labels, ignore_index=-100, label_smoothing=0.0):
     """``(nll_per_row, argmax)`` of the classification head ``log_softmax(x @ weight.T + bias)`` for int64 ``labels``:
     nll_per_row[r] = -log_softmax(z)[r, labels[r]], 0 where labels[r] == ignore_index.  Reductions stay with the caller.
     Gradients reach x, weight and bias.  On the tensor-core engines one fused op; a label outside [0, n_class) that is
     not ignore_index gives a NaN row (and NaN gradients) instead of torch's device assert.  On the 'simt' engine the
-    composed path (exact SIMT linear layer, then torch's log_softmax and nll_loss) with torch's semantics."""
+    composed path (exact SIMT linear layer, then torch's log_softmax and nll_loss) with torch's semantics.
+
+    ``label_smoothing`` = s in [0, 1] uses the target of the reference's ``utils.label_smoothing_log_loss``: 1 - s on
+    the label and s / (n_class - 1) on every other class, nll_per_row[r] = -sum_j t_j log_softmax(z)[r, j].  torch's
+    ``cross_entropy(label_smoothing=e)`` is this target with s = e (n_class - 1) / n_class.  At 0 the op is the plain
+    head above, bit for bit."""
     _require_cuda(x, weight, bias, labels)
     if x.dim() != 2 or weight.dim() != 2 or x.shape[1] != weight.shape[1]:
         raise ValueError("linear_nll: x (R, C) and weight (n_class, C) expected; got {} and {}".format(
             tuple(x.shape), tuple(weight.shape)))
     if labels.dtype != torch.int64 or labels.shape != (x.shape[0],):
         raise ValueError("linear_nll: labels must be int64 of shape ({},)".format(x.shape[0]))
+    s = float(label_smoothing)
+    if not 0.0 <= s <= 1.0 or (s > 0.0 and weight.shape[0] < 2):
+        raise ValueError("linear_nll: label_smoothing must lie in [0, 1] (and needs at least 2 classes when > 0); "
+                         "got {} with {} classes".format(label_smoothing, weight.shape[0]))
     if _engine == _lib.ENGINE_SIMT:
         z = mlp_apply([x], [weight], [bias])
+        if s > 0.0:
+            return _smoothed_nll(torch.log_softmax(z, dim=-1), labels, ignore_index, s), z.detach().argmax(dim=-1)
         nll = torch.nn.functional.nll_loss(torch.log_softmax(z, dim=-1), labels, reduction='none',
                                            ignore_index=ignore_index)
         return nll, z.detach().argmax(dim=-1)
+    if s > 0.0:
+        return LinearNLLFn.apply(x, weight, bias, labels, int(ignore_index), s)
     return LinearNLLFn.apply(x, weight, bias, labels, int(ignore_index))
 
 
@@ -1026,3 +1059,97 @@ def element_mean(x, elems, csr=None):
     if csr is None:
         csr = cached_element_csr(elems, x.shape[0])
     return ElementMeanFn.apply(x, elems, csr)
+
+
+# ---- mass-weighted mean over each mesh (outputs_at = 'global_mean') ---------------------------------------------------
+class Segments:
+    """Device tables of row segments for dn_global_mean_fwd / _bwd: segment b is rows [begin[b], begin[b] + rows[b])
+    of a (V, C) layout, each beginning on a 128-row tile, no two sharing a tile.  Built once on the host (a
+    ``batch.MeshBatch`` builds its own; ``single_segment`` caches the one of a single mesh per V), never read back."""
+
+    def __init__(self, begin, rows, V, device):
+        begin, rows = [int(b) for b in begin], [int(n) for n in rows]
+        V = int(V)
+        if not begin or len(begin) != len(rows):
+            raise ValueError("Segments: one begin and one row count per segment, at least one segment")
+        n_tiles = (V + 127) // 128
+        tile_seg = [-1] * n_tiles
+        for b, (r0, n) in enumerate(zip(begin, rows)):
+            if r0 % 128 or n < 0 or r0 + n > V:
+                raise ValueError("Segments: segment {} = rows [{}, {}) must begin on a 128-row tile inside [0, {})".format(
+                    b, r0, r0 + n, V))
+            for t in range(r0 // 128, (r0 + n + 127) // 128):
+                if tile_seg[t] != -1:
+                    raise ValueError("Segments: segments {} and {} share tile {}".format(tile_seg[t], b, t))
+                tile_seg[t] = b
+        self.n_seg, self.V = len(begin), V
+        i32 = dict(dtype=torch.int32, device=device)
+        self.begin = torch.tensor(begin, **i32)
+        self.rows = torch.tensor(rows, **i32)
+        self.tile_seg = torch.tensor(tile_seg, **i32)
+
+
+_single_segment_cache = {}
+
+
+def single_segment(V, device):
+    """Segments of one mesh: the single segment [0, V), built once per (V, device)."""
+    dev = torch.device(device)
+    key = (int(V), dev.index if dev.index is not None else torch.cuda.current_device())
+    hit = _single_segment_cache.get(key)
+    if hit is None:
+        hit = _single_segment_cache[key] = Segments([0], [V], V, dev)
+    return hit
+
+
+class GlobalMeanPoolFn(torch.autograd.Function):
+    """pooled[b] = sum_{v in b} mass[v] x[v] / sum_{v in b} mass[v] per segment: 2 launches forward
+    (dn_global_mean_fwd), 1 backward (dn_global_mean_bwd), bitwise reproducible.  Gradients reach x only."""
+
+    @staticmethod
+    @_device_guard
+    def forward(ctx, x, mass, seg):
+        x, mass = _f32c(x), _f32c(mass)
+        V, Cc = x.shape
+        pooled = torch.empty(seg.n_seg, Cc, dtype=torch.float32, device=x.device)
+        msum = torch.empty(seg.n_seg, dtype=torch.float32, device=x.device)
+        lib = _lib.load()
+        ws_bytes = lib.dn_global_mean_workspace_bytes(V, Cc)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        _lib.check(lib.dn_global_mean_fwd(x.data_ptr(), mass.data_ptr(), V, Cc, seg.begin.data_ptr(),
+                                          seg.rows.data_ptr(), seg.tile_seg.data_ptr(), seg.n_seg, pooled.data_ptr(),
+                                          msum.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "dn_global_mean_fwd")
+        ctx.save_for_backward(mass, msum)
+        ctx.seg, ctx.shape = seg, (V, Cc)
+        return pooled
+
+    @staticmethod
+    @_device_guard
+    def backward(ctx, g):
+        mass, msum = ctx.saved_tensors
+        seg = ctx.seg
+        V, Cc = ctx.shape
+        g = _f32c(g)
+        gx = torch.empty(V, Cc, dtype=torch.float32, device=g.device)
+        _lib.check(_lib.load().dn_global_mean_bwd(g.data_ptr(), mass.data_ptr(), msum.data_ptr(), V, Cc,
+                                                  seg.begin.data_ptr(), seg.rows.data_ptr(), seg.tile_seg.data_ptr(),
+                                                  seg.n_seg, gx.data_ptr(), _stream()), "dn_global_mean_bwd")
+        return gx, None, None
+
+
+def global_mean_pool(x, mass, segments=None):
+    """Mass-weighted mean of the (V, C) rows of ``x`` over each segment (reference layers.py:393-397 for one mesh):
+    (n_segments, C).  ``segments``: a ``Segments`` (a ``batch.MeshBatch``'s ``segments``: one per mesh, padding rows
+    never read and given a zero gradient); None for one mesh, [0, V).  C a multiple of 4 up to 256.  ``mass`` gets
+    no gradient."""
+    _require_cuda(x, mass)
+    if x.dim() != 2 or mass.shape != (x.shape[0],):
+        raise ValueError("global_mean_pool: x (V, C) and mass (V,) expected; got {} and {}".format(
+            tuple(x.shape), tuple(mass.shape)))
+    _no_operator_grads(("mass", mass))
+    if segments is None:
+        segments = single_segment(x.shape[0], x.device)
+    elif segments.V != x.shape[0]:
+        raise ValueError("global_mean_pool: x has {} rows, the segments a {}-row layout".format(x.shape[0],
+                                                                                               segments.V))
+    return GlobalMeanPoolFn.apply(x, mass, segments)

@@ -555,6 +555,23 @@ int dn_linear_nll_bwd(const float* x, const float* weight, const float* bias, co
                       float* grad_weight, float* grad_bias, void* workspace, int64_t ws_bytes, int engine,
                       dn_stream_t stream);
 
+/* The head with label smoothing: dn_linear_nll_fwd / _bwd with the smoothed target of the reference's
+ * utils.label_smoothing_log_loss (the classification experiment's loss).  With s = label_smoothing and
+ * s' = s / (n_class - 1), the target is t_j = 1 - s on the label and s' on every other class, and per row
+ *   nll[r] = -sum_j t_j log_softmax(z[r])_j,   dZ = grad_nll[r] (softmax(z[r]) - t)
+ * (torch's cross_entropy(label_smoothing = e) is this target with s = e (n_class - 1) / n_class).  The forward keeps one
+ * more running quantity per row, sum_j (max - z_j), so the smoothed sum of log-probabilities needs no cancellation.
+ * Everything else (shapes, engines, ignore_index and out-of-range labels, workspace, launch counts, determinism) is as
+ * for dn_linear_nll_fwd / _bwd; at s = 0 the results are theirs bit for bit.  s outside [0, 1] (or NaN), or s > 0 with
+ * n_class < 2, is DN_ERR_INVALID_ARGUMENT before anything is enqueued. */
+int dn_linear_nll_ls_fwd(const float* x, const float* weight, const float* bias, const int64_t* labels, int64_t R,
+                         int C, int n_class, int64_t ignore_index, float* nll, int64_t* argmax, float* lse, int engine,
+                         dn_stream_t stream, float label_smoothing);
+int dn_linear_nll_ls_bwd(const float* x, const float* weight, const float* bias, const int64_t* labels,
+                         const float* lse, const float* grad_nll, int64_t R, int C, int n_class, int64_t ignore_index,
+                         float* grad_x, float* grad_weight, float* grad_bias, void* workspace, int64_t ws_bytes,
+                         int engine, dn_stream_t stream, float label_smoothing);
+
 /* Element rows of the head for outputs_at = 'faces' / 'edges' (layers.py:394-398 takes the mean of the corner logits;
  * the mean commutes with last_lin, so the head runs on the mean of the corner features instead).
  *   fwd: out[e][c] = (sum_j x[elems[e][j]][c]) / k over the k corners in order, x (V, C), elems int64 (E, k) with every
@@ -567,6 +584,30 @@ int dn_element_mean_fwd(const float* x, int64_t V, int C, const int64_t* elems, 
                         dn_stream_t stream);
 int dn_element_mean_bwd(const float* grad_out, int64_t E, int C, const int32_t* rowptr, const int32_t* entries,
                         int64_t V, int k, float* grad_x, dn_stream_t stream);
+
+/* Rows of the head for outputs_at = 'global_mean': the mass-weighted mean of each mesh's features (layers.py:393-397
+ * weights the per-vertex logits by mass / sum(mass); the weights sum to 1, so the mean commutes with last_lin and the
+ * head runs on the pooled features).  x (V, C) fp32, C a multiple of 4 up to 256, x 16-byte aligned; mass (V).  Segment b
+ * is rows [seg_begin[b], seg_begin[b] + seg_rows[b]) (int32 device arrays of n_seg entries); every segment begins on a
+ * 128-row tile and every tile lies in at most one segment, named by tile_seg[t] (int32, ceil(V / 128) entries, -1 for
+ * a tile of no segment): a dn_mesh_batch layout with one segment per mesh, or one segment [0, V) for one mesh.  Rows
+ * outside every segment (a batch's padding rows) are never read.  The tables live on the device and nothing is read
+ * back, so both calls capture in a CUDA graph.
+ *   fwd: pooled[b][c] = sum_{v in b} mass[v] x[v][c] / M_b, M_b = sum_{v in b} mass[v]; pooled (n_seg, C) and mass_sum
+ *        (n_seg: M_b, what the backward needs) OVERWRITTEN.  2 launches whatever V, C and n_seg are: per-tile-run
+ *        partials in the workspace (dn_global_mean_workspace_bytes(V, C), 16-byte aligned), then one CTA per segment
+ *        sums its partials in tile order.  No atomics: two calls give bitwise-equal results.
+ *   bwd: grad_x[v][c] = mass[v] / M_b grad_pooled[b][c] for v in segment b and exactly 0 on every other row; grad_x
+ *        (V, C) OVERWRITTEN.  1 launch.
+ * C outside the envelope, V >= 2^31 or a misaligned x, pooled, grad_pooled, grad_x or workspace is DN_ERR_UNSUPPORTED,
+ * a short workspace DN_ERR_WORKSPACE, before anything is enqueued. */
+int64_t dn_global_mean_workspace_bytes(int64_t V, int C);
+int dn_global_mean_fwd(const float* x, const float* mass, int64_t V, int C, const int32_t* seg_begin,
+                       const int32_t* seg_rows, const int32_t* tile_seg, int n_seg, float* pooled, float* mass_sum,
+                       void* workspace, int64_t ws_bytes, dn_stream_t stream);
+int dn_global_mean_bwd(const float* grad_pooled, const float* mass, const float* mass_sum, int64_t V, int C,
+                       const int32_t* seg_begin, const int32_t* seg_rows, const int32_t* tile_seg, int n_seg,
+                       float* grad_x, dn_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -151,22 +151,32 @@ def atb_split(mode, V, I, J, sm, part_floats):
     return max(1, -(-chunks // cpc)), cpc * KC
 
 
-def _split_v(A, B, mode, sm, part_floats, ea=None, pert=(), stats=None, split=None):
+def _split_v(A, B, mode, sm, part_floats, ea=None, pert=(), stats=None, split=None, tree=None):
     """sum_v A[v]^T B[v] as atb / to_basis_partials + reduce_partials compute it: (gold, bound).  ``split``: (P, rows
-    per partial) of a planned mesh batch instead of the kernel's own split."""
+    per partial) of a planned mesh batch instead of the kernel's own split.  ``tree``: the partials are summed by
+    ``tree`` slices, each serially, then pairwise (spectral_scale_kernel: 4, the pack kernel's spectral job: 8) instead
+    of serially with the prefilled output added last."""
     V = A.shape[0]
     P, rps = split or atb_split(mode, V, A.shape[1], B.shape[1], sm, part_floats)
     if "drop_last_partial" in pert and P > 1:
         A = A.copy()
         A[(P - 1) * rps:] = 0
-    L = (3 if mode == "3x" else 1) * rps + P + 1
+    red = P + 1 if tree is None else -(-P // tree) + int(np.log2(tree))
+    L = (3 if mode == "3x" else 1) * rps + red
     return _contract(A.T, B, mode, L, ea=None if ea is None else ea.T, b_packed=False, stats=stats)
 
 
-def _dense(a, W, mode, ea=None, eW=None, emul=None, relu_mask=None, row_scale=None, stats=None):
-    """one run_chain layer out = a @ W (W (K, N) as the layer reads it), epilogue in rows_chain_kernel's order."""
+def _dense(a, W, mode, ea=None, eW=None, bias=None, relu=False, emul=None, relu_mask=None, row_scale=None,
+           residual=None, stats=None):
+    """one run_chain layer out = a @ W (W (K, N) as the layer reads it), epilogue in rows_chain_kernel's order: bias,
+    relu, emul, relu mask, row_scale, residual (fmaf with res_scale = 1)."""
     L = (3 if mode == "3x" else 1) * a.shape[1]
     z, b = _contract(a, W, mode, L, ea=ea, eb=eW, stats=stats)
+    if bias is not None:
+        z = z + bias[None, :]
+        b = b + U * np.abs(z)
+    if relu:                     # non-expansive: the band carries over
+        z = np.maximum(z, 0.0)
     if emul is not None:
         z = z * emul
         b = b * np.abs(emul) + U * np.abs(z)
@@ -176,6 +186,9 @@ def _dense(a, W, mode, ea=None, eW=None, emul=None, relu_mask=None, row_scale=No
     if row_scale is not None:
         z = z * row_scale[:, None]
         b = b * np.abs(row_scale)[:, None] + U * np.abs(z)
+    if residual is not None:
+        z = z + residual
+        b = b + U * np.abs(z)
     return z, b + U * np.abs(z)
 
 

@@ -14,8 +14,8 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libdiffusion_net_b200.so")
-SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_eig.cu", "dn_implicit.cu", "dn_fmap.cu", "dn_fmap_batch.cu", "dn_tc.cu",
-           "dn_head.cu", "dn_capi.cu"]
+SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_eig.cu", "dn_implicit.cu", "dn_implicit_batch.cu", "dn_fmap.cu",
+           "dn_fmap_batch.cu", "dn_tc.cu", "dn_head.cu", "dn_capi.cu"]
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "diffusion_net_b200.h")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -126,6 +126,11 @@ SIGNATURES = {
     "dn_implicit_diffusion_workspace_bytes": (_L, [_L, _I]),
     "dn_implicit_diffusion_fwd": (_I, [C.POINTER(dn_csr), _P, _P, _P, _L, _I, _D, _I, _P, _P, _P, _L, _P]),
     "dn_implicit_diffusion_bwd": (_I, [C.POINTER(dn_csr), _P, _P, _P, _P, _L, _I, _D, _I, _P, _P, _P, _P, _L, _P]),
+    "dn_implicit_diffusion_workspace_bytes_batched": (_L, [_L, _I, _I]),
+    "dn_implicit_diffusion_fwd_batched": (_I, [C.POINTER(dn_csr), _P, _P, _P, C.POINTER(dn_mesh_batch), _P, _L, _I, _D,
+                                               _I, _P, _P, _P, _L, _P]),
+    "dn_implicit_diffusion_bwd_batched": (_I, [C.POINTER(dn_csr), _P, _P, _P, _P, C.POINTER(dn_mesh_batch), _P, _L, _I,
+                                               _D, _I, _P, _P, _P, _P, _L, _P]),
     "dn_fmap_solve_fwd": (_I, [_P, _P, _P, _P, _I, _I, _D, _P, _P]),
     "dn_fmap_solve_bwd": (_I, [_P, _P, _P, _P, _I, _I, _D, _P, _P, _P, _P, _L, _P]),
     "dn_nearest_neighbor_workspace_bytes": (_L, [_L, _L, _I]),

@@ -519,6 +519,49 @@ int dn_implicit_diffusion_bwd(const dn_csr* L, const float* grad_out, const floa
                                    grad_x, grad_time, status, workspace, (cudaStream_t)stream);
 }
 
+int64_t dn_implicit_diffusion_workspace_bytes_batched(int64_t V, int C, int n_meshes) {
+  if (V < 0 || C <= 0 || n_meshes < 1) return -1;
+  return implicit_batched_ws_bytes(V, C, n_meshes);
+}
+
+static int implicit_batched_check(const dn_csr* L, const float* mass, const float* time, const float* rhs,
+                                  const dn_mesh_batch* batch, const int32_t* mesh_rows, int64_t V, int C, double rtol,
+                                  int max_iter, const float* out, const double* status, const void* workspace,
+                                  int64_t ws_bytes) {
+  if (!L || !batch || batch->n_meshes < 1 || !batch->tile_mesh || !mesh_rows || V <= 0 || V % 128 != 0 || C <= 0 ||
+      L->nnz < 0 || !(rtol >= 0.0) || max_iter < 1 || !time || !status || !L->rowptr || !mass || !rhs || !out ||
+      (L->nnz > 0 && (!L->colidx || !L->vals)))
+    return DN_ERR_INVALID_ARGUMENT;
+  if (C > 256 || L->nnz >= (1ll << 31) || V >= (1ll << 31) - 1 || (int64_t)batch->n_meshes * C >= (1ll << 31))
+    return DN_ERR_UNSUPPORTED;
+  if (!workspace || ws_bytes < implicit_batched_ws_bytes(V, C, batch->n_meshes)) return DN_ERR_WORKSPACE;
+  return DN_OK;
+}
+
+int dn_implicit_diffusion_fwd_batched(const dn_csr* L, const float* x, const float* mass, float* time,
+                                      const dn_mesh_batch* batch, const int32_t* mesh_rows, int64_t V, int C,
+                                      double rtol, int max_iter, float* x_diffuse, double* status, void* workspace,
+                                      int64_t ws_bytes, dn_stream_t stream) {
+  const int rc = implicit_batched_check(L, mass, time, x, batch, mesh_rows, V, C, rtol, max_iter, x_diffuse, status,
+                                        workspace, ws_bytes);
+  if (rc != DN_OK) return rc;
+  return launch_implicit_diffusion_batched(L, mass, time, x, nullptr, batch, mesh_rows, V, C, rtol, max_iter, 0,
+                                           x_diffuse, nullptr, status, workspace, (cudaStream_t)stream);
+}
+
+int dn_implicit_diffusion_bwd_batched(const dn_csr* L, const float* grad_out, const float* mass, const float* time,
+                                      const float* x_diffuse, const dn_mesh_batch* batch, const int32_t* mesh_rows,
+                                      int64_t V, int C, double rtol, int max_iter, float* grad_x, float* grad_time,
+                                      double* status, void* workspace, int64_t ws_bytes, dn_stream_t stream) {
+  const int rc = implicit_batched_check(L, mass, time, grad_out, batch, mesh_rows, V, C, rtol, max_iter, grad_x,
+                                        status, workspace, ws_bytes);
+  if (rc != DN_OK) return rc;
+  if (!grad_time || !x_diffuse) return DN_ERR_INVALID_ARGUMENT;
+  return launch_implicit_diffusion_batched(L, mass, const_cast<float*>(time), grad_out, x_diffuse, batch, mesh_rows, V,
+                                           C, rtol, max_iter, 1, grad_x, grad_time, status, workspace,
+                                           (cudaStream_t)stream);
+}
+
 int dn_compute_hks(const float* evals, const float* evecs, const float* scales, int64_t V, int K, int S, float* out,
                    dn_stream_t stream) {
   if (V < 0 || K <= 0 || S < 0 || ((V > 0 && S > 0) && (!evals || !evecs || !scales || !out)))

@@ -164,6 +164,13 @@ int64_t implicit_ws_bytes(int64_t V, int C);
 int launch_implicit_diffusion(const dn_csr* L, const float* mass, float* time, const float* rhs, const float* y,
                               int64_t V, int C, double rtol, int max_iter, int backward, float* out, float* grad_time,
                               double* status, void* ws, cudaStream_t st);
+// the same over a mesh batch (dn_implicit_batch.cu): one solve per (mesh, channel) pair; mesh_rows (device,
+// 2 n_meshes) holds each mesh's rows [begin, end)
+int64_t implicit_batched_ws_bytes(int64_t V, int C, int n_meshes);
+int launch_implicit_diffusion_batched(const dn_csr* L, const float* mass, float* time, const float* rhs, const float* y,
+                                      const dn_mesh_batch* batch, const int32_t* mesh_rows, int64_t V, int C,
+                                      double rtol, int max_iter, int backward, float* out, float* grad_time,
+                                      double* status, void* ws, cudaStream_t st);
 int launch_grad_spmm_pair(const dn_csr* g, const float* x, int64_t V, int C, float* out_vc2, cudaStream_t st);
 // R-order fused features: feat = tanh(gX*Bre + gY*Bim) from gathers of xd, P, Q (pq = [P|Q], ld 2C or C).
 int launch_spmm_features(const dn_csr* g, const float* xd, const float* pq, int rotations, int64_t V, int C,

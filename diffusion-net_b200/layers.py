@@ -178,9 +178,13 @@ class DiffusionNetBlock(nn.Module):
 
     def _forward_batch(self, batch, x_in):
         """Differentiable block over every mesh of a ``batch.MeshBatch`` (x_in in the batch layout): the per-mesh
-        spectral diffusion runs grouped (ops.BatchedDiffusionFn); the gradient features run on the block-diagonal CSR
-        and the MiniMLP row-wise, each once over the whole range.  Padding rows never reach a real row."""
-        x_diffuse = ops.BatchedDiffusionFn.apply(x_in, self.diffusion.diffusion_time, batch)
+        spectral diffusion runs grouped (ops.BatchedDiffusionFn), the implicit one as one solve over every (mesh,
+        channel) pair (ops.BatchedImplicitDiffusionFn); the gradient features run on the block-diagonal CSR and the
+        MiniMLP row-wise, each once over the whole range.  Padding rows never reach a real row."""
+        if self.diffusion.method == 'implicit_dense':
+            x_diffuse = ops.BatchedImplicitDiffusionFn.apply(x_in, self.diffusion.diffusion_time, batch)
+        else:
+            x_diffuse = ops.BatchedDiffusionFn.apply(x_in, self.diffusion.diffusion_time, batch)
         srcs = [x_in, x_diffuse]
         if self.with_gradient_features:
             A_re, A_im = self.gradient_features.weights()
@@ -280,9 +284,11 @@ class DiffusionNet(nn.Module):
         blocks run differentiably (``DiffusionNetBlock._forward_batch``): sum or average the per-mesh losses and the
         gradients are the per-mesh gradients accumulated, input gradients reaching each ``x_b``.  Dropout masks are
         drawn over the whole batch layout, one draw per hidden layer per block.  'faces' / 'edges' outputs need the
-        batch items to carry ``faces`` / ``edges``."""
-        if self.diffusion_method != 'spectral':
-            raise NotImplementedError("forward_batch: spectral diffusion only")
+        batch items to carry ``faces`` / ``edges``.
+
+        An implicit_dense net needs a batch whose items carry 'L'; it runs the differentiable route in inference as well
+        (batched solve, gradient features, MiniMLP)."""
+        self._check_batch(batch, "forward_batch")
         elems = None
         if self.outputs_at in ('edges', 'faces'):
             elems = batch.faces if self.outputs_at == 'faces' else batch.edges
@@ -315,9 +321,18 @@ class DiffusionNet(nn.Module):
                 self.C_in, x.shape[-1]))
         needs_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))
         dropout = any(blk.training and blk.dropout for blk in self.blocks)
-        if needs_grad or dropout:
+        if needs_grad or dropout or self.diffusion_method == 'implicit_dense':   # the fused block is spectral
             return ops.mlp_apply([self._forward_batch_blocks(batch, x)], [self.last_lin.weight], [self.last_lin.bias])
         return self._forward_batch_fused(batch, x)
+
+    def _check_batch(self, batch, what):
+        """The batch routes run spectral nets on batches with eigenpairs, implicit nets on batches with Laplacians."""
+        if self.diffusion_method == 'implicit_dense':
+            if batch is None or not batch.has_laplacian:
+                raise NotImplementedError("{}: a diffusion_method='implicit_dense' net needs a MeshBatch whose items "
+                                          "carry the Laplacian 'L'".format(what))
+        elif batch is not None and batch.K == 0:
+            raise ValueError("{}: a spectral net needs eigenpairs, and this MeshBatch has none (k_eig = 0)".format(what))
 
     def _forward_batch_blocks(self, batch, x):
         """The differentiable route of forward_batch from the packed input to the last block's (V, C_width) output."""
@@ -410,8 +425,7 @@ class DiffusionNet(nn.Module):
         predictions; ``losses.sum().backward()`` accumulates the gradients of the per-mesh loop.  The blocks run on
         forward_batch's differentiable route; padding rows of the batch layout carry ignore_index."""
         self._check_nll_head()
-        if self.diffusion_method != 'spectral':
-            raise NotImplementedError("forward_batch_nll: spectral diffusion only")
+        self._check_batch(batch, "forward_batch_nll")
         if len(labels) != batch.n_meshes:
             raise ValueError("forward_batch_nll: {} label tensors for {} meshes".format(len(labels), batch.n_meshes))
         x = xs if torch.is_tensor(xs) else batch.pack(xs)
@@ -481,11 +495,10 @@ class DiffusionNet(nn.Module):
         """forward_global_nll over a ``batch.MeshBatch``: ``labels`` an (n_meshes,) int64 tensor or a list of
         one-element int64 tensors.  Returns ``(losses, preds)``, both (n_meshes,); ``losses.sum().backward()``
         accumulates the gradients of the per-mesh loop.  The blocks run on forward_batch's differentiable route, then
-        one pool over every mesh (padding rows never read) and one fused head over the n_meshes pooled rows.  Spectral
-        diffusion only."""
+        one pool over every mesh (padding rows never read) and one fused head over the n_meshes pooled rows.  An
+        implicit_dense net needs a batch whose items carry 'L'."""
         self._check_global_head("forward_batch_global_nll")
-        if self.diffusion_method != 'spectral':
-            raise NotImplementedError("forward_batch_global_nll: spectral diffusion only")
+        self._check_batch(batch, "forward_batch_global_nll")
         if torch.is_tensor(labels):
             lab = labels
         else:

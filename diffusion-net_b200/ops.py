@@ -364,6 +364,21 @@ class LaplacianCSR:
                        "dn_csr_from_coo")
         self.csr = (_lib.dn_csr(rowptr.data_ptr(), colidx.data_ptr(), cv.data_ptr(), self.nnz), rowptr, colidx, cv)
 
+    @classmethod
+    def from_csr(cls, V, rowptr, colidx, vals2):
+        """Wrap a CSR already on the device: ``rowptr`` int32 (V+1), ``colidx`` int32 (nnz), ``vals2`` float32 (nnz, 2)
+        with L in column 0 (column 1 is not read).  batch.MeshBatch builds its block-diagonal Laplacian this way."""
+        self = cls.__new__(cls)
+        _require_cuda(rowptr, colidx, vals2)
+        self.V, self.device = int(V), rowptr.device
+        self.nnz = int(colidx.numel())
+        rowptr, colidx, cv = rowptr.contiguous(), colidx.contiguous(), vals2.contiguous().view(-1)
+        if self.nnz == 0:
+            colidx = torch.empty(1, dtype=torch.int32, device=self.device)
+            cv = torch.empty(2, dtype=torch.float32, device=self.device)
+        self.csr = (_lib.dn_csr(rowptr.data_ptr(), colidx.data_ptr(), cv.data_ptr(), self.nnz), rowptr, colidx, cv)
+        return self
+
 
 def prepare_laplacian(L):
     """Memoised like ``prepare_operators``: the CSR of the user's sparse ``L`` (coalesced COO (V, V) as get_operators
@@ -670,19 +685,33 @@ IMPLICIT_MAX_ITER = 20000   # a 200k-vertex mesh at t ~ 1 needs a few thousand i
 implicit_last_status = None  # host copy of the last solve's status (iterations per column, residuals; see the header)
 
 
-def _implicit_call(what, fn, V, Cc, device, args, outs):
+def _implicit_call(what, fn, V, Cc, device, args, outs, n_meshes=None):
     """Run one dn_implicit_diffusion_* call (``args`` before rtol / max_iter, ``outs`` after) and raise if a column did
-    not converge: one host read of the device status per solve."""
-    status = torch.empty(2 + 2 * Cc, dtype=torch.float64, device=device)
-    ws = torch.empty(int(_lib.load().dn_implicit_diffusion_workspace_bytes(V, Cc)), dtype=torch.uint8, device=device)
-    _lib.check(fn(*args, float(IMPLICIT_RTOL), int(IMPLICIT_MAX_ITER), *outs, status.data_ptr(), ws.data_ptr(),
-                  ws.numel(), _stream()), what)
+    not converge: one host read of the device status per solve.  ``n_meshes``: a _batched call, whose status has one
+    column per (mesh, channel) pair."""
+    lib = _lib.load()
+    n = Cc if n_meshes is None else n_meshes * Cc
+    status = torch.empty(2 + 2 * n, dtype=torch.float64, device=device)
+    nbytes = (lib.dn_implicit_diffusion_workspace_bytes(V, Cc) if n_meshes is None else
+              lib.dn_implicit_diffusion_workspace_bytes_batched(V, Cc, n_meshes))
+    ws = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+    max_iter = int(IMPLICIT_MAX_ITER)
+    _lib.check(fn(*args, float(IMPLICIT_RTOL), max_iter, *outs, status.data_ptr(), ws.data_ptr(), ws.numel(),
+                  _stream()), what)
     global implicit_last_status
     st = implicit_last_status = status.cpu()
     if st[0] > 0:
-        raise RuntimeError("diffusion_net_b200 {}: {} of {} columns did not converge in {} iterations (worst relative "
-                           "residual {:.3e}, tolerance {:.1e})".format(what, int(st[0]), Cc, IMPLICIT_MAX_ITER,
-                                                                      float(st[2 + Cc:].max()), IMPLICIT_RTOL))
+        if n_meshes is None:
+            raise RuntimeError("diffusion_net_b200 {}: {} of {} columns did not converge in {} iterations (worst "
+                               "relative residual {:.3e}, tolerance {:.1e})".format(
+                                   what, int(st[0]), Cc, max_iter, float(st[2 + Cc:].max()), IMPLICIT_RTOL))
+        # still iterating when the limit was reached: max_iter iterations and a residual above the tolerance
+        stuck = (st[2:2 + n] >= max_iter) & (st[2 + n:] > IMPLICIT_RTOL)
+        meshes = sorted({int(p) // Cc for p in torch.nonzero(stuck).flatten().tolist()})
+        raise RuntimeError("diffusion_net_b200 {}: {} of {} (mesh, channel) pairs did not converge in {} iterations, "
+                           "in meshes {} (worst relative residual {:.3e}, tolerance {:.1e})".format(
+                               what, int(st[0]), n, max_iter, meshes, float(st[2 + n:].nan_to_num(0.0).max()),
+                               IMPLICIT_RTOL))
     return st
 
 
@@ -723,6 +752,51 @@ class ImplicitDiffusionFn(torch.autograd.Function):
                        (C.byref(ctx.lap.csr[0]), g.data_ptr(), mass.data_ptr(), time.data_ptr(), y.data_ptr(), V, Cc),
                        (gx.data_ptr(), gt.data_ptr()))
         return gx, gt, None, None
+
+
+class BatchedImplicitDiffusionFn(torch.autograd.Function):
+    """ImplicitDiffusionFn over every mesh of a ``batch.MeshBatch`` whose items carry L (x in the batch layout): one
+    dn_implicit_diffusion_fwd_batched / _bwd_batched launch per solve whatever the mesh count, each (mesh, channel)
+    pair solved on its own, and one host read of the status.  Padding rows come out 0.  The kernel clamps ``time`` in
+    place, as the reference does on the Parameter (layers.py:48-49)."""
+
+    @staticmethod
+    @_device_guard
+    def forward(ctx, x, time, batch):
+        lib = _lib.load()
+        x = _f32c(x)
+        if time.dtype != torch.float32 or not time.is_contiguous():
+            raise RuntimeError("diffusion_time must be a contiguous float32 tensor")
+        if not batch.has_laplacian:
+            raise ValueError("implicit diffusion over a MeshBatch needs the Laplacian 'L' in every item")
+        V, Cc = x.shape
+        if V != batch.V or time.shape != (Cc,):
+            raise ValueError("implicit diffusion: x {} and time {} do not fit this batch ({} rows)".format(
+                tuple(x.shape), tuple(time.shape), batch.V))
+        y = torch.empty_like(x)
+        _implicit_call("dn_implicit_diffusion_fwd_batched", lib.dn_implicit_diffusion_fwd_batched, V, Cc, x.device,
+                       (C.byref(batch.lap.csr[0]), x.data_ptr(), batch.mass.data_ptr(), time.data_ptr(),
+                        C.byref(batch.desc), batch._mesh_rows.data_ptr(), V, Cc), (y.data_ptr(),),
+                       n_meshes=batch.n_meshes)
+        ctx.batch = batch
+        ctx.save_for_backward(time.detach().clone(), y)
+        return y
+
+    @staticmethod
+    @_device_guard
+    def backward(ctx, g):
+        lib = _lib.load()
+        time, y = ctx.saved_tensors
+        batch = ctx.batch
+        g = _f32c(g)
+        V, Cc = g.shape
+        gx = torch.empty_like(g)
+        gt = torch.zeros_like(time)
+        _implicit_call("dn_implicit_diffusion_bwd_batched", lib.dn_implicit_diffusion_bwd_batched, V, Cc, g.device,
+                       (C.byref(batch.lap.csr[0]), g.data_ptr(), batch.mass.data_ptr(), time.data_ptr(), y.data_ptr(),
+                        C.byref(batch.desc), batch._mesh_rows.data_ptr(), V, Cc), (gx.data_ptr(), gt.data_ptr()),
+                       n_meshes=batch.n_meshes)
+        return gx, gt, None
 
 
 def batched_diffusion_workspace_extra(n_meshes, K, C_):

@@ -464,6 +464,34 @@ int dn_from_basis_batched(const float* values, const float* basis, const float* 
                           int64_t V, int K, int C, float* out, void* workspace, int64_t ws_bytes, int engine,
                           dn_stream_t stream);
 
+/* dn_implicit_diffusion_fwd / _bwd (implicit diffusion, above) over a batch laid out as above, in one cooperative
+ * launch whatever the mesh count: for every mesh b and channel c (a "pair"), the rows of mesh b in column c of
+ * x_diffuse are (M_b + t_c L_b)^-1 M_b x_bc.  `L` is the batch's block-diagonal Laplacian (dn_csr with batch-global
+ * column indices, L at even positions of vals as above); `mass` (V) and x (V, C) are in the batch layout, V the padded
+ * total (a positive multiple of 128).  From `batch` only n_meshes and tile_mesh are read; `mesh_rows` (device,
+ * 2 n_meshes int32) holds the rows [begin, end) of mesh b, begin a multiple of 128 and the tiles of [begin, end) marked
+ * b in tile_mesh.  Every pair has its own step lengths, convergence test, freezing and NaN state, exactly as a column
+ * of the single-mesh call, so one mesh's iterations do not change another's.  Every sum over a mesh's rows is a sum of
+ * 32-row partials in a fixed order: results are bitwise reproducible and do not depend on the device's size.
+ * Padding rows (not in any [begin, end)) are written as exact zeros (x_diffuse, grad_x).
+ * `status` (device, 2 + 2 P doubles, P = n_meshes C, pair p = b C + c): [0] the number of pairs that did not converge
+ * within max_iter iterations, [1] the largest iteration count, [2 + p] the iterations of pair p, [2 + P + p] its final
+ * ||r|| / ||b|| (0 when b = 0, NaN for a non-finite pair).  When [0] > 0 no output is written and grad_time is not
+ * accumulated.  time is clamped in place by the forward as above.
+ *   bwd: grad_x = M_b w_bc on the rows of mesh b; grad_time[c] += -sum_b sum_v w_bc[v] (L_b x_diffuse_bc)[v], the meshes
+ *        added in mesh order (NaN when any pair of channel c is non-finite).
+ * Workspace: dn_implicit_diffusion_workspace_bytes_batched(V, C, n_meshes) (about 32 V C bytes). */
+int64_t dn_implicit_diffusion_workspace_bytes_batched(int64_t V, int C, int n_meshes);
+int dn_implicit_diffusion_fwd_batched(const dn_csr* L, const float* x, const float* mass, float* time,
+                                      const dn_mesh_batch* batch, const int32_t* mesh_rows, int64_t V, int C,
+                                      double rtol, int max_iter, float* x_diffuse, double* status, void* workspace,
+                                      int64_t ws_bytes, dn_stream_t stream);
+int dn_implicit_diffusion_bwd_batched(const dn_csr* L, const float* grad_out, const float* mass, const float* time,
+                                      const float* x_diffuse, const dn_mesh_batch* batch,
+                                      const int32_t* mesh_rows, int64_t V, int C, double rtol, int max_iter,
+                                      float* grad_x, float* grad_time, double* status, void* workspace,
+                                      int64_t ws_bytes, dn_stream_t stream);
+
 /* ---- functional maps over a pair batch ------------------------------------------------------------------------------
  * S shapes and P ordered pairs (x_p, y_p) of shape indices (self-pairs, repeats and unused shapes allowed).  The spectral
  * features are one stack F: shape s at F + s * ld_shape, n x d with row stride d (ld_shape >= n d, so a padded (S, K, d)

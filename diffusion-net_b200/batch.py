@@ -6,150 +6,397 @@ batch-global column indices and the small device tables of ``dn_mesh_batch`` (in
 ``DiffusionNet.forward_batch`` runs every stage of every block as ONE launch over all meshes
 (``dn_block_fwd_batched``): grouped split-V to_basis, one packed spectral multiplier per mesh, a from_basis chain that
 picks its weights per tile, and the per-vertex stages (gather, MiniMLP, first/last linear) over the whole range.
+
+``MeshDataset`` keeps a whole dataset's operators on the device, back to back without padding, and assembles any batch
+of its meshes (a shuffled training step) with one ``dn_batch_gather`` launch: the layout is planned on the host from the
+meshes' sizes, its tables go up in one pinned copy, and nothing is read back.  ``MeshBatch(items)`` is the dataset of
+``items`` gathered in order.
 """
 from __future__ import annotations
 
 import ctypes as C
+import operator
 
 import numpy as np
 import torch
 
 from . import _lib, ops
 
+# ranges of a gather table (dn_batch_gather): per batch mesh, (src_begin, dst_begin, n, n_dst) in units of
+R_ROWS, R_MESH, R_PTR, R_ENT, R_FACES, R_EDGES = range(6)   # rows, meshes, row pointers, CSR entries, faces, edges
+N_RANGES = 6
+_INT32_LIMIT = 2 ** 31
+
+
+def _check_items(items, device):
+    """MeshBatch's checks of the item dicts, before anything is copied or launched: (device, rows of every mesh, K,
+    whether the items carry L).  Every per-mesh array must have its mesh's row count, as the mesh's rows in the
+    concatenated dataset are placed by its mass alone."""
+    if len(items) < 1:
+        raise ValueError("MeshBatch needs at least one mesh")
+    dev = torch.device(device) if device is not None else items[0]["mass"].device
+    if dev.type != "cuda":
+        raise RuntimeError("diffusion_net_b200 runs on CUDA tensors only (no CPU fallback)")
+    for b, it in enumerate(items):
+        if it["mass"].dim() != 1:
+            raise ValueError("MeshBatch: mesh {}'s mass must be 1-D (V,), got shape {}".format(
+                b, tuple(it["mass"].shape)))
+    n_rows = [int(it["mass"].shape[0]) for it in items]
+    n_eig = lambda it: (int(it["evals"].shape[0]) if it.get("evals") is not None else 0,
+                        int(it["evecs"].shape[1]) if it.get("evecs") is not None else 0)
+    K = n_eig(items[0])[0]
+    if any(n_eig(it) != (K, K) for it in items):
+        raise ValueError("every mesh of a batch needs the same number of eigenpairs")
+    has_lap = [it.get("L") is not None for it in items]
+    if any(has_lap) and not all(has_lap):
+        raise ValueError("MeshBatch: 'L' must be given for every item or for none")
+    if K == 0 and not all(has_lap):
+        raise ValueError("MeshBatch: items without eigenpairs need the Laplacian 'L' (implicit diffusion)")
+    for b, (it, n) in enumerate(zip(items, n_rows)):
+        if K and (tuple(it["evals"].shape) != (K,) or tuple(it["evecs"].shape) != (n, K)):
+            raise ValueError("MeshBatch: mesh {} has {} vertices and {} eigenpairs but evals of shape {} and evecs of "
+                             "shape {}".format(b, n, K, tuple(it["evals"].shape), tuple(it["evecs"].shape)))
+        g = it["gradX"]
+        gV = (g.V, g.V) if isinstance(g, ops.GradOperators) else tuple(g.shape)
+        if gV != (n, n) or (not isinstance(g, ops.GradOperators) and tuple(it["gradY"].shape) != (n, n)):
+            raise ValueError("MeshBatch: mesh {} has {} vertices but gradient operators of shape {}".format(b, n, gV))
+    return dev, n_rows, K, all(has_lap)
+
+
+def _sm_count(dev):
+    sm, cc, smem = C.c_int(0), C.c_int(0), C.c_int64(0)
+    idx = dev.index if dev.index is not None else torch.cuda.current_device()
+    _lib.check(_lib.load().dn_device_query(idx, C.byref(sm), C.byref(cc), C.byref(smem)), "dn_device_query")
+    return int(sm.value)
+
+
+def plan_rows(n_rows, sm_count):
+    """dn_mesh_batch_plan (host): (row_begin [B + 1], tile_mesh [max(V / 128, 1)], tb_rows [2 n_ctas],
+    cta_begin [B + 1], n_ctas) as int32 arrays.  More than 1024 meshes, or a padded total of 2^31 - 256 rows or more,
+    raise RuntimeError (unsupported) before anything is allocated."""
+    n_rows = np.asarray(n_rows, dtype=np.int64)
+    B = len(n_rows)
+    padded = (n_rows + 127) // 128 * 128
+    if B < 1 or (n_rows < 0).any():
+        _lib.check(-1, "dn_mesh_batch_plan")
+    if int(padded.sum()) >= _INT32_LIMIT - 256:
+        _lib.check(-2, "dn_mesh_batch_plan")
+    row_begin = np.zeros(B + 1, dtype=np.int32)
+    tile_mesh = np.zeros(max(int(padded.sum()) // 128, 1), dtype=np.int32)
+    tb_rows = np.zeros(2 * 1024, dtype=np.int32)
+    cta_begin = np.zeros(B + 1, dtype=np.int32)
+    n32 = n_rows.astype(np.int32)
+    n_ctas = _lib.load().dn_mesh_batch_plan(B, n32.ctypes.data, int(sm_count), row_begin.ctypes.data,
+                                            tile_mesh.ctypes.data, tb_rows.ctypes.data, cta_begin.ctypes.data)
+    if n_ctas < 0:
+        _lib.check(n_ctas, "dn_mesh_batch_plan")
+    return row_begin, tile_mesh, tb_rows[:2 * n_ctas].copy(), cta_begin, int(n_ctas)
+
+
+def _starts(counts):
+    """Exclusive prefix sum (int64): where each mesh's units begin in the concatenation."""
+    out = np.zeros(len(counts) + 1, dtype=np.int64)
+    np.cumsum(counts, out=out[1:])
+    return out
+
+
+def gather_table(ids, n_rows, row_begin, n_ent, n_faces=None, n_edges=None):
+    """The (B, N_RANGES, 4) int64 table of dn_batch_gather for batch mesh b = dataset mesh ids[b], from sizes only:
+    the dataset's meshes have n_rows rows, n_ent CSR entries (gradient or Laplacian) and n_faces / n_edges elements
+    (None: not gathered), back to back; the batch's rows begin at row_begin (plan_rows).  A dataset row-pointer array
+    holds n_rows + 1 entries per mesh; the batch writes every mesh's padded rows, and the last mesh also row V."""
+    ids = np.asarray(ids, dtype=np.int64)
+    n_rows = np.asarray(n_rows, dtype=np.int64)
+    B = len(ids)
+    rb = np.asarray(row_begin, dtype=np.int64)
+    nb, pad = n_rows[ids], rb[1:] - rb[:-1]
+    src_row = _starts(n_rows)[ids]
+    last = np.zeros(B, dtype=np.int64)
+    last[-1] = 1
+    t = np.zeros((B, N_RANGES, 4), dtype=np.int64)
+    t[:, R_ROWS] = np.stack([src_row, rb[:-1], nb, pad], 1)
+    t[:, R_MESH] = np.stack([ids, np.arange(B), np.ones(B, np.int64), np.ones(B, np.int64)], 1)
+    t[:, R_PTR] = np.stack([src_row + ids, rb[:-1], nb + 1, pad + last], 1)
+    for r, cnt in ((R_ENT, n_ent), (R_FACES, n_faces), (R_EDGES, n_edges)):
+        if cnt is not None:
+            cnt = np.asarray(cnt, dtype=np.int64)
+            c = cnt[ids]
+            t[:, r] = np.stack([_starts(cnt)[ids], _starts(c)[:-1], c, c], 1)
+    return t
+
+
+def _int32_entries(t, what):
+    nnz = int(t[:, R_ENT, 2].sum())
+    if nnz >= _INT32_LIMIT:
+        raise ValueError("MeshBatch: the batch {} has {} entries, more than int32 indices hold".format(what, nnz))
+    return nnz
+
+
+def batch_tables(ids, n_rows, n_ent, n_faces=None, n_edges=None, sm_count=132, plan=None):
+    """Everything ``MeshDataset.batch`` builds on the host, from the dataset meshes' sizes only (no tensor, no GPU):
+    the dn_mesh_batch plan, the per-mesh row ranges of the implicit solve, the global-mean segments and the gather
+    table.  A batch that int32 indices cannot address is refused here (RuntimeError for rows, as dn_mesh_batch_plan
+    refuses them; ValueError for gradient entries).  ``plan``: plan_rows' result for these meshes, when the caller
+    already has it."""
+    ids = np.asarray(ids, dtype=np.int64)
+    nb = np.asarray(n_rows, dtype=np.int64)[ids]
+    row_begin, tile_mesh, tb_rows, cta_begin, n_ctas = plan if plan is not None else plan_rows(nb, sm_count)
+    V = int(row_begin[-1])
+    table = gather_table(ids, n_rows, row_begin, n_ent, n_faces, n_edges)
+    nnz = _int32_entries(table, "gradient operators")
+    seg_begin = row_begin[:-1].copy()
+    seg_rows = nb.astype(np.int32)
+    return dict(row_begin=row_begin, V=V, n_ctas=n_ctas, tile_mesh=tile_mesh[:max(V // 128, 1)].copy(),
+                tb_rows=tb_rows, cta_begin=cta_begin,
+                mesh_rows=np.stack([seg_begin, seg_begin + seg_rows], 1).reshape(-1).astype(np.int32),
+                seg_begin=seg_begin, seg_rows=seg_rows,
+                tile_seg=np.asarray(ops.Segments.tile_table(seg_begin, seg_rows, V), dtype=np.int32).reshape(-1),
+                table=table, nnz=nnz)
+
+
+def _upload(arrays, dev):
+    """Device copies of host int32 / int64 arrays through ONE pinned buffer and ONE non-blocking copy."""
+    offs, total = [], 0
+    for a in arrays:
+        offs.append(total)
+        total += (a.nbytes + 15) // 16 * 16
+    host = torch.empty(max(total, 16), dtype=torch.uint8, pin_memory=True)
+    hv = host.numpy()
+    for a, o in zip(arrays, offs):
+        hv[o:o + a.nbytes] = np.ascontiguousarray(a).view(np.uint8).reshape(-1)
+    d = host.to(dev, non_blocking=True)
+    tdt = {np.dtype(np.int32): torch.int32, np.dtype(np.int64): torch.int64}
+    return [d[o:o + a.nbytes].view(tdt[a.dtype]).view(a.shape) for a, o in zip(arrays, offs)]
+
+
+def _part(src, dst, op, width, rng, table_host, offset_range=0):
+    return _lib.dn_gather_part(src.data_ptr(), dst.data_ptr(), op, int(width), rng, offset_range,
+                               int(table_host[:, rng, 3].max()))
+
+
+def _gather(parts, table, n_meshes, dev):
+    """One dn_batch_gather launch; parts whose batch array is empty are left out (no launch when none is left)."""
+    parts = [p for p, dst in parts if dst.numel() > 0 and p.width > 0]
+    if not parts:
+        return
+    arr = (_lib.dn_gather_part * len(parts))(*parts)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().dn_batch_gather(arr, len(parts), table.data_ptr(), N_RANGES, n_meshes, ops._stream()),
+                   "dn_batch_gather")
+
+
+class _DatasetLaplacian:
+    """The dataset's per-mesh Laplacians, concatenated on first use (a spectral net never pays for them): local CSRs
+    back to back, every mesh's row pointers (V_b + 1 entries) kept."""
+
+    def __init__(self, Ls, n_rows, dev):
+        self._Ls, self.n_rows, self.device = Ls, n_rows, dev
+        self.arrays = None
+
+    def get(self):
+        if self.arrays is None and self._Ls is not None:
+            laps = []
+            for b, (L, n) in enumerate(zip(self._Ls, self.n_rows)):
+                lap = L if isinstance(L, ops.LaplacianCSR) else ops.prepare_laplacian(L.to(self.device))
+                if not isinstance(lap, ops.LaplacianCSR) or lap.V != n:
+                    raise ValueError("MeshBatch: mesh {} has {} vertices but its L is not a ({}, {}) Laplacian".format(
+                        b, n, n, n))
+                laps.append(lap)
+            self.arrays = (torch.cat([l.csr[1] for l in laps]), torch.cat([l.csr[2][:l.nnz] for l in laps]),
+                           torch.cat([l.csr[3][:2 * l.nnz] for l in laps]), [l.nnz for l in laps])
+            self._Ls = None
+        return self.arrays
+
+
+class MeshDataset:
+    """A dataset of meshes resident on the device, from which any batch is assembled on the GPU.
+
+    ``items``: the item dicts ``MeshBatch`` takes (mass, evals / evecs, gradX / gradY or a prepared
+    ``ops.GradOperators`` under 'gradX', optionally L (sparse or ``ops.LaplacianCSR``), faces, edges), checked as
+    ``MeshBatch`` checks them.  Everything is concatenated once on the device with device-to-device copies, without
+    padding (int64 offsets: a dataset may hold more than 2^31 rows or entries; only a batch must fit int32), and the
+    per-mesh sizes and offsets stay on the host (``n_meshes``, ``n_rows``, ``row_begin``, ``K``).  The caller may drop
+    the per-mesh tensors afterwards; Laplacians given as sparse L are kept until first used.
+
+    ``batch(ids)`` returns the ``MeshBatch`` of the meshes ``ids`` (repeats allowed) with one kernel launch, no host
+    synchronisation and no device-to-host transfer, so a shuffled training loop queues each step's batch behind the
+    previous step's work::
+
+        ds = MeshDataset(items)
+        for ids in torch.randperm(len(items), generator=g).split(32):
+            b = ds.batch(ids.tolist())
+            losses, _ = net.forward_batch_global_nll(b, ds.pack(features, b), labels[ids])
+    """
+
+    def __init__(self, items, device=None):
+        dev, n_rows, K, has_lap = _check_items(items, device)
+        self._build(items, dev, n_rows, K, has_lap, _sm_count(dev))
+
+    def _build(self, items, dev, n_rows, K, has_lap, sm):
+        """The concatenation, from what _check_items returned for ``items`` and the device's SM count."""
+        self.device, self.n_meshes, self.n_rows, self.K = dev, len(items), n_rows, K
+        self.row_begin = [int(v) for v in _starts(n_rows)]
+        self.V = self.row_begin[-1]
+        self._sm = sm
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.mass = torch.cat([it["mass"].to(**f32) for it in items])
+        self.evecs = torch.cat([it["evecs"].to(**f32) for it in items]) if K else torch.zeros(self.V, 0, **f32)
+        self.evals = torch.stack([it["evals"].to(**f32) for it in items]) if K else torch.zeros(self.n_meshes, 0, **f32)
+        grads = [it["gradX"] if isinstance(it["gradX"], ops.GradOperators) else
+                 ops.prepare_operators(it["gradX"].to(dev), it["gradY"].to(dev)) for it in items]
+        self._grad_nnz = [g.nnz for g in grads]
+        self._grad = (torch.cat([g.csr[1] for g in grads]), torch.cat([g.csr[2][:g.nnz] for g in grads]),
+                      torch.cat([g.csr[3][:2 * g.nnz] for g in grads]))
+        self._elems = {}
+        for name in ("faces", "edges"):
+            if all(it.get(name) is not None for it in items):
+                els = [torch.as_tensor(it[name]).to(device=dev, dtype=torch.int64) for it in items]
+                self._elems[name] = (torch.cat(els, 0), [int(e.shape[0]) for e in els])
+        self.has_laplacian = has_lap
+        self._lap = _DatasetLaplacian([it["L"] for it in items] if has_lap else None, n_rows, dev)
+
+    def __len__(self):
+        return self.n_meshes
+
+    def _ids(self, ids):
+        if torch.is_tensor(ids):
+            if ids.device.type != "cpu":
+                raise ValueError("MeshDataset.batch: ids must be a host list or a CPU tensor, got a tensor on {}: the "
+                                 "batch layout is planned on the host from the meshes' sizes".format(ids.device))
+            if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool or ids.dim() > 1:
+                raise TypeError("MeshDataset.batch: ids must be integers, got a {} tensor of shape {}".format(
+                    ids.dtype, tuple(ids.shape)))
+            ids = ids.tolist()
+        ids = [operator.index(i) for i in ids]
+        if not ids:
+            raise ValueError("MeshDataset.batch needs at least one mesh id")
+        bad = [i for i in ids if not 0 <= i < self.n_meshes]
+        if bad:
+            raise IndexError("MeshDataset.batch: mesh id {} is outside the dataset's {} meshes".format(bad[0],
+                                                                                                     self.n_meshes))
+        return ids
+
+    def batch(self, ids):
+        """The ``MeshBatch`` of dataset meshes ``ids`` (a host list or a CPU int tensor; repeats allowed), bitwise
+        what ``MeshBatch([items[i] for i in ids])`` builds.  One kernel launch; no host synchronisation."""
+        ids = self._ids(ids)
+        mb = MeshBatch.__new__(MeshBatch)
+        mb._gather_from(self, ids)
+        return mb
+
+    def pack(self, t, batch):
+        """A per-vertex tensor in the dataset layout (V_total,) or (V_total, C), float32 (features such as HKS or xyz)
+        or int64 (labels), in ``batch``'s layout with zero padding rows: one launch, no host synchronisation.  Data
+        only: a tensor that requires grad is refused (per-mesh lists still go through ``MeshBatch.pack``)."""
+        if getattr(batch, "_source", None) is not self._lap:
+            raise ValueError("MeshDataset.pack: the batch was not drawn from this dataset")
+        if not torch.is_tensor(t) or t.dim() not in (1, 2) or t.shape[0] != self.V or \
+                t.dtype not in (torch.float32, torch.int64):
+            raise ValueError("MeshDataset.pack: expected a float32 or int64 tensor of shape ({0},) or ({0}, C) in the "
+                             "dataset layout, got {1}".format(self.V, (tuple(t.shape), t.dtype) if torch.is_tensor(t)
+                                                              else type(t)))
+        if t.requires_grad:
+            raise ValueError("MeshDataset.pack gathers data; got a tensor that requires grad (pack per-mesh "
+                             "tensors with MeshBatch.pack to differentiate through the layout)")
+        ops._require_cuda(t)
+        if t.device != batch.device:
+            raise ValueError("MeshDataset.pack: the tensor is on {}, the dataset on {}".format(t.device, batch.device))
+        t = t.contiguous()
+        out = torch.empty((batch.V,) + tuple(t.shape[1:]), dtype=t.dtype, device=batch.device)
+        width = (t.shape[1] if t.dim() == 2 else 1) * (2 if t.dtype == torch.int64 else 1)
+        _gather([(_part(t, out, _lib.GATHER_COPY, width, R_ROWS, batch._table_host), out)], batch._table,
+                batch.n_meshes, batch.device)
+        return out
+
 
 class MeshBatch:
     """``items``: dicts with mass (V), evals (K), evecs (V,K), gradX, gradY (sparse COO (V,V) or a prepared
     ``ops.GradOperators`` under 'gradX') -- the reference's operator tuple per mesh -- and optionally faces (F,3) /
-    edges (E,2) for ``DiffusionNet.forward_batch`` with outputs_at 'faces' / 'edges'.  Build once, reuse every step.
+    edges (E,2) for ``DiffusionNet.forward_batch`` with outputs_at 'faces' / 'edges'.  Build once, reuse every step;
+    for a different set of meshes every step, draw the batches from a ``MeshDataset``.
 
     For nets with diffusion_method='implicit_dense', every item also carries 'L' (sparse COO (V,V) as get_operators
     returns it, or a prepared ``ops.LaplacianCSR``); the batch then holds one block-diagonal Laplacian CSR in its layout
     (``lap``, built on first use, so a spectral net never pays for it; None when the items carry no L;
     ``has_laplacian`` tells which without building it).  Such items may leave out 'evals' / 'evecs' (k_eig = 0): the batch then
-    has K = 0 and serves implicit nets only."""
+    has K = 0 and serves implicit nets only.
+
+    ``MeshBatch(items)`` is ``MeshDataset(items).batch(range(len(items)))``: the layout is planned (and a batch too
+    large for it refused) before anything is copied."""
 
     def __init__(self, items, device=None):
-        lib = _lib.load()
-        self.n_meshes = B = len(items)
-        if B < 1:
-            raise ValueError("MeshBatch needs at least one mesh")
-        dev = torch.device(device) if device is not None else items[0]["mass"].device
-        if dev.type != "cuda":
-            raise RuntimeError("diffusion_net_b200 runs on CUDA tensors only (no CPU fallback)")
-        self.device = dev
-        self.n_rows = [int(it["mass"].shape[0]) for it in items]
-        n_eig = lambda it: (int(it["evals"].shape[0]) if it.get("evals") is not None else 0,
-                            int(it["evecs"].shape[1]) if it.get("evecs") is not None else 0)
-        K = n_eig(items[0])[0]
-        if any(n_eig(it) != (K, K) for it in items):
-            raise ValueError("every mesh of a batch needs the same number of eigenpairs")
-        has_lap = [it.get("L") is not None for it in items]
-        if any(has_lap) and not all(has_lap):
-            raise ValueError("MeshBatch: 'L' must be given for every item or for none")
-        if K == 0 and not all(has_lap):
-            raise ValueError("MeshBatch: items without eigenpairs need the Laplacian 'L' (implicit diffusion)")
-        self.K = K
-        n_rows = np.asarray(self.n_rows, dtype=np.int32)
-        row_begin = np.zeros(B + 1, dtype=np.int32)
-        tiles_max = int(sum((v + 127) // 128 for v in self.n_rows))
-        tile_mesh = np.zeros(max(tiles_max, 1), dtype=np.int32)
-        tb_rows = np.zeros(2 * 1024, dtype=np.int32)
-        cta_begin = np.zeros(B + 1, dtype=np.int32)
-        sm = C.c_int(0)
-        cc = C.c_int(0)
-        smem = C.c_int64(0)
-        idx = dev.index if dev.index is not None else torch.cuda.current_device()
-        _lib.check(lib.dn_device_query(idx, C.byref(sm), C.byref(cc), C.byref(smem)), "dn_device_query")
-        n_ctas = lib.dn_mesh_batch_plan(B, n_rows.ctypes.data, int(sm.value), row_begin.ctypes.data, tile_mesh.ctypes.data,
-                                        tb_rows.ctypes.data, cta_begin.ctypes.data)
-        if n_ctas < 0:
-            _lib.check(n_ctas, "dn_mesh_batch_plan")
-        self.row_begin = [int(v) for v in row_begin]
-        self.V = V = self.row_begin[-1]
-        f32 = dict(dtype=torch.float32, device=dev)
-        self.mass = torch.zeros(V, **f32)
-        self.evecs = torch.zeros(V, K, **f32)
-        self.evals = torch.empty(B, K, **f32)
-        rp = [np.zeros(1, dtype=np.int64)]
-        cols, vals = [], []
-        nnz = 0
-        for b, it in enumerate(items):
-            r0, n = self.row_begin[b], self.n_rows[b]
-            self.mass[r0:r0 + n] = it["mass"].to(**f32)
-            if K:
-                self.evecs[r0:r0 + n] = it["evecs"].to(**f32)
-                self.evals[b] = it["evals"].to(**f32)
-            g = it["gradX"]
-            if not isinstance(g, ops.GradOperators):
-                g = ops.prepare_operators(it["gradX"].to(dev), it["gradY"].to(dev))
-            rowptr, colidx, gv = g.to_host_csr()
-            rowptr = np.asarray(rowptr, dtype=np.int64)
-            pad = (self.row_begin[b + 1] - r0) - n
-            rp.append(rowptr[1:] + nnz)
-            if pad:
-                rp.append(np.full(pad, rowptr[-1] + nnz, dtype=np.int64))
-            cols.append(np.asarray(colidx, dtype=np.int64) + r0)
-            vals.append(np.asarray(gv, dtype=np.float32).reshape(-1, 2))
-            nnz += int(rowptr[-1])
-        rowptr = torch.from_numpy(np.concatenate(rp).astype(np.int32)).to(dev)
-        colidx = torch.from_numpy(np.concatenate(cols).astype(np.int32)).to(dev)
-        vals_xy = torch.from_numpy(np.concatenate(vals)).to(dev)
-        self.gops = ops.GradOperators.from_csr(V, rowptr, colidx, vals_xy)
-        self._tile_mesh = torch.from_numpy(tile_mesh[:max(V // 128, 1)].copy()).to(dev)
-        self._tb_rows = torch.from_numpy(tb_rows[:2 * n_ctas].copy()).to(dev)
-        self._cta_begin = torch.from_numpy(cta_begin).to(dev)
-        self.desc = _lib.dn_mesh_batch(B, n_ctas, self._tile_mesh.data_ptr(), self._tb_rows.data_ptr(),
-                                       self._cta_begin.data_ptr())
-        # rows [begin, end) of every mesh, for the implicit solve, and the block-diagonal Laplacian
-        rows = np.stack([row_begin[:-1], row_begin[:-1] + n_rows], 1).astype(np.int32)
-        self._mesh_rows = torch.from_numpy(rows.reshape(-1).copy()).to(dev)
-        self.has_laplacian = all(has_lap)
-        self._laps = [it["L"] for it in items] if self.has_laplacian else None
-        self._lap = None
-        # one row segment per mesh, for the mass-weighted mean of outputs_at 'global_mean' (ops.global_mean_pool)
-        self.segments = ops.Segments(self.row_begin[:-1], self.n_rows, V, dev)
+        dev, n_rows, K, has_lap = _check_items(items, device)
+        sm = _sm_count(dev)
+        plan = plan_rows(n_rows, sm)        # more than 1024 meshes or int32 rows: refused before anything is copied
+        ds = MeshDataset.__new__(MeshDataset)
+        ds._build(items, dev, n_rows, K, has_lap, sm)
+        self._gather_from(ds, list(range(len(items))), plan)
+        self._private_source = True         # nothing else draws from this dataset: lap may drop it once built
+
+    def _gather_from(self, ds, ids, plan=None):
+        dev = ds.device
+        n_faces, n_edges = (ds._elems[k][1] if k in ds._elems else None for k in ("faces", "edges"))
+        t = batch_tables(ids, ds.n_rows, ds._grad_nnz, n_faces, n_edges, ds._sm, plan)
+        self.n_meshes = B = len(ids)
+        self.device, self.K = dev, ds.K
+        self.n_rows = [ds.n_rows[i] for i in ids]
+        self.row_begin = [int(v) for v in t["row_begin"]]
+        self.V = V = t["V"]
+        self._table_host = tab = t["table"]
+        (self._table, self._tile_mesh, self._tb_rows, self._cta_begin, self._mesh_rows, seg_begin, seg_rows,
+         tile_seg) = _upload([tab, t["tile_mesh"], t["tb_rows"], t["cta_begin"], t["mesh_rows"], t["seg_begin"],
+                              t["seg_rows"], t["tile_seg"]], dev)
+        f32, i32 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.int32, device=dev)
+        self.mass = torch.empty(V, **f32)
+        self.evecs = torch.empty(V, ds.K, **f32)
+        self.evals = torch.empty(B, ds.K, **f32)
+        rowptr, colidx = torch.empty(V + 1, **i32), torch.empty(t["nnz"], **i32)
+        vals_xy = torch.empty(t["nnz"], 2, **f32)
+        g_rowptr, g_colidx, g_vals = ds._grad
+        COPY, ADD32, ADD64 = _lib.GATHER_COPY, _lib.GATHER_ADD_I32, _lib.GATHER_ADD_I64
+        parts = [(_part(ds.mass, self.mass, COPY, 1, R_ROWS, tab), self.mass),
+                 (_part(ds.evecs, self.evecs, COPY, ds.K, R_ROWS, tab), self.evecs),
+                 (_part(ds.evals, self.evals, COPY, ds.K, R_MESH, tab), self.evals),
+                 (_part(g_rowptr, rowptr, ADD32, 1, R_PTR, tab, R_ENT), rowptr),
+                 (_part(g_colidx, colidx, ADD32, 1, R_ENT, tab, R_ROWS), colidx),
+                 (_part(g_vals, vals_xy, COPY, 2, R_ENT, tab), vals_xy)]
         # elements for outputs_at 'faces' / 'edges', vertex ids offset to batch rows (None unless every item has them)
         self.faces, self.edges, self._elem_counts = None, None, {}
-        for name in ("faces", "edges"):
-            if all(it.get(name) is not None for it in items):
-                els = [torch.as_tensor(it[name]).to(device=dev, dtype=torch.int64) for it in items]
-                setattr(self, name, torch.cat([e + r0 for e, r0 in zip(els, self.row_begin)], 0))
-                self._elem_counts[name] = [int(e.shape[0]) for e in els]
+        for name, rng in (("faces", R_FACES), ("edges", R_EDGES)):
+            if name in ds._elems:
+                src, counts = ds._elems[name]
+                out = torch.empty((int(tab[:, rng, 2].sum()),) + tuple(src.shape[1:]), dtype=torch.int64, device=dev)
+                parts.append((_part(src, out, ADD64, int(np.prod(src.shape[1:])), rng, tab, R_ROWS), out))
+                setattr(self, name, out)
+                self._elem_counts[name] = [counts[i] for i in ids]
+        _gather(parts, self._table, B, dev)
+        self.gops = ops.GradOperators.from_csr(V, rowptr, colidx, vals_xy)
+        self.desc = _lib.dn_mesh_batch(B, t["n_ctas"], self._tile_mesh.data_ptr(), self._tb_rows.data_ptr(),
+                                       self._cta_begin.data_ptr())
+        # one row segment per mesh, for the mass-weighted mean of outputs_at 'global_mean' (ops.global_mean_pool)
+        self.segments = ops.Segments.wrap(V, seg_begin, seg_rows, tile_seg)
+        self.has_laplacian = ds.has_laplacian
+        self._source, self._ids, self._lap, self._private_source = ds._lap, ids, None, False
 
     @property
     def lap(self):
-        """The batch's block-diagonal ops.LaplacianCSR (built once, on first use), or None without L."""
-        if self._lap is None and self._laps is not None:
-            self._lap = self._block_laplacian(self._laps, self.device)
-            self._laps = None
+        """The batch's block-diagonal ops.LaplacianCSR (built once, on first use, by a second dn_batch_gather), or
+        None without L."""
+        if self._lap is None and self.has_laplacian:
+            l_rowptr, l_colidx, l_vals, l_nnz = self._source.get()
+            tab = gather_table(self._ids, self._source.n_rows, self.row_begin, l_nnz)
+            nnz = _int32_entries(tab, "Laplacian")
+            table, = _upload([tab], self.device)
+            i32 = dict(dtype=torch.int32, device=self.device)
+            rowptr, colidx = torch.empty(self.V + 1, **i32), torch.empty(nnz, **i32)
+            vals = torch.empty(nnz, 2, dtype=torch.float32, device=self.device)
+            _gather([(_part(l_rowptr, rowptr, _lib.GATHER_ADD_I32, 1, R_PTR, tab, R_ENT), rowptr),
+                     (_part(l_colidx, colidx, _lib.GATHER_ADD_I32, 1, R_ENT, tab, R_ROWS), colidx),
+                     (_part(l_vals, vals, _lib.GATHER_COPY, 2, R_ENT, tab), vals)], table, self.n_meshes, self.device)
+            self._lap = ops.LaplacianCSR.from_csr(self.V, rowptr, colidx, vals)
+            if self._private_source:        # MeshBatch(items): its dataset's Laplacian copy is not needed any more
+                self._source = None
         return self._lap
-
-    def _block_laplacian(self, Ls, dev):
-        """One ops.LaplacianCSR over the batch layout: mesh b's CSR with its columns offset to its rows, padding rows
-        empty (the per-mesh CSRs are built or taken as prepared, then laid out on the host once)."""
-        rp = [np.zeros(1, dtype=np.int64)]
-        cols, vals = [], []
-        nnz = 0
-        for b, L in enumerate(Ls):
-            lap = L if isinstance(L, ops.LaplacianCSR) else ops.prepare_laplacian(L.to(dev))
-            r0, n = self.row_begin[b], self.n_rows[b]
-            if not isinstance(lap, ops.LaplacianCSR) or lap.V != n:
-                raise ValueError("MeshBatch: mesh {} has {} vertices but its L is not a ({}, {}) Laplacian".format(
-                    b, n, n, n))
-            _, rowptr, colidx, cv = lap.csr
-            rowptr = rowptr.cpu().numpy().astype(np.int64)
-            rp.append(rowptr[1:] + nnz)
-            pad = (self.row_begin[b + 1] - r0) - n
-            if pad:
-                rp.append(np.full(pad, rowptr[-1] + nnz, dtype=np.int64))
-            cols.append(colidx[:lap.nnz].cpu().numpy().astype(np.int64) + r0)
-            vals.append(cv[:2 * lap.nnz].cpu().numpy().reshape(-1, 2))
-            nnz += lap.nnz
-        if nnz >= 2 ** 31:
-            raise ValueError("MeshBatch: the batch Laplacian has {} entries, more than int32 indices hold".format(nnz))
-        return ops.LaplacianCSR.from_csr(self.V, torch.from_numpy(np.concatenate(rp).astype(np.int32)).to(dev),
-                                         torch.from_numpy(np.concatenate(cols).astype(np.int32)).to(dev),
-                                         torch.from_numpy(np.concatenate(vals).astype(np.float32)).to(dev))
 
     def elem_counts(self, name):
         """Number of 'faces' or 'edges' of every mesh (the split of the batch's element outputs)."""

@@ -1125,6 +1125,20 @@ int dn_mesh_batch_plan(int n_meshes, const int32_t* n_rows_host, int sm_count, i
   return n_ctas;
 }
 
+int dn_batch_gather(const dn_gather_part* parts_host, int n_parts, const int64_t* table, int n_ranges, int n_meshes,
+                    dn_stream_t stream) {
+  if (!parts_host || n_parts < 1 || n_parts > DN_GATHER_MAX_PARTS || !table || n_ranges < 1 || n_meshes < 1 ||
+      n_meshes > 65535)
+    return DN_ERR_INVALID_ARGUMENT;
+  for (int p = 0; p < n_parts; ++p) {
+    const dn_gather_part& q = parts_host[p];
+    if (!q.src || !q.dst || q.width < 1 || q.range < 0 || q.range >= n_ranges || q.max_units < 0) return DN_ERR_INVALID_ARGUMENT;
+    if (q.op != DN_GATHER_COPY && q.op != DN_GATHER_ADD_I32 && q.op != DN_GATHER_ADD_I64) return DN_ERR_INVALID_ARGUMENT;
+    if (q.op != DN_GATHER_COPY && (q.offset_range < 0 || q.offset_range >= n_ranges)) return DN_ERR_INVALID_ARGUMENT;
+  }
+  return launch_batch_gather(parts_host, n_parts, table, n_ranges, n_meshes, (cudaStream_t)stream);
+}
+
 int dn_block_fwd_profile(const float* x_in, const float* mass, const float* evals, const float* evecs,
                          const dn_csr* grad, const dn_block_params* p, int64_t V, int K, int C, float* out,
                          void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream, float* stage_ms_host) {

@@ -191,6 +191,10 @@ int launch_spectral_bwd(const float* gs_partial, int P, const float* evals, cons
 int launch_spectral_time_grad_batched(const float* G, const float* x_spec, const float* evals, const float* time,
                                       int n_meshes, int K, int C, float* grad_time, cudaStream_t st);
 
+// a mesh batch gathered from a dataset (dn_batch_gather.cu); parts were checked by dn_batch_gather
+int launch_batch_gather(const dn_gather_part* parts, int n_parts, const int64_t* table, int n_ranges, int n_meshes,
+                        cudaStream_t st);
+
 // ---- wgmma engine (dn_tc.cu) ----
 // Per-device table, filled on first use of a device: whether it runs the tensor-core kernels (sm_90, with their
 // >48 KB dynamic shared memory attributes set on it) and its SM count (1 if it cannot be queried), which sizes grids

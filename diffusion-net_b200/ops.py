@@ -1143,12 +1143,23 @@ class Segments:
 
     def __init__(self, begin, rows, V, device):
         begin, rows = [int(b) for b in begin], [int(n) for n in rows]
+        tile_seg = self.tile_table(begin, rows, V)
+        self.n_seg, self.V = len(begin), int(V)
+        i32 = dict(dtype=torch.int32, device=device)
+        self.begin = torch.tensor(begin, **i32)
+        self.rows = torch.tensor(rows, **i32)
+        self.tile_seg = torch.tensor(tile_seg, **i32)
+
+    @staticmethod
+    def tile_table(begin, rows, V):
+        """The segment of every 128-row tile of [0, V) (-1 for none), after checking the segments' invariants."""
         V = int(V)
-        if not begin or len(begin) != len(rows):
+        if len(begin) == 0 or len(begin) != len(rows):
             raise ValueError("Segments: one begin and one row count per segment, at least one segment")
         n_tiles = (V + 127) // 128
         tile_seg = [-1] * n_tiles
         for b, (r0, n) in enumerate(zip(begin, rows)):
+            r0, n = int(r0), int(n)
             if r0 % 128 or n < 0 or r0 + n > V:
                 raise ValueError("Segments: segment {} = rows [{}, {}) must begin on a 128-row tile inside [0, {})".format(
                     b, r0, r0 + n, V))
@@ -1156,11 +1167,16 @@ class Segments:
                 if tile_seg[t] != -1:
                     raise ValueError("Segments: segments {} and {} share tile {}".format(tile_seg[t], b, t))
                 tile_seg[t] = b
-        self.n_seg, self.V = len(begin), V
-        i32 = dict(dtype=torch.int32, device=device)
-        self.begin = torch.tensor(begin, **i32)
-        self.rows = torch.tensor(rows, **i32)
-        self.tile_seg = torch.tensor(tile_seg, **i32)
+        return tile_seg
+
+    @classmethod
+    def wrap(cls, V, begin, rows, tile_seg):
+        """Segments over device int32 tables already built by ``tile_table`` and uploaded (``batch.MeshDataset``
+        uploads them with the rest of a batch's tables in one copy)."""
+        self = cls.__new__(cls)
+        self.n_seg, self.V = int(begin.numel()), int(V)
+        self.begin, self.rows, self.tile_seg = begin, rows, tile_seg
+        return self
 
 
 _single_segment_cache = {}

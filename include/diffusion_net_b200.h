@@ -421,6 +421,34 @@ typedef struct dn_mesh_batch {
 int dn_mesh_batch_plan(int n_meshes, const int32_t* n_rows_host, int sm_count, int32_t* row_begin_host,
                        int32_t* tile_mesh_host, int32_t* tb_rows_host, int32_t* mesh_cta_begin_host);
 
+/* A batch gathered from a device-resident dataset (batch.MeshDataset): the dataset holds every mesh's arrays back to
+ * back (no padding, int64 offsets), and one call writes any batch of its meshes in the layout above.  Each "part" is one
+ * array, copied mesh by mesh in units (a row, a CSR entry, a face, a mesh) of `width` elements.  `table` (device int64
+ * [n_meshes][n_ranges][4]) names for batch mesh b and range r the tuple (src_begin, dst_begin, n, n_dst) in units:
+ * units [0, n) of the mesh come from src units [src_begin, src_begin + n) and go to dst units [dst_begin, ...); units
+ * [n, n_dst) are padding; only the first min(n, n_dst) source units are written when n > n_dst.  The ops:
+ *   DN_GATHER_COPY:    4-byte words copied as they are; padding written as 0 (fp32 rows, interleaved CSR values,
+ *                      eigenvalues, and int64 data as word pairs);
+ *   DN_GATHER_ADD_I32, DN_GATHER_ADD_I64: int32 / int64 entries plus the mesh's offset o = dst_begin of range
+ *                      `offset_range`; padding written as o + n of that range (mesh-local column and vertex indices
+ *                      rebased to batch rows, and mesh-local row pointers rebased to batch entries, padding rows empty).
+ * Every batch value must fit the element type (the caller checks: a batch is int32-indexed).  `max_units` is the largest
+ * n_dst of the part's range over the meshes; it sizes the grid only.  Parts must not overlap in dst.  One launch for up
+ * to DN_GATHER_MAX_PARTS parts and 65535 meshes; nothing is read back, so the call never waits on the device. */
+#define DN_GATHER_MAX_PARTS 16
+enum dn_gather_op { DN_GATHER_COPY = 0, DN_GATHER_ADD_I32 = 1, DN_GATHER_ADD_I64 = 2 };
+typedef struct dn_gather_part {
+  const void* src;       /* dataset array                                     */
+  void* dst;             /* batch array                                       */
+  int32_t op;            /* dn_gather_op                                      */
+  int32_t width;         /* elements per unit (4-byte words for DN_GATHER_COPY) */
+  int32_t range;         /* range of `table` that places this array's units   */
+  int32_t offset_range;  /* ADD ops: range whose dst_begin is added           */
+  int64_t max_units;
+} dn_gather_part;
+int dn_batch_gather(const dn_gather_part* parts_host, int n_parts, const int64_t* table, int n_ranges, int n_meshes,
+                    dn_stream_t stream);
+
 /* dn_block_fwd over a batch laid out as above (V = padded total, a multiple of 128).  Tensor-core engines only
  * (DN_ERR_UNSUPPORTED otherwise and for shapes outside the fused kernels' envelope: the caller loops over meshes). */
 int dn_block_fwd_batched(const float* x_in, const float* mass, const float* evals, const float* evecs,

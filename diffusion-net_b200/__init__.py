@@ -14,4 +14,4 @@ from .fmaps import (FunctionalMapCorrespondenceWithDiffusionNetFeatures, compute
                     pointwise_map, PairBatch, pointwise_map_batch)
 from .geometry import to_basis, from_basis  # noqa: F401,E402
 from .ops import set_engine, get_engine, prepare_operators  # noqa: F401,E402
-from .batch import MeshBatch, MeshDataset  # noqa: F401,E402
+from .batch import BatchSlot, MeshBatch, MeshDataset  # noqa: F401,E402

@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libdiffusion_net_b200.so")
 SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_eig.cu", "dn_implicit.cu", "dn_implicit_batch.cu", "dn_batch_gather.cu",
-           "dn_fmap.cu", "dn_fmap_batch.cu", "dn_tc.cu", "dn_head.cu", "dn_capi.cu"]
+           "dn_batch_plan.cu", "dn_fmap.cu", "dn_fmap_batch.cu", "dn_tc.cu", "dn_head.cu", "dn_capi.cu"]
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "diffusion_net_b200.h")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -76,6 +76,11 @@ class dn_gather_part(C.Structure):
 
 GATHER_COPY, GATHER_ADD_I32, GATHER_ADD_I64 = 0, 1, 2
 GATHER_MAX_PARTS = 16
+
+
+class dn_slot_plan(C.Structure):
+    _fields_ = [(name, C.c_void_p) for name in ("row_begin", "tile_mesh", "tb_rows", "mesh_cta_begin", "seg_begin",
+                                                "seg_rows", "tile_seg", "table", "status")]
 
 
 class dn_eig_batch(C.Structure):
@@ -146,6 +151,7 @@ SIGNATURES = {
     "dn_nearest_neighbor": (_I, [_P, _L, _P, _L, _I, _P, _P, _L, _P]),
     "dn_mesh_batch_plan": (_I, [_I, _P, _I, _P, _P, _P, _P]),
     "dn_batch_gather": (_I, [C.POINTER(dn_gather_part), _I, _P, _I, _I, _P]),
+    "dn_mesh_batch_plan_device": (_I, [_P, _I, _P, _L, _I, _L, _L, _I, _L, _I, C.POINTER(dn_slot_plan), _P]),
     "dn_block_fwd_ex": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),
                              C.POINTER(dn_head), _L, _I, _I, _P, _P, _L, _I, _P]),
     "dn_block_fwd_batched": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),

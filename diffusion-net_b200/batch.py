@@ -290,23 +290,51 @@ class MeshDataset:
         only: a tensor that requires grad is refused (per-mesh lists still go through ``MeshBatch.pack``)."""
         if getattr(batch, "_source", None) is not self._lap:
             raise ValueError("MeshDataset.pack: the batch was not drawn from this dataset")
-        if not torch.is_tensor(t) or t.dim() not in (1, 2) or t.shape[0] != self.V or \
-                t.dtype not in (torch.float32, torch.int64):
-            raise ValueError("MeshDataset.pack: expected a float32 or int64 tensor of shape ({0},) or ({0}, C) in the "
-                             "dataset layout, got {1}".format(self.V, (tuple(t.shape), t.dtype) if torch.is_tensor(t)
-                                                              else type(t)))
-        if t.requires_grad:
-            raise ValueError("MeshDataset.pack gathers data; got a tensor that requires grad (pack per-mesh "
-                             "tensors with MeshBatch.pack to differentiate through the layout)")
-        ops._require_cuda(t)
-        if t.device != batch.device:
-            raise ValueError("MeshDataset.pack: the tensor is on {}, the dataset on {}".format(t.device, batch.device))
+        self._check_pack(t, "MeshDataset.pack")
         t = t.contiguous()
         out = torch.empty((batch.V,) + tuple(t.shape[1:]), dtype=t.dtype, device=batch.device)
         width = (t.shape[1] if t.dim() == 2 else 1) * (2 if t.dtype == torch.int64 else 1)
         _gather([(_part(t, out, _lib.GATHER_COPY, width, R_ROWS, batch._table_host), out)], batch._table,
                 batch.n_meshes, batch.device)
         return out
+
+    def slot(self, n_meshes, max_rows=None, max_entries=None):
+        """A ``BatchSlot`` of ``n_meshes`` meshes of this dataset: a batch whose buffers never move, refilled on the
+        device from any mesh ids, so that a shuffled training step can be captured in one CUDA graph.  Its default
+        capacity holds any ``n_meshes`` distinct meshes; ``max_rows`` / ``max_entries`` set it instead."""
+        return BatchSlot(self, n_meshes, max_rows, max_entries)
+
+    def _check_pack(self, t, what):
+        if not torch.is_tensor(t) or t.dim() not in (1, 2) or t.shape[0] != self.V or \
+                t.dtype not in (torch.float32, torch.int64):
+            raise ValueError("{0}: expected a float32 or int64 tensor of shape ({1},) or ({1}, C) in the dataset layout, "
+                             "got {2}".format(what, self.V, (tuple(t.shape), t.dtype) if torch.is_tensor(t)
+                                              else type(t)))
+        if t.requires_grad:
+            raise ValueError("{} gathers data; got a tensor that requires grad (pack per-mesh tensors with "
+                             "MeshBatch.pack to differentiate through the layout)".format(what))
+        ops._require_cuda(t)
+        if t.device != self.device:
+            raise ValueError("{}: the tensor is on {}, the dataset on {}".format(what, t.device, self.device))
+
+    def _slot_tables(self):
+        """What every slot reads, built on first slot creation: the per-mesh size table on the device, and every mesh's
+        transposed gradient CSR back to back in the forward CSR's layout (the transpose of a block-diagonal matrix is
+        the block diagonal of the transposes, so a slot gathers it like the forward CSR and never transposes)."""
+        if getattr(self, "_slot_data", None) is None:
+            rowptr, colidx, vals = self._grad
+            parts, ent0 = [], 0
+            for i, (r0, n, nnz) in enumerate(zip(self.row_begin, self.n_rows, self._grad_nnz)):
+                g = ops.GradOperators.from_csr(n, rowptr[r0 + i:r0 + i + n + 1], colidx[ent0:ent0 + nnz],
+                                               vals[2 * ent0:2 * (ent0 + nnz)].view(-1, 2))
+                _, rt, ct, vt = g.csr_t
+                parts.append((rt, ct[:nnz], vt[:2 * nnz]))
+                ent0 += nnz
+            grad_t = tuple(torch.cat(p) for p in zip(*parts))
+            sizes = np.stack([np.asarray(self.n_rows, np.int64), np.asarray(self.row_begin[:-1], np.int64),
+                              np.asarray(self._grad_nnz, np.int64), _starts(self._grad_nnz)[:-1]], 1)
+            self._slot_data = (torch.from_numpy(sizes).to(self.device), grad_t)
+        return self._slot_data
 
 
 class MeshBatch:
@@ -413,6 +441,230 @@ class MeshBatch:
 
     def unpack(self, y):
         return [y[self.row_begin[b]:self.row_begin[b] + self.n_rows[b]] for b in range(self.n_meshes)]
+
+
+def slot_capacity(n_rows, n_ent, n_meshes, sm_count):
+    """(V_cap, entry_cap, n_tb_ctas) of a slot that holds any ``n_meshes`` distinct meshes of a dataset whose meshes
+    have ``n_rows`` rows and ``n_ent`` gradient entries: the sum of the n_meshes largest padded row counts (at least one
+    tile), the sum of the n_meshes largest entry counts (taken on their own: they may be other meshes'), and the
+    to_basis grid min(1024, sm_count + n_meshes).
+
+    The grid bound: dn_mesh_batch_plan gives mesh b want_b = round(chunks_b sm / total) CTAs, raised to 1, lowered to
+    chunks_b, lowered to 1 near the 1024 budget, then lowered again to ceil(chunks_b / per).  Rounding adds at most 1/2
+    and raising to 1 makes a value below 1/2 into 1, so want_b <= chunks_b sm / total + 1 and the batch uses at most
+    sum_b (chunks_b sm / total + 1) = sm + n_meshes CTAs, and never more than 1024."""
+    padded = sorted(((int(n) + 127) // 128 * 128 for n in n_rows), reverse=True)
+    v_cap = max(sum(padded[:n_meshes]), 128)
+    e_cap = sum(sorted((int(e) for e in n_ent), reverse=True)[:n_meshes])
+    return v_cap, e_cap, min(1024, int(sm_count) + n_meshes)
+
+
+_ST_BAD_ID, _ST_OVER_CAPACITY = 1, 2
+
+
+class BatchSlot:
+    """A batch of ``n_meshes`` meshes of a ``MeshDataset`` whose device buffers never move: ``fill(ids)`` rewrites
+    their contents from any mesh ids with a fixed launch sequence (a device planner, ``dn_mesh_batch_plan_device``, and
+    one ``dn_batch_gather``) that reads nothing back and allocates nothing, so a shuffled training step, fill
+    included, can be captured in one CUDA graph (``graphs.GraphedTrainStep``) and replayed with new ids::
+
+        slot = ds.slot(32)
+        ids = torch.zeros(32, dtype=torch.int64, device="cuda")
+        def step(net, ids):
+            slot.fill(ids)
+            return net.forward_batch_global_nll(slot, slot.pack(X), slot.take(Y), label_smoothing=0.2)[0].sum()
+        g = dn.graphs.GraphedTrainStep(net, step, (ids,))
+        for chunk in torch.randperm(len(ds), device="cuda").split(32):   # a short last chunk needs its own slot
+            if len(chunk) == 32:
+                ids.copy_(chunk); g.zero_grads(net); g.replay(); opt.step()
+
+    The reference's loop (one mesh per step, ``batch_size=None``) is ``ds.slot(1)`` with one graph.
+
+    Fixed for the slot's life: ``n_meshes``, ``V`` (the row capacity V_cap), the gradient entry capacity, the to_basis
+    grid and so every workspace size (``slot_capacity``).  A filled slot is ``ds.batch(ids)``'s layout on the batch's
+    rows, bitwise, and the rows past them up to V are padding of the last mesh (mass, evecs and features 0, no
+    gradient entries, tiles of the last mesh, outside every global-mean segment).  The to_basis CTAs past the batch's
+    own get empty row ranges that no mesh reduces.  The backward's transposed gradient CSR is gathered from per-mesh
+    transposes the dataset builds once.
+
+    A fill from host ids checks them first (``MeshDataset.batch``'s errors, and a ValueError for a batch past the
+    capacity, possible with repeats).  Device ids are checked on the device: an id outside the dataset or a batch past
+    the capacity reads nothing through the ids and plans every mesh empty, so the step computes NaN for every loss
+    (0 / 0 means) and NaN parameter gradients, and sets a sticky status that ``check()`` reads.
+
+    Spectral nets on ``forward_batch_global_nll`` and on ``forward_batch_nll`` with per-vertex labels in the batch
+    layout (``pack``).  A slot keeps no host copy of its layout: ``n_rows``, ``row_begin``, ``unpack``,
+    ``elem_counts``, ``forward_batch``, 'faces' / 'edges' outputs and implicit nets raise NotImplementedError."""
+
+    def __init__(self, ds, n_meshes, max_rows=None, max_entries=None):
+        n_meshes = operator.index(n_meshes)
+        if n_meshes < 1:
+            raise ValueError("MeshDataset.slot needs at least one mesh")
+        if n_meshes > 1024:
+            _lib.check(-2, "MeshDataset.slot ({} meshes; at most 1024)".format(n_meshes))
+        if ds.K == 0:
+            raise ValueError("MeshDataset.slot: the dataset has no eigenpairs (k_eig = 0); a slot serves spectral nets")
+        v_cap, e_cap, n_ctas = slot_capacity(ds.n_rows, ds._grad_nnz, n_meshes, ds._sm)
+        if max_rows is not None:
+            v_cap = max((operator.index(max_rows) + 127) // 128 * 128, 128)
+        if max_entries is not None:
+            e_cap = operator.index(max_entries)
+        if v_cap >= _INT32_LIMIT - 256:
+            _lib.check(-2, "MeshDataset.slot ({} rows)".format(v_cap))
+        if e_cap >= _INT32_LIMIT or e_cap < 0:
+            raise ValueError("MeshBatch: the batch gradient operators have {} entries, more than int32 indices "
+                             "hold".format(e_cap))
+        sizes, (g_rowptr_t, g_colidx_t, g_vals_t) = ds._slot_tables()
+        self._ds, self._sizes = ds, sizes
+        self.device, self.K, self.n_meshes, self.V = ds.device, ds.K, n_meshes, v_cap
+        self.entry_capacity = e_cap
+        B, dev = n_meshes, ds.device
+        # tail pieces no longer than the dataset's largest mesh: every gather grid is sized like ds.batch's
+        pad_max = max(max((n + 127) // 128 * 128 for n in ds.n_rows), 128)
+        self._tail = max(pad_max, -(-v_cap // (128 * B)) * 128)
+        i32, i64, f32 = (dict(dtype=t, device=dev) for t in (torch.int32, torch.int64, torch.float32))
+        self.ids = torch.zeros(B, **i64)
+        self.status = torch.zeros(3, **i64)
+        n_tiles = v_cap // 128
+        (self._row_begin, self._tile_mesh, self._tb_rows, self._cta_begin, seg_begin, seg_rows, tile_seg) = (
+            torch.zeros(n, **i32) for n in (B + 1, n_tiles, 2 * n_ctas, B + 1, B, B, n_tiles))
+        self._table = torch.zeros(2 * B, N_RANGES, 4, **i64)
+        self._plan = _lib.dn_slot_plan(*(t.data_ptr() for t in (
+            self._row_begin, self._tile_mesh, self._tb_rows, self._cta_begin, seg_begin, seg_rows, tile_seg,
+            self._table, self.status)))
+        self._n_ctas = n_ctas
+        self.mass = torch.zeros(v_cap, **f32)
+        self.evecs = torch.zeros(v_cap, ds.K, **f32)
+        self.evals = torch.zeros(B, ds.K, **f32)
+        rowptr, rowptr_t = torch.zeros(v_cap + 1, **i32), torch.zeros(v_cap + 1, **i32)
+        colidx, colidx_t = torch.zeros(e_cap, **i32), torch.zeros(e_cap, **i32)
+        vals, vals_t = torch.zeros(e_cap, 2, **f32), torch.zeros(e_cap, 2, **f32)
+        g_rowptr, g_colidx, g_vals = ds._grad
+        ent_max = max(ds._grad_nnz)
+        COPY, ADD32 = _lib.GATHER_COPY, _lib.GATHER_ADD_I32
+        part = lambda src, dst, op, width, rng, n, off=0: (_lib.dn_gather_part(src.data_ptr(), dst.data_ptr(), op,
+                                                                                width, rng, off, n), dst)
+        parts = [part(ds.mass, self.mass, COPY, 1, R_ROWS, self._tail),
+                 part(ds.evecs, self.evecs, COPY, ds.K, R_ROWS, self._tail),
+                 part(ds.evals, self.evals, COPY, ds.K, R_MESH, 1)]
+        for (r_src, c_src, v_src), (r_dst, c_dst, v_dst) in (((g_rowptr, g_colidx, g_vals), (rowptr, colidx, vals)),
+                                                              ((g_rowptr_t, g_colidx_t, g_vals_t),
+                                                               (rowptr_t, colidx_t, vals_t))):
+            parts += [part(r_src, r_dst, ADD32, 1, R_PTR, self._tail + 1, R_ENT),
+                      part(c_src, c_dst, ADD32, 1, R_ENT, ent_max, R_ROWS),
+                      part(v_src, v_dst, COPY, 2, R_ENT, ent_max)]
+        parts = [p for p, dst in parts if dst.numel() > 0]
+        self._parts = (_lib.dn_gather_part * len(parts))(*parts)
+        self.gops = ops.GradOperators.from_csr(v_cap, rowptr, colidx, vals)
+        self.gops._csr_t = (_lib.dn_csr(rowptr_t.data_ptr(), colidx_t.data_ptr(), vals_t.data_ptr(), e_cap),
+                            rowptr_t, colidx_t, vals_t)
+        self.desc = _lib.dn_mesh_batch(B, n_ctas, self._tile_mesh.data_ptr(), self._tb_rows.data_ptr(),
+                                       self._cta_begin.data_ptr())
+        self.segments = ops.Segments.wrap(v_cap, seg_begin, seg_rows, tile_seg)
+        self.has_laplacian, self.lap, self.faces, self.edges = False, None, None, None
+        self._mesh_ids = self._table[:B, R_MESH, 0]     # the filled ids; 0 for an invalid fill
+        self._static = {}
+
+    def fill(self, ids):
+        """Plan and gather the batch of dataset meshes ``ids``: a CUDA int64 tensor of n_meshes ids (checked on the
+        device), or a host list / CPU tensor (checked here first).  Two library launches whatever n_meshes is, no
+        host synchronisation, no allocation (host ids: one pinned upload).  Returns the slot."""
+        if torch.is_tensor(ids) and ids.device.type != "cpu":
+            if ids.dtype != torch.int64 or tuple(ids.shape) != (self.n_meshes,) or ids.device != self.device:
+                raise ValueError("BatchSlot.fill: device ids must be an int64 tensor of shape ({},) on {}, got {} of "
+                                 "shape {} on {}".format(self.n_meshes, self.device, ids.dtype, tuple(ids.shape),
+                                                         ids.device))
+            if ids.data_ptr() != self.ids.data_ptr():
+                self.ids.copy_(ids)
+        else:
+            ids = self._ds._ids(ids)
+            if len(ids) != self.n_meshes:
+                raise ValueError("BatchSlot.fill: {} ids for a slot of {} meshes".format(len(ids), self.n_meshes))
+            ds = self._ds
+            rows = sum((ds.n_rows[i] + 127) // 128 * 128 for i in ids)
+            ents = sum(ds._grad_nnz[i] for i in ids)
+            if rows > self.V or ents > self.entry_capacity:
+                raise ValueError("BatchSlot.fill: the batch needs {} rows and {} gradient entries, more than the slot's "
+                                 "capacity of {} and {}".format(rows, ents, self.V, self.entry_capacity))
+            self.ids.copy_(torch.tensor(ids, dtype=torch.int64).pin_memory(), non_blocking=True)
+        lib = _lib.load()
+        with torch.cuda.device(self.device):
+            st = ops._stream()
+            _lib.check(lib.dn_mesh_batch_plan_device(
+                self.ids.data_ptr(), self.n_meshes, self._sizes.data_ptr(), self._ds.n_meshes, self._ds._sm, self.V,
+                self.entry_capacity, self._n_ctas, self._tail, N_RANGES, C.byref(self._plan), st),
+                "dn_mesh_batch_plan_device")
+            if len(self._parts):
+                _lib.check(lib.dn_batch_gather(self._parts, len(self._parts), self._table.data_ptr(), N_RANGES,
+                                               2 * self.n_meshes, st), "dn_batch_gather")
+        return self
+
+    def check(self):
+        """Raise if a fill since the last check had invalid device ids (IndexError) or exceeded the capacity
+        (ValueError), naming the first offending position, and clear the status.  One device-to-host read."""
+        kind, pos, bad = self.status.tolist()
+        if kind:
+            self.status.zero_()
+        if kind == _ST_BAD_ID:
+            raise IndexError("BatchSlot.fill: mesh id {} at position {} is outside the dataset's {} meshes".format(
+                bad, pos, self._ds.n_meshes))
+        if kind == _ST_OVER_CAPACITY:
+            raise ValueError("BatchSlot.fill: the batch exceeds the slot's capacity of {} rows and {} gradient entries "
+                             "at position {}".format(self.V, self.entry_capacity, pos))
+
+    def _static_out(self, what, src, shape):
+        key = (what, src.data_ptr(), src.dtype, tuple(src.shape))
+        out = self._static.get(key)
+        if out is None:
+            out = self._static[key] = torch.zeros(shape, dtype=src.dtype, device=self.device)
+        return out
+
+    def pack(self, t):
+        """A dataset-layout float32 or int64 per-vertex tensor (V_total,) / (V_total, C) in the slot's layout, padding
+        rows 0: one launch into a buffer that is the same tensor on every call with the same ``t``."""
+        if isinstance(t, (list, tuple)):
+            raise NotImplementedError("BatchSlot.pack takes one tensor in the dataset layout; per-mesh lists need the "
+                                      "host layout of a MeshBatch")
+        self._ds._check_pack(t, "BatchSlot.pack")
+        out = self._static_out("pack", t, (self.V,) + tuple(t.shape[1:]))
+        t = t.contiguous()
+        width = (t.shape[1] if t.dim() == 2 else 1) * (2 if t.dtype == torch.int64 else 1)
+        if width:
+            part = _lib.dn_gather_part(t.data_ptr(), out.data_ptr(), _lib.GATHER_COPY, width, R_ROWS, 0, self._tail)
+            with torch.cuda.device(self.device):
+                _lib.check(_lib.load().dn_batch_gather(C.byref(part), 1, self._table.data_ptr(), N_RANGES,
+                                                       2 * self.n_meshes, ops._stream()), "dn_batch_gather")
+        return out
+
+    def take(self, per_mesh):
+        """``per_mesh[ids]`` (a per-mesh tensor of the dataset, e.g. whole-shape labels) into a buffer that is the same
+        tensor on every call with the same ``per_mesh``."""
+        if not torch.is_tensor(per_mesh) or per_mesh.dim() < 1 or per_mesh.shape[0] != self._ds.n_meshes or \
+                per_mesh.device != self.device:
+            raise ValueError("BatchSlot.take: expected a tensor of {} rows (one per dataset mesh) on {}, got {}".format(
+                self._ds.n_meshes, self.device, (tuple(per_mesh.shape), per_mesh.device) if torch.is_tensor(per_mesh)
+                else type(per_mesh)))
+        out = self._static_out("take", per_mesh, (self.n_meshes,) + tuple(per_mesh.shape[1:]))
+        torch.index_select(per_mesh, 0, self._mesh_ids, out=out)
+        return out
+
+    def _no_host_layout(self, what):
+        raise NotImplementedError("BatchSlot.{}: a slot keeps no host copy of its layout (it is planned on the device "
+                                  "at every fill); use ds.batch(ids) for per-mesh lists".format(what))
+
+    @property
+    def n_rows(self):
+        self._no_host_layout("n_rows")
+
+    @property
+    def row_begin(self):
+        self._no_host_layout("row_begin")
+
+    def unpack(self, y):
+        self._no_host_layout("unpack")
+
+    def elem_counts(self, name):
+        self._no_host_layout("elem_counts")
 
 
 def block_forward_batched_raw(batch, x_in, time, A_re, A_im, weights, biases, with_features, head=None):

@@ -1139,6 +1139,23 @@ int dn_batch_gather(const dn_gather_part* parts_host, int n_parts, const int64_t
   return launch_batch_gather(parts_host, n_parts, table, n_ranges, n_meshes, (cudaStream_t)stream);
 }
 
+int dn_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* dataset_sizes, int64_t n_dataset,
+                              int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas, int64_t tail_rows,
+                              int n_ranges, const dn_slot_plan* out_host, dn_stream_t stream) {
+  if (sm_count < 1) sm_count = 132;
+  const int64_t min_ctas = sm_count + (int64_t)n_meshes < 1024 ? sm_count + (int64_t)n_meshes : 1024;
+  if (!ids || !dataset_sizes || !out_host || n_meshes < 1 || n_meshes > 1024 || n_dataset < 1 || V_cap < 128 ||
+      V_cap % 128 || V_cap >= (1ll << 31) - 256 || entry_cap < 0 || entry_cap >= (1ll << 31) || n_tb_ctas < min_ctas ||
+      n_tb_ctas > 1024 || tail_rows < 1 || tail_rows * n_meshes < V_cap || n_ranges < 4)
+    return DN_ERR_INVALID_ARGUMENT;
+  const dn_slot_plan& o = *out_host;
+  if (!o.row_begin || !o.tile_mesh || !o.tb_rows || !o.mesh_cta_begin || !o.seg_begin || !o.seg_rows || !o.tile_seg ||
+      !o.table || !o.status)
+    return DN_ERR_INVALID_ARGUMENT;
+  return launch_mesh_batch_plan_device(ids, n_meshes, dataset_sizes, n_dataset, sm_count, V_cap, entry_cap, n_tb_ctas,
+                                       tail_rows, n_ranges, o, (cudaStream_t)stream);
+}
+
 int dn_block_fwd_profile(const float* x_in, const float* mass, const float* evals, const float* evecs,
                          const dn_csr* grad, const dn_block_params* p, int64_t V, int K, int C, float* out,
                          void* workspace, int64_t ws_bytes, int engine, dn_stream_t stream, float* stage_ms_host) {

@@ -234,6 +234,11 @@ class DiffusionNetBlock(nn.Module):
         return torch.stack(outs, dim=0)
 
 
+def _is_slot(batch):
+    from .batch import BatchSlot
+    return isinstance(batch, BatchSlot)
+
+
 class DiffusionNet(nn.Module):
 
     def __init__(self, C_in, C_out, C_width=128, N_block=4, last_activation=None, outputs_at='vertices',
@@ -289,6 +294,9 @@ class DiffusionNet(nn.Module):
         An implicit_dense net needs a batch whose items carry 'L'; it runs the differentiable route in inference as well
         (batched solve, gradient features, MiniMLP)."""
         self._check_batch(batch, "forward_batch")
+        if _is_slot(batch):
+            raise NotImplementedError("forward_batch returns per-mesh lists, and a BatchSlot keeps no host copy of its "
+                                      "layout: train on a slot with forward_batch_global_nll or forward_batch_nll")
         elems = None
         if self.outputs_at in ('edges', 'faces'):
             elems = batch.faces if self.outputs_at == 'faces' else batch.edges
@@ -327,6 +335,9 @@ class DiffusionNet(nn.Module):
 
     def _check_batch(self, batch, what):
         """The batch routes run spectral nets on batches with eigenpairs, implicit nets on batches with Laplacians."""
+        if self.diffusion_method == 'implicit_dense' and _is_slot(batch):
+            raise NotImplementedError("{}: a BatchSlot serves spectral nets only (the implicit solve reads its "
+                                      "convergence status on the host)".format(what))
         if self.diffusion_method == 'implicit_dense':
             if batch is None or not batch.has_laplacian:
                 raise NotImplementedError("{}: a diffusion_method='implicit_dense' net needs a MeshBatch whose items "
@@ -423,9 +434,19 @@ class DiffusionNet(nn.Module):
         """forward_nll over a ``batch.MeshBatch``: ``labels`` is the list of per-mesh label tensors (per vertex, or per
         face / edge).  Returns ``(losses, preds)``: the (n_meshes,) per-mesh mean losses and the list of per-mesh
         predictions; ``losses.sum().backward()`` accumulates the gradients of the per-mesh loop.  The blocks run on
-        forward_batch's differentiable route; padding rows of the batch layout carry ignore_index."""
+        forward_batch's differentiable route; padding rows of the batch layout carry ignore_index.
+
+        With outputs_at='vertices', ``labels`` may instead be one (V,) int64 tensor in the batch layout (``ds.pack``,
+        ``BatchSlot.pack``); the per-mesh losses are then formed on the device (the mean of the per-row nll over the
+        mesh's rows whose label is not ignore_index, NaN for a mesh without one), whatever the padding rows hold, and
+        ``preds`` is the (V,) prediction in the batch layout.  This is the route of a ``BatchSlot``."""
         self._check_nll_head()
         self._check_batch(batch, "forward_batch_nll")
+        if torch.is_tensor(labels):
+            return self._forward_batch_nll_layout(batch, xs, labels, ignore_index, label_smoothing)
+        if _is_slot(batch):
+            raise NotImplementedError("forward_batch_nll on a BatchSlot takes the labels as one (V,) tensor in the "
+                                      "batch layout (slot.pack(labels)): a slot keeps no host copy of its layout")
         if len(labels) != batch.n_meshes:
             raise ValueError("forward_batch_nll: {} label tensors for {} meshes".format(len(labels), batch.n_meshes))
         x = xs if torch.is_tensor(xs) else batch.pack(xs)
@@ -462,6 +483,34 @@ class DiffusionNet(nn.Module):
             labs = labels
         losses = torch.stack([v.sum() / (l != ignore_index).sum().to(v.dtype) for v, l in zip(nlls, labs)])
         return losses, preds
+
+    def _forward_batch_nll_layout(self, batch, xs, labels, ignore_index, label_smoothing):
+        """forward_batch_nll with (V,) labels in the batch layout: per-mesh losses from the device segment tables."""
+        if self.outputs_at != 'vertices':
+            err = NotImplementedError if _is_slot(batch) else ValueError
+            raise err("forward_batch_nll: labels in the batch layout are per vertex; outputs_at='{}' takes the list "
+                      "of per-mesh labels of a MeshBatch".format(self.outputs_at))
+        if labels.dtype != torch.int64 or tuple(labels.shape) != (batch.V,):
+            raise ValueError("forward_batch_nll: labels in the batch layout must be an int64 tensor of shape ({},), "
+                             "got {} of shape {}".format(batch.V, labels.dtype, tuple(labels.shape)))
+        x = xs if torch.is_tensor(xs) else batch.pack(xs)
+        if x.shape[-1] != self.C_in:
+            raise ValueError("DiffusionNet was constructed with C_in={}, but x_in has last dim={}".format(
+                self.C_in, x.shape[-1]))
+        ops._require_cuda(x, labels)
+        seg = batch.segments
+        x = self._forward_batch_blocks(batch, x)
+        # padding rows are ignored whatever label they hold (an out-of-range label would make its row NaN)
+        rows = torch.arange(batch.V, device=x.device)
+        s = seg.tile_seg.long()[rows >> 7]
+        sc = s.clamp(min=0)
+        real = (s >= 0) & (rows < (seg.begin.long() + seg.rows.long())[sc])
+        lab = torch.where(real, labels, torch.full_like(labels, ignore_index))
+        nll, pred = self._head_nll(x, lab, None, None, ignore_index, label_smoothing)
+        # per mesh: sum of nll / number of labelled rows, as the mass-weighted mean with weights (label != ignore)
+        w = (lab != ignore_index).to(nll.dtype)
+        losses = ops.global_mean_pool(torch.nn.functional.pad(nll[:, None], (0, 3)), w, seg)[:, 0]
+        return losses, pred
 
     def _check_global_head(self, what):
         if self.outputs_at != 'global_mean':

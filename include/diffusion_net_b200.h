@@ -449,6 +449,44 @@ typedef struct dn_gather_part {
 int dn_batch_gather(const dn_gather_part* parts_host, int n_parts, const int64_t* table, int n_ranges, int n_meshes,
                     dn_stream_t stream);
 
+/* DEVICE-side planner of a fixed-capacity batch slot (batch.BatchSlot): the layout above for the n_meshes dataset
+ * meshes ids[b] (device int64), planned in one single-CTA launch that reads nothing back, so it can be captured in a
+ * CUDA graph and replayed with new ids.  dataset_sizes (device int64 [n_dataset][4]) gives every dataset mesh's
+ * (rows, first row, gradient entries, first entry) in the dataset's concatenated arrays.  The slot's row range is
+ * V_cap rows (a multiple of 128) and its to_basis grid n_tb_ctas CTAs; both stay fixed while the batch changes.
+ * Written (device arrays of dn_slot_plan):
+ *   row_begin, tile_mesh, tb_rows, mesh_cta_begin: dn_mesh_batch_plan's for the same meshes (sm_count as there) on the
+ *     batch's rows; tiles past the batch's end map to the last mesh, and CTAs from mesh_cta_begin[n_meshes] up to
+ *     n_tb_ctas get the empty range [V, V) (V = row_begin[n_meshes]): no mesh's CTA range holds them;
+ *   seg_begin, seg_rows, tile_seg: one global-mean segment per mesh (tile_seg -1 past the batch's end);
+ *   table [2 n_meshes][n_ranges][4]: dn_batch_gather's table.  Entry b < n_meshes is batch mesh b, with ranges
+ *     0 rows, 1 meshes, 2 row pointers (n_rows + 1 per dataset mesh; the last batch mesh also writes row V), 3 gradient
+ *     entries, and every other range empty.  Entry n_meshes + k is piece k of the tail: rows
+ *     [V + k tail_rows, V + (k + 1) tail_rows) clipped to V_cap, written as padding (row pointers V + 1 ... V_cap equal
+ *     to the batch's entry count), so a gather grid sized by tail_rows covers it;
+ *   status [3]: sticky.  A fill whose ids hold an id outside [0, n_dataset) or whose rows or entries exceed V_cap or
+ *     entry_cap reads nothing through its ids and is planned with every mesh empty (V = 0, every mesh one empty CTA,
+ *     no gathered data), and if status[0] is 0 it records (1 = bad id / 2 = over capacity, first offending position,
+ *     the id there).  The caller reads and clears it.
+ * Requires 1 <= n_meshes <= 1024, V_cap a multiple of 128 below 2^31 - 256, entry_cap < 2^31,
+ * min(1024, sm_count + n_meshes) <= n_tb_ctas <= 1024 (the host planner never uses more CTAs: each mesh gets at most
+ * chunks_b sm_count / chunks_total + 1), n_meshes * tail_rows >= V_cap and n_ranges >= 4; DN_ERR_INVALID_ARGUMENT
+ * otherwise, before any launch. */
+typedef struct dn_slot_plan {
+  int32_t* row_begin;        /* [n_meshes + 1]          */
+  int32_t* tile_mesh;        /* [V_cap / 128]           */
+  int32_t* tb_rows;          /* [2 * n_tb_ctas]         */
+  int32_t* mesh_cta_begin;   /* [n_meshes + 1]          */
+  int32_t* seg_begin;        /* [n_meshes]              */
+  int32_t* seg_rows;         /* [n_meshes]              */
+  int32_t* tile_seg;         /* [V_cap / 128]           */
+  int64_t* table;            /* [2 n_meshes][n_ranges][4] */
+  int64_t* status;           /* [3]                     */
+} dn_slot_plan;
+int dn_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* dataset_sizes, int64_t n_dataset,
+                              int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas, int64_t tail_rows,
+                              int n_ranges, const dn_slot_plan* out_host, dn_stream_t stream);
+
 /* dn_block_fwd over a batch laid out as above (V = padded total, a multiple of 128).  Tensor-core engines only
  * (DN_ERR_UNSUPPORTED otherwise and for shapes outside the fused kernels' envelope: the caller loops over meshes). */
 int dn_block_fwd_batched(const float* x_in, const float* mass, const float* evals, const float* evecs,

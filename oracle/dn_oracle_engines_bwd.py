@@ -199,10 +199,11 @@ def _last_tile(V):
 # ------------------------------------------------------------------------------------------------
 # the entry points
 # ------------------------------------------------------------------------------------------------
-def from_basis(values, basis, row_scale, engine, pert=(), eW=None, stats=None):
-    """dn_from_basis: out = row_scale * (basis @ values)."""
+def from_basis(values, basis, row_scale, engine, pert=(), eW=None, stats=None, mode=None):
+    """dn_from_basis: out = row_scale * (basis @ values).  ``mode``: the chain's mode where from_basis is the first
+    layer of a longer chain (the fused block's front); its own plan's when None."""
     K, C = values.shape
-    mode = _mode(layer_mode(engine, [K], K, C), pert)
+    mode = _mode(mode or layer_mode(engine, [K], K, C), pert)
     rs = None if row_scale is None else np.asarray(row_scale, np.float64)
     if rs is not None and "row_scale_last_tile" in pert:
         rs = rs.copy()

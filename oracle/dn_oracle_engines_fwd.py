@@ -24,11 +24,16 @@ Where the forward rounds, beyond the contractions of ``dn_oracle_engines_bwd``:
   Programming Guide's documented maximum errors (Intrinsic Functions): __expf(y) within 2 + floor(|1.173 y|) ulp,
   __fdividef(x, y) within 2 ulp for |y| in [2^-126, 2^126] (0 above it); the add and the subtraction round once.
 * the MiniMLP: run_chain's epilogue, bias, relu, emul (dropout), then on the last layer the residual (fmaf).
+* the fused block's head (dn_block_fwd_ex with a dn_head, DiffusionNet.last_lin in the MiniMLP epilogue): fp32 fmaf
+  chains over the finished fp32 row, C / 4 terms per lane, a 2-level butterfly over 4 lanes, then + b.
 * dn_compute_hks: out[v, s] = sum_k expf(-(lambda_k s)) phi_vk^2.  Each lane runs an fmaf chain over its
   ceil(K / 32) eigenpairs, and a 5-level butterfly over the 32 lanes sums them (hks_warp_kernel and
   hks_generic_kernel alike).  Every term is >= 0, so the bound is relative to the element.
 
-``PERTURBATIONS``: named structural errors for the sensitivity tests."""
+``tree_sum`` restates, bitwise, the fp32 sums of the split-V partials that spectral_scale_kernel (4 slices) and the pack
+kernel's spectral job (8 slices) form; the fused block keeps only the partials, so its x_spec is checked on that sum.
+
+``PERTURBATIONS``, ``HEAD_PERTURBATIONS``: named structural errors for the sensitivity tests."""
 from __future__ import annotations
 
 import numpy as np
@@ -37,8 +42,8 @@ from dn_oracle_engines import _mlp_modes
 from dn_oracle_engines_bwd import (C_SAFE, PARTIAL_FLOATS, PASSES, U, _dense, _last_tile, _mode, _split_v, from_basis,
                                    layer_mode, to_basis_mode)
 
-__all__ = ["diffusion_fwd", "clamped_time", "to_basis_batched", "from_basis_batched", "features_fwd", "tanh_error",
-           "mini_mlp_fwd", "compute_hks", "routes", "mlp_on_tc", "PERTURBATIONS"]
+__all__ = ["diffusion_fwd", "tree_sum", "head_fwd", "clamped_time", "to_basis_batched", "from_basis_batched", "features_fwd", "tanh_error",
+           "mini_mlp_fwd", "compute_hks", "routes", "mlp_on_tc", "PERTURBATIONS", "HEAD_PERTURBATIONS"]
 
 TIME_MIN = np.float32(1e-8)   # dn_clamp_time
 TIME_COL = 4                  # the channel whose time "time_scaled" perturbs (0 .. 3 are the edge times)
@@ -50,6 +55,7 @@ PERTURBATIONS = {
             "wrong_w0_block", "bf16_for_1x"),
     "hks": ("drop_eig", "scale_scaled"),
 }
+HEAD_PERTURBATIONS = ("head_wrong_bias", "head_drop_col", "head_before_residual")   # head_fwd's, for the fused block
 _f = lambda v: None if v is None else np.asarray(v, np.float64)
 
 
@@ -68,12 +74,13 @@ def clamped_time(time, pert=()):
 
 
 def diffusion_fwd(x, mass, evals, evecs, time, engine, x_spec_out=None, sm=132, part_floats=PARTIAL_FLOATS, pert=(),
-                  stats=None, split=None, tree=4, cache=None):
+                  stats=None, split=None, tree=4, cache=None, fb_mode=None):
     """dn_learned_time_diffusion_fwd: {"x_spec": (gold, bound), "time": fp32, "x_diffuse": (gold, bound)}.
 
     x_diffuse is checked on ``x_spec_out`` (the call's own fp32 sums; the gold's x_spec when None).  One mesh of the
     batched call with ``split`` = its CTA plan's (P, rows per CTA) and ``tree`` = 8.  ``cache``: a dict shared by the
-    calls on the same inputs, so that engines whose to_basis rounds alike share its gold."""
+    calls on the same inputs, so that engines whose to_basis rounds alike share its gold.  ``fb_mode``: from_basis's
+    mode when it leads a longer chain (the fused block's front, dn_oracle_engines.dispatch)."""
     xv, m, lam, phi = _f(x), _f(mass), _f(evals), _f(evecs)
     K, C = phi.shape[1], xv.shape[1]
     tb = _mode(to_basis_mode(engine, K, C, sm, part_floats), pert)
@@ -96,8 +103,20 @@ def diffusion_fwd(x, mass, evals, evecs, time, engine, x_spec_out=None, sm=132, 
     xk = xs if x_spec_out is None else _f(x_spec_out)
     S = e * xk
     eS = np.abs(xk) * ee + U * np.abs(S)
-    res["x_diffuse"] = from_basis(S, phi, None, engine, pert=pert, eW=eS, stats=stats)
+    res["x_diffuse"] = from_basis(S, phi, None, engine, pert=pert, eW=eS, stats=stats, mode=fb_mode)
     return res
+
+
+def tree_sum(partials, tree):
+    """The fp32 sum over the partials (P, ...) as the kernels reduce them: slice s adds partials s, s + tree, ... serially
+    from 0, then the ``tree`` slice sums pairwise (dn_internal.h pairwise_sum).  Bitwise, in IEEE fp32."""
+    p = np.asarray(partials, np.float32)
+    red = [np.zeros(p.shape[1:], np.float32) for _ in range(tree)]
+    for q in range(p.shape[0]):
+        red[q % tree] = red[q % tree] + p[q]
+    while len(red) > 1:
+        red = [red[i] + red[i + 1] for i in range(0, len(red), 2)]
+    return red[0]
 
 
 def to_basis_batched(values, mass, evecs, engine, split, sm=132):
@@ -154,17 +173,19 @@ def _pq_weight(A_re, A_im, pert):
     return np.vstack([A_re, A_im]).T
 
 
-def features_fwd(gX, gY, x_diffuse, A_re, A_im, engine, pq_out=None, pert=(), stats=None):
+def features_fwd(gX, gY, x_diffuse, A_re, A_im, engine, pq_out=None, pert=(), stats=None, mode=None):
     """dn_gradient_features_fwd: {"pq": (gold, bound), "features": (gold, bound), "arg": (gold, band)}.  gX, gY:
     scipy.sparse CSR (V, V) on one pattern with fp32 values; A_im None without rotations.  The features are checked on
-    ``pq_out`` (the call's own [P|Q]; the gold's when None) and the exact x_diffuse."""
+    ``pq_out`` (the call's own [P|Q]; the gold's when None) and the exact x_diffuse.  ``mode``: the [P|Q] layers' mode
+    in the fused block (dn_oracle_engines.dispatch: a front chain's, or P and Q as two layers); the single layer's plan
+    when None."""
     import scipy.sparse as sp
     rot = A_im is not None
     xd = _f(x_diffuse)
     V, C = xd.shape
     W = _pq_weight(A_re, A_im, pert)
     npq = W.shape[1]
-    mode = _mode(layer_mode(engine, [C], C, npq), pert)
+    mode = _mode(mode or layer_mode(engine, [C], C, npq), pert)
     res = {"pq": _dense(xd, W, mode, stats=stats)}
     pq = res["pq"][0] if pq_out is None else _f(pq_out)
     Pm, Qm = pq[:, :C], (pq[:, C:2 * C] if rot else None)
@@ -255,6 +276,25 @@ def mini_mlp_fwd(srcs, weights, biases, drops, residual, engine, hidden=None, pe
             res["hidden"].append(z)
             a = z[0] if hidden is None else _f(hidden[l])
     return res
+
+
+def head_fwd(out, weight, bias, x_in=None, pert=()):
+    """The head in the MiniMLP epilogue: (out W^T + b, bound), (V, n_out), on the block output ``out`` the chain
+    finished (fp32).  Each element is at most C fmaf roundings, two butterfly adds and the bias add, each within u of
+    a partial sum bounded by |W||out| + |b|: 2 (C + 1) u (|W||out| + |b|).  ``x_in``: the residual, for the
+    "head_before_residual" perturbation."""
+    o, W = _f(out), _f(weight)
+    b = np.zeros(W.shape[0]) if bias is None else _f(bias)
+    C = W.shape[1]
+    bound = 2 * (C + 1) * U * (np.abs(o) @ np.abs(W).T + np.abs(b)[None, :])
+    if "head_before_residual" in pert:
+        o = o - _f(x_in)
+    if "head_drop_col" in pert:
+        W = W.copy()
+        W[:, C - 1] = 0
+    if "head_wrong_bias" in pert:
+        b = np.roll(b, -1)
+    return o @ W.T + b[None, :], bound
 
 
 # ------------------------------------------------------------------------------------------------

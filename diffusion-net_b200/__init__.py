@@ -11,7 +11,7 @@ from . import _lib, ops, geometry, layers, synthetic, streaming, dist, graphs, b
 from .layers import (DiffusionNet, DiffusionNetBlock, LearnedTimeDiffusion,  # noqa: F401,E402
                      SpatialGradientFeatures, MiniMLP)
 from .fmaps import (FunctionalMapCorrespondenceWithDiffusionNetFeatures, compute_correspondence,  # noqa: F401,E402
-                    pointwise_map, PairBatch, pointwise_map_batch)
+                    pointwise_map, PairBatch, PairDataset, pointwise_map_batch)
 from .geometry import to_basis, from_basis  # noqa: F401,E402
 from .ops import set_engine, get_engine, prepare_operators  # noqa: F401,E402
 from .batch import BatchSlot, MeshBatch, MeshDataset  # noqa: F401,E402

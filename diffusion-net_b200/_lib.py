@@ -15,7 +15,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libdiffusion_net_b200.so")
 SOURCES = ["dn_simt.cu", "dn_geom.cu", "dn_eig.cu", "dn_implicit.cu", "dn_implicit_batch.cu", "dn_batch_gather.cu",
-           "dn_batch_plan.cu", "dn_fmap.cu", "dn_fmap_batch.cu", "dn_tc.cu", "dn_head.cu", "dn_capi.cu"]
+           "dn_batch_rotate.cu", "dn_batch_plan.cu", "dn_fmap.cu", "dn_fmap_batch.cu", "dn_fmap_gt.cu", "dn_tc.cu",
+           "dn_head.cu", "dn_capi.cu"]
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "diffusion_net_b200.h")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -152,6 +153,7 @@ SIGNATURES = {
     "dn_mesh_batch_plan": (_I, [_I, _P, _I, _P, _P, _P, _P]),
     "dn_batch_gather": (_I, [C.POINTER(dn_gather_part), _I, _P, _I, _I, _P]),
     "dn_mesh_batch_plan_device": (_I, [_P, _I, _P, _L, _I, _L, _L, _I, _L, _I, C.POINTER(dn_slot_plan), _P]),
+    "dn_rotate_rows": (_I, [_P, _L, _P, _I, _P, _P, _P]),
     "dn_block_fwd_ex": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),
                              C.POINTER(dn_head), _L, _I, _I, _P, _P, _L, _I, _P]),
     "dn_block_fwd_batched": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),
@@ -167,6 +169,8 @@ SIGNATURES = {
     "dn_fmap_solve_bwd_batched": (_I, [_P, _L, _P, _L, _I, _P, _P, _I, _P, _P, _I, _I, _D, _P, _P, _P, _L, _P]),
     "dn_fmap_pointwise_map_batched_workspace_bytes": (_L, [_I, _I, _P, _P, _P, _P, _I]),
     "dn_fmap_pointwise_map_batched": (_I, [_P, _I, _P, _L, _P, _P, _I, _P, _P, _I, _P, _P, _L, _P]),
+    "dn_fmap_ground_truth_workspace_bytes": (_L, [_I, _I, _L]),
+    "dn_fmap_ground_truth": (_I, [_P, _L, _I, _P, _P, _L, _P, _L, _P, _I, _L, _P, _P, _P, _L, _P]),
     "dn_linear_nll_workspace_bytes": (_L, [_L, _I, _I]),
     "dn_linear_nll_fwd": (_I, [_P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _I, _P]),
     "dn_linear_nll_bwd": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _P, _L, _I, _P]),

@@ -284,18 +284,25 @@ class MeshDataset:
         mb._gather_from(self, ids)
         return mb
 
-    def pack(self, t, batch):
+    def pack(self, t, batch, rotations=None):
         """A per-vertex tensor in the dataset layout (V_total,) or (V_total, C), float32 (features such as HKS or xyz)
         or int64 (labels), in ``batch``'s layout with zero padding rows: one launch, no host synchronisation.  Data
-        only: a tensor that requires grad is refused (per-mesh lists still go through ``MeshBatch.pack``)."""
+        only: a tensor that requires grad is refused (per-mesh lists still go through ``MeshBatch.pack``).
+
+        ``rotations``: (batch.n_meshes, 3, 3) float32 (``random_rotations``) for float32 (V_total, 3) data such as
+        vertex positions: every batch mesh's rows are multiplied by its matrix, ``x_b @ R_b`` as the reference's
+        ``random_rotate_points`` does, by one more launch (``rotate_rows``)."""
         if getattr(batch, "_source", None) is not self._lap:
             raise ValueError("MeshDataset.pack: the batch was not drawn from this dataset")
         self._check_pack(t, "MeshDataset.pack")
+        _check_rotated(t, rotations, batch, "MeshDataset.pack")
         t = t.contiguous()
         out = torch.empty((batch.V,) + tuple(t.shape[1:]), dtype=t.dtype, device=batch.device)
         width = (t.shape[1] if t.dim() == 2 else 1) * (2 if t.dtype == torch.int64 else 1)
         _gather([(_part(t, out, _lib.GATHER_COPY, width, R_ROWS, batch._table_host), out)], batch._table,
                 batch.n_meshes, batch.device)
+        if rotations is not None:
+            _rotate(out, batch, rotations, out)
         return out
 
     def slot(self, n_meshes, max_rows=None, max_entries=None):
@@ -619,14 +626,18 @@ class BatchSlot:
             out = self._static[key] = torch.zeros(shape, dtype=src.dtype, device=self.device)
         return out
 
-    def pack(self, t):
+    def pack(self, t, rotations=None):
         """A dataset-layout float32 or int64 per-vertex tensor (V_total,) / (V_total, C) in the slot's layout, padding
-        rows 0: one launch into a buffer that is the same tensor on every call with the same ``t``."""
+        rows 0: one launch into a buffer that is the same tensor on every call with the same ``t``.  ``rotations``:
+        (n_meshes, 3, 3) float32, one matrix per slot mesh, for float32 (V_total, 3) data, as in ``MeshDataset.pack``
+        (one more launch; the rotated rows go to a buffer of their own, so ``pack(t)`` and ``pack(t, rotations=R)``
+        do not overwrite each other)."""
         if isinstance(t, (list, tuple)):
             raise NotImplementedError("BatchSlot.pack takes one tensor in the dataset layout; per-mesh lists need the "
                                       "host layout of a MeshBatch")
         self._ds._check_pack(t, "BatchSlot.pack")
-        out = self._static_out("pack", t, (self.V,) + tuple(t.shape[1:]))
+        _check_rotated(t, rotations, self, "BatchSlot.pack")
+        out = self._static_out("pack" if rotations is None else "pack_rotated", t, (self.V,) + tuple(t.shape[1:]))
         t = t.contiguous()
         width = (t.shape[1] if t.dim() == 2 else 1) * (2 if t.dtype == torch.int64 else 1)
         if width:
@@ -634,6 +645,8 @@ class BatchSlot:
             with torch.cuda.device(self.device):
                 _lib.check(_lib.load().dn_batch_gather(C.byref(part), 1, self._table.data_ptr(), N_RANGES,
                                                        2 * self.n_meshes, ops._stream()), "dn_batch_gather")
+        if rotations is not None:
+            _rotate(out, self, rotations, out)
         return out
 
     def take(self, per_mesh):
@@ -665,6 +678,86 @@ class BatchSlot:
 
     def elem_counts(self, name):
         self._no_host_layout("elem_counts")
+
+
+# ------------------------------------------------------------------------------------------------
+# random rotations (the reference's xyz augmentation), per mesh of a batch or slot
+# ------------------------------------------------------------------------------------------------
+def rotation_from_uniforms(u, axis=None):
+    """(n, 3, 3) float64 rotations from uniforms in [0, 1), with the reference's constructions (utils.py):
+    ``axis=None``: u (n, 3), ``random_rotation_matrix`` (Graphics Gems III: a rotation by 2 pi u0 about z, then the
+    Householder-type map (V V^T - I) with V from 2 pi u1 and 2 u2), uniform over SO(3);
+    ``axis='y'``: u (n,) or (n, 1), ``random_rotate_points_y``'s rotation by 2 pi u about y.
+    Torch ops only, on u's device."""
+    u = u.to(torch.float64)
+    two_pi = 2.0 * np.pi
+    if axis == 'y':
+        a = u.reshape(-1) * two_pi
+        c, s = torch.cos(a), torch.sin(a)
+        o, z = torch.ones_like(a), torch.zeros_like(a)
+        return torch.stack([c, z, s, z, o, z, -s, z, c], -1).view(-1, 3, 3)
+    if axis is not None:
+        raise ValueError("rotation axis must be None (uniform over SO(3)) or 'y', got {!r}".format(axis))
+    if u.dim() != 2 or u.shape[1] != 3:
+        raise ValueError("rotation_from_uniforms: expected (n, 3) uniforms, got {}".format(tuple(u.shape)))
+    theta, phi, z = u[:, 0] * two_pi, u[:, 1] * two_pi, u[:, 2] * 2.0
+    r = torch.sqrt(z)
+    V = torch.stack([torch.sin(phi) * r, torch.cos(phi) * r, torch.sqrt(2.0 - z)], -1)
+    st, ct = torch.sin(theta), torch.cos(theta)
+    o, zero = torch.ones_like(st), torch.zeros_like(st)
+    Rz = torch.stack([ct, st, zero, -st, ct, zero, zero, zero, o], -1).view(-1, 3, 3)
+    H = V.unsqueeze(-1) * V.unsqueeze(-2) - torch.eye(3, dtype=torch.float64, device=u.device)
+    return (H.unsqueeze(-1) * Rz.unsqueeze(-3)).sum(-2)          # (V V^T - I) Rz
+
+
+def random_rotations(n, axis=None, generator=None, device="cuda"):
+    """(n, 3, 3) float32 random rotations, one per mesh, for ``pack(..., rotations=)``: the distributions of the
+    reference's ``random_rotate_points`` (``axis=None``, uniform over SO(3) from 3 uniforms) and
+    ``random_rotate_points_y`` (``axis='y'``, a uniform angle about y).  The same distributions, not the same random
+    stream: the uniforms come from ``torch.rand`` on ``device`` (with ``generator`` if given) and the matrices are
+    built with torch ops there (``rotation_from_uniforms``), so a step captured in a CUDA graph draws new rotations
+    at every replay."""
+    k = 1 if axis == 'y' else 3
+    u = torch.rand(int(n), k, generator=generator, device=device, dtype=torch.float64)
+    return rotation_from_uniforms(u, axis).to(torch.float32)
+
+
+def _check_rotated(t, rotations, batch, what):
+    if rotations is None:
+        return
+    if t.dtype != torch.float32 or t.dim() != 2 or t.shape[1] != 3:
+        raise ValueError("{}: rotations apply to float32 (V_total, 3) data, got {} of shape {}".format(
+            what, t.dtype, tuple(t.shape)))
+    if not torch.is_tensor(rotations) or tuple(rotations.shape) != (batch.n_meshes, 3, 3) or \
+            rotations.dtype != torch.float32 or rotations.device != batch.device:
+        raise ValueError("{}: rotations must be a float32 ({}, 3, 3) tensor on {}, got {}".format(
+            what, batch.n_meshes, batch.device, (tuple(rotations.shape), rotations.dtype, rotations.device)
+            if torch.is_tensor(rotations) else type(rotations)))
+    if rotations.requires_grad:
+        raise ValueError("{}: rotations are data; got a tensor that requires grad".format(what))
+
+
+def _rotate(x, batch, R, out):
+    R = R.contiguous()
+    with torch.cuda.device(batch.device):
+        _lib.check(_lib.load().dn_rotate_rows(x.data_ptr(), batch.V, R.data_ptr(), batch.n_meshes,
+                                              batch._tile_mesh.data_ptr(), out.data_ptr(), ops._stream()),
+                   "dn_rotate_rows")
+    return out
+
+
+def rotate_rows(x, batch, rotations):
+    """(V, 3) float32 rows ``x`` in the layout of ``batch`` (a ``MeshBatch`` or ``BatchSlot``) rotated per mesh:
+    ``x_b @ R_b`` on the rows of mesh b (``dn_rotate_rows``, one launch; the mesh of a row comes from the layout's
+    tile table, so no host layout is needed).  Padding rows, 0 in ``x``, stay 0.  Data only (no autograd)."""
+    ops._require_cuda(x)
+    if x.dtype != torch.float32 or tuple(x.shape) != (batch.V, 3):
+        raise ValueError("rotate_rows: expected float32 ({}, 3) rows in the batch layout, got {} of shape {}".format(
+            batch.V, x.dtype, tuple(x.shape)))
+    _check_rotated(x, rotations, batch, "rotate_rows")
+    if x.requires_grad:
+        raise ValueError("rotate_rows rotates data; got rows that require grad")
+    return _rotate(x.contiguous(), batch, rotations, torch.empty_like(x))
 
 
 def block_forward_batched_raw(batch, x_in, time, A_re, A_im, weights, biases, with_features, head=None):

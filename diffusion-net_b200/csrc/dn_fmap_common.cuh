@@ -15,6 +15,28 @@ inline int64_t solve_smem_bytes(int n) {
   return (int64_t)sizeof(double) * ((int64_t)n * (n + 1) + 2 * n) + (int64_t)sizeof(float) * (n * kChunkLd + kChunk);
 }
 
+// Right-looking Cholesky of the symmetric n x n matrix S (lower triangle, row stride ld) in place; the diagonal ends as
+// L_kk.  Returns true (the same on every thread) at the first pivot k that is not above piv_floor[k] (not above 0 when
+// piv_floor is null; a NaN pivot always stops), leaving S partly factored.  Run by all kSolveThreads threads of a CTA.
+__device__ __forceinline__ bool cholesky_lower(double* S, int ld, int n, const double* piv_floor) {
+  const int tid = threadIdx.x;
+  for (int k = 0; k < n; ++k) {
+    __syncthreads();
+    const double piv = S[k * ld + k];
+    if (!(piv > (piv_floor ? piv_floor[k] : 0.0))) return true;  // every thread reads the same pivot: a uniform exit
+    const double lkk = sqrt(piv);
+    for (int j = k + 1 + tid; j < n; j += kSolveThreads) S[j * ld + k] /= lkk;
+    __syncthreads();
+    if (tid == 0) S[k * ld + k] = lkk;
+    const int m = n - k - 1;
+    for (int e = tid; e < m * m; e += kSolveThreads) {
+      const int j = k + 1 + e / m, l = k + 1 + e % m;
+      if (l <= j) S[j * ld + l] -= S[j * ld + k] * S[l * ld + k];
+    }
+  }
+  return false;
+}
+
 // Factor S_i and solve for row i of one pair (A, B: n x d, row stride d).  Forward (G == null): C_out[i] = c_i in fp32
 // (NaN when singular).  Backward: Cd[i] = c_i and Wd[i] = w_i = S_i^-1 g_i in fp64.  Run by all kSolveThreads threads of
 // a CTA with the dynamic shared memory of solve_smem_bytes(n).
@@ -66,25 +88,7 @@ __device__ __forceinline__ void row_solve(const float* __restrict__ A, const flo
     const double dl = (double)ex[j] - (double)ey[i];
     S[j * ld + j] += lambda * (dl * dl);
   }
-  // right-looking Cholesky, lower triangle in place; the diagonal ends as L_kk
-  bool singular = false;
-  for (int k = 0; k < n; ++k) {
-    __syncthreads();
-    const double piv = S[k * ld + k];
-    if (!(piv > 0.0)) {  // every thread reads the same pivot: a uniform exit
-      singular = true;
-      break;
-    }
-    const double lkk = sqrt(piv);
-    for (int j = k + 1 + tid; j < n; j += kSolveThreads) S[j * ld + k] /= lkk;
-    __syncthreads();
-    if (tid == 0) S[k * ld + k] = lkk;
-    const int m = n - k - 1;
-    for (int e = tid; e < m * m; e += kSolveThreads) {
-      const int j = k + 1 + e / m, l = k + 1 + e % m;
-      if (l <= j) S[j * ld + l] -= S[j * ld + k] * S[l * ld + k];
-    }
-  }
+  const bool singular = cholesky_lower(S, ld, n, nullptr);
   __syncthreads();
   if (!singular && tid < 32) {  // L y = r, then L^T x = y (both right-hand sides in the backward), one warp
     const int lane = tid;

@@ -14,12 +14,17 @@ evaluation's pointwise map (``functional_correspondence.py:194-196``) on the GPU
   (the training and evaluation loops of functional_correspondence.py): features once per shape (``forward_batch``),
   one batched projection, one batched solve, and the pointwise maps of all pairs, each pair's result what the per-pair
   calls give.
+* ``PairDataset`` / ``PairSlot``: shuffled pairs of a device-resident ``MeshDataset``, their ground-truth maps from the
+  template correspondences (faust_scape_dataset.py:186-190, ``dn_fmap_ground_truth``), and fixed-buffer pair slots on
+  which a whole training step, pair draw and random rotations included, captures in one CUDA graph.
 """
 from __future__ import annotations
 
 import ctypes as C
 import weakref
+from operator import index as operator_index
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -165,7 +170,11 @@ class FunctionalMapCorrespondenceWithDiffusionNetFeatures(nn.Module):
         features run once per shape through ``feature_extractor.forward_batch``'s route, so in training mode a shape
         used by several pairs gets ONE dropout mask per step (the reference draws one per forward call); then
         ``project_batched`` and ``fmap_solve_batched``.  The loss over all pairs backpropagates through each shape's
-        features once, with the per-pair gradients summed in a fixed order."""
+        features once, with the per-pair gradients summed in a fixed order.
+
+        On a ``PairSlot`` (``PairDataset.slot``; ``xs`` one tensor in the slot layout, e.g. ``slot.pack(verts,
+        rotations=...)``) the same launch sequence runs on the slot's fixed buffers, so the step captures in one CUDA
+        graph; ``feats`` is then the (V_cap, n_feat) features in the slot layout (a slot has no per-shape split)."""
         n = self.n_fmap
         if pair_batch.n != n:
             raise ValueError("forward_pairs: the pair batch was built for n_fmap = {}, the model uses {}".format(
@@ -174,6 +183,8 @@ class FunctionalMapCorrespondenceWithDiffusionNetFeatures(nn.Module):
         feat = self.feature_extractor._forward_batch_layout(mb, xs)
         F_hat = project_batched(feat, pair_batch)
         C_pred = fmap_solve_batched(F_hat, pair_batch.evals, pair_batch.pairs, n, self.lambda_param)
+        if isinstance(pair_batch, PairSlot):
+            return C_pred, feat
         return C_pred, mb.unpack(feat)
 
 
@@ -307,8 +318,19 @@ class PairBatch:
         K = min(int(it["evals"].shape[0]) for it in items)
         if K < n:
             raise ValueError("PairBatch: K = {} eigenpairs is fewer than n_fmap = {}".format(K, n))
-        self.n, self.n_shapes, self.n_pairs = n, S, len(pairs)
-        self.mesh_batch = mb = MeshBatch(items)
+        self._build(MeshBatch(items), pairs, n)
+
+    @classmethod
+    def _of(cls, mb, pairs, n):
+        """The pair batch of an already gathered MeshBatch (``PairDataset.batch``; the caller checked the pairs)."""
+        pb = cls.__new__(cls)
+        pb._build(mb, pairs, n)
+        return pb
+
+    def _build(self, mb, pairs, n):
+        self.n, self.n_shapes, self.n_pairs = n, mb.n_meshes, len(pairs)
+        self.mesh_batch = mb
+        S = mb.n_meshes
         self.device = mb.device
         self.pairs = PairList(pairs, S, mb.device)
         self.kp = kp = (n + 7) // 8 * 8
@@ -448,3 +470,253 @@ def pointwise_map_batch(C_pred, pair_batch, n_fmap=30):
                                                      px, py, P, out.data_ptr(), ws.data_ptr(), ws.numel(),
                                                      ops._stream()), "dn_fmap_pointwise_map_batched")
     return list(torch.split(out, counts))
+
+
+# ------------------------------------------------------------------------------------------------
+# pair datasets: shuffled pairs of a MeshDataset, their ground-truth maps, and pair slots for CUDA-graph training
+# ------------------------------------------------------------------------------------------------
+_GT_BAD_PAIR, _GT_SINGULAR = 1, 2
+
+
+def _ground_truth_into(pds, ids, out, status, ws):
+    """dn_fmap_ground_truth of device int64 pair ids into ``out`` (P, n, n); ``ws`` sized for P."""
+    _lib.check(_lib.load().dn_fmap_ground_truth(
+        pds.ds.evecs.data_ptr(), pds.ds.K, pds.n, pds._vts_rows.data_ptr(), pds._vts_begin.data_ptr(), pds.ds.n_meshes,
+        pds.pairs.data_ptr(), pds.n_table, ids.data_ptr(), ids.shape[0], pds.max_m, out.data_ptr(), status.data_ptr(),
+        ws.data_ptr(), ws.numel(), ops._stream()), "dn_fmap_ground_truth")
+    return out
+
+
+def _gt_workspace(pds, P):
+    b = int(_lib.load().dn_fmap_ground_truth_workspace_bytes(P, pds.n, pds.max_m))
+    if b < 0:
+        _lib.check(b, "dn_fmap_ground_truth_workspace_bytes")
+    return torch.empty(b, dtype=torch.uint8, device=pds.device)
+
+
+def _raise_gt_status(st, n_table):
+    kind, pos, pid = st
+    if kind == _GT_BAD_PAIR:
+        raise IndexError("pair index {} at position {} is outside the dataset's {} pairs".format(pid, pos, n_table))
+    if kind == _GT_SINGULAR:
+        raise RuntimeError("pair {} at position {}: the ground-truth system A^T A is singular (its correspondences "
+                           "do not determine an n x n map); its C_gt is NaN".format(pid, pos))
+
+
+class PairDataset:
+    """Ordered shape pairs of a ``batch.MeshDataset`` with their correspondences, for the functional-map model's
+    training loop (functional_correspondence.py:100-143) on the device.
+
+    ``ds``: the MeshDataset (K >= n_fmap eigenpairs); ``vts``: one int64 tensor per mesh, the vertex of that mesh
+    matching each template vertex (faust_scape_dataset.py's ``vts``; repeats allowed); ``pairs``: the table of allowed
+    ordered pairs (x, y), e.g. ``itertools.permutations(range(80), 2)`` as the reference trains FAUST.  Checked once on
+    the host: indices, vertices inside their mesh, ``len(vts[x]) == len(vts[y])`` for every pair.  The correspondences,
+    rebased to dataset rows and concatenated, and the pair table stay on the device.
+
+    * ``batch(pair_ids)``: the eager ``PairBatch`` of those pairs (``ds.batch(xs + ys)`` with pairs (p, P + p)), for
+      ``forward_pairs`` and ``pointwise_map_batch``.
+    * ``ground_truth(pair_ids)``: (P, n, n) ground-truth maps (``dn_fmap_ground_truth``).
+    * ``slot(n_pairs)``: a ``PairSlot`` whose whole training step, pair draw included, captures in one CUDA graph.
+
+    The ground truth is the reference's least squares C_gt = X^T, X = argmin ||Phi_x[vts_x, :n] X -
+    Phi_y[vts_y, :n]||, solved by fp64 normal equations.  Where the reference's ``lstsq`` returns some solution for a
+    rank-deficient system (fewer than n distinct correspondence rows, say), that pair's C_gt here is NaN and a status
+    is set that ``check()`` (or ``PairSlot.check()``) raises on."""
+
+    def __init__(self, ds, vts, pairs, n_fmap=30):
+        n = int(n_fmap)
+        _check_n(n, "PairDataset")
+        if n < 1:
+            raise ValueError("PairDataset: n_fmap must be at least 1, got {}".format(n))
+        if ds.K < n:
+            raise ValueError("PairDataset: K = {} eigenpairs is fewer than n_fmap = {}".format(ds.K, n))
+        vts = list(vts)
+        if len(vts) != ds.n_meshes:
+            raise ValueError("PairDataset: {} correspondence tensors for {} meshes".format(len(vts), ds.n_meshes))
+        host = []
+        for s, v in enumerate(vts):
+            v = torch.as_tensor(v)
+            if v.dim() != 1 or v.dtype.is_floating_point or v.dtype.is_complex or v.dtype == torch.bool:
+                raise ValueError("PairDataset: vts[{}] must be a 1-D integer tensor, got {} of shape {}".format(
+                    s, v.dtype, tuple(v.shape)))
+            v = v.cpu().to(torch.int64)
+            if v.numel() and (int(v.min()) < 0 or int(v.max()) >= ds.n_rows[s]):
+                raise IndexError("PairDataset: vts[{}] holds a vertex outside the mesh's {} vertices".format(
+                    s, ds.n_rows[s]))
+            host.append(v)
+        counts = [int(v.numel()) for v in host]
+        table = torch.as_tensor([[int(a), int(b)] for a, b in pairs], dtype=torch.int64).reshape(-1, 2)
+        if table.shape[0] == 0:
+            raise ValueError("PairDataset needs at least one pair")
+        S = ds.n_meshes
+        for p, (a, b) in enumerate(table.tolist()):
+            if not (0 <= a < S and 0 <= b < S):
+                raise ValueError("PairDataset: pair {} = ({}, {}) indexes a mesh outside [0, {})".format(p, a, b, S))
+            if counts[a] != counts[b]:
+                raise ValueError("PairDataset: pair {} = ({}, {}) has {} and {} correspondences; the ground truth needs "
+                                 "as many on both shapes".format(p, a, b, counts[a], counts[b]))
+        self.ds, self.n, self.device = ds, n, ds.device
+        self.n_table = int(table.shape[0])
+        self.pair_x_host = table[:, 0].tolist()
+        self.pair_y_host = table[:, 1].tolist()
+        self.max_m = max(counts[a] for a in self.pair_x_host)
+        self.pairs = table.to(ds.device)
+        self._vts_rows = torch.cat([v + r0 for v, r0 in zip(host, ds.row_begin)]).to(ds.device)
+        self._vts_begin = torch.tensor([0] + np.cumsum(counts).tolist(), dtype=torch.int64).to(ds.device)
+        self.status = torch.zeros(3, dtype=torch.int64, device=ds.device)
+
+    def __len__(self):
+        return self.n_table
+
+    def _host_ids(self, ids, what):
+        if torch.is_tensor(ids):
+            ids = ids.tolist()
+        ids = [int(i) for i in ids]
+        if not ids:
+            raise ValueError("PairDataset.{} needs at least one pair index".format(what))
+        bad = [(q, i) for q, i in enumerate(ids) if not 0 <= i < self.n_table]
+        if bad:
+            raise IndexError("PairDataset.{}: pair index {} at position {} is outside the dataset's {} pairs".format(
+                what, bad[0][1], bad[0][0], self.n_table))
+        return ids
+
+    def batch(self, pair_ids):
+        """The ``PairBatch`` of pairs ``pair_ids`` (host ints; repeats allowed): shapes x_0 .. x_{P-1}, y_0 ..
+        y_{P-1} drawn by one ``ds.batch`` and pairs (p, P + p)."""
+        ids = self._host_ids(pair_ids, "batch")
+        if 2 * len(ids) > MAX_SHAPES:
+            raise ValueError("PairDataset.batch: {} pairs need {} shapes, more than the {} a pair batch takes".format(
+                len(ids), 2 * len(ids), MAX_SHAPES))
+        P = len(ids)
+        mb = self.ds.batch([self.pair_x_host[i] for i in ids] + [self.pair_y_host[i] for i in ids])
+        return PairBatch._of(mb, [(p, P + p) for p in range(P)], self.n)
+
+    def ground_truth(self, pair_ids):
+        """(P, n, n) float32 ground-truth maps of pairs ``pair_ids``: host ints (checked here) or a CUDA int64 tensor
+        (checked on the device: an invalid index gives a NaN map and sets the status ``check()`` reads).  Two
+        launches, no host synchronisation for device ids."""
+        if torch.is_tensor(pair_ids) and pair_ids.device.type != "cpu":
+            if pair_ids.dtype != torch.int64 or pair_ids.dim() != 1 or pair_ids.device != self.device:
+                raise ValueError("PairDataset.ground_truth: device pair ids must be a 1-D int64 tensor on {}".format(
+                    self.device))
+            ids = pair_ids.contiguous()
+        else:
+            ids = torch.tensor(self._host_ids(pair_ids, "ground_truth"), dtype=torch.int64).to(self.device)
+        P = ids.shape[0]
+        if not 1 <= P <= MAX_PAIRS:
+            raise ValueError("PairDataset.ground_truth takes 1 .. {} pairs, got {}".format(MAX_PAIRS, P))
+        out = torch.empty(P, self.n, self.n, dtype=torch.float32, device=self.device)
+        with ops._on(out):
+            return _ground_truth_into(self, ids, out, self.status, _gt_workspace(self, P))
+
+    def check(self):
+        """Raise if a ground_truth call since the last check met an invalid pair index (IndexError) or a singular
+        system (RuntimeError), and clear the status.  One device-to-host read."""
+        st = self.status.tolist()
+        if st[0]:
+            self.status.zero_()
+        _raise_gt_status(st, self.n_table)
+
+    def slot(self, n_pairs, max_rows=None, max_entries=None):
+        """A ``PairSlot`` of ``n_pairs`` pairs (see there)."""
+        return PairSlot(self, n_pairs, max_rows, max_entries)
+
+
+class PairSlot:
+    """``n_pairs`` pairs of a ``PairDataset`` on buffers that never move, refilled on the device from any pair indices,
+    so that the functional-map model's whole training step (pair draw, rotations, features, projection, solve, ground
+    truth, loss and backward) captures in one CUDA graph (``graphs.GraphedTrainStep``)::
+
+        slot = pds.slot(P)
+        ids = torch.zeros(P, dtype=torch.int64, device="cuda")
+        def step(model, ids):
+            slot.fill(ids)
+            x = slot.pack(verts, rotations=dn.batch.random_rotations(2 * P, device="cuda"))
+            C_pred, _ = model.forward_pairs(slot, x)
+            return (C_pred - slot.ground_truth()).square().mean()
+        g = dn.graphs.GraphedTrainStep(model, step, (ids,))
+        for chunk in torch.randint(len(pds), (n_steps, P), device="cuda"):
+            ids.copy_(chunk); g.zero_grads(model); g.replay(); opt.step()
+
+    It wraps a ``batch.BatchSlot`` of 2 P meshes filled with ``cat(pair_x[ids], pair_y[ids])`` (``mesh_batch``), with
+    the fixed ``PairList`` (p, P + p) (so the solve's shape -> (pair, role) lists never change), a fixed (V_cap, kp)
+    projection basis refreshed at every fill and a fixed (P, n, n) ground-truth buffer.  The default capacity is 2 P
+    times the dataset's largest padded mesh and gradient entry count: a pair draw repeats shapes, which
+    ``BatchSlot``'s default (any distinct meshes) does not cover.
+
+    A pair index outside the table gives every mesh of the slot an invalid id: the step computes NaN (loss and
+    gradients), and ``check()`` raises IndexError; the next valid fill recovers.  Dropout masks are drawn over the
+    whole slot layout, as ``forward_pairs`` draws them on a ``PairBatch``."""
+
+    def __init__(self, pds, n_pairs, max_rows=None, max_entries=None):
+        from .batch import BatchSlot
+        P = operator_index(n_pairs)
+        if P < 1 or 2 * P > MAX_SHAPES:
+            raise ValueError("PairDataset.slot takes 1 .. {} pairs, got {}".format(MAX_SHAPES // 2, P))
+        ds = pds.ds
+        pad_max = max((r + 127) // 128 * 128 for r in ds.n_rows)
+        self.pds, self.n, self.n_pairs, self.n_shapes, self.device = pds, pds.n, P, 2 * P, ds.device
+        self.mesh_batch = BatchSlot(ds, 2 * P, 2 * P * pad_max if max_rows is None else max_rows,
+                                    2 * P * max(ds._grad_nnz) if max_entries is None else max_entries)
+        self.pairs = PairList([(p, P + p) for p in range(P)], 2 * P, ds.device)
+        self.kp = kp = (self.n + 7) // 8 * 8
+        self.basis = torch.zeros(self.mesh_batch.V, kp, dtype=torch.float32, device=ds.device)
+        self.evals = self.mesh_batch.evals       # (2 P, K): the solve reads the first n of every row
+        self.ids = torch.zeros(P, dtype=torch.int64, device=ds.device)
+        self.C_gt = torch.zeros(P, self.n, self.n, dtype=torch.float32, device=ds.device)
+        self.status = torch.zeros(3, dtype=torch.int64, device=ds.device)
+        self._ws = _gt_workspace(pds, P)
+
+    def fill(self, ids):
+        """Draw pairs ``ids``: a CUDA int64 tensor of n_pairs pair indices (checked on the device, nothing read back)
+        or host ints (checked here).  A few small torch ops map the pairs to their 2 P meshes (an invalid index to
+        an invalid mesh id), then ``BatchSlot.fill`` and one copy of the basis.  Returns the slot."""
+        P = self.n_pairs
+        if torch.is_tensor(ids) and ids.device.type != "cpu":
+            if ids.dtype != torch.int64 or tuple(ids.shape) != (P,) or ids.device != self.device:
+                raise ValueError("PairSlot.fill: device ids must be an int64 tensor of shape ({},) on {}".format(
+                    P, self.device))
+            if ids.data_ptr() != self.ids.data_ptr():
+                self.ids.copy_(ids)
+        else:
+            h = self.pds._host_ids(ids, "slot fill")
+            if len(h) != P:
+                raise ValueError("PairSlot.fill: {} pair indices for a slot of {} pairs".format(len(h), P))
+            self.ids.copy_(torch.tensor(h, dtype=torch.int64).pin_memory(), non_blocking=True)
+        valid = (self.ids >= 0) & (self.ids < self.pds.n_table)
+        xy = torch.index_select(self.pds.pairs, 0, torch.where(valid, self.ids, 0))
+        xy = torch.where(valid.unsqueeze(1), xy, -1)
+        mesh_ids = self.mesh_batch.ids
+        mesh_ids[:P].copy_(xy[:, 0])
+        mesh_ids[P:].copy_(xy[:, 1])
+        self.mesh_batch.fill(mesh_ids)
+        self.basis[:, :self.n].copy_(self.mesh_batch.evecs[:, :self.n])
+        return self
+
+    def pack(self, t, rotations=None):
+        """``BatchSlot.pack`` of the slot's 2 P meshes (x shapes first, then y shapes); ``rotations`` (2 P, 3, 3)."""
+        return self.mesh_batch.pack(t, rotations=rotations)
+
+    def ground_truth(self):
+        """The (P, n, n) ground-truth maps of the drawn pairs, written into the slot's fixed buffer (two launches)."""
+        with ops._on(self.C_gt):
+            return _ground_truth_into(self.pds, self.ids, self.C_gt, self.status, self._ws)
+
+    def check(self):
+        """Raise if a fill since the last check had an invalid pair index (IndexError) or exceeded the capacity
+        (ValueError), or a ground truth was singular (RuntimeError), and clear the status.  One device-to-host read."""
+        st = torch.cat([self.status, self.mesh_batch.status]).tolist()
+        gt, ms = st[:3], st[3:]
+        if gt[0]:
+            self.status.zero_()
+        if ms[0]:
+            self.mesh_batch.status.zero_()
+        if gt[0] == _GT_BAD_PAIR or ms[0] == 1:
+            if gt[0] == _GT_BAD_PAIR:
+                _raise_gt_status(gt, self.pds.n_table)
+            raise IndexError("PairSlot.fill: the pair index at position {} is outside the dataset's {} pairs".format(
+                ms[1] % self.n_pairs, self.pds.n_table))
+        if ms[0]:
+            raise ValueError("PairSlot.fill: the drawn pairs exceed the slot's capacity of {} rows and {} gradient "
+                             "entries".format(self.mesh_batch.V, self.mesh_batch.entry_capacity))
+        _raise_gt_status(gt, self.pds.n_table)

@@ -115,8 +115,10 @@ class GraphedTrainStep:
     recipe: warm-up on a side stream, ``.grad`` buffers allocated before capture) and replayed every step; gradients
     ACCUMULATE into the parameters' ``.grad`` exactly like eager ``backward()`` does, so a data-parallel step is
     ``zero_grads(); for g in graphs: g.replay(); all-reduce; optimizer.step()``.  The inputs are the tensors passed at
-    construction (update them in place to change the data); dropout must be off (the mask generation is host RNG
-    plumbing, see layers.MiniMLP)."""
+    construction (update them in place to change the data).  Random draws inside the step (dropout masks,
+    ``batch.random_rotations``) come from torch's CUDA generator, which a graph replays from its current seed and
+    offset: every replay draws new masks and rotations, and a replay after ``torch.cuda.manual_seed(s)`` draws what an
+    eager step would after the same seed."""
 
     def __init__(self, net, loss_fn, inputs, warmup=3):
         _refuse_implicit(net)

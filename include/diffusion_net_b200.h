@@ -487,6 +487,15 @@ int dn_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* d
                               int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas, int64_t tail_rows,
                               int n_ranges, const dn_slot_plan* out_host, dn_stream_t stream);
 
+/* Per-mesh rotations of the (V, 3) rows of a batch laid out as above (the reference's random_rotate_points on every
+ * mesh of a batch or slot): out[v] = x[v] @ R[tile_mesh[v / 128]], R device (n_meshes, 3, 3) row-major, each output
+ * one fp32 FMA chain x0 R[0][j], + x1 R[1][j], + x2 R[2][j].  tile_mesh is the batch's (device, V / 128 entries), so
+ * a host-planned batch and a device-planned slot are served alike; padding rows, 0 in x, stay 0.  A row whose tile
+ * names no mesh in [0, n_meshes) is written as NaN.  x and out may be the same array.  V a positive multiple of 128.
+ * 1 launch; nothing is read back. */
+int dn_rotate_rows(const float* x, int64_t V, const float* R, int n_meshes, const int32_t* tile_mesh, float* out,
+                   dn_stream_t stream);
+
 /* dn_block_fwd over a batch laid out as above (V = padded total, a multiple of 128).  Tensor-core engines only
  * (DN_ERR_UNSUPPORTED otherwise and for shapes outside the fused kernels' envelope: the caller loops over meshes). */
 int dn_block_fwd_batched(const float* x_in, const float* mass, const float* evals, const float* evecs,
@@ -601,6 +610,35 @@ int dn_fmap_pointwise_map_batched(const float* C, int n, const float* evecs, int
                                   const int32_t* row_begin_host, const int32_t* n_rows_host, int n_shapes,
                                   const int32_t* pair_x_host, const int32_t* pair_y_host, int n_pairs,
                                   int64_t* out_index, void* workspace, int64_t ws_bytes, dn_stream_t stream);
+
+/* Ground-truth functional maps of shape pairs (faust_scape_dataset.py:186-190, the functional-map model's training
+ * target): for pair p with table entry (x, y) = pair_table[pair_ids[p]], A = Phi_x[vts_x, :n] and B = Phi_y[vts_y, :n]
+ * (m rows each), C_gt[p] = X^T with X = argmin ||A X - B||, solved from the normal equations A^T A X = A^T B.
+ *   evecs (dataset rows, row stride ld_evecs >= n): the eigenvectors of every shape, back to back;
+ *   vts_rows (device int64): the correspondences of every shape as evecs rows (already rebased to the dataset), shape s
+ *     owning vts_rows[vts_begin[s] .. vts_begin[s + 1]) (vts_begin device int64 [n_shapes + 1]);
+ *   pair_table (device int64 [n_table][2]) the allowed ordered pairs, pair_ids (device int64 [n_pairs]) the drawn ones.
+ * The caller checks that every table pair's shapes have equal correspondence counts m <= max_m and that every row is in
+ * evecs.  A and B are gathered straight from evecs in shared memory (never materialised); A^T A and A^T B are summed in
+ * fp64 over fixed 512-row chunks, each chunk's partial one FMA chain in row order, the partials added in chunk order;
+ * A^T A is factored by the fp64 Cholesky of the functional-map solve and the n columns solved; C_gt is written in fp32.
+ * A pair's result depends on its own rows only: bitwise the same alone or among other pairs, at any position.
+ * 2 launches; the grid is sized from max_m and n_pairs, not from the drawn pairs, and nothing is read back, so the
+ * call captures in a CUDA graph and replays for any draw.
+ * Where the reference's least squares returns a solution, a pair whose A^T A has a pivot at or below 1e-10 of its
+ * diagonal entry gets NaN in all of C_gt[p]: a rank-deficient system (fewer than n distinct rows, for instance), and
+ * also a full-rank but near-singular one (a column of A within about 1e-5 radians of the span of the others, so
+ * roughly kappa(A) >= 1e5), whose fp64 normal equations would lose every digit of fp32 accuracy.  So does a pair
+ * index outside [0, n_table).  Either sets the sticky status (device int64 [3]) when status[0] is 0: (1 = bad pair
+ * index / 2 = singular, position p, pair_ids[p]).  The caller reads and clears it.
+ * 1 <= n <= 128 (DN_ERR_UNSUPPORTED above), n_pairs <= 65535, max_m < 2^31.
+ * Workspace: dn_fmap_ground_truth_workspace_bytes(n_pairs, n, max_m), each part rounded up to 256 bytes:
+ *   16 n^2 n_pairs max(1, ceil(max_m / 512)) + 8 n^2 n_pairs bytes. */
+int64_t dn_fmap_ground_truth_workspace_bytes(int n_pairs, int n, int64_t max_m);
+int dn_fmap_ground_truth(const float* evecs, int64_t ld_evecs, int n, const int64_t* vts_rows,
+                         const int64_t* vts_begin, int64_t n_shapes, const int64_t* pair_table, int64_t n_table,
+                         const int64_t* pair_ids, int n_pairs, int64_t max_m, float* C_gt, int64_t* status,
+                         void* workspace, int64_t ws_bytes, dn_stream_t stream);
 
 /* Linear head fused behind a block (SURVEY.md 8f-1): `DiffusionNet.last_lin` (layers.py:366-370 -- the nn.Linear applied
  * to the last block's output) computed in the epilogue of that block's MiniMLP chain, in exact fp32, so that the

@@ -37,7 +37,8 @@ WORKLOADS = {"shrec11": dict(n_data=600, batch=32, v_lo=250, v_hi=750, nm=(12, 4
              "large": dict(n_data=64, batch=8, v_lo=5000, v_hi=10000, nm=(60, 130))}
 
 
-def dataset_items(w, seed=0):
+def dataset_items(w, seed=0, faces=False):
+    """The workload's synthetic tori; ``faces``: each item also carries its grid's faces (synthetic.torus_mesh)."""
     g = torch.Generator().manual_seed(seed)
     out = []
     while len(out) < w["n_data"]:
@@ -47,6 +48,8 @@ def dataset_items(w, seed=0):
             for _ in range(2):         # resident operators: the CSR and the locality decision are made before timing
                 dn.prepare_operators(gX, gY)
             out.append(dict(mass=mass, evals=evals, evecs=evecs, gradX=gX, gradY=gY))
+            if faces:
+                out[-1]["faces"] = dn.synthetic.torus_mesh(n, m)[1].cuda()
     return out
 
 

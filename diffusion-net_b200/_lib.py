@@ -84,6 +84,12 @@ class dn_slot_plan(C.Structure):
                                                 "seg_rows", "tile_seg", "table", "status")]
 
 
+class dn_slot_elements(C.Structure):
+    _fields_ = [("capacity", C.c_int64), ("tail", C.c_int64), ("k", C.c_int32), ("range", C.c_int32),
+                ("csr_range", C.c_int32), ("begin", C.c_void_p), ("count", C.c_void_p), ("tile_seg", C.c_void_p)]
+
+
+
 class dn_eig_batch(C.Structure):
     _fields_ = [("n_meshes", C.c_int32), ("n_tiles", C.c_int32), ("n_slices", C.c_int32), ("row_begin", C.c_void_p),
                 ("tile_mesh", C.c_void_p), ("tile_begin", C.c_void_p), ("slice_mesh", C.c_void_p),
@@ -153,6 +159,8 @@ SIGNATURES = {
     "dn_mesh_batch_plan": (_I, [_I, _P, _I, _P, _P, _P, _P]),
     "dn_batch_gather": (_I, [C.POINTER(dn_gather_part), _I, _P, _I, _I, _P]),
     "dn_mesh_batch_plan_device": (_I, [_P, _I, _P, _L, _I, _L, _L, _I, _L, _I, C.POINTER(dn_slot_plan), _P]),
+    "dn_mesh_batch_plan_device_elements": (_I, [_P, _I, _P, _I, _L, _I, _L, _L, _I, _L, _I, C.POINTER(dn_slot_plan),
+                                                C.POINTER(dn_slot_elements), _I, _I, _P]),
     "dn_rotate_rows": (_I, [_P, _L, _P, _I, _P, _P, _P]),
     "dn_block_fwd_ex": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),
                              C.POINTER(dn_head), _L, _I, _I, _P, _P, _L, _I, _P]),

@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import ctypes as C
 import operator
+import types
 
 import numpy as np
 import torch
@@ -25,6 +26,11 @@ from . import _lib, ops
 # ranges of a gather table (dn_batch_gather): per batch mesh, (src_begin, dst_begin, n, n_dst) in units of
 R_ROWS, R_MESH, R_PTR, R_ENT, R_FACES, R_EDGES = range(6)   # rows, meshes, row pointers, CSR entries, faces, edges
 N_RANGES = 6
+# a BatchSlot holding elements adds: the corners' offset and padding row (the mesh's first row), and the vertex ->
+# element CSR entries of faces and edges
+R_CORNER_OFF, R_FACES_CSR, R_EDGES_CSR = range(6, 9)
+N_SLOT_RANGES = 9
+ELEMENT_KINDS = (("faces", R_FACES, R_FACES_CSR), ("edges", R_EDGES, R_EDGES_CSR))
 _INT32_LIMIT = 2 ** 31
 
 
@@ -305,17 +311,22 @@ class MeshDataset:
             _rotate(out, batch, rotations, out)
         return out
 
-    def slot(self, n_meshes, max_rows=None, max_entries=None):
+    def slot(self, n_meshes, max_rows=None, max_entries=None, elements=(), max_elements=None):
         """A ``BatchSlot`` of ``n_meshes`` meshes of this dataset: a batch whose buffers never move, refilled on the
         device from any mesh ids, so that a shuffled training step can be captured in one CUDA graph.  Its default
-        capacity holds any ``n_meshes`` distinct meshes; ``max_rows`` / ``max_entries`` set it instead."""
-        return BatchSlot(self, n_meshes, max_rows, max_entries)
+        capacity holds any ``n_meshes`` distinct meshes; ``max_rows`` / ``max_entries`` set it instead.
+        ``elements``: 'faces', 'edges' or both (a sequence), for outputs_at 'faces' / 'edges' training: the slot then
+        also holds those elements of the batch (the dataset's items must carry them), with ``max_elements`` (an int
+        for every kind, or a dict by kind) setting their capacity; a slot sized for repeated ids by ``max_rows`` needs
+        ``max_elements`` too."""
+        return BatchSlot(self, n_meshes, max_rows, max_entries, elements, max_elements)
 
-    def _check_pack(self, t, what):
-        if not torch.is_tensor(t) or t.dim() not in (1, 2) or t.shape[0] != self.V or \
+    def _check_pack(self, t, what, n=None):
+        n = self.V if n is None else n
+        if not torch.is_tensor(t) or t.dim() not in (1, 2) or t.shape[0] != n or \
                 t.dtype not in (torch.float32, torch.int64):
             raise ValueError("{0}: expected a float32 or int64 tensor of shape ({1},) or ({1}, C) in the dataset layout, "
-                             "got {2}".format(what, self.V, (tuple(t.shape), t.dtype) if torch.is_tensor(t)
+                             "got {2}".format(what, n, (tuple(t.shape), t.dtype) if torch.is_tensor(t)
                                               else type(t)))
         if t.requires_grad:
             raise ValueError("{} gathers data; got a tensor that requires grad (pack per-mesh tensors with "
@@ -325,9 +336,10 @@ class MeshDataset:
             raise ValueError("{}: the tensor is on {}, the dataset on {}".format(what, t.device, self.device))
 
     def _slot_tables(self):
-        """What every slot reads, built on first slot creation: the per-mesh size table on the device, and every mesh's
-        transposed gradient CSR back to back in the forward CSR's layout (the transpose of a block-diagonal matrix is
-        the block diagonal of the transposes, so a slot gathers it like the forward CSR and never transposes)."""
+        """What every slot reads, built on first slot creation: the per-mesh size table on the device (rows, first row,
+        gradient entries, first entry), and every mesh's transposed gradient CSR back to back in the forward CSR's
+        layout (the transpose of a block-diagonal matrix is the block diagonal of the transposes, so a slot gathers it
+        like the forward CSR and never transposes)."""
         if getattr(self, "_slot_data", None) is None:
             rowptr, colidx, vals = self._grad
             parts, ent0 = [], 0
@@ -342,6 +354,46 @@ class MeshDataset:
                               np.asarray(self._grad_nnz, np.int64), _starts(self._grad_nnz)[:-1]], 1)
             self._slot_data = (torch.from_numpy(sizes).to(self.device), grad_t)
         return self._slot_data
+
+    def _slot_element_tables(self, names):
+        """What a slot holding the element kinds ``names`` reads besides _slot_tables': the size table with the columns
+        dn_mesh_batch_plan_device_elements reads (_slot_tables' four, then (elements, first element) per kind), and
+        per kind every mesh's vertex -> element CSR (ops.element_csr of its own elements: n_rows + 1 row pointers and
+        k mesh-local element indices per element) back to back like the elements, so a slot gathers it and never
+        sorts.  Each kind's CSR is built once, on the first slot that asks for that kind."""
+        if getattr(self, "_slot_elem", None) is None:
+            self._slot_elem = {}
+        for name in names:
+            if name not in self._slot_elem:
+                els, counts = self._elems[name]
+                self._check_elements(name, els, counts)
+                rowptrs, entries, e0 = [], [], 0
+                for n, cnt in zip(self.n_rows, counts):
+                    rowptr, ent = ops.element_csr(els[e0:e0 + cnt], n)
+                    rowptrs.append(rowptr)
+                    entries.append(ent)
+                    e0 += cnt
+                self._slot_elem[name] = (torch.cat(rowptrs), torch.cat(entries))
+        sizes = self._slot_tables()[0]
+        cols = [sizes] + [torch.from_numpy(np.stack([np.asarray(self._elems[n][1], np.int64),
+                                                     _starts(self._elems[n][1])[:-1]], 1)).to(self.device)
+                          for n in names]
+        return torch.cat(cols, 1).contiguous(), {n: self._slot_elem[n] for n in names}
+
+    def _check_elements(self, name, els, counts):
+        """Every corner of every mesh's elements names one of the mesh's vertices (one device-to-host read): a slot
+        gathers and sorts them on the device, where an index out of range would read past its rows."""
+        if els.shape[0] == 0:
+            return
+        dev = els.device
+        mesh = torch.repeat_interleave(torch.arange(self.n_meshes, device=dev), torch.tensor(counts, device=dev))
+        n = torch.tensor(self.n_rows, dtype=torch.int64, device=dev)[mesh]
+        bad = ((els < 0) | (els >= n[:, None])).any(dim=1)
+        if bool(bad.any()):
+            e = int(bad.nonzero()[0, 0])
+            m = int(mesh[e])
+            raise ValueError("MeshDataset.slot: {} {} of mesh {} has a corner outside the mesh's {} vertices".format(
+                name[:-1], e - int(_starts(counts)[m]), m, self.n_rows[m]))
 
 
 class MeshBatch:
@@ -466,6 +518,14 @@ def slot_capacity(n_rows, n_ent, n_meshes, sm_count):
     return v_cap, e_cap, min(1024, int(sm_count) + n_meshes)
 
 
+def slot_element_capacity(n_elems, n_meshes):
+    """The element capacity of a slot that holds any ``n_meshes`` distinct meshes whose meshes have ``n_elems``
+    elements of one kind: the sum of the n_meshes largest counts, each padded to a 128-element tile (at least one
+    tile), as slot_capacity sizes the rows."""
+    padded = sorted(((int(n) + 127) // 128 * 128 for n in n_elems), reverse=True)
+    return max(sum(padded[:n_meshes]), 128)
+
+
 _ST_BAD_ID, _ST_OVER_CAPACITY = 1, 2
 
 
@@ -499,11 +559,28 @@ class BatchSlot:
     the capacity reads nothing through the ids and plans every mesh empty, so the step computes NaN for every loss
     (0 / 0 means) and NaN parameter gradients, and sets a sticky status that ``check()`` reads.
 
-    Spectral nets on ``forward_batch_global_nll`` and on ``forward_batch_nll`` with per-vertex labels in the batch
-    layout (``pack``).  A slot keeps no host copy of its layout: ``n_rows``, ``row_begin``, ``unpack``,
-    ``elem_counts``, ``forward_batch``, 'faces' / 'edges' outputs and implicit nets raise NotImplementedError."""
+    Elements: a slot made with ``elements='faces'`` (and / or 'edges', which the dataset's items must carry) holds them
+    too, in an element layout of fixed capacity (``element_capacity[name]``: by default the sum of the n_meshes largest
+    element counts, each padded to 128, so any n_meshes distinct meshes fit; ``max_elements`` sets it, and a slot
+    sized for repeated ids needs it as much as ``max_rows``) planned and gathered by the same two launches.  A slot
+    made without ``elements`` holds none, whatever the items carry, and plans and gathers exactly what it did before
+    elements existed.  Every mesh's elements
+    begin on a 128-element tile; ``faces`` / ``edges`` are int64 (capacity, k) with vertex ids in slot rows, each
+    padding element's corners the first row of its mesh (row 0 past the batch), so every corner names a row.
+    ``element_segments[name]`` is one ``ops.Segments`` per mesh over the element layout and ``element_csr(name)`` the
+    vertex -> element CSR of the real elements (ops.element_csr's format, gathered from per-mesh CSRs the dataset
+    builds once): no vertex's entries reach a padding element.  ``pack_elements(t, name)`` brings per-element data
+    (labels) into the element layout.  A batch whose elements exceed the capacity is over capacity like one whose rows
+    do.
 
-    def __init__(self, ds, n_meshes, max_rows=None, max_entries=None):
+    Spectral nets on ``forward_batch_global_nll``, on ``forward_batch_nll`` with per-vertex labels in the batch layout
+    (``pack``), and for outputs_at 'faces' / 'edges' on ``forward_batch_nll`` with labels in the element layout
+    (``pack_elements``).  A slot keeps no host copy of its layout: ``n_rows``, ``row_begin``, ``unpack``,
+    ``elem_counts``, ``forward_batch`` and implicit nets raise NotImplementedError."""
+
+    element_capacity = types.MappingProxyType({})     # element kind -> capacity (read-only); none unless asked for
+
+    def __init__(self, ds, n_meshes, max_rows=None, max_entries=None, elements=(), max_elements=None):
         n_meshes = operator.index(n_meshes)
         if n_meshes < 1:
             raise ValueError("MeshDataset.slot needs at least one mesh")
@@ -521,7 +598,34 @@ class BatchSlot:
         if e_cap >= _INT32_LIMIT or e_cap < 0:
             raise ValueError("MeshBatch: the batch gradient operators have {} entries, more than int32 indices "
                              "hold".format(e_cap))
+        names = (elements,) if isinstance(elements, str) else tuple(elements or ())
+        for name in names:
+            if name not in ("faces", "edges") or names.count(name) > 1:
+                raise ValueError("MeshDataset.slot: elements are 'faces' and / or 'edges', each once; got {!r}".format(
+                    elements))
+            if name not in ds._elems:
+                raise ValueError("MeshDataset.slot: elements={!r}, but the dataset's items carry no '{}'".format(
+                    elements, name))
+        if max_elements is not None and not names:
+            raise ValueError("MeshDataset.slot: max_elements sizes the elements the slot holds; pass elements= too")
+        if isinstance(max_elements, dict) and set(max_elements) - set(names):
+            raise ValueError("MeshDataset.slot: max_elements names {} the slot does not hold ({})".format(
+                sorted(set(max_elements) - set(names)), list(names)))
+        kinds = [(name, rng, csr_rng) for name, rng, csr_rng in ELEMENT_KINDS if name in names]
+        capacity = {}
+        for name, _, _ in kinds:
+            cap = slot_element_capacity(ds._elems[name][1], n_meshes)
+            m = max_elements.get(name) if isinstance(max_elements, dict) else max_elements
+            if m is not None:
+                cap = max((operator.index(m) + 127) // 128 * 128, 128)
+            if cap * int(ds._elems[name][0].shape[1]) >= _INT32_LIMIT:
+                raise ValueError("MeshDataset.slot: {} {} have more corners than int32 indices hold".format(cap, name))
+            capacity[name] = cap
+        self.element_capacity = types.MappingProxyType(capacity)      # element kind -> capacity, fixed
         sizes, (g_rowptr_t, g_colidx_t, g_vals_t) = ds._slot_tables()
+        elem_csr = {}
+        if kinds:
+            sizes, elem_csr = ds._slot_element_tables([name for name, _, _ in kinds])
         self._ds, self._sizes = ds, sizes
         self.device, self.K, self.n_meshes, self.V = ds.device, ds.K, n_meshes, v_cap
         self.entry_capacity = e_cap
@@ -535,7 +639,9 @@ class BatchSlot:
         n_tiles = v_cap // 128
         (self._row_begin, self._tile_mesh, self._tb_rows, self._cta_begin, seg_begin, seg_rows, tile_seg) = (
             torch.zeros(n, **i32) for n in (B + 1, n_tiles, 2 * n_ctas, B + 1, B, B, n_tiles))
-        self._table = torch.zeros(2 * B, N_RANGES, 4, **i64)
+        self._static = {}
+        self._n_ranges = N_SLOT_RANGES if kinds else N_RANGES
+        self._table = torch.zeros(2 * B, self._n_ranges, 4, **i64)
         self._plan = _lib.dn_slot_plan(*(t.data_ptr() for t in (
             self._row_begin, self._tile_mesh, self._tb_rows, self._cta_begin, seg_begin, seg_rows, tile_seg,
             self._table, self.status)))
@@ -560,6 +666,32 @@ class BatchSlot:
             parts += [part(r_src, r_dst, ADD32, 1, R_PTR, self._tail + 1, R_ENT),
                       part(c_src, c_dst, ADD32, 1, R_ENT, ent_max, R_ROWS),
                       part(v_src, v_dst, COPY, 2, R_ENT, ent_max)]
+        # elements: corners offset by (and padded with) the mesh's first row, the CSR's row pointers placed like the
+        # gradient CSR's and offset to the mesh's first CSR entry, its entries offset to the mesh's first element
+        ADD64 = _lib.GATHER_ADD_I64
+        self.faces = self.edges = None
+        self.element_segments, self._elem_csr, self._elem_tail, self._elem_begin, kind_structs = {}, {}, {}, {}, []
+        for name, rng, csr_rng in kinds:
+            src, counts = ds._elems[name]
+            cap, k = self.element_capacity[name], int(src.shape[1])
+            pad_max = max(max((c + 127) // 128 * 128 for c in counts), 128)
+            tail = self._elem_tail[name] = max(pad_max, -(-cap // (128 * B)) * 128)
+            els = torch.zeros(cap, k, **i64)            # row 0 until the first fill: every corner names a row
+            e_rowptr, e_ent = torch.zeros(v_cap + 1, **i32), torch.zeros(cap * k, **i32)
+            begin, count, e_tile_seg = (torch.zeros(n, **i32) for n in (B + 1, B, cap // 128))
+            src_rowptr, src_ent = elem_csr[name]
+            if src.numel():
+                parts += [part(src, els, ADD64, k, rng, tail, R_CORNER_OFF),
+                          part(src_ent, e_ent, ADD32, 1, csr_rng, k * max(counts), rng)]
+            parts.append(part(src_rowptr, e_rowptr, ADD32, 1, R_PTR, self._tail + 1, csr_rng))
+            setattr(self, name, els)
+            self._elem_csr[name] = (e_rowptr, e_ent)
+            self.element_segments[name] = ops.Segments.wrap(cap, begin[:B], count, e_tile_seg)
+            kind_structs.append(_lib.dn_slot_elements(cap, tail, k, rng, csr_rng, begin.data_ptr(), count.data_ptr(),
+                                                      e_tile_seg.data_ptr()))
+            self._elem_begin[name] = begin
+        self._kinds = (_lib.dn_slot_elements * max(len(kind_structs), 1))(*kind_structs)
+        self._n_kinds = len(kind_structs)
         parts = [p for p, dst in parts if dst.numel() > 0]
         self._parts = (_lib.dn_gather_part * len(parts))(*parts)
         self.gops = ops.GradOperators.from_csr(v_cap, rowptr, colidx, vals)
@@ -568,9 +700,8 @@ class BatchSlot:
         self.desc = _lib.dn_mesh_batch(B, n_ctas, self._tile_mesh.data_ptr(), self._tb_rows.data_ptr(),
                                        self._cta_begin.data_ptr())
         self.segments = ops.Segments.wrap(v_cap, seg_begin, seg_rows, tile_seg)
-        self.has_laplacian, self.lap, self.faces, self.edges = False, None, None, None
+        self.has_laplacian, self.lap = False, None
         self._mesh_ids = self._table[:B, R_MESH, 0]     # the filled ids; 0 for an invalid fill
-        self._static = {}
 
     def fill(self, ids):
         """Plan and gather the batch of dataset meshes ``ids``: a CUDA int64 tensor of n_meshes ids (checked on the
@@ -590,21 +721,34 @@ class BatchSlot:
             ds = self._ds
             rows = sum((ds.n_rows[i] + 127) // 128 * 128 for i in ids)
             ents = sum(ds._grad_nnz[i] for i in ids)
-            if rows > self.V or ents > self.entry_capacity:
-                raise ValueError("BatchSlot.fill: the batch needs {} rows and {} gradient entries, more than the slot's "
-                                 "capacity of {} and {}".format(rows, ents, self.V, self.entry_capacity))
+            elems = {name: sum((ds._elems[name][1][i] + 127) // 128 * 128 for i in ids)
+                     for name in self.element_capacity}
+            if rows > self.V or ents > self.entry_capacity or \
+                    any(e > self.element_capacity[name] for name, e in elems.items()):
+                raise ValueError("BatchSlot.fill: the batch needs {}, more than the slot's capacity of {}".format(
+                    self._amounts(rows, ents, elems), self._capacity_text()))
             self.ids.copy_(torch.tensor(ids, dtype=torch.int64).pin_memory(), non_blocking=True)
         lib = _lib.load()
         with torch.cuda.device(self.device):
             st = ops._stream()
-            _lib.check(lib.dn_mesh_batch_plan_device(
-                self.ids.data_ptr(), self.n_meshes, self._sizes.data_ptr(), self._ds.n_meshes, self._ds._sm, self.V,
-                self.entry_capacity, self._n_ctas, self._tail, N_RANGES, C.byref(self._plan), st),
-                "dn_mesh_batch_plan_device")
+            _lib.check(lib.dn_mesh_batch_plan_device_elements(
+                self.ids.data_ptr(), self.n_meshes, self._sizes.data_ptr(), int(self._sizes.shape[1]),
+                self._ds.n_meshes, self._ds._sm, self.V, self.entry_capacity, self._n_ctas, self._tail,
+                self._n_ranges, C.byref(self._plan), self._kinds, self._n_kinds, R_CORNER_OFF, st),
+                "dn_mesh_batch_plan_device_elements")
             if len(self._parts):
-                _lib.check(lib.dn_batch_gather(self._parts, len(self._parts), self._table.data_ptr(), N_RANGES,
+                _lib.check(lib.dn_batch_gather(self._parts, len(self._parts), self._table.data_ptr(), self._n_ranges,
                                                2 * self.n_meshes, st), "dn_batch_gather")
         return self
+
+    @staticmethod
+    def _amounts(rows, ents, elems):
+        words = ["{} rows".format(rows), "{} gradient entries".format(ents)]
+        words += ["{} {}".format(e, name) for name, e in elems.items()]
+        return ", ".join(words[:-1]) + " and " + words[-1]
+
+    def _capacity_text(self):
+        return self._amounts(self.V, self.entry_capacity, self.element_capacity)
 
     def check(self):
         """Raise if a fill since the last check had invalid device ids (IndexError) or exceeded the capacity
@@ -616,8 +760,8 @@ class BatchSlot:
             raise IndexError("BatchSlot.fill: mesh id {} at position {} is outside the dataset's {} meshes".format(
                 bad, pos, self._ds.n_meshes))
         if kind == _ST_OVER_CAPACITY:
-            raise ValueError("BatchSlot.fill: the batch exceeds the slot's capacity of {} rows and {} gradient entries "
-                             "at position {}".format(self.V, self.entry_capacity, pos))
+            raise ValueError("BatchSlot.fill: the batch exceeds the slot's capacity of {} at position {}".format(
+                self._capacity_text(), pos))
 
     def _static_out(self, what, src, shape):
         key = (what, src.data_ptr(), src.dtype, tuple(src.shape))
@@ -643,11 +787,42 @@ class BatchSlot:
         if width:
             part = _lib.dn_gather_part(t.data_ptr(), out.data_ptr(), _lib.GATHER_COPY, width, R_ROWS, 0, self._tail)
             with torch.cuda.device(self.device):
-                _lib.check(_lib.load().dn_batch_gather(C.byref(part), 1, self._table.data_ptr(), N_RANGES,
+                _lib.check(_lib.load().dn_batch_gather(C.byref(part), 1, self._table.data_ptr(), self._n_ranges,
                                                        2 * self.n_meshes, ops._stream()), "dn_batch_gather")
         if rotations is not None:
             _rotate(out, self, rotations, out)
         return out
+
+    def _element_kind(self, name, what):
+        if name not in self.element_capacity:
+            raise ValueError("BatchSlot.{}: the slot holds no {!r}: it holds {} (the elements every item of the "
+                             "dataset carries)".format(what, name, sorted(self.element_capacity) or "none"))
+        return dict((n, r) for n, r, _ in ELEMENT_KINDS)[name]
+
+    def pack_elements(self, t, name):
+        """A per-element float32 or int64 tensor (E_total,) / (E_total, C) in the dataset's element layout of kind
+        ``name`` ('faces' or 'edges': every mesh's elements back to back, as its items list them), in the slot's
+        element layout, padding elements 0: one launch into a buffer that is the same tensor on every call with the
+        same ``t``.  Labels for forward_batch_nll of a 'faces' / 'edges' net."""
+        rng = self._element_kind(name, "pack_elements")
+        self._ds._check_pack(t, "BatchSlot.pack_elements", self._ds._elems[name][0].shape[0])
+        out = self._static_out("pack_" + name, t, (self.element_capacity[name],) + tuple(t.shape[1:]))
+        t = t.contiguous()
+        width = (t.shape[1] if t.dim() == 2 else 1) * (2 if t.dtype == torch.int64 else 1)
+        if width and t.numel():
+            part = _lib.dn_gather_part(t.data_ptr(), out.data_ptr(), _lib.GATHER_COPY, width, rng, 0,
+                                       self._elem_tail[name])
+            with torch.cuda.device(self.device):
+                _lib.check(_lib.load().dn_batch_gather(C.byref(part), 1, self._table.data_ptr(), self._n_ranges,
+                                                       2 * self.n_meshes, ops._stream()), "dn_batch_gather")
+        return out
+
+    def element_csr(self, name):
+        """(rowptr int32 (V + 1), entries int32): the vertex -> element CSR of the filled batch's real elements of
+        kind ``name``, in ops.element_csr's format on the slot's rows and element layout (ops.element_mean's ``csr``).
+        Gathered at every fill into the same buffers."""
+        self._element_kind(name, "element_csr")
+        return self._elem_csr[name]
 
     def take(self, per_mesh):
         """``per_mesh[ids]`` (a per-mesh tensor of the dataset, e.g. whole-shape labels) into a buffer that is the same

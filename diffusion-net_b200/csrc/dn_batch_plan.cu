@@ -3,7 +3,8 @@
 // batch.batch_tables build on the host, so a training step over any meshes can be captured in one CUDA graph.  One
 // thread per batch mesh; row, entry and CTA starts are block scans.  The host planner's CTA count has one sequential
 // rule (a running count forces one CTA per mesh near the 1024-CTA budget); when the parallel result shows that the
-// rule fires, thread 0 replays the host loop.
+// rule fires, thread 0 replays the host loop.  Element kinds (faces, edges) are planned in the same launch: every mesh's
+// elements start on a 128-element tile, and their vertex -> element CSR entries follow each other without gaps.
 #include "dn_internal.h"
 
 namespace {
@@ -15,10 +16,12 @@ enum { ST_OK = 0, ST_BAD_ID = 1, ST_OVER_CAPACITY = 2 };
 
 struct PlanArgs {
   const int64_t* ids;
-  const int64_t* sizes;              // [n_dataset][4]: rows, first row, gradient entries, first entry
+  // [n_dataset][size_cols]: rows, first row, gradient entries, first entry, then per element kind (count, first)
+  const int64_t* sizes;
   int64_t n_dataset, V_cap, entry_cap, tail_rows;
-  int n_meshes, sm_count, n_tb_ctas, n_ranges;
+  int n_meshes, sm_count, n_tb_ctas, n_ranges, size_cols, n_kinds, corner_range;
   dn_slot_plan out;
+  dn_slot_elements kind[DN_SLOT_MAX_ELEMENT_KINDS];
 };
 
 // inclusive sum over the block's threads; *total gets the sum over all of them
@@ -61,10 +64,12 @@ __global__ void __launch_bounds__(kThreads) plan_kernel(const __grid_constant__ 
   __syncthreads();
 
   int64_t id = 0, n = 0, src_row = 0, ent = 0, src_ent = 0;
+  bool id_ok = false;
   if (b < B) {
     id = a.ids[b];
-    if (id >= 0 && id < a.n_dataset) {
-      const int64_t* s = a.sizes + 4 * id;
+    id_ok = id >= 0 && id < a.n_dataset;
+    if (id_ok) {
+      const int64_t* s = a.sizes + a.size_cols * id;
       n = s[0]; src_row = s[1]; ent = s[2]; src_ent = s[3];
     } else {
       atomicMin(&s_first_bad, b);
@@ -74,6 +79,12 @@ __global__ void __launch_bounds__(kThreads) plan_kernel(const __grid_constant__ 
   int64_t row_end = block_scan(padded, warp_tot, &rows_total);
   int64_t ent_end = block_scan(ent, warp_tot, &ents_total);
   if (b < B && (row_end > a.V_cap || ent_end > a.entry_cap)) atomicMin(&s_first_over, b);
+  for (int q = 0; q < a.n_kinds; ++q) {
+    const int64_t ne = id_ok ? a.sizes[a.size_cols * id + 4 + 2 * q] : 0;
+    int64_t elems_total;
+    const int64_t elem_end = block_scan((ne + 127) / 128 * 128, warp_tot, &elems_total);
+    if (b < B && elem_end > a.kind[q].capacity) atomicMin(&s_first_over, b);
+  }
   __syncthreads();
   // an invalid batch is planned with every mesh empty: nothing is read for it, every loss over it is 0 / 0
   const bool bad = s_first_bad < B || s_first_over < B;
@@ -145,6 +156,8 @@ __global__ void __launch_bounds__(kThreads) plan_kernel(const __grid_constant__ 
     put_range(t + 4 * R_ROWS, 0, start, 0, len);
     put_range(t + 4 * R_PTR, 0, start + 1, 0, len);        // empty rows: every pointer is the batch's entry count
     put_range(t + 4 * R_ENT, 0, ents_total, 0, 0);
+    // element corners are offset by the mesh's first row and padded with it (the tail's with row 0): always a row
+    if (a.n_kinds > 0) put_range(e + 4 * a.corner_range, 0, row0, 0, 0);
   }
   if (b == 0) {
     o.row_begin[B] = (int32_t)rows_total;
@@ -174,18 +187,61 @@ __global__ void __launch_bounds__(kThreads) plan_kernel(const __grid_constant__ 
     o.tile_mesh[tile] = lo;
     o.tile_seg[tile] = r < rows_total ? lo : -1;
   }
+  // element kinds: mesh b's elements at a 128-aligned begin, padded to its tile end; its CSR entries right after the
+  // previous mesh's (so no vertex's entry range crosses a padding element); the tail pieces pad [total, capacity)
+  for (int q = 0; q < a.n_kinds; ++q) {
+    const dn_slot_elements& k = a.kind[q];
+    int64_t ne = 0, src_el = 0;
+    if (b < B && !bad) {
+      const int64_t* s = a.sizes + a.size_cols * id + 4 + 2 * q;
+      ne = s[0]; src_el = s[1];
+    }
+    const int64_t pe = (ne + 127) / 128 * 128, nc = ne * k.k;
+    int64_t elems_total, corners_total;
+    const int64_t e0 = block_scan(pe, warp_tot, &elems_total) - pe;
+    const int64_t c0 = block_scan(nc, warp_tot, &corners_total) - nc;
+    if (b < B) {
+      s_row_begin[b] = (int32_t)e0;
+      k.begin[b] = (int32_t)e0;
+      k.count[b] = (int32_t)ne;
+      int64_t* e = a.out.table + (int64_t)b * a.n_ranges * 4;
+      put_range(e + 4 * k.range, src_el, e0, ne, pe);
+      put_range(e + 4 * k.csr_range, src_el * k.k, c0, nc, nc);
+      int64_t* t = a.out.table + (int64_t)(B + b) * a.n_ranges * 4;
+      const int64_t start = elems_total + b * k.tail;
+      int64_t len = k.capacity - start;
+      len = len < 0 ? 0 : (len > k.tail ? k.tail : len);
+      put_range(t + 4 * k.range, 0, start, 0, len);
+      put_range(t + 4 * k.csr_range, 0, corners_total, 0, 0);
+    }
+    if (b == 0) k.begin[B] = (int32_t)elems_total;
+    __syncthreads();
+    for (int64_t tile = b; tile < k.capacity / 128; tile += kThreads) {
+      const int64_t r = tile * 128;
+      int lo = 0, hi = B - 1;
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) / 2;
+        if (s_row_begin[mid] <= r) lo = mid; else hi = mid - 1;
+      }
+      k.tile_seg[tile] = r < elems_total ? lo : -1;
+    }
+    __syncthreads();
+  }
 }
 
 }  // namespace
 
-int launch_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* sizes, int64_t n_dataset,
-                                  int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas, int64_t tail_rows,
-                                  int n_ranges, const dn_slot_plan& out, cudaStream_t st) {
-  PlanArgs a;
+int launch_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* sizes, int size_cols,
+                                  int64_t n_dataset, int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas,
+                                  int64_t tail_rows, int n_ranges, const dn_slot_plan& out,
+                                  const dn_slot_elements* kinds, int n_kinds, int corner_range, cudaStream_t st) {
+  PlanArgs a = {};
   a.ids = ids; a.sizes = sizes; a.n_dataset = n_dataset;
   a.V_cap = V_cap; a.entry_cap = entry_cap; a.tail_rows = tail_rows;
   a.n_meshes = n_meshes; a.sm_count = sm_count; a.n_tb_ctas = n_tb_ctas; a.n_ranges = n_ranges;
+  a.size_cols = size_cols; a.n_kinds = n_kinds; a.corner_range = corner_range;
   a.out = out;
+  for (int q = 0; q < n_kinds; ++q) a.kind[q] = kinds[q];
   plan_kernel<<<1, kThreads, 0, st>>>(a);
   DN_LAUNCH_CHECK();
   return DN_OK;

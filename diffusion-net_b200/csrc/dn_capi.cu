@@ -1142,6 +1142,35 @@ int dn_batch_gather(const dn_gather_part* parts_host, int n_parts, const int64_t
 int dn_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* dataset_sizes, int64_t n_dataset,
                               int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas, int64_t tail_rows,
                               int n_ranges, const dn_slot_plan* out_host, dn_stream_t stream) {
+  return dn_mesh_batch_plan_device_elements(ids, n_meshes, dataset_sizes, 4, n_dataset, sm_count, V_cap, entry_cap,
+                                            n_tb_ctas, tail_rows, n_ranges, out_host, nullptr, 0, 0, stream);
+}
+
+int dn_mesh_batch_plan_device_elements(const int64_t* ids, int n_meshes, const int64_t* dataset_sizes, int size_cols,
+                                       int64_t n_dataset, int sm_count, int64_t V_cap, int64_t entry_cap,
+                                       int n_tb_ctas, int64_t tail_rows, int n_ranges, const dn_slot_plan* out_host,
+                                       const dn_slot_elements* elements_host, int n_kinds, int corner_range,
+                                       dn_stream_t stream) {
+  if (n_kinds < 0 || n_kinds > DN_SLOT_MAX_ELEMENT_KINDS || (n_kinds > 0 && !elements_host) ||
+      size_cols < 4 + 2 * n_kinds)
+    return DN_ERR_INVALID_ARGUMENT;
+  if (n_kinds > 0) {                   // corner_range, every range and csr_range: distinct, past the four fixed ones
+    int used[2 * DN_SLOT_MAX_ELEMENT_KINDS + 1] = {corner_range};
+    int n_used = 1;
+    for (int q = 0; q < n_kinds; ++q) {
+      const dn_slot_elements& k = elements_host[q];
+      if (k.capacity < 128 || k.capacity % 128 || k.k < 1 || k.capacity * k.k >= (1ll << 31) || k.tail < 1 ||
+          k.tail * n_meshes < k.capacity || !k.begin || !k.count || !k.tile_seg)
+        return DN_ERR_INVALID_ARGUMENT;
+      used[n_used++] = k.range;
+      used[n_used++] = k.csr_range;
+    }
+    for (int i = 0; i < n_used; ++i) {
+      if (used[i] < 4 || used[i] >= n_ranges) return DN_ERR_INVALID_ARGUMENT;
+      for (int j = 0; j < i; ++j)
+        if (used[i] == used[j]) return DN_ERR_INVALID_ARGUMENT;
+    }
+  }
   if (sm_count < 1) sm_count = 132;
   const int64_t min_ctas = sm_count + (int64_t)n_meshes < 1024 ? sm_count + (int64_t)n_meshes : 1024;
   if (!ids || !dataset_sizes || !out_host || n_meshes < 1 || n_meshes > 1024 || n_dataset < 1 || V_cap < 128 ||
@@ -1152,8 +1181,9 @@ int dn_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* d
   if (!o.row_begin || !o.tile_mesh || !o.tb_rows || !o.mesh_cta_begin || !o.seg_begin || !o.seg_rows || !o.tile_seg ||
       !o.table || !o.status)
     return DN_ERR_INVALID_ARGUMENT;
-  return launch_mesh_batch_plan_device(ids, n_meshes, dataset_sizes, n_dataset, sm_count, V_cap, entry_cap, n_tb_ctas,
-                                       tail_rows, n_ranges, o, (cudaStream_t)stream);
+  return launch_mesh_batch_plan_device(ids, n_meshes, dataset_sizes, size_cols, n_dataset, sm_count, V_cap, entry_cap,
+                                       n_tb_ctas, tail_rows, n_ranges, o, elements_host, n_kinds, corner_range,
+                                       (cudaStream_t)stream);
 }
 
 int dn_block_fwd_profile(const float* x_in, const float* mass, const float* evals, const float* evecs,

@@ -195,9 +195,10 @@ int launch_spectral_time_grad_batched(const float* G, const float* x_spec, const
 int launch_batch_gather(const dn_gather_part* parts, int n_parts, const int64_t* table, int n_ranges, int n_meshes,
                         cudaStream_t st);
 // a batch slot's layout planned on the device (dn_batch_plan.cu); arguments checked by dn_mesh_batch_plan_device
-int launch_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* sizes, int64_t n_dataset,
-                                  int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas, int64_t tail_rows,
-                                  int n_ranges, const dn_slot_plan& out, cudaStream_t st);
+int launch_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* sizes, int size_cols,
+                                  int64_t n_dataset, int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas,
+                                  int64_t tail_rows, int n_ranges, const dn_slot_plan& out,
+                                  const dn_slot_elements* kinds, int n_kinds, int corner_range, cudaStream_t st);
 
 // ---- wgmma engine (dn_tc.cu) ----
 // Per-device table, filled on first use of a device: whether it runs the tensor-core kernels (sm_90, with their

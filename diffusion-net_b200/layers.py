@@ -439,7 +439,11 @@ class DiffusionNet(nn.Module):
         With outputs_at='vertices', ``labels`` may instead be one (V,) int64 tensor in the batch layout (``ds.pack``,
         ``BatchSlot.pack``); the per-mesh losses are then formed on the device (the mean of the per-row nll over the
         mesh's rows whose label is not ignore_index, NaN for a mesh without one), whatever the padding rows hold, and
-        ``preds`` is the (V,) prediction in the batch layout.  This is the route of a ``BatchSlot``."""
+        ``preds`` is the (V,) prediction in the batch layout.  This is the route of a ``BatchSlot``.  With outputs_at
+        'faces' / 'edges' on a ``BatchSlot`` that holds those elements, ``labels`` is one (E_cap,) int64 tensor in the
+        slot's element layout (``BatchSlot.pack_elements``): the head runs on the slot's elements with its gathered
+        vertex -> element CSR, and the losses are formed the same way over the element segments, whatever the padding
+        elements hold; ``preds`` is (E_cap,)."""
         self._check_nll_head()
         self._check_batch(batch, "forward_batch_nll")
         if torch.is_tensor(labels):
@@ -485,28 +489,38 @@ class DiffusionNet(nn.Module):
         return losses, preds
 
     def _forward_batch_nll_layout(self, batch, xs, labels, ignore_index, label_smoothing):
-        """forward_batch_nll with (V,) labels in the batch layout: per-mesh losses from the device segment tables."""
+        """forward_batch_nll with (V,) labels in the batch layout, or (E_cap,) labels in a slot's element layout:
+        per-mesh losses from the device segment tables."""
+        elems = csr = None
         if self.outputs_at != 'vertices':
-            err = NotImplementedError if _is_slot(batch) else ValueError
-            raise err("forward_batch_nll: labels in the batch layout are per vertex; outputs_at='{}' takes the list "
-                      "of per-mesh labels of a MeshBatch".format(self.outputs_at))
-        if labels.dtype != torch.int64 or tuple(labels.shape) != (batch.V,):
+            cap = batch.element_capacity.get(self.outputs_at) if _is_slot(batch) else None
+            if cap is None or labels.dim() != 1 or labels.shape[0] != cap:
+                err = NotImplementedError if _is_slot(batch) else ValueError
+                raise err("forward_batch_nll: labels in the batch layout are per vertex; outputs_at='{0}' takes the "
+                          "list of per-mesh labels of a MeshBatch, or ({1},) labels in the element layout of a "
+                          "BatchSlot holding '{0}' (ds.slot(n, elements='{0}'), slot.pack_elements)".format(self.outputs_at,
+                                                                               "E_cap" if cap is None else cap))
+            elems, csr = getattr(batch, self.outputs_at), batch.element_csr(self.outputs_at)
+            seg, n = batch.element_segments[self.outputs_at], cap
+        else:
+            seg, n = batch.segments, batch.V
+        if labels.dtype != torch.int64 or tuple(labels.shape) != (n,):
             raise ValueError("forward_batch_nll: labels in the batch layout must be an int64 tensor of shape ({},), "
-                             "got {} of shape {}".format(batch.V, labels.dtype, tuple(labels.shape)))
+                             "got {} of shape {}".format(n, labels.dtype, tuple(labels.shape)))
         x = xs if torch.is_tensor(xs) else batch.pack(xs)
         if x.shape[-1] != self.C_in:
             raise ValueError("DiffusionNet was constructed with C_in={}, but x_in has last dim={}".format(
                 self.C_in, x.shape[-1]))
         ops._require_cuda(x, labels)
-        seg = batch.segments
         x = self._forward_batch_blocks(batch, x)
-        # padding rows are ignored whatever label they hold (an out-of-range label would make its row NaN)
-        rows = torch.arange(batch.V, device=x.device)
+        # padding rows / elements are ignored whatever label they hold (an out-of-range label would make its row NaN)
+        rows = torch.arange(n, device=x.device)
         s = seg.tile_seg.long()[rows >> 7]
         sc = s.clamp(min=0)
         real = (s >= 0) & (rows < (seg.begin.long() + seg.rows.long())[sc])
         lab = torch.where(real, labels, torch.full_like(labels, ignore_index))
-        nll, pred = self._head_nll(x, lab, None, None, ignore_index, label_smoothing)
+        # elements: the slot's gathered CSR, never cached_element_csr (a fill rewrites the elements in place)
+        nll, pred = self._head_nll(x, lab, elems, csr, ignore_index, label_smoothing)
         # per mesh: sum of nll / number of labelled rows, as the mass-weighted mean with weights (label != ignore)
         w = (lab != ignore_index).to(nll.dtype)
         losses = ops.global_mean_pool(torch.nn.functional.pad(nll[:, None], (0, 3)), w, seg)[:, 0]

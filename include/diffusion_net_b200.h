@@ -487,6 +487,42 @@ int dn_mesh_batch_plan_device(const int64_t* ids, int n_meshes, const int64_t* d
                               int sm_count, int64_t V_cap, int64_t entry_cap, int n_tb_ctas, int64_t tail_rows,
                               int n_ranges, const dn_slot_plan* out_host, dn_stream_t stream);
 
+/* The same planner for a slot that also holds element kinds (faces, edges: outputs_at 'faces' / 'edges' training).
+ * dataset_sizes is [n_dataset][size_cols], size_cols >= 4 + 2 n_kinds: the four columns above, then for kind q the
+ * dataset mesh's (elements, first element) at columns 4 + 2q and 5 + 2q.  With n_kinds = 0 and size_cols = 4 this is
+ * dn_mesh_batch_plan_device, bitwise.  For every kind, in the same launch:
+ *   begin [n_meshes + 1], count [n_meshes]: batch mesh b's elements are [begin[b], begin[b] + count[b]) of the slot's
+ *     element layout of `capacity` elements; every begin is a multiple of 128 (so an element tile belongs to one mesh),
+ *     begin[n_meshes] is the padded total; tile_seg [capacity / 128]: the mesh of every element tile, -1 past the
+ *     total.  (begin, count, tile_seg) are one global-mean segment per mesh over the element layout;
+ *   table range `range` of entry b: (first element, begin[b], count[b], padded count) for the corners, which
+ *     dn_batch_gather offsets by (and pads with) dst_begin of range `corner_range` = the mesh's first row, so every
+ *     padding corner names a row of the slot; tail piece entries pad [begin[n_meshes], capacity) in pieces of `tail`
+ *     elements, their corners row 0;
+ *   table range `csr_range` of entry b: (k * first element, c_b, k count[b], k count[b]) for the mesh's vertex -> element
+ *     CSR entries, c_b the sum of k count over the earlier meshes: no gaps between meshes, so with the row pointers
+ *     gathered through range 2 (offset range csr_range) no vertex's entries reach a padding element.
+ * The kinds' element totals join the capacity check: a batch whose padded elements of a kind exceed its capacity is
+ * over capacity (status 2) and planned empty like any invalid fill.  Requires, besides the above: 0 <= n_kinds <=
+ * DN_SLOT_MAX_ELEMENT_KINDS, every capacity a positive multiple of 128 with k capacity < 2^31, k >= 1, n_meshes tail >=
+ * capacity, and corner_range, every range and every csr_range distinct, in [4, n_ranges). */
+#define DN_SLOT_MAX_ELEMENT_KINDS 2
+typedef struct dn_slot_elements {
+  int64_t capacity;          /* elements of the slot's element layout   */
+  int64_t tail;              /* elements per tail piece                  */
+  int32_t k;                 /* corners per element: 3 faces, 2 edges    */
+  int32_t range;             /* table range of the elements (corners)    */
+  int32_t csr_range;         /* table range of the vertex -> element CSR */
+  int32_t* begin;            /* [n_meshes + 1]                           */
+  int32_t* count;            /* [n_meshes]                               */
+  int32_t* tile_seg;         /* [capacity / 128]                         */
+} dn_slot_elements;
+int dn_mesh_batch_plan_device_elements(const int64_t* ids, int n_meshes, const int64_t* dataset_sizes, int size_cols,
+                                       int64_t n_dataset, int sm_count, int64_t V_cap, int64_t entry_cap,
+                                       int n_tb_ctas, int64_t tail_rows, int n_ranges, const dn_slot_plan* out_host,
+                                       const dn_slot_elements* elements_host, int n_kinds, int corner_range,
+                                       dn_stream_t stream);
+
 /* Per-mesh rotations of the (V, 3) rows of a batch laid out as above (the reference's random_rotate_points on every
  * mesh of a batch or slot): out[v] = x[v] @ R[tile_mesh[v / 128]], R device (n_meshes, 3, 3) row-major, each output
  * one fp32 FMA chain x0 R[0][j], + x1 R[1][j], + x2 R[2][j].  tile_mesh is the batch's (device, V / 128 entries), so

@@ -4,12 +4,20 @@ The shared object is built IN-TREE (``diffusion-net_b200/libdiffusion_net_b200.s
 with nvcc for sm_90a (H100) and loaded with ctypes -- plain pointers and sizes, no torch
 types cross the boundary.  There is no CPU or library fallback: if the library is
 missing or a call fails, a RuntimeError is raised.
+
+The header is the only place a signature or constant is written: every ``dn_*``
+declaration is bound from it (``SIGNATURES``), and its integer ``DN_*`` macros and
+enum members are this module's names without the prefix (``ENGINE_TC3X``,
+``GATHER_MAX_PARTS``, ``ERR_UNSUPPORTED``, ``ABI_VERSION``, ``PROFILE_STAGES``, ...).
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 import subprocess
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
@@ -21,8 +29,6 @@ HEADER = os.path.join(os.path.dirname(_HERE), "include", "diffusion_net_b200.h")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
-
-ENGINE_SIMT, ENGINE_TC3X, ENGINE_TC1X, ENGINE_BF16 = 0, 1, 2, 3
 
 
 def _stale() -> bool:
@@ -75,10 +81,6 @@ class dn_gather_part(C.Structure):
                 ("offset_range", C.c_int32), ("max_units", C.c_int64)]
 
 
-GATHER_COPY, GATHER_ADD_I32, GATHER_ADD_I64 = 0, 1, 2
-GATHER_MAX_PARTS = 16
-
-
 class dn_slot_plan(C.Structure):
     _fields_ = [(name, C.c_void_p) for name in ("row_begin", "tile_mesh", "tb_rows", "mesh_cta_begin", "seg_begin",
                                                 "seg_rows", "tile_seg", "table", "status")]
@@ -100,96 +102,58 @@ class dn_head(C.Structure):
     _fields_ = [("weight", C.c_void_p), ("bias", C.c_void_p), ("n_out", C.c_int32), ("out", C.c_void_p), ("ld_out", C.c_int64)]
 
 
-_P, _I, _L, _D = C.c_void_p, C.c_int, C.c_int64, C.c_double
-_PP = C.POINTER(C.c_void_p)
-_IP = C.POINTER(C.c_int)
+_STRUCTS = {cls.__name__: cls for cls in (dn_patches, dn_csr, dn_block_params, dn_mesh_batch, dn_gather_part,
+                                           dn_slot_plan, dn_slot_elements, dn_eig_batch, dn_head)}
+_SCALARS = {"int": C.c_int, "int64_t": C.c_int64, "double": C.c_double, "float": C.c_float,
+            "dn_stream_t": C.c_void_p}      # dn_stream_t is a typedef of void*
 
-# name -> (restype, argtypes): every symbol include/diffusion_net_b200.h declares
-SIGNATURES = {
-    "dn_abi_version": (_I, []),
-    "dn_error_string": (C.c_char_p, [_I]),
-    "dn_device_query": (_I, [_I, _IP, _IP, C.POINTER(_L)]),
-    "dn_kernel_launch_count": (_L, []),
-    "dn_workspace_bytes": (_L, [_L, _I, _I]),
-    "dn_csr_from_coo": (_I, [_P, _P, _P, _P, _L, _L, _P, _P, _P, _P]),
-    "dn_patch_build": (_L, [_L, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
-    "dn_csr_transpose": (_I, [C.POINTER(dn_csr), _L, _P, _P, _P, _P, _L, _P]),
-    "dn_compute_hks": (_I, [_P, _P, _P, _L, _I, _I, _P, _P]),
-    "dn_to_basis": (_I, [_P, _P, _P, _L, _I, _I, _P, _P, _L, _I, _P]),
-    "dn_from_basis": (_I, [_P, _P, _P, _L, _I, _I, _P, _P, _L, _I, _P]),
-    "dn_learned_time_diffusion_fwd": (_I, [_P, _P, _P, _P, _P, _L, _I, _I, _P, _P, _P, _L, _I, _P]),
-    "dn_learned_time_diffusion_bwd": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _P, _P, _P, _L, _I, _P]),
-    "dn_grad_spmm": (_I, [C.POINTER(dn_csr), _P, _L, _I, _P, _P]),
-    "dn_spatial_gradient_features_fwd": (_I, [_P, _P, _P, _I, _L, _I, _P, _P, _L, _I, _P]),
-    "dn_gradient_features_fwd": (_I, [C.POINTER(dn_csr), _P, _P, _P, _I, _L, _I, _P, _P, _P, _L, _I, _P]),
-    "dn_gradient_features_bwd": (_I, [C.POINTER(dn_csr), C.POINTER(dn_csr), _P, _P, _P, _P, _P, _P, _I, _L, _I,
-                                      _P, _P, _P, _P, _L, _I, _P]),
-    "dn_mini_mlp_fwd": (_I, [_PP, _IP, _I, _PP, _PP, _IP, _I, _PP, _P, _L, _PP, _P, _P, _L, _I, _P]),
-    "dn_mini_mlp_bwd": (_I, [_P, _PP, _IP, _I, _PP, _IP, _I, _PP, _PP, _L, _PP, _PP, _PP, _P, _L, _I, _P]),
-    "dn_block_fwd": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), _L, _I, _I, _P, _P, _L,
-                          _I, _P]),
-    "dn_block_fwd_profile": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), _L, _I, _I, _P, _P, _L,
-                                  _I, _P, C.POINTER(C.c_float)]),
-    "dn_build_grad": (_I, [_P, _P, _P, _P, _L, _L, _P, _P, _P, _P, _L, _P]),
-    "dn_mesh_laplacian": (_I, [_P, _P, _L, _L, _D, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P]),
-    "dn_vertex_frames": (_I, [_P, _P, _L, _L, _P, _P, _P, _P, _P, _L, _P]),
-    "dn_eig_filter": (_I, [_P, _P, _P, _P, _L, _I, _P, _P, _L, _D, _D, _D, _P, _P]),
-    "dn_eig_gram": (_I, [_P, _L, _P, _L, _L, _I, _I, _P, _P, _L, _P]),
-    "dn_eig_rotate": (_I, [_P, _L, _P, _L, _L, _I, _I, _D, _P, _L, _P]),
-    "dn_eig_residual_norms": (_I, [_P, _L, _P, _L, _P, _L, _I, _P, _P, _L, _P]),
-    "dn_eig_finalize": (_I, [_P, _L, _P, _I, _P, _L, _P, _P, _L, _P]),
-    "dn_mesh_laplacian_batched": (_I, [_P, _P, _L, _L, _I, _P, _D, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P]),
-    "dn_eig_filter_batched": (_I, [_P, _P, _P, _P, C.POINTER(dn_eig_batch), _I, _P, _P, _L, _P, _P, _P, _P, _P, _P]),
-    "dn_eig_gram_batched": (_I, [_P, _L, _P, _L, C.POINTER(dn_eig_batch), _I, _I, _P, _P, _P, _L, _P]),
-    "dn_eig_rotate_batched": (_I, [_P, _L, _P, C.POINTER(dn_eig_batch), _I, _I, _D, _P, _P, _L, _P]),
-    "dn_eig_residual_norms_batched": (_I, [_P, _L, _P, _L, _P, C.POINTER(dn_eig_batch), _I, _P, _P, _P, _L, _P]),
-    "dn_eig_finalize_batched": (_I, [_P, _L, _P, _I, _P, C.POINTER(dn_eig_batch), _P, _P, _L, _P]),
-    "dn_implicit_diffusion_workspace_bytes": (_L, [_L, _I]),
-    "dn_implicit_diffusion_fwd": (_I, [C.POINTER(dn_csr), _P, _P, _P, _L, _I, _D, _I, _P, _P, _P, _L, _P]),
-    "dn_implicit_diffusion_bwd": (_I, [C.POINTER(dn_csr), _P, _P, _P, _P, _L, _I, _D, _I, _P, _P, _P, _P, _L, _P]),
-    "dn_implicit_diffusion_workspace_bytes_batched": (_L, [_L, _I, _I]),
-    "dn_implicit_diffusion_fwd_batched": (_I, [C.POINTER(dn_csr), _P, _P, _P, C.POINTER(dn_mesh_batch), _P, _L, _I, _D,
-                                               _I, _P, _P, _P, _L, _P]),
-    "dn_implicit_diffusion_bwd_batched": (_I, [C.POINTER(dn_csr), _P, _P, _P, _P, C.POINTER(dn_mesh_batch), _P, _L, _I,
-                                               _D, _I, _P, _P, _P, _P, _L, _P]),
-    "dn_fmap_solve_fwd": (_I, [_P, _P, _P, _P, _I, _I, _D, _P, _P]),
-    "dn_fmap_solve_bwd": (_I, [_P, _P, _P, _P, _I, _I, _D, _P, _P, _P, _P, _L, _P]),
-    "dn_nearest_neighbor_workspace_bytes": (_L, [_L, _L, _I]),
-    "dn_nearest_neighbor": (_I, [_P, _L, _P, _L, _I, _P, _P, _L, _P]),
-    "dn_mesh_batch_plan": (_I, [_I, _P, _I, _P, _P, _P, _P]),
-    "dn_batch_gather": (_I, [C.POINTER(dn_gather_part), _I, _P, _I, _I, _P]),
-    "dn_mesh_batch_plan_device": (_I, [_P, _I, _P, _L, _I, _L, _L, _I, _L, _I, C.POINTER(dn_slot_plan), _P]),
-    "dn_mesh_batch_plan_device_elements": (_I, [_P, _I, _P, _I, _L, _I, _L, _L, _I, _L, _I, C.POINTER(dn_slot_plan),
-                                                C.POINTER(dn_slot_elements), _I, _I, _P]),
-    "dn_rotate_rows": (_I, [_P, _L, _P, _I, _P, _P, _P]),
-    "dn_block_fwd_ex": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),
-                             C.POINTER(dn_head), _L, _I, _I, _P, _P, _L, _I, _P]),
-    "dn_block_fwd_batched": (_I, [_P, _P, _P, _P, C.POINTER(dn_csr), C.POINTER(dn_block_params), C.POINTER(dn_mesh_batch),
-                                  _L, _I, _I, _P, _P, _L, _I, _P]),
-    "dn_learned_time_diffusion_fwd_batched": (_I, [_P, _P, _P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P, _P,
-                                                   _L, _I, _P]),
-    "dn_learned_time_diffusion_bwd_batched": (_I, [_P, _P, _P, _P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P,
-                                                   _P, _L, _I, _P]),
-    "dn_to_basis_batched": (_I, [_P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P, _L, _I, _P]),
-    "dn_from_basis_batched": (_I, [_P, _P, _P, C.POINTER(dn_mesh_batch), _L, _I, _I, _P, _P, _L, _I, _P]),
-    "dn_fmap_solve_batched_workspace_bytes": (_L, [_I, _I, _I]),
-    "dn_fmap_solve_fwd_batched": (_I, [_P, _L, _P, _L, _I, _P, _P, _I, _I, _I, _D, _P, _P]),
-    "dn_fmap_solve_bwd_batched": (_I, [_P, _L, _P, _L, _I, _P, _P, _I, _P, _P, _I, _I, _D, _P, _P, _P, _L, _P]),
-    "dn_fmap_pointwise_map_batched_workspace_bytes": (_L, [_I, _I, _P, _P, _P, _P, _I]),
-    "dn_fmap_pointwise_map_batched": (_I, [_P, _I, _P, _L, _P, _P, _I, _P, _P, _I, _P, _P, _L, _P]),
-    "dn_fmap_ground_truth_workspace_bytes": (_L, [_I, _I, _L]),
-    "dn_fmap_ground_truth": (_I, [_P, _L, _I, _P, _P, _L, _P, _L, _P, _I, _L, _P, _P, _P, _L, _P]),
-    "dn_linear_nll_workspace_bytes": (_L, [_L, _I, _I]),
-    "dn_linear_nll_fwd": (_I, [_P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _I, _P]),
-    "dn_linear_nll_bwd": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _P, _L, _I, _P]),
-    "dn_element_mean_fwd": (_I, [_P, _L, _I, _P, _L, _I, _P, _P]),
-    "dn_element_mean_bwd": (_I, [_P, _L, _I, _P, _P, _L, _I, _P, _P]),
-    "dn_linear_nll_ls_fwd": (_I, [_P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _I, _P, C.c_float]),
-    "dn_linear_nll_ls_bwd": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _L, _P, _P, _P, _P, _L, _I, _P, C.c_float]),
-    "dn_global_mean_workspace_bytes": (_L, [_L, _I]),
-    "dn_global_mean_fwd": (_I, [_P, _P, _L, _I, _P, _P, _P, _I, _P, _P, _P, _L, _P]),
-    "dn_global_mean_bwd": (_I, [_P, _P, _P, _L, _I, _P, _P, _P, _I, _P, _P]),
-}
+
+def _ctype(decl, ctype, structs, result=False):
+    """The ctypes type of a header type: a scalar, a `const char*` return, a pointer to a header struct, or any
+    other pointer (device data, host arrays, T* const*), passed as a plain address."""
+    words = ctype.replace("*", " * ").split()
+    base = [w for w in words if w not in ("const", "*")]
+    stars = words.count("*")
+    if stars == 0 and len(base) == 1 and base[0] in _SCALARS:
+        return _SCALARS[base[0]]
+    if result and words == ["const", "char", "*"]:
+        return C.c_char_p
+    if stars == 1 and len(base) == 1 and base[0] in structs:
+        if base[0] not in _STRUCTS:
+            raise RuntimeError("diffusion_net_b200: {}: struct {} has no ctypes class".format(decl, base[0]))
+        return C.POINTER(_STRUCTS[base[0]])
+    if stars and not result:
+        return C.c_void_p
+    raise RuntimeError("diffusion_net_b200: {}: unsupported type '{}' in {}".format(decl, " ".join(words), HEADER))
+
+
+def parse_header(text):
+    """(signatures, constants) of the C-ABI header: name -> (restype, argtypes) for every dn_* declaration, and
+    name -> value for every integer #define and enum member named DN_*."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", "", text, flags=re.S)
+    constants = {k: int(v) for k, v in re.findall(r"^#define[ \t]+(DN_\w+)[ \t]+(-?\d+)[ \t]*$", text, re.M)}
+    for body in re.findall(r"\benum\s+\w+\s*\{([^}]*)\}", text):
+        value = -1
+        for member in filter(None, (m.strip() for m in body.split(","))):
+            name, _, v = member.partition("=")
+            value = int(v) if v.strip() else value + 1
+            constants[name.strip()] = value
+    structs = set(re.findall(r"\bstruct\s+(\w+)", text))
+    signatures = {}
+    for stmt in re.split(r"[;{}]", re.sub(r"^#[^\n]*", "", text, flags=re.M)):
+        m = re.fullmatch(r"\s*([\w\s*]+?)\s*\b(dn_\w+)\s*\(([^()]*)\)\s*", stmt)
+        if m is None:
+            continue
+        ret, name, params = m.groups()
+        params = [] if params.strip() in ("", "void") else params.split(",")
+        signatures[name] = (_ctype(name, ret, structs, result=True),
+                            [_ctype(name, re.sub(r"\w+\s*$", "", p), structs) for p in params])
+    return signatures, constants
+
+
+with open(HEADER) as _fh:
+    SIGNATURES, _constants = parse_header(_fh.read())
+globals().update({k[len("DN_"):]: v for k, v in _constants.items()})
 
 _lib = None
 
@@ -209,7 +173,7 @@ def load():
         fn = getattr(lib, name)          # AttributeError if a declared symbol is not exported
         fn.restype = res
         fn.argtypes = args
-    if lib.dn_abi_version() != 5:
+    if lib.dn_abi_version() != ABI_VERSION:
         raise RuntimeError("diffusion_net_b200: ABI version mismatch")
     _lib = lib
     return lib
@@ -219,6 +183,18 @@ def check(code: int, what: str = ""):
     if code != 0:
         msg = load().dn_error_string(code).decode()
         raise RuntimeError("diffusion_net_b200 {} failed ({}): {}".format(what, code, msg))
+
+
+def addresses(args):
+    """``args`` with every torch.Tensor replaced by its data_ptr(); every other argument (ints, floats, None, ctypes
+    objects) as it is."""
+    return [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+
+
+def call(name, *args):
+    """Call the entry point ``name``, whose int return is a status, with ``addresses(args)`` (the tensors stay
+    referenced until the call returns), and raise as ``check`` does unless it is DN_OK."""
+    check(getattr(load(), name)(*addresses(args)), name)
 
 
 def ptr_array(ptrs):

@@ -72,7 +72,7 @@ def _check_items(items, device):
 def _sm_count(dev):
     sm, cc, smem = C.c_int(0), C.c_int(0), C.c_int64(0)
     idx = dev.index if dev.index is not None else torch.cuda.current_device()
-    _lib.check(_lib.load().dn_device_query(idx, C.byref(sm), C.byref(cc), C.byref(smem)), "dn_device_query")
+    _lib.call("dn_device_query", idx, C.byref(sm), C.byref(cc), C.byref(smem))
     return int(sm.value)
 
 
@@ -84,9 +84,9 @@ def plan_rows(n_rows, sm_count):
     B = len(n_rows)
     padded = (n_rows + 127) // 128 * 128
     if B < 1 or (n_rows < 0).any():
-        _lib.check(-1, "dn_mesh_batch_plan")
+        _lib.check(_lib.ERR_INVALID_ARGUMENT, "dn_mesh_batch_plan")
     if int(padded.sum()) >= _INT32_LIMIT - 256:
-        _lib.check(-2, "dn_mesh_batch_plan")
+        _lib.check(_lib.ERR_UNSUPPORTED, "dn_mesh_batch_plan")
     row_begin = np.zeros(B + 1, dtype=np.int32)
     tile_mesh = np.zeros(max(int(padded.sum()) // 128, 1), dtype=np.int32)
     tb_rows = np.zeros(2 * 1024, dtype=np.int32)
@@ -187,8 +187,7 @@ def _gather(parts, table, n_meshes, dev):
         return
     arr = (_lib.dn_gather_part * len(parts))(*parts)
     with torch.cuda.device(dev):
-        _lib.check(_lib.load().dn_batch_gather(arr, len(parts), table.data_ptr(), N_RANGES, n_meshes, ops._stream()),
-                   "dn_batch_gather")
+        _lib.call("dn_batch_gather", arr, len(parts), table, N_RANGES, n_meshes, ops._stream())
 
 
 class _DatasetLaplacian:
@@ -585,7 +584,7 @@ class BatchSlot:
         if n_meshes < 1:
             raise ValueError("MeshDataset.slot needs at least one mesh")
         if n_meshes > 1024:
-            _lib.check(-2, "MeshDataset.slot ({} meshes; at most 1024)".format(n_meshes))
+            _lib.check(_lib.ERR_UNSUPPORTED, "MeshDataset.slot ({} meshes; at most 1024)".format(n_meshes))
         if ds.K == 0:
             raise ValueError("MeshDataset.slot: the dataset has no eigenpairs (k_eig = 0); a slot serves spectral nets")
         v_cap, e_cap, n_ctas = slot_capacity(ds.n_rows, ds._grad_nnz, n_meshes, ds._sm)
@@ -594,7 +593,7 @@ class BatchSlot:
         if max_entries is not None:
             e_cap = operator.index(max_entries)
         if v_cap >= _INT32_LIMIT - 256:
-            _lib.check(-2, "MeshDataset.slot ({} rows)".format(v_cap))
+            _lib.check(_lib.ERR_UNSUPPORTED, "MeshDataset.slot ({} rows)".format(v_cap))
         if e_cap >= _INT32_LIMIT or e_cap < 0:
             raise ValueError("MeshBatch: the batch gradient operators have {} entries, more than int32 indices "
                              "hold".format(e_cap))
@@ -728,17 +727,15 @@ class BatchSlot:
                 raise ValueError("BatchSlot.fill: the batch needs {}, more than the slot's capacity of {}".format(
                     self._amounts(rows, ents, elems), self._capacity_text()))
             self.ids.copy_(torch.tensor(ids, dtype=torch.int64).pin_memory(), non_blocking=True)
-        lib = _lib.load()
         with torch.cuda.device(self.device):
             st = ops._stream()
-            _lib.check(lib.dn_mesh_batch_plan_device_elements(
-                self.ids.data_ptr(), self.n_meshes, self._sizes.data_ptr(), int(self._sizes.shape[1]),
-                self._ds.n_meshes, self._ds._sm, self.V, self.entry_capacity, self._n_ctas, self._tail,
-                self._n_ranges, C.byref(self._plan), self._kinds, self._n_kinds, R_CORNER_OFF, st),
-                "dn_mesh_batch_plan_device_elements")
+            _lib.call("dn_mesh_batch_plan_device_elements", self.ids, self.n_meshes, self._sizes,
+                      int(self._sizes.shape[1]), self._ds.n_meshes, self._ds._sm, self.V, self.entry_capacity,
+                      self._n_ctas, self._tail, self._n_ranges, C.byref(self._plan), self._kinds, self._n_kinds,
+                      R_CORNER_OFF, st)
             if len(self._parts):
-                _lib.check(lib.dn_batch_gather(self._parts, len(self._parts), self._table.data_ptr(), self._n_ranges,
-                                               2 * self.n_meshes, st), "dn_batch_gather")
+                _lib.call("dn_batch_gather", self._parts, len(self._parts), self._table, self._n_ranges,
+                          2 * self.n_meshes, st)
         return self
 
     @staticmethod
@@ -787,8 +784,8 @@ class BatchSlot:
         if width:
             part = _lib.dn_gather_part(t.data_ptr(), out.data_ptr(), _lib.GATHER_COPY, width, R_ROWS, 0, self._tail)
             with torch.cuda.device(self.device):
-                _lib.check(_lib.load().dn_batch_gather(C.byref(part), 1, self._table.data_ptr(), self._n_ranges,
-                                                       2 * self.n_meshes, ops._stream()), "dn_batch_gather")
+                _lib.call("dn_batch_gather", C.byref(part), 1, self._table, self._n_ranges, 2 * self.n_meshes,
+                          ops._stream())
         if rotations is not None:
             _rotate(out, self, rotations, out)
         return out
@@ -813,8 +810,8 @@ class BatchSlot:
             part = _lib.dn_gather_part(t.data_ptr(), out.data_ptr(), _lib.GATHER_COPY, width, rng, 0,
                                        self._elem_tail[name])
             with torch.cuda.device(self.device):
-                _lib.check(_lib.load().dn_batch_gather(C.byref(part), 1, self._table.data_ptr(), self._n_ranges,
-                                                       2 * self.n_meshes, ops._stream()), "dn_batch_gather")
+                _lib.call("dn_batch_gather", C.byref(part), 1, self._table, self._n_ranges, 2 * self.n_meshes,
+                          ops._stream())
         return out
 
     def element_csr(self, name):
@@ -913,11 +910,8 @@ def _check_rotated(t, rotations, batch, what):
 
 
 def _rotate(x, batch, R, out):
-    R = R.contiguous()
     with torch.cuda.device(batch.device):
-        _lib.check(_lib.load().dn_rotate_rows(x.data_ptr(), batch.V, R.data_ptr(), batch.n_meshes,
-                                              batch._tile_mesh.data_ptr(), out.data_ptr(), ops._stream()),
-                   "dn_rotate_rows")
+        _lib.call("dn_rotate_rows", x, batch.V, R.contiguous(), batch.n_meshes, batch._tile_mesh, out, ops._stream())
     return out
 
 

@@ -82,10 +82,6 @@ class LaplaceOperator:
         self.bound = float(bound)
 
 
-def _check(code, what):
-    _lib.check(code, what)
-
-
 class _Solver:
     def __init__(self, op, k, B, seed):
         self.op, self.k, self.B, self.V = op, k, B, op.V
@@ -109,29 +105,25 @@ class _Solver:
 
     def filt(self, src, prev, dst, c0, alpha, beta, gamma):
         op = self.op
-        _check(self.lib.dn_eig_filter(op.rowptr.data_ptr(), op.colidx.data_ptr(), op.avals.data_ptr(),
-                                      op.adiag.data_ptr(), self.V, self.B - c0, self._p(src, c0),
-                                      self._p(prev, c0) if prev is not None else None, self.B, alpha, beta, gamma,
-                                      self._p(dst, c0), ops._stream()), "dn_eig_filter")
+        _lib.call("dn_eig_filter", op.rowptr, op.colidx, op.avals, op.adiag, self.V, self.B - c0, self._p(src, c0),
+                  self._p(prev, c0) if prev is not None else None, self.B, alpha, beta, gamma, self._p(dst, c0),
+                  ops._stream())
 
     def gram(self, X, xc0, xn, Y, yc0, yn):
         out = torch.empty(xn, yn, dtype=torch.float64, device=self.dev)
-        _check(self.lib.dn_eig_gram(self._p(X, xc0), self.B, self._p(Y, yc0), self.B, self.V, xn, yn, out.data_ptr(),
-                                    self.ws.data_ptr(), self.ws.numel(), ops._stream()), "dn_eig_gram")
+        _lib.call("dn_eig_gram", self._p(X, xc0), self.B, self._p(Y, yc0), self.B, self.V, xn, yn, out, self.ws,
+                  self.ws.numel(), ops._stream())
         return out
 
     def rotate(self, X, xc0, kd, Cm, Z, zc0, n, beta=0.0):
-        Cm = Cm.contiguous()
-        _check(self.lib.dn_eig_rotate(self._p(X, xc0), self.B, Cm.data_ptr(), n, self.V, kd, n, beta, self._p(Z, zc0),
-                                      self.B, ops._stream()), "dn_eig_rotate")
+        _lib.call("dn_eig_rotate", self._p(X, xc0), self.B, Cm.contiguous(), n, self.V, kd, n, beta, self._p(Z, zc0),
+                  self.B, ops._stream())
 
     def residuals(self, Wb, Qb, c0, theta):
         n = self.B - c0
         out = torch.empty(n, dtype=torch.float64, device=self.dev)
-        theta = theta.contiguous()
-        _check(self.lib.dn_eig_residual_norms(self._p(Wb, c0), self.B, self._p(Qb, c0), self.B, theta.data_ptr(),
-                                              self.V, n, out.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
-                                              ops._stream()), "dn_eig_residual_norms")
+        _lib.call("dn_eig_residual_norms", self._p(Wb, c0), self.B, self._p(Qb, c0), self.B, theta.contiguous(), self.V,
+                  n, out, self.ws, self.ws.numel(), ops._stream())
         return out
 
     # ---- the steps of one outer iteration ------------------------------------------------------------------------
@@ -247,8 +239,8 @@ def lowest_eigenpairs(op, k, seed=0, stats=None):
     idx = torch.sort(theta_all, stable=True).indices[:k]
     cols = idx.to(torch.int32).contiguous()
     evecs = torch.empty(V, k, dtype=torch.float64, device=dev)
-    _check(s.lib.dn_eig_finalize(s.Q.data_ptr(), B, cols.data_ptr(), k, op.mass.data_ptr(), V, evecs.data_ptr(),
-                                 s.ws.data_ptr(), s.ws.numel(), ops._stream()), "dn_eig_finalize")
+    _lib.check(s.lib.dn_eig_finalize(*_lib.addresses((s.Q, B, cols, k, op.mass, V, evecs, s.ws, s.ws.numel(),
+                                                      ops._stream()))), "dn_eig_finalize")
     evals = theta_all[idx].clamp_min(0.0)
     if stats is not None:
         torch.cuda.synchronize(dev)
@@ -262,7 +254,7 @@ def lowest_eigenpairs(op, k, seed=0, stats=None):
 # ----------------------------------------------------------------------------------------------------------------------
 # the same iteration for a batch of small meshes, as one launch sequence
 # ----------------------------------------------------------------------------------------------------------------------
-TILE_ROWS, SLICE_ROWS = 64, 1024        # DN_EIG_TILE_ROWS, DN_EIG_SLICE_ROWS of the header
+TILE_ROWS, SLICE_ROWS = _lib.EIG_TILE_ROWS, _lib.EIG_SLICE_ROWS
 
 
 class BatchPlan:
@@ -290,7 +282,6 @@ class _BatchSolver:
     def __init__(self, ops_, k, B, seed):
         import ctypes
         self.k, self.B, self.n = k, B, len(ops_)
-        self.lib = _lib.load()
         dev = self.dev = ops_[0].mass.device
         f64 = torch.float64
         self.plan = BatchPlan([op.V for op in ops_], dev)
@@ -331,23 +322,18 @@ class _BatchSolver:
 
     def filt(self, src, prev, dst, coef):
         """coef: (3, n) device rows alpha, beta, gamma"""
-        _check(self.lib.dn_eig_filter_batched(self.rowptr.data_ptr(), self.colidx.data_ptr(), self.avals.data_ptr(),
-                                              self.adiag.data_ptr(), self.bt, self.B, src.data_ptr(),
-                                              prev.data_ptr() if prev is not None else None, self.B, coef[0].data_ptr(),
-                                              coef[1].data_ptr(), coef[2].data_ptr(), self.active.data_ptr(),
-                                              dst.data_ptr(), ops._stream()), "dn_eig_filter_batched")
+        _lib.call("dn_eig_filter_batched", self.rowptr, self.colidx, self.avals, self.adiag, self.bt, self.B, src, prev,
+                  self.B, coef[0], coef[1], coef[2], self.active, dst, ops._stream())
 
     def gram(self, X, Y):
-        _check(self.lib.dn_eig_gram_batched(X.data_ptr(), self.B, Y.data_ptr(), self.B, self.bt, self.B, self.B,
-                                            self.active.data_ptr(), self.G.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
-                                            ops._stream()), "dn_eig_gram_batched")
+        _lib.call("dn_eig_gram_batched", X, self.B, Y, self.B, self.bt, self.B, self.B, self.active, self.G, self.ws,
+                  self.ws.numel(), ops._stream())
         G = self.G[self.act]
         return 0.5 * (G + G.transpose(1, 2))
 
     def rotate(self, X, Cm, Z):
-        _check(self.lib.dn_eig_rotate_batched(X.data_ptr(), self.B, Cm.data_ptr(), self.bt, self.B, self.B, 0.0,
-                                              self.active.data_ptr(), Z.data_ptr(), self.B, ops._stream()),
-               "dn_eig_rotate_batched")
+        _lib.call("dn_eig_rotate_batched", X, self.B, Cm, self.bt, self.B, self.B, 0.0, self.active, Z, self.B,
+                  ops._stream())
 
     def _dense(self, fn):
         a = _event()
@@ -400,10 +386,8 @@ class _BatchSolver:
         self._dense(dense)
         self.rotate(Z, self.Cm, self.Q)
         self.rotate(self.W, self.Cm, self.W2)
-        _check(self.lib.dn_eig_residual_norms_batched(self.W2.data_ptr(), self.B, self.Q.data_ptr(), self.B,
-                                                      theta_all.data_ptr(), self.bt, self.B, self.active.data_ptr(),
-                                                      res_all.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
-                                                      ops._stream()), "dn_eig_residual_norms_batched")
+        _lib.call("dn_eig_residual_norms_batched", self.W2, self.B, self.Q, self.B, theta_all, self.bt, self.B,
+                  self.active, res_all, self.ws, self.ws.numel(), ops._stream())
 
 
 def lowest_eigenpairs_batch(ops_, k, seed=0, stats=None, first=0):
@@ -486,9 +470,7 @@ def lowest_eigenpairs_batch(ops_, k, seed=0, stats=None, first=0):
         # eigh returns every mesh's Ritz values ascending and nothing was locked: the k lowest are the first k columns
         cols = torch.arange(k, dtype=torch.int32, device=dev).repeat(m, 1).contiguous()
         evecs = torch.empty(s.plan.V, k, dtype=torch.float64, device=dev)
-        _check(s.lib.dn_eig_finalize_batched(s.Q.data_ptr(), B, cols.data_ptr(), k, s.mass.data_ptr(), s.bt,
-                                             evecs.data_ptr(), s.ws.data_ptr(), s.ws.numel(), ops._stream()),
-               "dn_eig_finalize_batched")
+        _lib.call("dn_eig_finalize_batched", s.Q, B, cols, k, s.mass, s.bt, evecs, s.ws, s.ws.numel(), ops._stream())
         evals = theta_all[:, :k].clamp_min(0.0)
         rb = s.plan.row_begin
         for b, i in enumerate(stack):

@@ -55,9 +55,7 @@ class FmapSolveFn(torch.autograd.Function):
         n, d = A.shape
         _check_n(n, "functional-map solve")
         out = torch.empty(n, n, dtype=torch.float32, device=A.device)
-        _lib.check(_lib.load().dn_fmap_solve_fwd(A.data_ptr(), B.data_ptr(), ex.data_ptr(), ey.data_ptr(), n, d,
-                                                 float(lambda_param), out.data_ptr(), ops._stream()),
-                   "dn_fmap_solve_fwd")
+        _lib.call("dn_fmap_solve_fwd", A, B, ex, ey, n, d, float(lambda_param), out, ops._stream())
         ctx.lam = float(lambda_param)
         ctx.save_for_backward(A, B, ex, ey)
         return out
@@ -70,9 +68,7 @@ class FmapSolveFn(torch.autograd.Function):
         n, d = A.shape
         gA, gB = torch.empty_like(A), torch.empty_like(B)
         ws = torch.empty(16 * n * n, dtype=torch.uint8, device=A.device)
-        _lib.check(_lib.load().dn_fmap_solve_bwd(A.data_ptr(), B.data_ptr(), ex.data_ptr(), ey.data_ptr(), n, d, ctx.lam,
-                                                 g.data_ptr(), gA.data_ptr(), gB.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                 ops._stream()), "dn_fmap_solve_bwd")
+        _lib.call("dn_fmap_solve_bwd", A, B, ex, ey, n, d, ctx.lam, g, gA, gB, ws, ws.numel(), ops._stream())
         return gA, gB, None, None, None
 
 
@@ -204,12 +200,10 @@ def nearest_neighbor(source, target):
     Vt = target.shape[0]
     _check_n(n, "nearest_neighbor")
     out = torch.empty(Vs, dtype=torch.int64, device=source.device)
-    lib = _lib.load()
     with ops._on(source):
-        ws = torch.empty(max(int(lib.dn_nearest_neighbor_workspace_bytes(Vs, Vt, n)), 1), dtype=torch.uint8,
+        ws = torch.empty(max(int(_lib.load().dn_nearest_neighbor_workspace_bytes(Vs, Vt, n)), 1), dtype=torch.uint8,
                          device=source.device)
-        _lib.check(lib.dn_nearest_neighbor(source.data_ptr(), Vs, target.data_ptr(), Vt, n, out.data_ptr(),
-                                           ws.data_ptr(), ws.numel(), ops._stream()), "dn_nearest_neighbor")
+        _lib.call("dn_nearest_neighbor", source, Vs, target, Vt, n, out, ws, ws.numel(), ops._stream())
     return out
 
 
@@ -220,9 +214,7 @@ def _apply_basis_exact(values, basis):
     out = torch.empty(V, Cc, dtype=torch.float32, device=values.device)
     with ops._on(values):
         ws = ops.workspace(V, K, Cc, values.device)
-        _lib.check(_lib.load().dn_from_basis(values.data_ptr(), basis.data_ptr(), None, V, K, Cc, out.data_ptr(),
-                                             ws.data_ptr(), ws.numel(), _lib.ENGINE_SIMT, ops._stream()),
-                   "dn_from_basis")
+        _lib.call("dn_from_basis", values, basis, None, V, K, Cc, out, ws, ws.numel(), _lib.ENGINE_SIMT, ops._stream())
     return out
 
 
@@ -362,9 +354,8 @@ class ProjectBatchedFn(torch.autograd.Function):
         Cc = feat.shape[1]
         out = torch.empty(mb.n_meshes, pb.kp, Cc, dtype=torch.float32, device=feat.device)
         ws = _spectral_ws(pb, Cc)
-        _lib.check(_lib.load().dn_to_basis_batched(feat.data_ptr(), pb.basis.data_ptr(), mb.mass.data_ptr(),
-                                                   C.byref(mb.desc), mb.V, pb.kp, Cc, out.data_ptr(), ws.data_ptr(),
-                                                   ws.numel(), ops._engine, ops._stream()), "dn_to_basis_batched")
+        _lib.call("dn_to_basis_batched", feat, pb.basis, mb.mass, C.byref(mb.desc), mb.V, pb.kp, Cc, out, ws, ws.numel(),
+                  ops._engine, ops._stream())
         ctx.pb = pb
         return out
 
@@ -377,9 +368,8 @@ class ProjectBatchedFn(torch.autograd.Function):
         Cc = g.shape[2]
         gx = torch.empty(mb.V, Cc, dtype=torch.float32, device=g.device)
         ws = _spectral_ws(pb, Cc)
-        _lib.check(_lib.load().dn_from_basis_batched(g.data_ptr(), pb.basis.data_ptr(), mb.mass.data_ptr(),
-                                                     C.byref(mb.desc), mb.V, pb.kp, Cc, gx.data_ptr(), ws.data_ptr(),
-                                                     ws.numel(), ops._engine, ops._stream()), "dn_from_basis_batched")
+        _lib.call("dn_from_basis_batched", g, pb.basis, mb.mass, C.byref(mb.desc), mb.V, pb.kp, Cc, gx, ws, ws.numel(),
+                  ops._engine, ops._stream())
         return gx, None
 
 
@@ -405,10 +395,8 @@ class FmapSolveBatchedFn(torch.autograd.Function):
                              "n = {}".format(tuple(F_hat.shape), tuple(evals.shape), pairs.n_shapes, n))
         S, m, d = F_hat.shape
         out = torch.empty(pairs.n_pairs, n, n, dtype=torch.float32, device=F_hat.device)
-        _lib.check(_lib.load().dn_fmap_solve_fwd_batched(
-            F_hat.data_ptr(), m * d, evals.data_ptr(), evals.shape[1], S, pairs.pair_x.data_ptr(),
-            pairs.pair_y.data_ptr(), pairs.n_pairs, n, d, float(lambda_param), out.data_ptr(), ops._stream()),
-            "dn_fmap_solve_fwd_batched")
+        _lib.call("dn_fmap_solve_fwd_batched", F_hat, m * d, evals, evals.shape[1], S, pairs.pair_x, pairs.pair_y,
+                  pairs.n_pairs, n, d, float(lambda_param), out, ops._stream())
         ctx.pairs, ctx.n, ctx.lam = pairs, n, float(lambda_param)
         ctx.save_for_backward(F_hat, evals)
         return out
@@ -420,15 +408,12 @@ class FmapSolveBatchedFn(torch.autograd.Function):
         pairs, n = ctx.pairs, ctx.n
         g = ops._f32c(g)
         S, m, d = F_hat.shape
-        lib = _lib.load()
         gF = torch.zeros_like(F_hat)
-        ws = torch.empty(int(lib.dn_fmap_solve_batched_workspace_bytes(pairs.n_pairs, n, d)), dtype=torch.uint8,
+        ws = torch.empty(int(_lib.load().dn_fmap_solve_batched_workspace_bytes(pairs.n_pairs, n, d)), dtype=torch.uint8,
                          device=F_hat.device)
-        _lib.check(lib.dn_fmap_solve_bwd_batched(
-            F_hat.data_ptr(), m * d, evals.data_ptr(), evals.shape[1], S, pairs.pair_x.data_ptr(),
-            pairs.pair_y.data_ptr(), pairs.n_pairs, pairs._role_begin.data_ptr(), pairs._role_list.data_ptr(), n, d,
-            ctx.lam, g.data_ptr(), gF.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()),
-            "dn_fmap_solve_bwd_batched")
+        _lib.call("dn_fmap_solve_bwd_batched", F_hat, m * d, evals, evals.shape[1], S, pairs.pair_x, pairs.pair_y,
+                  pairs.n_pairs, pairs._role_begin, pairs._role_list, n, d, ctx.lam, g, gF, ws, ws.numel(),
+                  ops._stream())
         return gF, None, None, None, None
 
 
@@ -455,20 +440,18 @@ def pointwise_map_batch(C_pred, pair_batch, n_fmap=30):
         raise ValueError("pointwise_map_batch: C_pred {} does not hold {} pairs of n_fmap = {} (K = {})".format(
             tuple(C_pred.shape), P, n, mb.K))
     _check_n(n, "pointwise_map_batch")
-    lib = _lib.load()
     px, py = _lib.int_array(pb.pairs.pair_x_host), _lib.int_array(pb.pairs.pair_y_host)
     rb, nr = _lib.int_array(pb.row_begin_host), _lib.int_array(pb.n_rows_host)
     counts = [pb.n_rows_host[y] for y in pb.pairs.pair_y_host]
     with torch.no_grad(), ops._on(C_pred):
         Cm = ops._f32c(C_pred[:, :n, :n].contiguous())
         out = torch.empty(sum(counts), dtype=torch.int64, device=C_pred.device)
-        wsb = int(lib.dn_fmap_pointwise_map_batched_workspace_bytes(n, P, px, py, rb, nr, pb.n_shapes))
+        wsb = int(_lib.load().dn_fmap_pointwise_map_batched_workspace_bytes(n, P, px, py, rb, nr, pb.n_shapes))
         if wsb < 0:
             _lib.check(wsb, "dn_fmap_pointwise_map_batched_workspace_bytes")
         ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=C_pred.device)
-        _lib.check(lib.dn_fmap_pointwise_map_batched(Cm.data_ptr(), n, mb.evecs.data_ptr(), mb.K, rb, nr, pb.n_shapes,
-                                                     px, py, P, out.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                     ops._stream()), "dn_fmap_pointwise_map_batched")
+        _lib.call("dn_fmap_pointwise_map_batched", Cm, n, mb.evecs, mb.K, rb, nr, pb.n_shapes, px, py, P, out, ws,
+                  ws.numel(), ops._stream())
     return list(torch.split(out, counts))
 
 
@@ -480,10 +463,8 @@ _GT_BAD_PAIR, _GT_SINGULAR = 1, 2
 
 def _ground_truth_into(pds, ids, out, status, ws):
     """dn_fmap_ground_truth of device int64 pair ids into ``out`` (P, n, n); ``ws`` sized for P."""
-    _lib.check(_lib.load().dn_fmap_ground_truth(
-        pds.ds.evecs.data_ptr(), pds.ds.K, pds.n, pds._vts_rows.data_ptr(), pds._vts_begin.data_ptr(), pds.ds.n_meshes,
-        pds.pairs.data_ptr(), pds.n_table, ids.data_ptr(), ids.shape[0], pds.max_m, out.data_ptr(), status.data_ptr(),
-        ws.data_ptr(), ws.numel(), ops._stream()), "dn_fmap_ground_truth")
+    _lib.call("dn_fmap_ground_truth", pds.ds.evecs, pds.ds.K, pds.n, pds._vts_rows, pds._vts_begin, pds.ds.n_meshes,
+              pds.pairs, pds.n_table, ids, ids.shape[0], pds.max_m, out, status, ws, ws.numel(), ops._stream())
     return out
 
 

@@ -11,7 +11,7 @@ import os
 import numpy as np
 import torch
 
-from . import ops
+from . import _lib, ops
 
 
 def to_basis(values, basis, massvec):
@@ -246,8 +246,7 @@ def _vertex_normals(v64, f64, frames):
     nrm = torch.empty(V, 3, dtype=torch.float64, device=dev)
     nbad = torch.zeros(1, dtype=torch.int32, device=dev)
     ws = torch.empty(12 * F + 8 * V + 1024, dtype=torch.uint8, device=dev)
-    _lib_check(_lib_load().dn_vertex_frames(v64.data_ptr(), f64.data_ptr(), F, V, None, nrm.data_ptr(), frames.data_ptr(),
-                                            nbad.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()), "dn_vertex_frames")
+    _lib.call("dn_vertex_frames", v64, f64, F, V, None, nrm, frames, nbad, ws, ws.numel(), ops._stream())
     return nrm, int(nbad.item()) > 0
 
 
@@ -255,9 +254,9 @@ def _frames_from_normals(normals, dtype, frames):
     """dn_vertex_frames from given (V,3) normals into ``frames`` (V,3,3) fp64; the normals are rounded to ``dtype``
     first, as the reference converts them (geometry.py:144)."""
     nbad = torch.zeros(1, dtype=torch.int32, device=frames.device)
-    n_in = normals.to(device=frames.device, dtype=dtype).to(torch.float64).contiguous()
-    _lib_check(_lib_load().dn_vertex_frames(None, None, 0, int(frames.shape[0]), n_in.data_ptr(), None, frames.data_ptr(),
-                                            nbad.data_ptr(), None, 0, ops._stream()), "dn_vertex_frames")
+    _lib.call("dn_vertex_frames", None, None, 0, int(frames.shape[0]),
+              normals.to(device=frames.device, dtype=dtype).to(torch.float64).contiguous(), None, frames, nbad, None, 0,
+              ops._stream())
     return frames
 
 
@@ -294,7 +293,6 @@ def mesh_laplacian(v64, f64, eps=EPS, row_begin=None, first=0):
     hold): dn_mesh_laplacian_batched, which gives each mesh its own mass shift and bound.  ``bound`` is then a numpy
     array of n, an eighth value holds the offsets ``rowptr[row_begin]`` of the meshes' entries (numpy int64), and the
     NaN errors name their mesh, counted from ``first``."""
-    lib = _lib_load()
     V, F = int(v64.shape[0]), int(f64.shape[0])
     n = 1 if row_begin is None else int(row_begin.numel()) - 1
     dev = v64.device
@@ -308,16 +306,14 @@ def mesh_laplacian(v64, f64, eps=EPS, row_begin=None, first=0):
     bound = torch.empty(n, dtype=torch.float64, device=dev)
     nan = torch.empty(n, 2, dtype=torch.int32, device=dev)
     ws = torch.empty(120 * F + 12 * V + 2048, dtype=torch.uint8, device=dev)
-    out = (rowptr.data_ptr(), colidx.data_ptr(), lvals.data_ptr(), mass.data_ptr(), avals.data_ptr(), adiag.data_ptr(),
-           bound.data_ptr(), nan.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream())
+    out = (rowptr, colidx, lvals, mass, avals, adiag, bound, nan, ws, ws.numel(), ops._stream())
     if row_begin is None:
-        _lib_check(lib.dn_mesh_laplacian(v64.data_ptr(), f64.data_ptr(), F, V, eps, *out), "dn_mesh_laplacian")
+        _lib.call("dn_mesh_laplacian", v64, f64, F, V, eps, *out)
         ends = rowptr[-1:]
     else:
-        _lib_check(lib.dn_mesh_laplacian_batched(v64.data_ptr(), f64.data_ptr(), F, V, n, row_begin.data_ptr(), eps, *out),
-                   "dn_mesh_laplacian_batched")
+        _lib.call("dn_mesh_laplacian_batched", v64, f64, F, V, n, row_begin, eps, *out)
         ends = rowptr[row_begin.long()]
-    del ws
+    del ws, out
     host = torch.cat((bound, nan.flatten().double(), ends.double())).cpu().numpy()      # one read of all three
     bound_h, nan_h, nzb = host[:n], host[n:3 * n].reshape(n, 2), host[3 * n:].astype(np.int64)
     for b in range(n):
@@ -329,16 +325,6 @@ def mesh_laplacian(v64, f64, eps=EPS, row_begin=None, first=0):
     nnz = int(nzb[-1])
     csr = (rowptr, colidx[:nnz], lvals[:nnz], mass, avals[:nnz], adiag)
     return csr + (float(bound_h[0]),) if row_begin is None else csr + (bound_h, nzb)
-
-
-def _lib_load():
-    from . import _lib
-    return _lib.load()
-
-
-def _lib_check(code, what):
-    from . import _lib
-    _lib.check(code, what)
 
 
 def compute_operators(verts, faces, k_eig, normals=None, device=None, stats=None):
@@ -592,8 +578,6 @@ def build_grad_operators(verts, frames, edges, edge_tangent=None):
     range check and the entry count); fp64 2x2 solves like numpy; 1e-6-grade agreement with the reference
     (tests/test_gpu_parity.py).  Raises IndexError for edges outside [0, V), ValueError for an ``edge_tangent`` that is
     not (E, 2)."""
-    import ctypes as C
-    from . import _lib
     V = int(verts.shape[0])
     _check_edges(edges, V, edge_tangent)
     ops._require_cuda(verts)
@@ -608,9 +592,7 @@ def build_grad_operators(verts, frames, edges, edge_tangent=None):
     vals = torch.empty(max(E + V, 1), 2, dtype=torch.float32, device=dev)
     ws = torch.empty(max(4 * V, 4), dtype=torch.uint8, device=dev)
     with ops._on(verts):
-        _lib.check(_lib.load().dn_build_grad(verts.data_ptr(), frames.data_ptr(), et.data_ptr() if et is not None else None,
-                                             edges.data_ptr(), E, V, rowptr.data_ptr(), colidx.data_ptr(), vals.data_ptr(),
-                                             ws.data_ptr(), ws.numel(), ops._stream()), "dn_build_grad")
+        _lib.call("dn_build_grad", verts, frames, et, edges, E, V, rowptr, colidx, vals, ws, ws.numel(), ops._stream())
     nnz = int(rowptr[-1].item()) if V > 0 else 0
     return ops.GradOperators.from_csr(V, rowptr, colidx[:max(nnz, 1)] if nnz else colidx[:0], vals[:nnz])
 

@@ -102,13 +102,10 @@ class GradOperators:
         self._csr_t = None
 
     def _build(self, rows, cols, vx, vy):
-        lib = _lib.load()
         rowptr = torch.empty(self.V + 1, dtype=torch.int32, device=self.device)
         colidx = torch.empty(max(self.nnz, 1), dtype=torch.int32, device=self.device)
         vals = torch.empty(2 * max(self.nnz, 1), dtype=torch.float32, device=self.device)
-        _lib.check(lib.dn_csr_from_coo(rows.data_ptr(), cols.data_ptr(), vx.data_ptr(), vy.data_ptr(),
-                                       self.nnz, self.V, rowptr.data_ptr(), colidx.data_ptr(), vals.data_ptr(),
-                                       _stream()), "dn_csr_from_coo")
+        _lib.call("dn_csr_from_coo", rows, cols, vx, vy, self.nnz, self.V, rowptr, colidx, vals, _stream())
         st = _lib.dn_csr(rowptr.data_ptr(), colidx.data_ptr(), vals.data_ptr(), self.nnz)
         return (st, rowptr, colidx, vals)   # keep the tensors alive next to the struct
 
@@ -135,9 +132,8 @@ class GradOperators:
         vals = torch.empty(2 * max(self.nnz, 1), dtype=torch.float32, device=dev)
         scratch = torch.empty(max(self.V, 1), dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(_lib.load().dn_csr_transpose(C.byref(st_t), self.V, rowptr.data_ptr(), colidx.data_ptr(),
-                                                    vals.data_ptr(), scratch.data_ptr(), 4 * scratch.numel(),
-                                                    _stream()), "dn_csr_transpose")
+            _lib.call("dn_csr_transpose", C.byref(st_t), self.V, rowptr, colidx, vals, scratch, 4 * scratch.numel(),
+                      _stream())
         self.csr = (_lib.dn_csr(rowptr.data_ptr(), colidx.data_ptr(), vals.data_ptr(), self.nnz),
                     rowptr, colidx, vals)
         self._coo = None
@@ -205,7 +201,7 @@ class GradOperators:
         hp = lambda a: C.c_void_p(a.ctypes.data)
         n = _lib.load().dn_patch_build(V, hp(rp), hp(ci), int(max_targets), int(max_src), hp(tgt_ptr), hp(tgt),
                                        hp(src_ptr), hp(src_rows), hp(ent_ptr), hp(lcol), hp(perm), hp(worst))
-        if n == -2:                     # a row with more than max_src entries: the plain kernel keeps serving it
+        if n == _lib.ERR_UNSUPPORTED:   # a row with more than max_src entries: the plain kernel keeps serving it
             self._patches = False
             return self
         if n < 0:
@@ -244,9 +240,8 @@ class GradOperators:
             vt = torch.empty(2 * max(self.nnz, 1), dtype=torch.float32, device=self.device)
             scratch = torch.empty(max(self.V, 1), dtype=torch.int32, device=self.device)
             with torch.cuda.device(self.device):
-                _lib.check(_lib.load().dn_csr_transpose(C.byref(self.csr[0]), self.V, rt.data_ptr(), ct.data_ptr(),
-                                                        vt.data_ptr(), scratch.data_ptr(), 4 * scratch.numel(),
-                                                        _stream()), "dn_csr_transpose")
+                _lib.call("dn_csr_transpose", C.byref(self.csr[0]), self.V, rt, ct, vt, scratch, 4 * scratch.numel(),
+                          _stream())
             self._csr_t = (_lib.dn_csr(rt.data_ptr(), ct.data_ptr(), vt.data_ptr(), self.nnz), rt, ct, vt)
         if self._csr_t is None:
             rows, cols, vx, vy = self._coo
@@ -353,15 +348,12 @@ class LaplacianCSR:
         idx = Lc.indices()
         self.nnz = int(idx.shape[1])
         vals = _f32c(Lc.values())
-        lib = _lib.load()
         rowptr = torch.empty(self.V + 1, dtype=torch.int32, device=self.device)
         colidx = torch.empty(max(self.nnz, 1), dtype=torch.int32, device=self.device)
         cv = torch.empty(2 * max(self.nnz, 1), dtype=torch.float32, device=self.device)
-        rows, cols = idx[0].contiguous(), idx[1].contiguous()
         with _on(vals):
-            _lib.check(lib.dn_csr_from_coo(rows.data_ptr(), cols.data_ptr(), vals.data_ptr(), None, self.nnz, self.V,
-                                           rowptr.data_ptr(), colidx.data_ptr(), cv.data_ptr(), _stream()),
-                       "dn_csr_from_coo")
+            _lib.call("dn_csr_from_coo", idx[0].contiguous(), idx[1].contiguous(), vals, None, self.nnz, self.V, rowptr,
+                      colidx, cv, _stream())
         self.csr = (_lib.dn_csr(rowptr.data_ptr(), colidx.data_ptr(), cv.data_ptr(), self.nnz), rowptr, colidx, cv)
 
     @classmethod
@@ -428,13 +420,10 @@ def to_basis_raw(values, basis, massvec):
     V, K = basis.shape
     Cc = values.shape[-1]
     out = torch.empty(K, Cc, dtype=torch.float32, device=values.device)
-    mv = _f32c(massvec) if massvec is not None else None
     with _on(values):
         ws = workspace(V, K, Cc, values.device)
-        _lib.check(_lib.load().dn_to_basis(values.data_ptr(), basis.data_ptr(),
-                                           mv.data_ptr() if mv is not None else None, V, K, Cc,
-                                           out.data_ptr(), ws.data_ptr(), ws.numel(), _engine, _stream()),
-                   "dn_to_basis")
+        _lib.call("dn_to_basis", values, basis, _f32c(massvec) if massvec is not None else None, V, K, Cc, out, ws,
+                  ws.numel(), _engine, _stream())
     return out
 
 
@@ -444,12 +433,10 @@ def from_basis_raw(values, basis, row_scale=None):
     V, K = basis.shape
     Cc = values.shape[-1]
     out = torch.empty(V, Cc, dtype=torch.float32, device=values.device)
-    rs = _f32c(row_scale) if row_scale is not None else None
     with _on(values):
         ws = workspace(V, K, Cc, values.device)
-        _lib.check(_lib.load().dn_from_basis(values.data_ptr(), basis.data_ptr(),
-                                             rs.data_ptr() if rs is not None else None, V, K, Cc, out.data_ptr(),
-                                             ws.data_ptr(), ws.numel(), _engine, _stream()), "dn_from_basis")
+        _lib.call("dn_from_basis", values, basis, _f32c(row_scale) if row_scale is not None else None, V, K, Cc, out,
+                  ws, ws.numel(), _engine, _stream())
     return out
 
 
@@ -527,8 +514,7 @@ def compute_hks_raw(evals, evecs, scales):
     S = scales.shape[0]
     out = torch.empty(V, S, dtype=torch.float32, device=evecs.device)
     with torch.cuda.device(evecs.device):
-        _lib.check(_lib.load().dn_compute_hks(evals.data_ptr(), evecs.data_ptr(), scales.data_ptr(), V, K, S,
-                                              out.data_ptr(), _stream()), "dn_compute_hks")
+        _lib.call("dn_compute_hks", evals, evecs, scales, V, K, S, out, _stream())
     return out
 
 
@@ -537,8 +523,7 @@ def grad_spmm_raw(ops: GradOperators, x):
     V, Cc = x.shape
     out = torch.empty(V, Cc, 2, dtype=torch.float32, device=x.device)
     with _on(x):
-        _lib.check(_lib.load().dn_grad_spmm(C.byref(ops.csr[0]), x.data_ptr(), V, Cc, out.data_ptr(), _stream()),
-                   "dn_grad_spmm")
+        _lib.call("dn_grad_spmm", C.byref(ops.csr[0]), x, V, Cc, out, _stream())
     return out
 
 
@@ -546,14 +531,10 @@ def spatial_gradient_features_raw(vectors, A_re, A_im):
     vectors = _f32c(vectors)
     V, Cc, _ = vectors.shape
     out = torch.empty(V, Cc, dtype=torch.float32, device=vectors.device)
-    a_re = _f32c(A_re)                                  # contiguous copies stay referenced until the call returns
-    a_im = _f32c(A_im) if A_im is not None else None
     with _on(vectors):
         ws = workspace(V, Cc, Cc, vectors.device)
-        _lib.check(_lib.load().dn_spatial_gradient_features_fwd(
-            vectors.data_ptr(), a_re.data_ptr(), a_im.data_ptr() if a_im is not None else None,
-            1 if a_im is not None else 0, V, Cc, out.data_ptr(), ws.data_ptr(), ws.numel(), _engine, _stream()),
-            "dn_spatial_gradient_features_fwd")
+        _lib.call("dn_spatial_gradient_features_fwd", vectors, _f32c(A_re), _f32c(A_im) if A_im is not None else None,
+                  1 if A_im is not None else 0, V, Cc, out, ws, ws.numel(), _engine, _stream())
     return out
 
 
@@ -579,7 +560,6 @@ def block_forward_raw(x_in, mass, evals, evecs, ops, time, A_re, A_im, weights, 
     (see batch.MeshBatch) when ``x_in`` / the operators are a batch laid out as one vertex range.  ``out``: a
     contiguous fp32 tensor on ``x_in``'s device that receives the result ((V, C), or (V, n_out) with ``head``) and is
     returned; it must not overlap ``x_in``.  None allocates it."""
-    lib = _lib.load()
     x_in, mass, evals, evecs = _f32c(x_in), _f32c(mass), _f32c(evals), _f32c(evecs)
     V, Cc = x_in.shape
     K = evecs.shape[1]
@@ -591,7 +571,7 @@ def block_forward_raw(x_in, mass, evals, evecs, ops, time, A_re, A_im, weights, 
         raise ValueError("block_forward_raw: out must be a contiguous float32 ({}, {}) tensor on {}".format(
             V, n_res, x_in.device))
     dims = [weights[0].shape[1]] + [w.shape[0] for w in weights]
-    # contiguous copies (if any were needed) must outlive the launch: keep them in locals, not temporaries
+    # the parameter struct holds raw pointers: contiguous copies (if any were needed) must outlive the launch
     wc = [_f32c(w) for w in weights]
     bc = [_f32c(b) if b is not None else None for b in biases]
     a_re = _f32c(A_re) if A_re is not None else None
@@ -615,25 +595,23 @@ def block_forward_raw(x_in, mass, evals, evecs, ops, time, A_re, A_im, weights, 
                 hb = _f32c(head[1]) if head[1] is not None else None
                 hd = _lib.dn_head(hw.data_ptr(), hb.data_ptr() if hb is not None else None, int(hw.shape[0]),
                                   out.data_ptr(), int(hw.shape[0]))
-            rc = lib.dn_block_fwd_ex(x_in.data_ptr(), mass.data_ptr(), evals.data_ptr(), evecs.data_ptr(), csr, C.byref(prm),
-                                     C.byref(batch_desc) if batch_desc is not None else None,
-                                     C.byref(hd) if hd is not None else None, V, K, Cc,
-                                     None if head is not None else out.data_ptr(), ws.data_ptr(), ws.numel(), _engine,
-                                     _stream())
-            if rc == -2 and head is not None:      # DN_ERR_UNSUPPORTED: the chain that would carry the head is not available
+            rc = _lib.load().dn_block_fwd_ex(x_in.data_ptr(), mass.data_ptr(), evals.data_ptr(), evecs.data_ptr(), csr,
+                                             C.byref(prm), C.byref(batch_desc) if batch_desc is not None else None,
+                                             C.byref(hd) if hd is not None else None, V, K, Cc,
+                                             None if head is not None else out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                             _engine, _stream())
+            if rc == _lib.ERR_UNSUPPORTED and head is not None:   # the chain that would carry the head is not available
                 raise HeadNotFused()
             _lib.check(rc, "dn_block_fwd_ex")
             return out
         if profile is not None:
-            ms = (C.c_float * 6)()
-            _lib.check(lib.dn_block_fwd_profile(x_in.data_ptr(), mass.data_ptr(), evals.data_ptr(), evecs.data_ptr(),
-                                                csr, C.byref(prm), V, K, Cc, out.data_ptr(), ws.data_ptr(),
-                                                ws.numel(), _engine, _stream(), ms), "dn_block_fwd_profile")
+            ms = (C.c_float * _lib.PROFILE_STAGES)()
+            _lib.call("dn_block_fwd_profile", x_in, mass, evals, evecs, csr, C.byref(prm), V, K, Cc, out, ws,
+                      ws.numel(), _engine, _stream(), ms)
             profile[:] = [float(v) for v in ms]
             return out
-        _lib.check(lib.dn_block_fwd(x_in.data_ptr(), mass.data_ptr(), evals.data_ptr(), evecs.data_ptr(), csr,
-                                    C.byref(prm), V, K, Cc, out.data_ptr(), ws.data_ptr(), ws.numel(), _engine,
-                                    _stream()), "dn_block_fwd")
+        _lib.call("dn_block_fwd", x_in, mass, evals, evecs, csr, C.byref(prm), V, K, Cc, out, ws, ws.numel(), _engine,
+                  _stream())
     return out
 
 
@@ -647,7 +625,6 @@ class DiffusionFn(torch.autograd.Function):
     @staticmethod
     @_device_guard
     def forward(ctx, x, time, mass, evals, evecs):
-        lib = _lib.load()
         x, mass, evals, evecs = _f32c(x), _f32c(mass), _f32c(evals), _f32c(evecs)
         V, Cc = x.shape
         K = evecs.shape[1]
@@ -655,17 +632,14 @@ class DiffusionFn(torch.autograd.Function):
         x_spec = torch.empty(K, Cc, dtype=torch.float32, device=x.device)
         ws = workspace(V, K, Cc, x.device)
         # the kernel clamps `time` in place, as the reference does on the Parameter (layers.py:48-49)
-        _lib.check(lib.dn_learned_time_diffusion_fwd(x.data_ptr(), mass.data_ptr(), evals.data_ptr(),
-                                                     evecs.data_ptr(), time.data_ptr(), V, K, Cc, xd.data_ptr(),
-                                                     x_spec.data_ptr(), ws.data_ptr(), ws.numel(), _engine,
-                                                     _stream()), "dn_learned_time_diffusion_fwd")
+        _lib.call("dn_learned_time_diffusion_fwd", x, mass, evals, evecs, time, V, K, Cc, xd, x_spec, ws, ws.numel(),
+                  _engine, _stream())
         ctx.save_for_backward(mass, evals, evecs, time.detach().clone(), x_spec)
         return xd
 
     @staticmethod
     @_device_guard
     def backward(ctx, g):
-        lib = _lib.load()
         mass, evals, evecs, time, x_spec = ctx.saved_tensors
         g = _f32c(g)
         V, Cc = g.shape
@@ -673,10 +647,8 @@ class DiffusionFn(torch.autograd.Function):
         gx = torch.empty_like(g)
         gt = torch.zeros_like(time)
         ws = workspace(V, K, Cc, g.device)
-        _lib.check(lib.dn_learned_time_diffusion_bwd(g.data_ptr(), mass.data_ptr(), evals.data_ptr(),
-                                                     evecs.data_ptr(), time.data_ptr(), x_spec.data_ptr(), V, K, Cc,
-                                                     gx.data_ptr(), gt.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                     _engine, _stream()), "dn_learned_time_diffusion_bwd")
+        _lib.call("dn_learned_time_diffusion_bwd", g, mass, evals, evecs, time, x_spec, V, K, Cc, gx, gt, ws,
+                  ws.numel(), _engine, _stream())
         return gx, gt, None, None, None
 
 
@@ -686,7 +658,8 @@ implicit_last_status = None  # host copy of the last solve's status (iterations 
 
 
 def _implicit_call(what, fn, V, Cc, device, args, outs, n_meshes=None):
-    """Run one dn_implicit_diffusion_* call (``args`` before rtol / max_iter, ``outs`` after) and raise if a column did
+    """Run one dn_implicit_diffusion_* call ``fn`` (``args`` before rtol / max_iter, ``outs`` after; tensors passed as
+    their addresses) and raise if a column did
     not converge: one host read of the device status per solve.  ``n_meshes``: a _batched call, whose status has one
     column per (mesh, channel) pair."""
     lib = _lib.load()
@@ -696,8 +669,8 @@ def _implicit_call(what, fn, V, Cc, device, args, outs, n_meshes=None):
               lib.dn_implicit_diffusion_workspace_bytes_batched(V, Cc, n_meshes))
     ws = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
     max_iter = int(IMPLICIT_MAX_ITER)
-    _lib.check(fn(*args, float(IMPLICIT_RTOL), max_iter, *outs, status.data_ptr(), ws.data_ptr(), ws.numel(),
-                  _stream()), what)
+    _lib.check(fn(*_lib.addresses((*args, float(IMPLICIT_RTOL), max_iter, *outs, status, ws, ws.numel(), _stream()))),
+               what)
     global implicit_last_status
     st = implicit_last_status = status.cpu()
     if st[0] > 0:
@@ -733,8 +706,7 @@ class ImplicitDiffusionFn(torch.autograd.Function):
                 tuple(x.shape), tuple(mass.shape), tuple(time.shape), lap.V, lap.V))
         y = torch.empty_like(x)
         _implicit_call("dn_implicit_diffusion_fwd", lib.dn_implicit_diffusion_fwd, V, Cc, x.device,
-                       (C.byref(lap.csr[0]), x.data_ptr(), mass.data_ptr(), time.data_ptr(), V, Cc),
-                       (y.data_ptr(),))
+                       (C.byref(lap.csr[0]), x, mass, time, V, Cc), (y,))
         ctx.lap = lap
         ctx.save_for_backward(mass, time.detach().clone(), y)
         return y
@@ -749,8 +721,7 @@ class ImplicitDiffusionFn(torch.autograd.Function):
         gx = torch.empty_like(g)
         gt = torch.zeros_like(time)
         _implicit_call("dn_implicit_diffusion_bwd", lib.dn_implicit_diffusion_bwd, V, Cc, g.device,
-                       (C.byref(ctx.lap.csr[0]), g.data_ptr(), mass.data_ptr(), time.data_ptr(), y.data_ptr(), V, Cc),
-                       (gx.data_ptr(), gt.data_ptr()))
+                       (C.byref(ctx.lap.csr[0]), g, mass, time, y, V, Cc), (gx, gt))
         return gx, gt, None, None
 
 
@@ -775,9 +746,8 @@ class BatchedImplicitDiffusionFn(torch.autograd.Function):
                 tuple(x.shape), tuple(time.shape), batch.V))
         y = torch.empty_like(x)
         _implicit_call("dn_implicit_diffusion_fwd_batched", lib.dn_implicit_diffusion_fwd_batched, V, Cc, x.device,
-                       (C.byref(batch.lap.csr[0]), x.data_ptr(), batch.mass.data_ptr(), time.data_ptr(),
-                        C.byref(batch.desc), batch._mesh_rows.data_ptr(), V, Cc), (y.data_ptr(),),
-                       n_meshes=batch.n_meshes)
+                       (C.byref(batch.lap.csr[0]), x, batch.mass, time, C.byref(batch.desc), batch._mesh_rows, V, Cc),
+                       (y,), n_meshes=batch.n_meshes)
         ctx.batch = batch
         ctx.save_for_backward(time.detach().clone(), y)
         return y
@@ -793,9 +763,8 @@ class BatchedImplicitDiffusionFn(torch.autograd.Function):
         gx = torch.empty_like(g)
         gt = torch.zeros_like(time)
         _implicit_call("dn_implicit_diffusion_bwd_batched", lib.dn_implicit_diffusion_bwd_batched, V, Cc, g.device,
-                       (C.byref(batch.lap.csr[0]), g.data_ptr(), batch.mass.data_ptr(), time.data_ptr(), y.data_ptr(),
-                        C.byref(batch.desc), batch._mesh_rows.data_ptr(), V, Cc), (gx.data_ptr(), gt.data_ptr()),
-                       n_meshes=batch.n_meshes)
+                       (C.byref(batch.lap.csr[0]), g, batch.mass, time, y, C.byref(batch.desc), batch._mesh_rows, V,
+                        Cc), (gx, gt), n_meshes=batch.n_meshes)
         return gx, gt, None
 
 
@@ -812,7 +781,6 @@ class BatchedDiffusionFn(torch.autograd.Function):
     @staticmethod
     @_device_guard
     def forward(ctx, x, time, batch):
-        lib = _lib.load()
         x = _f32c(x)
         V, Cc = x.shape
         K, B = batch.K, batch.n_meshes
@@ -822,10 +790,8 @@ class BatchedDiffusionFn(torch.autograd.Function):
         x_spec = torch.empty(B, K, Cc, dtype=torch.float32, device=x.device)
         ws = workspace(V, K, Cc, x.device, extra=batched_diffusion_workspace_extra(B, K, Cc))
         # the kernel clamps `time` in place, as the reference does on the Parameter (layers.py:48-49)
-        _lib.check(lib.dn_learned_time_diffusion_fwd_batched(
-            x.data_ptr(), batch.mass.data_ptr(), batch.evals.data_ptr(), batch.evecs.data_ptr(), time.data_ptr(),
-            C.byref(batch.desc), V, K, Cc, xd.data_ptr(), x_spec.data_ptr(), ws.data_ptr(), ws.numel(), _engine,
-            _stream()), "dn_learned_time_diffusion_fwd_batched")
+        _lib.call("dn_learned_time_diffusion_fwd_batched", x, batch.mass, batch.evals, batch.evecs, time,
+                  C.byref(batch.desc), V, K, Cc, xd, x_spec, ws, ws.numel(), _engine, _stream())
         ctx.batch = batch
         ctx.save_for_backward(time.detach().clone(), x_spec)
         return xd
@@ -833,7 +799,6 @@ class BatchedDiffusionFn(torch.autograd.Function):
     @staticmethod
     @_device_guard
     def backward(ctx, g):
-        lib = _lib.load()
         time, x_spec = ctx.saved_tensors
         batch = ctx.batch
         g = _f32c(g)
@@ -842,10 +807,8 @@ class BatchedDiffusionFn(torch.autograd.Function):
         gx = torch.empty_like(g)
         gt = torch.zeros_like(time)
         ws = workspace(V, K, Cc, g.device, extra=batched_diffusion_workspace_extra(B, K, Cc))
-        _lib.check(lib.dn_learned_time_diffusion_bwd_batched(
-            g.data_ptr(), batch.mass.data_ptr(), batch.evals.data_ptr(), batch.evecs.data_ptr(), time.data_ptr(),
-            x_spec.data_ptr(), C.byref(batch.desc), V, K, Cc, gx.data_ptr(), gt.data_ptr(), ws.data_ptr(), ws.numel(),
-            _engine, _stream()), "dn_learned_time_diffusion_bwd_batched")
+        _lib.call("dn_learned_time_diffusion_bwd_batched", g, batch.mass, batch.evals, batch.evecs, time, x_spec,
+                  C.byref(batch.desc), V, K, Cc, gx, gt, ws, ws.numel(), _engine, _stream())
         return gx, gt, None
 
 
@@ -855,7 +818,6 @@ class GradFeaturesFn(torch.autograd.Function):
     @staticmethod
     @_device_guard
     def forward(ctx, xd, A_re, A_im, ops):
-        lib = _lib.load()
         xd, A_re = _f32c(xd), _f32c(A_re)
         A_im = _f32c(A_im) if A_im is not None else None
         V, Cc = xd.shape
@@ -863,10 +825,8 @@ class GradFeaturesFn(torch.autograd.Function):
         feat = torch.empty_like(xd)
         pq = torch.empty(V, (2 if rot else 1) * Cc, dtype=torch.float32, device=xd.device)
         ws = workspace(V, Cc, Cc, xd.device)
-        _lib.check(lib.dn_gradient_features_fwd(C.byref(ops.csr[0]), xd.data_ptr(), A_re.data_ptr(),
-                                                A_im.data_ptr() if rot else None, 1 if rot else 0, V, Cc,
-                                                feat.data_ptr(), pq.data_ptr(), ws.data_ptr(), ws.numel(), _engine,
-                                                _stream()), "dn_gradient_features_fwd")
+        _lib.call("dn_gradient_features_fwd", C.byref(ops.csr[0]), xd, A_re, A_im, 1 if rot else 0, V, Cc, feat, pq, ws,
+                  ws.numel(), _engine, _stream())
         ctx.ops = ops
         ctx.rot = rot
         ctx.save_for_backward(xd, pq, feat, A_re, A_im if rot else A_re)
@@ -875,7 +835,6 @@ class GradFeaturesFn(torch.autograd.Function):
     @staticmethod
     @_device_guard
     def backward(ctx, g):
-        lib = _lib.load()
         xd, pq, feat, A_re, A_im = ctx.saved_tensors
         ops, rot = ctx.ops, ctx.rot
         g = _f32c(g)
@@ -884,11 +843,8 @@ class GradFeaturesFn(torch.autograd.Function):
         gAre = torch.zeros_like(A_re)
         gAim = torch.zeros_like(A_im) if rot else None
         ws = workspace(V, Cc, Cc, xd.device)
-        _lib.check(lib.dn_gradient_features_bwd(
-            C.byref(ops.csr[0]), C.byref(ops.csr_t[0]), g.data_ptr(), xd.data_ptr(), pq.data_ptr(), feat.data_ptr(),
-            A_re.data_ptr(), A_im.data_ptr() if rot else None, 1 if rot else 0, V, Cc, gx.data_ptr(),
-            gAre.data_ptr(), gAim.data_ptr() if rot else None, ws.data_ptr(), ws.numel(), _engine, _stream()),
-            "dn_gradient_features_bwd")
+        _lib.call("dn_gradient_features_bwd", C.byref(ops.csr[0]), C.byref(ops.csr_t[0]), g, xd, pq, feat, A_re,
+                  A_im if rot else None, 1 if rot else 0, V, Cc, gx, gAre, gAim, ws, ws.numel(), _engine, _stream())
         return gx, gAre, gAim, None
 
 
@@ -901,7 +857,6 @@ class MLPFn(torch.autograd.Function):
     @staticmethod
     @_device_guard
     def forward(ctx, n_src, n_layers, has_res, drop_p, *t):
-        lib = _lib.load()
         srcs = [_f32c(s) for s in t[:n_src]]
         weights = [_f32c(w) for w in t[n_src:n_src + n_layers]]
         biases = [(_f32c(b) if b is not None else None) for b in t[n_src + n_layers:n_src + 2 * n_layers]]
@@ -922,14 +877,13 @@ class MLPFn(torch.autograd.Function):
                      .mul_(1.0 / (1.0 - drop_p)) for l in range(n_layers - 1)]
         out = torch.empty(V, dims[-1], dtype=torch.float32, device=dev)
         ws = workspace(V, max(dims[1:]), max(max(dims[1:]), (max(dims) + 2) // 3), dev)
-        _lib.check(lib.dn_mini_mlp_fwd(
-            _lib.ptr_array([s.data_ptr() for s in srcs]), _lib.int_array([s.shape[1] for s in srcs]), n_src,
-            _lib.ptr_array([w.data_ptr() for w in weights]),
-            _lib.ptr_array([b.data_ptr() if b is not None else None for b in biases]), _lib.int_array(dims),
-            n_layers, _lib.ptr_array([m.data_ptr() for m in masks]) if masks else None,
-            residual.data_ptr() if residual is not None else None, V,
-            _lib.ptr_array([h.data_ptr() for h in hidden]) if hidden else None, out.data_ptr(), ws.data_ptr(),
-            ws.numel(), _engine, _stream()), "dn_mini_mlp_fwd")
+        _lib.call("dn_mini_mlp_fwd",
+                  _lib.ptr_array([s.data_ptr() for s in srcs]), _lib.int_array([s.shape[1] for s in srcs]), n_src,
+                  _lib.ptr_array([w.data_ptr() for w in weights]),
+                  _lib.ptr_array([b.data_ptr() if b is not None else None for b in biases]), _lib.int_array(dims),
+                  n_layers, _lib.ptr_array([m.data_ptr() for m in masks]) if masks else None, residual, V,
+                  _lib.ptr_array([h.data_ptr() for h in hidden]) if hidden else None, out, ws, ws.numel(), _engine,
+                  _stream())
         ctx.meta = (n_src, n_layers, has_res, dims, [b is not None for b in biases])
         ctx.save_for_backward(*srcs, *weights, *hidden, *masks)
         ctx.n_hidden, ctx.n_masks = len(hidden), len(masks)
@@ -938,7 +892,6 @@ class MLPFn(torch.autograd.Function):
     @staticmethod
     @_device_guard
     def backward(ctx, g):
-        lib = _lib.load()
         n_src, n_layers, has_res, dims, has_bias = ctx.meta
         sv = ctx.saved_tensors
         srcs = sv[:n_src]
@@ -953,14 +906,14 @@ class MLPFn(torch.autograd.Function):
         gb = [torch.zeros(w.shape[0], dtype=torch.float32, device=dev) if hb else None
               for w, hb in zip(weights, has_bias)]
         ws = workspace(V, max(dims[1:]), max(max(dims[1:]), (max(dims) + 2) // 3), dev)
-        _lib.check(lib.dn_mini_mlp_bwd(
-            g.data_ptr(), _lib.ptr_array([s.data_ptr() for s in srcs]),
-            _lib.int_array([s.shape[1] for s in srcs]), n_src, _lib.ptr_array([w.data_ptr() for w in weights]),
-            _lib.int_array(dims), n_layers, _lib.ptr_array([h.data_ptr() for h in hidden]) if hidden else None,
-            _lib.ptr_array([m.data_ptr() for m in masks]) if masks else None, V,
-            _lib.ptr_array([x.data_ptr() for x in gs]), _lib.ptr_array([x.data_ptr() for x in gw]),
-            _lib.ptr_array([x.data_ptr() if x is not None else None for x in gb]), ws.data_ptr(), ws.numel(),
-            _engine, _stream()), "dn_mini_mlp_bwd")
+        _lib.call("dn_mini_mlp_bwd",
+                  g, _lib.ptr_array([s.data_ptr() for s in srcs]), _lib.int_array([s.shape[1] for s in srcs]), n_src,
+                  _lib.ptr_array([w.data_ptr() for w in weights]), _lib.int_array(dims), n_layers,
+                  _lib.ptr_array([h.data_ptr() for h in hidden]) if hidden else None,
+                  _lib.ptr_array([m.data_ptr() for m in masks]) if masks else None, V,
+                  _lib.ptr_array([x.data_ptr() for x in gs]), _lib.ptr_array([x.data_ptr() for x in gw]),
+                  _lib.ptr_array([x.data_ptr() if x is not None else None for x in gb]), ws, ws.numel(), _engine,
+                  _stream())
         res = (g,) if has_res else ()
         return (None, None, None, None, *gs, *gw, *gb, *res)
 
@@ -988,13 +941,11 @@ class LinearNLLFn(torch.autograd.Function):
         nll = torch.empty(R, dtype=torch.float32, device=x.device)
         lse = torch.empty(R, dtype=torch.float32, device=x.device)
         pred = torch.empty(R, dtype=torch.int64, device=x.device)
-        lib = _lib.load()
-        args = (x.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None else None, labels.data_ptr(), R,
-                Cc, n_class, int(ignore_index), nll.data_ptr(), pred.data_ptr(), lse.data_ptr(), _engine, _stream())
+        args = (x, weight, bias, labels, R, Cc, n_class, int(ignore_index), nll, pred, lse, _engine, _stream())
         if label_smoothing:
-            _lib.check(lib.dn_linear_nll_ls_fwd(*args, float(label_smoothing)), "dn_linear_nll_ls_fwd")
+            _lib.call("dn_linear_nll_ls_fwd", *args, float(label_smoothing))
         else:
-            _lib.check(lib.dn_linear_nll_fwd(*args), "dn_linear_nll_fwd")
+            _lib.call("dn_linear_nll_fwd", *args)
         ctx.save_for_backward(x, weight, bias, labels, lse)
         ctx.ignore_index = int(ignore_index)
         ctx.label_smoothing = float(label_smoothing)
@@ -1011,16 +962,14 @@ class LinearNLLFn(torch.autograd.Function):
         gx = torch.empty_like(x)
         gw = torch.empty_like(weight)
         gb = torch.empty_like(bias) if bias is not None else None
-        lib = _lib.load()
-        ws_bytes = lib.dn_linear_nll_workspace_bytes(R, Cc, n_class)
+        ws_bytes = _lib.load().dn_linear_nll_workspace_bytes(R, Cc, n_class)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        args = (x.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None else None, labels.data_ptr(),
-                lse.data_ptr(), g.data_ptr(), R, Cc, n_class, ctx.ignore_index, gx.data_ptr(), gw.data_ptr(),
-                gb.data_ptr() if gb is not None else None, ws.data_ptr(), ws_bytes, _engine, _stream())
+        args = (x, weight, bias, labels, lse, g, R, Cc, n_class, ctx.ignore_index, gx, gw, gb, ws, ws_bytes, _engine,
+                _stream())
         if ctx.label_smoothing:
-            _lib.check(lib.dn_linear_nll_ls_bwd(*args, ctx.label_smoothing), "dn_linear_nll_ls_bwd")
+            _lib.call("dn_linear_nll_ls_bwd", *args, ctx.label_smoothing)
         else:
-            _lib.check(lib.dn_linear_nll_bwd(*args), "dn_linear_nll_bwd")
+            _lib.call("dn_linear_nll_bwd", *args)
         return gx, gw, gb, None, None, None
 
 
@@ -1093,8 +1042,7 @@ class ElementMeanFn(torch.autograd.Function):
         V, Cc = x.shape
         E, k = elems.shape
         out = torch.empty(E, Cc, dtype=torch.float32, device=x.device)
-        _lib.check(_lib.load().dn_element_mean_fwd(x.data_ptr(), V, Cc, elems.data_ptr(), E, k, out.data_ptr(),
-                                                   _stream()), "dn_element_mean_fwd")
+        _lib.call("dn_element_mean_fwd", x, V, Cc, elems, E, k, out, _stream())
         ctx.save_for_backward(*csr)
         ctx.shape = (V, Cc, E, k)
         return out
@@ -1106,8 +1054,7 @@ class ElementMeanFn(torch.autograd.Function):
         V, Cc, E, k = ctx.shape
         g = _f32c(g)
         gx = torch.empty(V, Cc, dtype=torch.float32, device=g.device)
-        _lib.check(_lib.load().dn_element_mean_bwd(g.data_ptr(), E, Cc, rowptr.data_ptr(), ent.data_ptr(), V, k,
-                                                   gx.data_ptr(), _stream()), "dn_element_mean_bwd")
+        _lib.call("dn_element_mean_bwd", g, E, Cc, rowptr, ent, V, k, gx, _stream())
         return gx, None, None
 
 
@@ -1203,12 +1150,10 @@ class GlobalMeanPoolFn(torch.autograd.Function):
         V, Cc = x.shape
         pooled = torch.empty(seg.n_seg, Cc, dtype=torch.float32, device=x.device)
         msum = torch.empty(seg.n_seg, dtype=torch.float32, device=x.device)
-        lib = _lib.load()
-        ws_bytes = lib.dn_global_mean_workspace_bytes(V, Cc)
+        ws_bytes = _lib.load().dn_global_mean_workspace_bytes(V, Cc)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        _lib.check(lib.dn_global_mean_fwd(x.data_ptr(), mass.data_ptr(), V, Cc, seg.begin.data_ptr(),
-                                          seg.rows.data_ptr(), seg.tile_seg.data_ptr(), seg.n_seg, pooled.data_ptr(),
-                                          msum.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "dn_global_mean_fwd")
+        _lib.call("dn_global_mean_fwd", x, mass, V, Cc, seg.begin, seg.rows, seg.tile_seg, seg.n_seg, pooled, msum, ws,
+                  ws_bytes, _stream())
         ctx.save_for_backward(mass, msum)
         ctx.seg, ctx.shape = seg, (V, Cc)
         return pooled
@@ -1221,9 +1166,8 @@ class GlobalMeanPoolFn(torch.autograd.Function):
         V, Cc = ctx.shape
         g = _f32c(g)
         gx = torch.empty(V, Cc, dtype=torch.float32, device=g.device)
-        _lib.check(_lib.load().dn_global_mean_bwd(g.data_ptr(), mass.data_ptr(), msum.data_ptr(), V, Cc,
-                                                  seg.begin.data_ptr(), seg.rows.data_ptr(), seg.tile_seg.data_ptr(),
-                                                  seg.n_seg, gx.data_ptr(), _stream()), "dn_global_mean_bwd")
+        _lib.call("dn_global_mean_bwd", g, mass, msum, V, Cc, seg.begin, seg.rows, seg.tile_seg, seg.n_seg, gx,
+                  _stream())
         return gx, None, None
 
 
